@@ -45,10 +45,14 @@ METRIC = "candidate schedules/sec"
 UNIT = "candidates/s"
 J, S, G = 256, 8, 8
 WORKLOAD = "C4: J=256 jobs x S=8 strategies x G=1..8 GPUs, synthetic T (seed 0), integer starts"
-WAVE = 148 * 8 * 32           # candidates in one half wave of 32-candidate tiles (148 SMs x 16 resident warps / 2)
-B_PER_GPU = WAVE * 28         # 1,060,864 candidates = 14 whole tiles for every resident warp of the persistent
-                              # grid (no idle warps in a last partial wave) = 543 MB of encodings per step (> 126 MB L2)
-FALLBACK_HBM_GBS = 6650.0
+WAVE = 132 * 8 * 32           # candidates in one half wave of 32-candidate tiles (H100 SXM: 132 SMs x 16 resident warps / 2)
+B_PER_GPU = WAVE * 28         # 946,176 candidates = 14 whole tiles for every resident warp of the persistent grid on an
+                              # H100 SXM (no idle warps in a last partial wave) = 484 MB of encodings per step (> 50 MB L2).
+                              # A constant, not the device's SM count, so that the workload and --dump-outputs are the
+                              # same on every machine; on a part with another SM count the last wave is partial.
+FALLBACK_HBM_GBS = 3350.0     # H100 SXM data sheet (not a measurement)
+DUMP_LIMIT = 4 * 1024 * 1024  # --dump-outputs: at most this many makespans; a larger batch dumps a seeded sample of them
+                              # plus their indices: 4 B + 8 B per entry = 48 MiB at most, under the 64 MB cap
 
 
 def bytes_per_candidate(j):
@@ -57,7 +61,7 @@ def bytes_per_candidate(j):
 
 
 class ClockSampler:
-    """nvidia-smi sampler running during the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampler (read-only queries) running during the timed region: SM clock and throttle reasons."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -114,7 +118,7 @@ def measured_peak():
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return FALLBACK_HBM_GBS, "fallback (B200_PROFILING.md)"
+        return FALLBACK_HBM_GBS, "fallback (H100 SXM data sheet, 3.35 TB/s)"
 
 
 def ncu_traffic():
@@ -128,11 +132,27 @@ def ncu_traffic():
         return None, None
 
 
+def dump_outputs(d, out, key):
+    """What the timed path hands its caller: the makespan of every candidate (float32; a seeded sample of
+    DUMP_LIMIT of them, with their indices, for larger batches) and the folded arg-min key, split into the
+    best makespan (float32) and the id of the candidate that reached it (float64, exact)."""
+    os.makedirs(d, exist_ok=True)
+    mk = out.cpu().numpy().astype(np.float32)
+    if mk.size > DUMP_LIMIT:
+        idx = np.sort(np.random.default_rng(0).choice(mk.size, DUMP_LIMIT, replace=False))
+        np.save(os.path.join(d, "makespans_index.npy"), idx.astype(np.float64))
+        mk = mk[idx]
+    np.save(os.path.join(d, "makespans.npy"), mk)
+    k = int(key.item())
+    np.save(os.path.join(d, "best_makespan.npy"), np.array([k >> 32], dtype=np.uint32).view(np.float32))
+    np.save(os.path.join(d, "best_candidate.npy"), np.array([k & 0xffffffff], dtype=np.float64))
+
+
 def static_config(ints=True, config="C4"):
     """The `config` object both arms print (identical for the same run shape, so the driver's same_config holds)."""
     return {"workload": WORKLOAD, "integer_starts": bool(ints),
             "l2": "no flush needed: every step streams its whole input once — GPU arm %.0f MB of candidate encodings "
-                  "per GPU per step (> 126 MB L2); CPU arm >= 2 M candidate evaluations per step" % (
+                  "per GPU per step (> 50 MB L2); CPU arm >= 2 M candidate evaluations per step" % (
                       B_PER_GPU * 2 * 256 / 1e6)}
 
 
@@ -229,7 +249,7 @@ def milp_leg_finish(proc, eng, c4_tasks, c4_plan_makespan, c4_wall):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=200)
+    ap.add_argument("--steps", type=int, default=None, help="timed steps (default 200; 5 for --impl reference)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--batch", type=int, default=B_PER_GPU, help="candidates per GPU per step")
@@ -243,11 +263,15 @@ def main():
     ap.add_argument("--solve-devices", type=int, default=0,
                     help="N = 1 only, opt-in: also time saturn.solver.solve(..., devices=D) — ONE process driving D GPUs "
                          "(it touches GPUs beyond --gpus, so it is never run by default)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed to DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
     if args.impl == "reference":
-        if args.steps == 200:
+        if args.steps is None:
             args.steps = 5                                            # default K for the CPU arm: minutes, not hours
         return run_reference(args)
+    if args.steps is None:
+        args.steps = 200
     args.warmup = max(args.warmup, 3)
 
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -367,6 +391,8 @@ def main():
     e1.record()
     barrier()
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out, key)
     if use_xchg:
         eng.xchg_check()
     ms_total = e0.elapsed_time(e1)
@@ -546,8 +572,7 @@ def main():
                                           "encoding of the J > 512 search)" if by_pos else
                                           "job-indexed opt, full table" if name == "C3" else
                                           "job-indexed opt, all 8 strategies (256 KB of table): rows re-ordered on the "
-                                          "device, position-major kernel reading the table through L1 (round 1: tile "
-                                          "kernel path 4, 1.2e8)")}
+                                          "device, position-major kernel reading the table through L1")}
             del oc, pc, outc
         # the kernel shape the north star sketches (slot times across lanes + warp shuffles), same C4 candidates
         eng.set_table(T)
@@ -580,8 +605,8 @@ def main():
                 "traffic": dram if headline else None, "eval_path": kernel_path,
                 "kernel": "k_eval_tiles<1,%s,true>" % ("true" if ints else "false"),
                 "kernel_ms": kern_ms_max, "algorithmic_bytes_per_launch": alg, "peak_source": peak_src,
-                "note": "instruction-issue / ALU-pipe bound, not HBM bound: one list-scheduling step is ~51 SASS "
-                        "instructions per warp of 32 candidates for 64 bytes of input; see DESIGN.md 5.1 and profiles/"}
+                "note": "instruction-issue / ALU-pipe bound, not HBM bound: one list-scheduling step is dozens of SASS "
+                        "instructions per warp of 32 candidates for 64 bytes of input; see DESIGN.md 5.1"}
         cpu = None
         milp = None
         if world == 1 and not args.no_cpu:

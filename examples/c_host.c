@@ -5,7 +5,7 @@
  *   prob.solve(), milp.py:321-327) -> sb_decode (replaces reading the MILP variables, milp.py:330-352)
  *
  * Build:  gcc -O2 -Iinclude examples/c_host.c -Lsaturn_b200 -lsaturn_b200 -Wl,-rpath,$PWD/saturn_b200 -lm -o c_host
- * Run:    ./c_host [J] [seed]          (prints the plan; needs a B200)
+ * Run:    ./c_host [J] [seed]          (prints the plan; needs an H100)
  * Output is line-oriented so that tests/test_gpu_solver.py can re-score the plan with the CPU oracle. */
 #include <math.h>
 #include <stdint.h>

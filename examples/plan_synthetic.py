@@ -1,4 +1,4 @@
-"""Plan a synthetic multi-model workload with the B200 solver through Saturn's own API.
+"""Plan a synthetic multi-model workload with the H100 solver through Saturn's own API.
 
     python examples/plan_synthetic.py [--jobs 32] [--nodes 1] [--devices 1] [--dense]
 

@@ -1,11 +1,11 @@
-/* saturn_b200.h — C ABI of the B200-native SPASE solver hot path.
+/* saturn_b200.h — C ABI of the H100-native SPASE solver hot path.
  *
  * This is the drop-in boundary for the ONE path of knagrecha/saturn that this
  * repository accelerates: `saturn.solver.solve()` (reference
  * saturn/solver/milp.py:23-445), whose arithmetic the reference delegates to a
  * third-party MILP binary (PuLP -> Gurobi/CBC, milp.py:321-327).  The library
  * replaces that solver call with a parallel search over list-schedule
- * candidates evaluated by hand-written sm_100a CUDA kernels.
+ * candidates evaluated by hand-written sm_90a CUDA kernels.
  *
  * Conventions
  *   - extern "C", plain pointers and sizes, no torch / Python types.
@@ -31,7 +31,7 @@
  *   B * row_stride elements (the last row included: the aligned paths fetch whole 16- / 32-byte
  *   chunks of every row, and sb_eval_host copies B * row_stride elements per buffer).  Rows that are
  *   32-byte aligned (base pointers and byte strides multiples of 32) take the
- *   fast path (TMA bulk copies + 256-bit streaming loads); 16-byte aligned rows
+ *   fast path (TMA bulk copies + 32-byte streaming loads); 16-byte aligned rows
  *   use TMA bulk copies only; anything else is fetched with plain loads.
  *
  * Evaluation rule (one node, 8 GPU slots; reference milp.py:62,139-149,209-319)
@@ -90,7 +90,7 @@ typedef enum sb_status {
                                      slot times spread over 8 lanes and combined with warp shuffles (the shape
                                      BASELINE.json's north_star sketches), 4 candidates per warp.  Same results;
                                      kept to be measured against the shipped lane-per-candidate kernel
-                                     (profiles/r02_alt_shape.md), not to be used. */
+                                     (bench.py configs.C4_alt_shape), not to be used. */
 #define SB_IPC_HANDLE_BYTES 64
 
 typedef struct sb_handle sb_handle;
@@ -138,10 +138,9 @@ int sb_eval(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, int64
  *     on the device (a scratch buffer of B * row_stride bytes owned by the handle, grow-only) and scored by the
  *     position-major kernel as under 5 / 8,
  * 8 = position-major kernel with the table in global memory, read through L1 / L2 (a one-node table beyond one
- *     SM's shared memory), 7 = the same with the table split over the shared memory of CTA pairs (test hook:
- *     measured, slower than 8),
+ *     SM's shared memory), 7 = the same with the table split over the shared memory of CTA pairs (test hook),
  * 6 = the alternate warp-shuffle kernel (SB_FLAG_ALT_WARPSCAN),
- * 5 = position-major kernel (SB_FLAG_OPT_BY_POSITION): both rows streamed with 256-bit loads,
+ * 5 = position-major kernel (SB_FLAG_OPT_BY_POSITION): both rows streamed, 32 bytes per lane per load,
  * 4 = as 3 but with the runtime table read from global memory (it does not fit in shared memory; what
  *     sb_eval_host, whose speed is PCIe's, still takes),
  * 3 = tile kernel, opt rows by TMA bulk copy + prio rows streamed with 256-bit loads (rows 32-byte
@@ -221,8 +220,7 @@ typedef struct sb_search_params {
                          * with (r - 1) % resample_every == 0 — inside the round kernel where the rows are resident
                          * in shared memory (rivals = the 32 chains of a warp, re-dealt between launches), with the
                          * sb_search_resample kernel otherwise.  0: only when the caller calls sb_search_resample.  -1: automatic
-                         * (2 where the tournament runs inside the round kernel, 4 where it is a copy of the population;
-                         * profiles/r01_search_round.md). */
+                         * (2 where the tournament runs inside the round kernel, 4 where it is a copy of the population). */
 } sb_search_params;
 
 int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_opt /*host, nullable*/,
@@ -290,7 +288,7 @@ int sb_search_run_multi(sb_handle** handles, int n, const sb_search_params* p, c
                         void* prio_out /*host [J]*/, sb_search_result* result);
 /* Population size that fills the device exactly once with the round kernel this table gets (resident warps
  * per SM x 32 lanes x SMs).  A population that is a whole multiple of it leaves no partially filled last
- * wave: 131,072 chains on 148 SMs x 12 warps are 2.3 waves and cost 3. */
+ * wave: 131,072 chains on 132 SMs x 12 warps are 2.6 waves and cost 3. */
 int sb_search_wave(sb_handle* h, unsigned flags, int64_t* chains);
 /* 1 if rounds run as ONE fused kernel (move + evaluate + accept), 0 if they run as propose / evaluate /
  * accept kernels.  Fused rounds keep both rows of a tile's 32 candidates in shared memory when they fit

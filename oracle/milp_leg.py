@@ -60,8 +60,7 @@ def main():
                        "formula": "vars = J*S + J*N + 2*N*G*J + J*(J-1) + 1; rows = 2J + N*G*J*S + 4*J*N*S + 2*J*N*S*G + "
                                   "2*S*N*G*J*(J-1), N=1, G=8 (SURVEY §8a A2/A3)",
                        "result": "not built: 8.4 M rows of Python/PuLP expression objects (milp.py:277-319 is an "
-                                 "O(G*J^2*S) Python loop); HiGHS has no incumbent at J=24 within 30 s already "
-                                 "(profiles/r01_milp_vs_gpu.md)"}
+                                 "O(G*J^2*S) Python loop); HiGHS has no incumbent at J=24 within 30 s already"}
     print(json.dumps(out), flush=True)
 
 

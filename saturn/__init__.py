@@ -1,4 +1,4 @@
-"""Import-path alias: `import saturn` resolves to the B200-native implementation in saturn_b200.
+"""Import-path alias: `import saturn` resolves to the H100-native implementation in saturn_b200.
 
 Keeps the reference's entry points (saturn/__init__.py:1, saturn/solver/__init__.py:1-2,
 saturn/core/representations/__init__.py:1-2) importable without PuLP, Ray or Gurobi.  Submodules

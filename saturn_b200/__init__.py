@@ -1,4 +1,4 @@
-"""saturn_b200 — Blackwell-native SPASE solver hot path behind Saturn's own solver API.
+"""saturn_b200 — Hopper-native (H100, sm_90a) SPASE solver hot path behind Saturn's own solver API.
 
 Public surface (mirrors the reference's module layout, see the `saturn/` alias package):
     saturn_b200.solver.solve / convert_into_comprehensible     <- saturn.solver

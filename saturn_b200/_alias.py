@@ -58,6 +58,6 @@ def reference_attr(pkg_name, module_file, attr):
                     raise
             return getattr(mod, attr)
     raise ImportError(
-        "%s.%s is not part of the B200 solver drop-in (it implements saturn.solver, saturn.orchestrate, "
+        "%s.%s is not part of the saturn_b200 solver drop-in (it implements saturn.solver, saturn.orchestrate, "
         "saturn.core.representations and saturn.executor.forecast only) and no reference `saturn` "
         "distribution was found on sys.path to fall through to" % (pkg_name, attr))

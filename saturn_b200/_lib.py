@@ -58,7 +58,7 @@ def load():
         return _lib
     if not os.path.exists(SO_PATH):
         raise SaturnB200Error(
-            "%s is missing — build it with `python -m saturn_b200.build` (nvcc, sm_100a). "
+            "%s is missing — build it with `python -m saturn_b200.build` (nvcc, sm_90a). "
             "saturn_b200 has no CPU fallback." % SO_PATH)
     lib = C.CDLL(SO_PATH)
     vp, i64, u32, ci = C.c_void_p, C.c_int64, C.c_uint, C.c_int

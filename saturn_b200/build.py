@@ -1,4 +1,4 @@
-"""In-tree build of libsaturn_b200.so (nvcc, sm_100a only).
+"""In-tree build of libsaturn_b200.so (nvcc, sm_90a only).
 
     python -m saturn_b200.build [--force]
 
@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "libsaturn_b200.so")
 SOURCES = ["sb_api.cu", "sb_eval.cu", "sb_eval_alt.cu", "sb_table.cu", "sb_search.cu", "sb_xchg.cu"]
 HEADERS = ["sb_common.cuh", "sb_lane.cuh", "sb_internal.h", "sb_search.h", os.path.join("..", "..", "include", "saturn_b200.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
 

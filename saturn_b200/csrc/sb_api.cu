@@ -169,8 +169,8 @@ int sb_create(int device, void* stream, sb_handle** out) {
   CK(cudaSetDevice(device));
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major < 10)
-    return fail(SB_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_100a only", device, prop.major,
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(SB_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major,
                 prop.minor);
   sb_handle* h = new (std::nothrow) sb_handle();
   if (!h) return fail(SB_ERR_NOMEM, "out of host memory");
@@ -355,8 +355,7 @@ int sb_eval(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, int64
   // Job-indexed rows where the tile kernel runs short of shared memory — a table that does not fit beside the
   // tiles (C5 with all strategies: 256 KB, tile kernel path 4) or J >= 1024 (33 KB of opt tile per warp: 5 warps
   // per SM): re-order the opt bytes into schedule order on the device (h->by_pos, B x row_stride bytes, grow-only)
-  // and score them with the position-major kernel.  Measured on C5, 227,328 candidates: 3.6e8 against 1.3e8
-  // candidates/s (full table), 3.9e8 against 3.3e8 (reduced table); profiles/r02_table_homes.md.
+  // and score them with the position-major kernel, which keeps no tile and streams both rows.
   // Test hooks: 0x00200000 takes this route at any size, 0x00100000 never.
   {
     const bool hooks = (flags & (0x80000000u | 0x40000000u | 0x00100000u | SB_FLAG_POST_KEY | SB_FLAG_FOLD_PREV |
@@ -1111,8 +1110,8 @@ static int search_run_impl(sb_handle** hs, int n, const sb_search_params* p, con
     if (!wired && (rc = sb_xchg_connect_local(hs, n))) return rc;
   }
   // population set-up (allocation on first use, initialisation, first scoring, LPT seeds: several host
-  // synchronisations per device) runs on one host thread per device — done one device after the other it was
-  // 0.75 s of a 1.03 s C5 search on 8 devices (profiles/r02_c5_anneal_8dev_v1.md)
+  // synchronisations per device) runs on one host thread per device — done one device after the other it
+  // dominates a short multi-device search
   auto setup = [&](int i) -> int {
     sb_search_params pp = *p;
     pp.total_rounds = c->rounds;

@@ -1,12 +1,12 @@
-// sb_common.cuh — shared device helpers for the SPASE candidate evaluator (sm_100a only).
+// sb_common.cuh — shared device helpers for the SPASE candidate evaluator (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include "../../include/saturn_b200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "saturn_b200 kernels target sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "saturn_b200 kernels target sm_90a (H100) only"
 #endif
 
 namespace sb {
@@ -97,9 +97,8 @@ __device__ __forceinline__ void tma_bulk_g2s(void* dst_smem, const void* src_gme
 // window) is produced by a 3-stage barrel shifter on the bits of km1: no dynamic register
 // indexing, no divergence.
 //
-// Instruction mix, shaped by the ncu captures in profiles/r01_summary.md — the kernel is bound by
-// instruction issue, and before that by the ALU pipe, so work is spread over the pipes at the
-// lowest instruction count found (54 per step):
+// Instruction mix: the step is bound by instruction issue, and before that by the ALU pipe, so work
+// is spread over the ALU and FMA pipes at a low instruction count:
 //   stage "by 4", lower half : 4 FSEL (ALU); predicates come from the bit inside the asm so that
 //                              ptxas derives all three stage predicates with ONE R2P of the opt byte
 //   stage "by 4", upper half : x = f + m with m = bit ? +inf : -0.0  (1 FSEL + 4 FADD, FMA pipe;
@@ -129,11 +128,8 @@ __device__ __forceinline__ float psel(float a, float b, int bit) {
   return r;
 }
 
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));  // one FMNMX3
-  return d;
-}
+// sm_90 has no 3-input max.f32: two FMNMX (max is exact, so the grouping does not change the result)
+__device__ __forceinline__ float fmax3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
 
 // kTrackMk: fold this job's completion (s + rt) into mk.  Needed with integer starts (the slot
 // state holds s + ceil(rt), not the completion) and with several nodes (no single f[7] at the end).

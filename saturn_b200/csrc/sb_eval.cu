@@ -12,13 +12,13 @@
 //     TMA bulk copy into a padded shared-memory row (the opt bytes are gathered by job id, so
 //     they must be resident), completion on a per-warp mbarrier — no CTA-wide barrier after
 //     start-up.  The prio row is consumed in order, so in the STREAM variant (rows 32-byte
-//     aligned) each lane streams it straight from HBM with 256-bit loads (one full 32-byte sector
-//     per lane, prefetched 32 steps ahead) and it never touches shared memory: 8.7 KB of smem per
-//     warp instead of 17.4 KB -> 16 resident warps per SM instead of 8 (ncu r01b: with 2 warps per
-//     scheduler 31 % of issue slots were lost to dependency waits).  Unaligned rows fall back to
+//     aligned) each lane streams it straight from HBM, one full 32-byte sector per lane (two
+//     128-bit loads, prefetched 32 steps ahead), and it never touches shared memory: 8.7 KB of smem
+//     per warp instead of 17.4 KB -> 16 resident warps per SM instead of 8 (with 2 warps per
+//     scheduler, dependency waits leave issue slots empty).  Unaligned rows fall back to
 //     the non-STREAM variant (prio rows staged in shared memory, TMA or plain loads);
 //   * one candidate per LANE: the 8 slot ready-times live sorted in 8 registers and one
-//     scheduling step is ~51 instructions (sb_common.cuh: ls_step) — fp32 min/max/add and byte
+//     scheduling step is a few dozen instructions (sb_common.cuh: ls_step) — fp32 min/max/add and byte
 //     indexing only, no tensor cores;
 //   * MULTI variant (several nodes, milp.py:117-137: a gang stays inside one node): the sorted
 //     state of every node lives in a lane-private shared-memory column (2 x float4 per node,
@@ -107,9 +107,8 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
   // warp), and only spins — bounded — after its last tile.  The publish of this round is in the tail.
   bool fold_pending = a.xp.counter != nullptr && a.xp.fold_prev && a.xp.seq > 1 && blockIdx.x == 0 && warp == 0;
   // a look = two loads per lane (round number with acquire, then the key), ISSUED at one tile boundary and
-  // CONSUMED at the next: the NVLink round trip (~2 us) overlaps the tile's 16 us of evaluation instead of
-  // stalling this warp — every warp has the same number of tiles, so the folding warp's stalls were the
-  // kernel's tail (+4 us per step at N > 1 in the first round-2 version, profiles/r02_bench_8gpu.md)
+  // CONSUMED at the next: the NVLink round trip overlaps the tile's evaluation instead of stalling this
+  // warp — every warp has the same number of tiles, so the folding warp's stalls would be the kernel's tail
   unsigned long long pf_seen = 0ull, pf_key = ~0ull;
   auto look_issue = [&]() {
     if (lane < a.xp.x.world) {
@@ -263,9 +262,8 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
       }
       const uint4* prow = reinterpret_cast<const uint4*>(prio_row_s);
       // ONE copy of the unrolled step body in this loop: the kernel is instruction-fetch bound as soon as the
-      // hot path spans several unrolled bodies (the first version, a window loop around CPW unrolled reads and
-      // three inlined call sites, ran at 29 % issue-active with 6.9 "no instruction" stalls per issue,
-      // profiles/r02_search_inc_v1_raw.csv)
+      // hot path spans several unrolled bodies (a window loop around CPW unrolled reads and three inlined call
+      // sites stalls on instruction fetch)
 #pragma unroll 1
       for (int c = w0 * CPW; c < nch; ++c) {
         if (save && c > w0 * CPW && (c % CPW) == 0) {
@@ -352,8 +350,8 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
             // ... and its boundary snapshots, from the rival's current buffers into this lane's current buffers.
             // ALL loads of a batch (up to 7 boundaries = 63 words; the evaluation registers are free here) are
             // issued before the first store, so a tournament costs one trip to L2 / HBM per batch, not one per
-            // boundary (the first version copied boundary by boundary: 7 dependent round trips every other round
-            // made the incremental kernel 2x SLOWER than scoring from position 0, profiles/r02_incremental.md).
+            // boundary (copying boundary by boundary costs 7 dependent round trips every other round, enough to
+            // make incremental scoring slower than scoring from position 0).
             const uint32_t rpar = __shfl_sync(0xffffffffu, par, rival);
             constexpr int kBatch = 7;
             for (int b0s = 0; b0s < nwin - 1; b0s += kBatch) {
@@ -786,8 +784,7 @@ static cudaError_t dispatch_search(const Device& dev, const TileArgs& a, const T
 
 // 2 = both rows of a candidate fit in shared memory for at least 8 warps: the tile kernel runs the fused
 // round (all moves); 0 = they do not: the search keeps a position-major population (sb_search.cu: 16 warps
-// at any J; already 1.5x faster per round at J = 400 where only 5 tile warps fit,
-// profiles/r01_search_round.md) or, when even the table does not fit, runs unfused rounds
+// at any J, where only a few tile warps would fit) or, when even the table does not fit, runs unfused rounds
 int search_round_mode(const Device& dev, int J, int SG, int nodes) {
   const int pb = J <= 256 ? 1 : 2;
   TilePlan tp;

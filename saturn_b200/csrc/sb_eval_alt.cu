@@ -4,7 +4,7 @@
 // It exists to be measured next to the shipped kernel (one candidate per LANE, sb_eval.cu), not to be used:
 // SURVEY.md §7 H2 asked for the alternates behind the same ABI with ncu / the clock deciding, and DESIGN.md
 // §5.1 only argued by instruction count.  Selected with SB_FLAG_ALT_WARPSCAN; same inputs, bit-identical
-// makespans (tests/test_gpu_parity.py); numbers in profiles/r02_alt_shape.md.
+// makespans (tests/test_gpu_parity.py); bench.py reports its rate as configs.C4_alt_shape.
 //
 // Shape: 8 slots = 8 lanes, so a warp carries 4 candidates (lever (i) of SURVEY H2 — one candidate per
 // 32-lane warp would leave 24 lanes idle in every instruction below).  The 8 ready-times of a candidate are

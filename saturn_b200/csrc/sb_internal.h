@@ -10,7 +10,7 @@ namespace sb {
 struct Device {
   int ordinal = 0;
   int sm_count = 0;
-  size_t smem_optin = 0;  // max dynamic shared memory per CTA (227 KB on B200)
+  size_t smem_optin = 0;  // max dynamic shared memory per CTA (227 KB on H100)
 };
 
 // peer-memory MIN exchange (sb_xchg.cu)

@@ -10,16 +10,19 @@ struct PrioChunk {
 };
 // kReadOnly: the rows are not written during the kernel (evaluation) -> non-coherent path; the fused
 // search round writes accepted moves back into the same rows, so it uses the coherent form.
+// sm_90 has no 256-bit global load: the 32-byte chunk (p 32-byte aligned, one sector) is two 128-bit loads.
 template <bool kReadOnly>
 __device__ __forceinline__ PrioChunk ld_prio32(const uint8_t* p) {
   PrioChunk c;
   if (kReadOnly) {
-    asm volatile("ld.global.nc.L1::no_allocate.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+    asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
+                 "ld.global.nc.L1::no_allocate.v4.u32 {%4,%5,%6,%7}, [%8+16];"
                  : "=r"(c.w[0]), "=r"(c.w[1]), "=r"(c.w[2]), "=r"(c.w[3]), "=r"(c.w[4]), "=r"(c.w[5]), "=r"(c.w[6]),
                    "=r"(c.w[7])
                  : "l"(p));
   } else {
-    asm volatile("ld.global.L1::no_allocate.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+    asm volatile("ld.global.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
+                 "ld.global.L1::no_allocate.v4.u32 {%4,%5,%6,%7}, [%8+16];"
                  : "=r"(c.w[0]), "=r"(c.w[1]), "=r"(c.w[2]), "=r"(c.w[3]), "=r"(c.w[4]), "=r"(c.w[5]), "=r"(c.w[6]),
                    "=r"(c.w[7])
                  : "l"(p)
@@ -32,7 +35,7 @@ __device__ __forceinline__ PrioChunk ld_prio32(const uint8_t* p) {
 // ADDR = 1 (shared-memory table and opt rows only): the two look-up addresses of a step are formed with
 // `mad.lo` on run-time multipliers, which ptxas must issue as IMAD on the FMA pipe instead of IADD3 / LEA on
 // the ALU pipe — the step is bound by the ALU pipe (half rate) and by issue together, so the same instruction
-// count with two fewer ALU instructions is the cheaper mix (profiles/r02_summary.md).
+// count with two fewer ALU instructions is the cheaper mix.
 template <bool INT, bool MULTI, int ADDR = 0>
 struct LaneState {
   float f[8];
@@ -177,7 +180,7 @@ __device__ __forceinline__ void keep_best_tail(const SearchFuse& sf) {
 // are the chains' CURRENT candidates; every lane applies its own random move to its private
 // shared-memory rows, scores the result, decides acceptance and — only when accepted — writes the
 // few changed bytes back to the chain's rows in HBM.  No proposal buffer, no separate propose /
-// accept kernels (they cost 60 % of an unfused round at 1 M chains, profiles/r01_search_round.md).
+// accept kernels (the bulk of an unfused round's traffic).
 struct Move {
   int kind;  // 0 none, 1 opt byte of job a changed, 2 positions a,b swapped, 3 positions [a..b] rewritten
   int a, b;

@@ -59,9 +59,8 @@ __global__ void k_init_population(SearchDev s) {
 }
 
 // ---- initial population, built in SHARED memory: one thread per chain shuffles its priority row there
-// (the Fisher-Yates swaps are dependent random accesses: ~30 clk each in shared memory instead of a
-// global-memory round trip — the serial per-thread version above cost 3.7 ms per 1 M chains,
-// profiles/r01_launch_shares.md), then the CTA writes the finished rows out with coalesced 32-bit stores
+// (the Fisher-Yates swaps are dependent random accesses: a shared-memory access each instead of the
+// global-memory round trip of the serial per-thread version above), then the CTA writes the finished rows out with coalesced 32-bit stores
 // (padding included, so the rows need no memset).  The shuffle draws from a per-chain 32-bit LCG seeded by the
 // counter-based generator (one IMAD per draw on the serial path instead of two 64-bit mixes); the option
 // bytes are independent of each other, so they are not staged at all: the write-out derives the four bytes of a
@@ -418,8 +417,8 @@ __device__ __forceinline__ PosMove make_pos_move_win(const SearchFuse& sf, int r
 // 1 = left in global memory and read through L1 / L2 (the default for such tables: this kernel keeps no tile
 // in shared memory, so the launch asks for the whole array as L1);
 // 2 = split over the shared memory of a CTA PAIR (cluster of 2): each CTA loads one half with TMA and every
-// look-up is a `ld.shared::cluster` to whichever CTA owns the entry (distributed shared memory) — built and
-// measured, 3x slower than 1, kept behind a test hook (profiles/r02_table_homes.md).
+// look-up is a `ld.shared::cluster` to whichever CTA owns the entry (distributed shared memory) — the
+// alternative to 1, kept behind a test hook.
 template <int PB, bool INT, bool MULTI, bool EVAL = false, int TAB = 0>
 __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
   static_assert(TAB == 0 || (EVAL && !MULTI), "tables outside the CTA's shared memory: scoring only, one node");
@@ -844,10 +843,9 @@ cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float
 
 // Where the position-major scoring kernel keeps a table of J x SG entries: 0 = every CTA's shared memory;
 // a one-node table that does not fit there: 1 = global memory, read through L1 / L2 (with no tile in shared
-// memory the SM's whole array is L1: 5.4e8 candidates/s on the 256 KB C5 table against 6.2e8 for a table in
-// shared memory, profiles/r02_table_homes.md); -1 = nowhere (multi-node table beyond shared memory).
-// Test hooks in flags: 0x00400000 forces 2 (split over CTA pairs — measured, 3x slower than 1: scattered 4-byte
-// ld.shared::cluster), 0x00800000 forces 1.
+// memory the SM's whole array is L1); -1 = nowhere (multi-node table beyond shared memory).
+// Test hooks in flags: 0x00400000 forces 2 (split over CTA pairs: scattered 4-byte ld.shared::cluster),
+// 0x00800000 forces 1.
 int eval_pos_home(const Device& dev, int J, int SG, int nodes, unsigned flags) {
   const bool pair_ok = nodes == 1 && static_cast<size_t>(pos_tab_half(J, SG)) * 4 + 16 <= dev.smem_optin;
   if (flags & 0x00400000u) return pair_ok ? 2 : -1;

@@ -5,7 +5,7 @@
     python scripts/anneal.py --config C5 --devices 8 ...      # ONE process driving 8 devices (sb_search_run_multi)
 
 Prints the best-makespan-vs-time curve (rank 0) as a markdown table: the "1e9-candidate anneal on
-8xB200; makespan vs reference MILP wall-clock" item of BASELINE.json (the MILP column is "no
+8xH100; makespan vs reference MILP wall-clock" item of BASELINE.json (the MILP column is "no
 incumbent": HiGHS finds none at J = 24 in 30 s and the J = 1024 model has 134 M rows).
 """
 import argparse
@@ -71,7 +71,7 @@ def main():
                 t, n, mk = h[i]
                 print("| %.3f | %.2e | %.1f | %.2f %% |" % (t, n, mk, 100 * (mk / lb - 1)))
         print("\nreference MILP on the same T: model of %d x %d tasks/options cannot be built (SURVEY §8a: 134 M rows "
-              "at J=1024; HiGHS has no incumbent at J=24 after 30 s, profiles/r01_milp_vs_gpu.md)" % (J, 8))
+              "at J=1024; HiGHS has no incumbent at J=24 after 30 s)" % (J, 8))
     if world > 1 and args.devices <= 1:
         dist.destroy_process_group()
 

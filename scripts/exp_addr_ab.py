@@ -10,9 +10,10 @@ from saturn_b200.engine import Engine, random_candidates  # noqa: E402
 from saturn_b200.synth import synth_table  # noqa: E402
 
 eng = Engine(0)
+SMS = torch.cuda.get_device_properties(0).multi_processor_count
 T, valid = synth_table(256, 8, 8, seed=0)
 eng.set_table(T)
-B = 148 * 8 * 32 * 28
+B = SMS * 8 * 32 * 28
 opt, prio = random_candidates(eng, B, valid, seed=1)
 out = torch.empty(B, dtype=torch.float32, device="cuda")
 ref = eng.eval(opt, prio, _plain_addr=True).clone()

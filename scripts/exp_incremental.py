@@ -2,7 +2,7 @@
 incremental (snapshots).  Prints a markdown table: ms per round at ~1 M chains (C4, reduced table) and the
 plan quality / wall time of whole searches at the solve() population.
 
-    python scripts/exp_incremental.py > profiles/r02_incremental.md
+    python scripts/exp_incremental.py
 """
 import os
 import sys

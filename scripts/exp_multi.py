@@ -4,10 +4,11 @@ import numpy as np, torch
 from saturn_b200.engine import Engine, random_candidates
 from saturn_b200.synth import synth_table
 eng = Engine(0)
+SMS = torch.cuda.get_device_properties(0).multi_processor_count
 for nodes in (2, 4):
     T, valid = synth_table(256, 1, 8, seed=0, masked=False)
     eng.set_table(T, nodes=nodes)
-    B = 148 * 16 * 32 * 8
+    B = SMS * 16 * 32 * 8
     opt, prio = random_candidates(eng, B, valid, seed=1, nodes=nodes)
     for _ in range(3): eng.eval(opt, prio, reduced=True)
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)

@@ -7,8 +7,9 @@ from saturn_b200.engine import Engine, random_candidates, opt_by_position
 from saturn_b200.synth import synth_table
 
 eng = Engine(0)
+SMS = torch.cuda.get_device_properties(0).multi_processor_count
 J, S, G = 1024, 8, 8
-B = 148 * 16 * 32 * 3          # 3 tiles per resident warp of the position-major kernel
+B = SMS * 16 * 32 * 3          # 3 tiles per resident warp of the position-major kernel
 T, valid = synth_table(J, S, G, seed=0)
 eng.set_table(T)
 stream = torch.cuda.current_stream()

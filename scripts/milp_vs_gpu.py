@@ -1,6 +1,6 @@
 """GPU search vs the reference's CPU MILP on the same T, same box (SURVEY §8d metric 2).
 
-    python scripts/milp_vs_gpu.py [--limit 30] > profiles/r01_milp_vs_gpu.md
+    python scripts/milp_vs_gpu.py [--limit 30]
 
 For each instance: the reference MILP restated for scipy/HiGHS (oracle/ref_milp.py — the reference
 tree and PuLP/Gurobi/CBC are not on the GPU box) runs with a wall-clock limit and its incumbent is

@@ -14,7 +14,8 @@ from saturn_b200.synth import synth_table  # noqa: E402
 
 which = sys.argv[1] if len(sys.argv) > 1 else "eval"
 eng = Engine(0)
-WAVE = 148 * 8 * 32
+SMS = torch.cuda.get_device_properties(0).multi_processor_count
+WAVE = SMS * 8 * 32
 if which in ("eval", "eval_plain"):
     T, valid = synth_table(256, 8, 8, seed=0)
     eng.set_table(T)

@@ -8,7 +8,8 @@ from saturn_b200.synth import synth_table
 
 which = sys.argv[1] if len(sys.argv) > 1 else "all"
 eng = Engine(0)
-WAVE = 148 * 16 * 32
+SMS = torch.cuda.get_device_properties(0).multi_processor_count
+WAVE = SMS * 16 * 32
 if which in ("all", "search"):
     T, valid = synth_table(256, 8, 8, seed=0)
     eng.set_table(T)
@@ -27,7 +28,7 @@ if which in ("all", "c5"):
     Tr = np.where(valid, T, np.inf).min(axis=1, keepdims=True)
     vr = np.isfinite(Tr)
     eng.set_table(np.where(vr, Tr, 1e8).astype(np.float32))
-    opt, prio = random_candidates(eng, 148 * 6 * 32 * 8, vr, seed=1)
+    opt, prio = random_candidates(eng, SMS * 6 * 32 * 8, vr, seed=1)
     for _ in range(4):
         eng.eval(opt, prio)
     torch.cuda.synchronize()

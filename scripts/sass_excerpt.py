@@ -1,11 +1,11 @@
 """SASS evidence for the hot kernels (runs on the build box: cuobjdump only, no GPU).
 
-    python scripts/sass_excerpt.py > profiles/r02_sass.md
+    python scripts/sass_excerpt.py
 
 For each kernel of interest: instruction count of the fully unrolled 32-step block of the hot loop, the
 opcode histogram per scheduling step, and an excerpt of one step; plus the whole-library counts of the
-Blackwell-specific opcodes (UBLKCP = TMA bulk copy, SYNCS = mbarrier, LDG.E.*.256 = 256-bit loads,
-FMNMX3 = 3-input min/max) and the absence of tensor-core opcodes (the path has no contraction).
+Hopper opcodes the path relies on (UBLKCP = TMA bulk copy, SYNCS = mbarrier, LDG.E.*.128 = 128-bit loads)
+and the absence of tensor-core opcodes (the path has no contraction).
 """
 import collections
 import os
@@ -67,12 +67,11 @@ def main():
     for x in allins:
         t = x.split()
         op = t[1] if t[0].startswith("@") else t[0]
-        if ".256" in op:
-            full["LDG.*.256 (256-bit global loads)"] += 1
+        if op.startswith("LDG") and ".128" in op:
+            full["LDG.*.128"] += 1
     print("Whole library: %d kernels, %d instructions.  UBLKCP (TMA bulk copy) %d, SYNCS (mbarrier) %d, %s %d, "
-          "FMNMX3 %d, R2P %d; tensor-core opcodes (HMMA / IMMA / UTCHMMA / UTCQMMA / QGMMA): %d.\n" % (
-              len(fns), len(allins), hist["UBLKCP"], hist["SYNCS"], "LDG.*.256", full["LDG.*.256 (256-bit global loads)"],
-              hist["FMNMX3"], hist["R2P"],
+          "R2P %d; tensor-core opcodes (HMMA / IMMA / UTCHMMA / UTCQMMA / QGMMA): %d.\n" % (
+              len(fns), len(allins), hist["UBLKCP"], hist["SYNCS"], "LDG.*.128", full["LDG.*.128"], hist["R2P"],
               sum(hist[k] for k in hist if k in ("HMMA", "IMMA", "UTCHMMA", "UTCQMMA", "QGMMA", "UTCIMMA", "BMMA"))))
     want = [("_ZN2sb12k_eval_tilesILi1ELb1ELb1ELb0ELb0ELb0ELi1EEEvNS_8TileArgsE", "the measured kernel (bench `value`): C4, integer starts, prio streamed, look-up addresses on the FMA pipe", 32),
             ("_ZN2sb12k_eval_tilesILi1ELb1ELb1ELb0ELb0ELb0ELi0EEEvNS_8TileArgsE", "the same kernel with plain C++ addressing (test hook 0x02000000; the round-1 form)", 32),
@@ -99,7 +98,7 @@ def main():
             for x in blk[a:b]:
                 print("    " + x)
             print("```\n")
-    mem = [x for x in fns.get(want[0][0], []) if re.search(r"UBLKCP|SYNCS|LDG\.E\.\S*256|ATOMG|STG|ld\.acquire|LDG\.E\.64\.STRONG\.SYS|ST\.E\S*STRONG\.SYS|STG\.E\S*STRONG\.SYS", x)]
+    mem = [x for x in fns.get(want[0][0], []) if re.search(r"UBLKCP|SYNCS|LDG\.E\.\S*128|ATOMG|STG|ld\.acquire|LDG\.E\.64\.STRONG\.SYS|ST\.E\S*STRONG\.SYS|STG\.E\S*STRONG\.SYS", x)]
     print("## Memory / synchronisation instructions of the measured kernel (deduplicated)\n\n```")
     seen = set()
     for x in mem:

@@ -23,6 +23,7 @@ def _run(args, timeout):
 def test_reference_arm_line():
     d = _run(["--impl", "reference", "--steps", "1", "--warmup", "0"], 300)
     assert d["impl"] == "reference" and BASE_KEYS <= set(d)
+    assert d["steps"] == 1                                   # --steps sets the number of timed steps exactly
     assert d["metric"] == "candidate schedules/sec" and d["unit"] == "candidates/s" and d["higher_is_better"] is True
     assert d["value"] > 0 and d["e2e"]["value"] == d["value"] and d["e2e"]["h2d_bytes_per_step"] == 0
     assert d["cpu_baseline"]["kind"] == "port" and d["cpu_baseline"]["cores"] >= 1 and d["gpu_launches"] == 0
@@ -34,9 +35,62 @@ def test_reference_arm_line():
     assert d["cpu_baseline"]["cores"] <= (os.cpu_count() or 1) and "physical cores" in d["run"]["cores_how"]
 
 
+def _load_dump(d):
+    import numpy as np
+    return {f[:-4]: np.load(os.path.join(d, f)) for f in sorted(os.listdir(d))}
+
+
+def test_dump_outputs_layout_and_size_cap(tmp_path):
+    """--dump-outputs writes float32 / float64 arrays only, stays under 64 MB for any batch (a seeded sample plus
+    its indices above DUMP_LIMIT makespans), and writes the same files for the same outputs."""
+    import numpy as np
+    import torch
+    sys.path.insert(0, ROOT)
+    import bench
+    key = torch.tensor([(int(np.float32(3.5).view(np.uint32)) << 32) | 12345], dtype=torch.int64)
+    for n in (1000, 9_000_000):
+        out = torch.arange(n, dtype=torch.float32)
+        runs = []
+        for r in ("a", "b"):
+            d = tmp_path / ("%d_%s" % (n, r))
+            bench.dump_outputs(str(d), out, key)
+            assert sum(f.stat().st_size for f in d.iterdir()) <= 64 * 10 ** 6
+            runs.append(_load_dump(str(d)))
+        a, b = runs
+        assert a.keys() == b.keys() and all(np.array_equal(a[k], b[k]) for k in a)
+        assert all(v.dtype in (np.float32, np.float64) for v in a.values())
+        assert a["best_makespan"][0] == np.float32(3.5) and a["best_candidate"][0] == 12345
+        if n <= bench.DUMP_LIMIT:
+            assert set(a) == {"makespans", "best_makespan", "best_candidate"}
+            assert np.array_equal(a["makespans"], out.numpy())
+        else:
+            idx = a["makespans_index"].astype(np.int64)
+            assert len(idx) == bench.DUMP_LIMIT and np.all(np.diff(idx) > 0)
+            assert np.array_equal(a["makespans"], out.numpy()[idx])
+
+
+@pytest.mark.gpu
+def test_dump_outputs_reproduce_the_timed_path(tmp_path):
+    """Two runs with the same arguments dump identical outputs, and the dumped key is the arg-min of the dumped
+    makespans (first index of the minimum)."""
+    import numpy as np
+    args = ["--steps", "2", "--warmup", "3", "--batch", str(132 * 16 * 32), "--no-cpu", "--no-e2e"]
+    dumps = []
+    for r in ("a", "b"):
+        d = _run(args + ["--dump-outputs", str(tmp_path / r)], 600)
+        assert d["steps"] == 2 and d["gpu_launches"] == 2
+        dumps.append(_load_dump(str(tmp_path / r)))
+    a, b = dumps
+    assert set(a) == {"makespans", "best_makespan", "best_candidate"}
+    assert all(np.array_equal(a[k], b[k]) for k in a)
+    mk = a["makespans"]
+    assert mk.dtype == np.float32 and mk.shape == (132 * 16 * 32,)
+    assert a["best_makespan"][0] == mk.min() and int(a["best_candidate"][0]) == int(np.argmin(mk))
+
+
 @pytest.mark.gpu
 def test_our_arm_line():
-    d = _run(["--steps", "4", "--warmup", "3", "--batch", str(148 * 16 * 32 * 2), "--no-cpu"], 600)
+    d = _run(["--steps", "4", "--warmup", "3", "--batch", str(132 * 16 * 32 * 2), "--no-cpu"], 600)
     assert BASE_KEYS <= set(d) and {"roofline", "clocks"} <= set(d)
     assert d["metric"] == "candidate schedules/sec" and d["n_gpus"] == 1 and d["steps"] == 4 and d["warmup"] >= 3
     assert d["scaling"] == "weak" and d["vs_baseline"] is None and d["dtype"] == "f32" and d["data"] == "synthetic"

@@ -326,9 +326,9 @@ def test_fuzz_small_and_odd_shapes(engine):
 
 
 def test_large_batch_64bit_indexing(engine):
-    """9.4 M candidates of J = 256: each encoding array is 2.4 GB, so row offsets exceed 2^31 bytes."""
+    """9.5 M candidates of J = 256: each encoding array is 2.4 GB, so row offsets exceed 2^31 bytes."""
     J, S, G = 256, 8, 8
-    B = 148 * 16 * 32 * 124                                  # 9,396,224
+    B = 132 * 16 * 32 * 140                                  # 9,461,760
     T, valid = R.synth_table(J, S, G, seed=0)
     engine.set_table(T)
     opt, prio = random_candidates(engine, B, valid, seed=77)

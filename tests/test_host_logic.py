@@ -259,11 +259,17 @@ def test_forecast_matches_reference_forecast():
 
 
 # ------------------------------------------------------------------------------------------ round 2
-def test_alias_package_falls_through_to_an_installed_reference():
+def test_alias_package_falls_through_to_an_installed_reference(tmp_path):
     """`import saturn` is this repository's alias; submodules it does not implement resolve in a reference
-    distribution when one is on sys.path (saturn_b200/_alias.py) and raise a clear ImportError otherwise."""
+    distribution when one is on sys.path (saturn_b200/_alias.py) and raise a clear ImportError otherwise.
+    The reference distribution is a stand-in with the reference's package layout, written to tmp_path."""
     import subprocess
     import sys
+    ref = tmp_path / "reference"
+    for pkg, body in (("saturn", ""), ("saturn/library", "ORIGIN = 'reference'\n"), ("saturn/executor", "")):
+        (ref / pkg).mkdir(parents=True)
+        (ref / pkg / "__init__.py").write_text(body)
+    (ref / "saturn" / "executor" / "executor.py").write_text("def execute(*args):\n    return 'reference execute'\n")
     code = r'''
 import sys
 sys.path.insert(0, %r)
@@ -279,20 +285,19 @@ try:
     E.execute
     raise SystemExit("saturn.executor.execute must not resolve without a reference distribution")
 except ImportError as e:
-    assert "not part of the B200 solver drop-in" in str(e)
-ref = "/root/reference"
-import os
-if os.path.isdir(ref):
-    sys.path.append(ref)
-    for m in [m for m in sys.modules if m == "saturn" or m.startswith("saturn.")]:
-        del sys.modules[m]
-    import saturn, saturn.solver, saturn.library
-    assert saturn.library.__file__.startswith(ref)                      # fell through
-    assert saturn.solver.solve.__module__ == "saturn_b200.solver"       # the drop-in still wins
-    assert saturn.orchestrate.__module__ == "saturn_b200.orchestrator"
+    assert "not part of the saturn_b200 solver drop-in" in str(e)
+ref = %r
+sys.path.append(ref)
+for m in [m for m in sys.modules if m == "saturn" or m.startswith("saturn.")]:
+    del sys.modules[m]
+import saturn, saturn.solver, saturn.library, saturn.executor as E
+assert saturn.library.__file__.startswith(ref) and saturn.library.ORIGIN == "reference"   # fell through
+assert E.execute() == "reference execute"
+assert saturn.solver.solve.__module__ == "saturn_b200.solver"       # the drop-in still wins
+assert saturn.orchestrate.__module__ == "saturn_b200.orchestrator"
 print("ok")
-''' % ROOT
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, cwd="/tmp")
+''' % (ROOT, str(ref))
+    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, cwd=str(tmp_path))
     assert r.returncode == 0 and r.stdout.strip().endswith("ok"), r.stdout + r.stderr
 
 
