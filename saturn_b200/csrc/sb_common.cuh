@@ -128,8 +128,13 @@ __device__ __forceinline__ float psel(float a, float b, int bit) {
   return r;
 }
 
-// sm_90 has no 3-input max.f32: two FMNMX (max is exact, so the grouping does not change the result)
-__device__ __forceinline__ float fmax3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
+// sm_90 has no 3-input max.f32, but it has the 3-input integer max (VIMNMX3).  The makespan fold only sees
+// mk >= +0 and completions s + rt of non-negative runtimes: non-negative fp32 values order exactly like their bit
+// patterns as signed integers, and a negative value (sign bit set) loses to mk either way.  One VIMNMX3 instead
+// of two FMNMX, with the same result.
+__device__ __forceinline__ float fmax3_mk(float mk, float b, float c) {
+  return __int_as_float(__vimax3_s32(__float_as_int(mk), __float_as_int(b), __float_as_int(c)));
+}
 
 // kTrackMk: fold this job's completion (s + rt) into mk.  Needed with integer starts (the slot
 // state holds s + ceil(rt), not the completion) and with several nodes (no single f[7] at the end).
@@ -163,7 +168,7 @@ __device__ __forceinline__ void ls_step(float (&f)[8], float& mk, float& pend, f
     const float e = kIntegerStarts ? s + rt : v;
     if (ph < 0) mk = fmaxf(mk, e);
     else if (ph == 0) pend = e;
-    else mk = fmax3(mk, pend, e);
+    else mk = fmax3_mk(mk, pend, e);
   }
   f[0] = fmaxf(f[0], fminf(v, x1));
   f[1] = fmaxf(f[1], fminf(v, x2));

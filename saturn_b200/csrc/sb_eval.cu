@@ -203,7 +203,55 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
     auto evaluate = [&](const uint8_t* prio_row_s) -> float {
       st.reset(a.nodes);
       const int J = a.J;
-      if (STREAM) {
+      if constexpr (STREAM && ADDR == 1) {
+        // The look-ups of a step do not depend on the slot state, but each is two dependent shared-memory
+        // gathers on random banks.  So the full chunks run in batches of kBatch positions: the gathers of
+        // batch n + 1 (all opt bytes, then all runtimes) are issued before the steps of batch n, which read
+        // their look-ups from registers.  The last batch of a chunk resolves the first batch of the next
+        // full chunk, so the pipeline runs across chunks; a partial last chunk takes the plain steps.
+        constexpr int STEPS = 32;
+        constexpr int kBatch = 8;  // 90 registers, no spills: within the 128 that 16 warps per SM allow
+        const int nch = (J + STEPS - 1) / STEPS, nfull = J / STEPS;
+        uint32_t ob[kBatch];
+        float rb[kBatch];
+        auto resolve = [&](const uint32_t* w) {  // w: the kBatch / 4 words that hold the batch's job ids
+          int js[kBatch];
+#pragma unroll
+          for (int i = 0; i < kBatch; ++i) js[i] = prio_at<1>(w, i);
+#pragma unroll
+          for (int i = 0; i < kBatch; ++i) ob[i] = st.gather_opt(js[i]);
+#pragma unroll
+          for (int i = 0; i < kBatch; ++i) rb[i] = st.gather_rt(js[i], ob[i]);
+        };
+        if (nfull > 0) resolve(q.w);
+        for (int c = 0; c < nfull; ++c) {
+          PrioChunk nxt = q;
+          if (c + 1 < nch) nxt = ld_prio32<true>(pg + (c + 1) * 32);
+          // a partial next chunk is not resolved ahead (its bytes past J are not job ids): the last batch then
+          // re-resolves this chunk's first batch, and the result is not used
+          const bool ahead = c + 1 < nfull;
+          uint32_t head[kBatch / 4];
+#pragma unroll
+          for (int i = 0; i < kBatch / 4; ++i) head[i] = ahead ? nxt.w[i] : q.w[i];
+#pragma unroll
+          for (int b = 0; b < STEPS / kBatch; ++b) {
+            uint32_t oc[kBatch];
+            float rc[kBatch];
+#pragma unroll
+            for (int i = 0; i < kBatch; ++i) { oc[i] = ob[i]; rc[i] = rb[i]; }
+            resolve(b + 1 < STEPS / kBatch ? q.w + (b + 1) * (kBatch / 4) : head);
+#pragma unroll
+            for (int i = 0; i < kBatch; ++i) st.step_resolved(static_cast<int>(oc[i]), rc[i], i & 1);
+          }
+          q = nxt;
+        }
+        if (nfull < nch) {
+          const int rem = J - nfull * STEPS;
+#pragma unroll
+          for (int t = 0; t < STEPS; ++t)
+            if (t < rem) st.step(prio_at<1>(q.w, t), t & 1);
+        }
+      } else if (STREAM) {
         constexpr int STEPS = 32 / PB;  // schedule positions per 256-bit load
         const int nch = (J + STEPS - 1) / STEPS;
         for (int c = 0; c < nch; ++c) {

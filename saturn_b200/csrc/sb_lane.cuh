@@ -89,16 +89,26 @@ struct LaneState {
       ls_step<INT, true>(f, mk, pend, rt, o & 7, one, ph);
     }
   }
+  // ADDR = 1: the two look-ups as separate gathers, so that the streamed loop of k_eval_tiles can issue a whole
+  // batch of opt-byte gathers, then the batch's runtime gathers, ahead of the steps that consume them
+  __device__ __forceinline__ uint32_t gather_opt(int j) const {
+    uint32_t oa, o;
+    asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(oa) : "r"(j), "r"(one), "r"(orow_s));
+    asm("ld.shared.u8 %0, [%1];" : "=r"(o) : "r"(oa));
+    return o;
+  }
+  __device__ __forceinline__ float gather_rt(int j, uint32_t o) const {
+    uint32_t idx, ta;
+    float rt;
+    asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(idx) : "r"(j), "r"(SG), "r"(o));
+    asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(ta) : "r"(idx), "r"(four), "r"(tab_s));
+    asm("ld.shared.f32 %0, [%1];" : "=f"(rt) : "r"(ta));
+    return rt;
+  }
   __device__ __forceinline__ void step(int j, int ph = -1) {
     if (!MULTI && ADDR == 1) {
-      uint32_t oa, o, idx, ta;
-      float rt;
-      asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(oa) : "r"(j), "r"(one), "r"(orow_s));
-      asm("ld.shared.u8 %0, [%1];" : "=r"(o) : "r"(oa));
-      asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(idx) : "r"(j), "r"(SG), "r"(o));
-      asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(ta) : "r"(idx), "r"(four), "r"(tab_s));
-      asm("ld.shared.f32 %0, [%1];" : "=f"(rt) : "r"(ta));
-      ls_step<INT>(f, mk, pend, rt, static_cast<int>(o & 7u), one, ph);
+      const uint32_t o = gather_opt(j);
+      ls_step<INT>(f, mk, pend, gather_rt(j, o), static_cast<int>(o & 7u), one, ph);
       return;
     }
     const int o = orow[j];
