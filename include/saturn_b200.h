@@ -41,6 +41,10 @@
  *       start = max(ready[sel])
  *       ready[sel] = start + (integer_starts ? ceil(rt) : rt)
  *   makespan = max_j (start_j + rt_j)
+ * With SB_FLAG_SUM_COMPLETION the score is the sum of completion times instead:
+ *   total = sum_j (start_j + rt_j), in fp32 a left fold in schedule order, acc = acc + (start + rt) from +0
+ * (one add per job, never paired or reassociated; the oracle folds the same way and agrees bit for bit).
+ * The schedule, every start and every slot mask are the same under both objectives.
  * With integer_starts the slot state is the integer time a slot becomes usable, start + ceil(rt);
  * SURVEY.md §8a writes the same rule as `start = ceil(max ready)` over real-valued ready times.  Starts,
  * makespans and the set of k slots taken are identical (ceil is monotone); the one observable difference
@@ -91,6 +95,16 @@ typedef enum sb_status {
                                      BASELINE.json's north_star sketches), 4 candidates per warp.  Same results;
                                      kept to be measured against the shipped lane-per-candidate kernel
                                      (bench.py configs.C4_alt_shape), not to be used. */
+#define SB_FLAG_SUM_COMPLETION 64u /* objective = sum of completion times (the mean job completion time x J) instead of
+                                     the makespan.  Accepted by sb_eval, sb_eval_host, sb_eval_full, sb_decode and the
+                                     search (sb_search_params.flags).  EVERY score the library emits then holds that
+                                     sum: makespan_out, sb_decode's makespan, the packed best keys (a non-negative
+                                     fp32, so the key is still an arg-min), sb_search_best's and
+                                     sb_search_result's makespan, the history; sb_search_control.target_makespan
+                                     then targets the sum.  Starts and slot masks do not change.  The search's
+                                     temperature unit becomes the incumbent's MEAN completion (sum / J), and
+                                     sb_search_seed_lpt plants shortest-processing-time orders.  Not available with
+                                     SB_FLAG_ALT_WARPSCAN (SB_ERR_UNSUPPORTED). */
 #define SB_IPC_HANDLE_BYTES 64
 
 typedef struct sb_handle sb_handle;
@@ -213,7 +227,8 @@ typedef struct sb_search_params {
   int64_t chains;       /* candidates in this GPU's population */
   uint64_t chain_base;  /* global id of chain 0 (rank * chains) */
   unsigned flags;       /* SB_FLAG_* */
-  float t_start;        /* initial temperature as a fraction of the incumbent makespan */
+  float t_start;        /* initial temperature as a fraction of the incumbent makespan (SB_FLAG_SUM_COMPLETION:
+                         * of the incumbent's mean completion time, its sum / J) */
   float t_end;          /* final temperature fraction */
   int total_rounds;     /* cooling horizon */
   int resample_every;   /* > 0: sb_search_round itself resamples the population by tournament before every round r
@@ -244,7 +259,8 @@ int sb_search_resample(sb_handle* h);
 /* ---- the whole single-GPU search in one call (what prob.solve(solver) is to the reference, milp.py:321-327)
  * sb_search_seed_lpt plants three longest-processing-time candidates (every job on its fastest option / on its
  * least GPU-seconds option / in between; nodes filled greedily by GPU-seconds) into an eighth of the
- * population each and scores them.  sb_search_run = sb_search_init + seeds + `rounds` rounds in groups of
+ * population each and scores them; with SB_FLAG_SUM_COMPLETION the orders are shortest-processing-time
+ * instead (ascending runtime of the chosen option), same options and node fill.  sb_search_run = sb_search_init + seeds + `rounds` rounds in groups of
  * `sync_every` (tournament resampling every `resample_every` rounds inside a group is only another launch;
  * the host reads the incumbent key once per group and applies the stopping rules) + sb_search_best.
  * The multi-GPU driver (saturn_b200/search.py) runs the same steps with a key exchange per group. */

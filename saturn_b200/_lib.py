@@ -12,6 +12,7 @@ FLAG_OPT_BY_POSITION = 4
 FLAG_POST_KEY = 8
 FLAG_FOLD_PREV = 16
 FLAG_ALT_WARPSCAN = 32
+FLAG_SUM_COMPLETION = 64
 IPC_HANDLE_BYTES = 64
 _FLAG_FORCE_GENERIC = 0x80000000
 

@@ -40,7 +40,7 @@ struct SearchState {
   bool ready = false;
   SearchDev d;
   sb_search_params p;
-  float scale = 0.f;  // temperature unit: incumbent makespan after initialisation
+  float scale = 0.f;  // temperature unit: incumbent makespan after initialisation (SB_FLAG_SUM_COMPLETION: sum / J)
   long long evaluated = 0;
   int rounds_done = 0;
   bool fused_ok = true;  // run rounds with the fused kernel while its tiles fit
@@ -382,6 +382,9 @@ int sb_eval(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, int64
     }
   }
   if (flags & SB_FLAG_ALT_WARPSCAN) {
+    if (flags & SB_FLAG_SUM_COMPLETION)
+      return fail(SB_ERR_UNSUPPORTED, "SB_FLAG_ALT_WARPSCAN scores the makespan only: it cannot be combined with "
+                  "SB_FLAG_SUM_COMPLETION");
     if (flags & (SB_FLAG_POST_KEY | SB_FLAG_FOLD_PREV))
       return fail(SB_ERR_UNSUPPORTED, "SB_FLAG_ALT_WARPSCAN cannot be combined with the fused key exchange");
     cudaError_t e = eval_alt_launch(h->dev, c, h->stream);
@@ -812,7 +815,9 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
   uint32_t bits = static_cast<uint32_t>(key >> 32);
   float mk;
   memcpy(&mk, &bits, 4);
-  s.scale = isfinite(mk) ? mk : 1.0f;
+  // the temperature unit: the incumbent's makespan, or its mean completion time (the sum / J), so that t_start /
+  // t_end mean the same fraction of a typical score difference under both objectives
+  s.scale = isfinite(mk) ? ((p->flags & SB_FLAG_SUM_COMPLETION) ? mk / static_cast<float>(J) : mk) : 1.0f;
   s.evaluated = d.chains;
   s.rounds_done = 0;
   s.launches = 0;
@@ -1028,6 +1033,7 @@ int sb_search_seed_lpt(sb_handle* h) {
   const int J = h->J, nodes = h->nodes;
   const bool reduced = (s.p.flags & SB_FLAG_REDUCED) != 0;
   const float* tmin = h->h_tmin.data();
+  const bool spt = (s.p.flags & SB_FLAG_SUM_COMPLETION) != 0;  // shortest first: the order that favours the sum
   const double INF = HUGE_VAL;
   // usable cells: below the sentinel threshold; a job with none falls back to any finite cell
   std::vector<double> usable(static_cast<size_t>(J) * kSlots);
@@ -1064,7 +1070,8 @@ int sb_search_seed_lpt(sb_handle* h) {
       weight[j] = rt[j] * sqrt(best + 1.0);
       order[j] = j;
     }
-    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return weight[a] > weight[b]; });
+    if (spt) std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return rt[a] < rt[b]; });
+    else std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return weight[a] > weight[b]; });
     std::vector<double> load(nodes, 0.0);
     for (int j = 0; j < J; ++j) opt[j] = static_cast<uint8_t>(col[j]);
     if (nodes > 1) {

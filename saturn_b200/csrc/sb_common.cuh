@@ -142,7 +142,10 @@ __device__ __forceinline__ float fmax3_mk(float mk, float b, float c) {
 // completion in `pend`, 1 folds max(mk, pend, completion); callers with unrolled loops pass t & 1 (a
 // compile-time constant after unrolling), others pass -1 for the plain 2-input max.  A parked value
 // that is never folded is picked up by the final max(mk, pend) (LaneState::result).
-template <bool kIntegerStarts, bool kTrackMk = kIntegerStarts>
+// kSum (SB_FLAG_SUM_COMPLETION): mk is the running SUM of completions instead, one add per step in schedule
+// order (acc = acc + (s + rt), the oracle's left fold bit for bit); `ph` and `pend` are unused, and the
+// completion is tracked whatever kTrackMk says.  The slot update is the same: only the score differs.
+template <bool kIntegerStarts, bool kTrackMk = kIntegerStarts, bool kSum = false>
 __device__ __forceinline__ void ls_step(float (&f)[8], float& mk, float& pend, float rt, int km1, int one, int ph) {
   const float INF = inf_f();
   const int b2 = km1 & 4, b1 = km1 & 2, b0 = km1 & 1;
@@ -164,7 +167,10 @@ __device__ __forceinline__ void ls_step(float (&f)[8], float& mk, float& pend, f
   } else {
     v = s + rt;
   }
-  if (kTrackMk) {
+  if (kSum) {
+    const float e = kIntegerStarts ? s + rt : v;
+    mk = mk + e;
+  } else if (kTrackMk) {
     const float e = kIntegerStarts ? s + rt : v;
     if (ph < 0) mk = fmaxf(mk, e);
     else if (ph == 0) pend = e;

@@ -24,7 +24,9 @@
 //     state of every node lives in a lane-private shared-memory column (2 x float4 per node,
 //     conflict-free); a step loads the state of the job's node, updates it, stores it back;
 //   * makespans are written coalesced (128 B per warp); an optional 64-bit arg-min key is
-//     folded with one redux + one atomicMin per warp.
+//     folded with one redux + one atomicMin per warp;
+//   * SUM (SB_FLAG_SUM_COMPLETION): every kernel here also comes in a form that scores the sum of completion
+//     times instead of the makespan (ls_step<..., kSum>); the schedule, and every start, is the same.
 #include "sb_lane.cuh"
 
 namespace sb {
@@ -51,7 +53,8 @@ struct TileArgs {
 
 // TABG: the runtime table stays in global memory (read through L1/L2) — for tables larger than the
 // shared memory left beside the opt tiles (e.g. J = 1024 with 8 strategies: 256 KB).
-template <int PB, bool INT, bool STREAM, bool MULTI, bool SEARCH = false, bool TABG = false, int ADDR = 0>
+template <int PB, bool INT, bool STREAM, bool MULTI, bool SEARCH = false, bool TABG = false, int ADDR = 0,
+          bool SUM = false>
 __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const TileArgs a) {
   static_assert(!(SEARCH && (STREAM || TABG)), "the fused search round runs on shared-memory tiles only");
   static_assert(ADDR == 0 || (!TABG && !MULTI && !SEARCH), "ADDR = 1 needs the table and the opt rows in shared memory");
@@ -89,7 +92,7 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
     }
   }
 
-  LaneState<INT, MULTI, ADDR> st;
+  LaneState<INT, MULTI, ADDR, SUM> st;
   if (TABG) st.tab = a.tab;
   else st.tab = tab_s;
   st.SG = a.SG;
@@ -291,8 +294,9 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
     // SEARCH rounds: score the lane's rows from window `w0` on (warp-uniform).  w0 > 0 resumes from the
     // snapshot taken in front of that window (buffer bit w0-1 of `par`); `save` stores the state in front of
     // every later window into the OTHER buffer (the proposal's boundary states; the caller flips the bits of
-    // `par` if it accepts the move).  Snapshot = the 8 sorted slot times + the running makespan; a completion
-    // parked in `pend` is always folded at a window boundary (even number of steps per window).
+    // `par` if it accepts the move).  Snapshot = the 8 sorted slot times + the running score (makespan, or the
+    // running sum with SUM); a completion parked in `pend` is always folded at a window boundary (even number of
+    // steps per window) — the sum parks nothing, so its snapshot is exact at any step.
     [[maybe_unused]] auto eval_from = [&](const uint8_t* prio_row_s, int w0, uint32_t par, bool save,
                                           float* snap_t) -> float {
       const int J = a.J;
@@ -319,7 +323,7 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
           float* sp = snap_t + ((b * 2 + (((par >> b) & 1u) ^ 1u)) * 9) * 32 + lane;
 #pragma unroll
           for (int i = 0; i < 8; ++i) __stcg(sp + i * 32, st.f[i]);
-          __stcg(sp + 8 * 32, fmaxf(st.mk, st.pend));
+          __stcg(sp + 8 * 32, st.running());
         }
         const uint4 p = prow[c];
         const uint32_t wd[4] = {p.x, p.y, p.z, p.w};
@@ -532,7 +536,7 @@ struct GenericArgs {
   int one;
 };
 
-template <int PB, bool INT, bool MULTI>
+template <int PB, bool INT, bool MULTI, bool SUM = false>
 __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
   extern __shared__ __align__(128) uint8_t smem[];
   const float* tab = a.tab;
@@ -546,7 +550,7 @@ __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
     tab = tab_s;
   }
   const int lane = threadIdx.x & 31;
-  LaneState<INT, MULTI> st;
+  LaneState<INT, MULTI, 0, SUM> st;
   st.tab = tab;
   st.SG = a.SG;
   st.one = a.one;
@@ -603,7 +607,7 @@ struct FullArgs {
   uint32_t* slotmask;   // [B][J] by job, nullable
 };
 
-template <int PB, bool INT>
+template <int PB, bool INT, bool SUM = false>
 __global__ void __launch_bounds__(128) k_eval_full(const FullArgs a) {
   const long long nthreads = static_cast<long long>(gridDim.x) * blockDim.x;
   const bool multi = a.nodes > 1;
@@ -639,7 +643,8 @@ __global__ void __launch_bounds__(128) k_eval_full(const FullArgs a) {
       const float nxt = s + hold;
       for (int g = 0; g < kSlots; ++g)
         if ((taken >> g) & 1u) rd[g] = nxt;
-      mk = fmaxf(mk, s + rt);
+      if (SUM) mk = mk + (s + rt);  // the left fold in schedule order of ls_step<..., kSum>
+      else mk = fmaxf(mk, s + rt);
       if (a.start) a.start[b * a.J + j] = s;
       if (a.slotmask) a.slotmask[b * a.J + j] = (static_cast<uint32_t>(node) << 16) | taken;
     }
@@ -709,9 +714,9 @@ int plan_tiles(const Device& dev, int J, int SG, int pb, bool stream, int nodes,
   return nw;
 }
 
-template <int PB, bool INT, bool STREAM, bool MULTI, bool TABG = false, int ADDR = 0>
+template <int PB, bool INT, bool STREAM, bool MULTI, bool TABG = false, int ADDR = 0, bool SUM = false>
 static cudaError_t launch_tiles(const Device& dev, const TileArgs& a, const TilePlan& tp, cudaStream_t st) {
-  auto kern = k_eval_tiles<PB, INT, STREAM, MULTI, false, TABG, ADDR>;
+  auto kern = k_eval_tiles<PB, INT, STREAM, MULTI, false, TABG, ADDR, SUM>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(tp.smem));
   if (e != cudaSuccess) return e;
   long long ctas = (a.ntiles + tp.warps - 1) / tp.warps;
@@ -720,19 +725,21 @@ static cudaError_t launch_tiles(const Device& dev, const TileArgs& a, const Tile
   return cudaGetLastError();
 }
 
-template <int PB, bool INT>
+template <int PB, bool INT, bool SUM>
 static cudaError_t dispatch_tiles(const Device& dev, const TileArgs& a, const TilePlan& tp, bool stream, bool multi,
                                   cudaStream_t st) {
   if (stream) {
-    return multi ? launch_tiles<PB, INT, true, true>(dev, a, tp, st) : launch_tiles<PB, INT, true, false>(dev, a, tp, st);
+    return multi ? launch_tiles<PB, INT, true, true, false, 0, SUM>(dev, a, tp, st)
+                 : launch_tiles<PB, INT, true, false, false, 0, SUM>(dev, a, tp, st);
   }
-  return multi ? launch_tiles<PB, INT, false, true>(dev, a, tp, st) : launch_tiles<PB, INT, false, false>(dev, a, tp, st);
+  return multi ? launch_tiles<PB, INT, false, true, false, 0, SUM>(dev, a, tp, st)
+               : launch_tiles<PB, INT, false, false, false, 0, SUM>(dev, a, tp, st);
 }
 
-template <int PB, bool INT, bool MULTI>
+template <int PB, bool INT, bool MULTI, bool SUM>
 static cudaError_t launch_generic(const Device& dev, const GenericArgs& a0, cudaStream_t st) {
   GenericArgs a = a0;
-  auto kern = k_eval_generic<PB, INT, MULTI>;
+  auto kern = k_eval_generic<PB, INT, MULTI, SUM>;
   const size_t tab_bytes = static_cast<size_t>(a.J) * a.SG * 4;
   size_t smem = MULTI ? static_cast<size_t>(4) * a.nodes * 1024u : 0u;  // 4 warps per CTA
   a.tab_in_smem = 0;
@@ -752,8 +759,8 @@ static cudaError_t launch_generic(const Device& dev, const GenericArgs& a0, cuda
   return cudaGetLastError();
 }
 
-cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, int* path_used) {
-  if (c.B <= 0) return cudaSuccess;
+template <bool SUM>
+static cudaError_t eval_launch_obj(const Device& dev, const EvalCall& c, cudaStream_t st, int* path_used) {
   const int pb = c.J <= 256 ? 1 : 2;
   const bool ints = (c.flags & SB_FLAG_INTEGER_STARTS) != 0;
   const bool multi = c.nodes > 1;
@@ -789,15 +796,22 @@ cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, i
     a.xp = c.xp;
     if (path_used) *path_used = tabg ? 4 : (stream ? 3 : (a.use_bulk ? 2 : 1));
     if (tabg) {
-      if (pb == 1) return ints ? launch_tiles<1, true, true, false, true>(dev, a, tp, st) : launch_tiles<1, false, true, false, true>(dev, a, tp, st);
-      return ints ? launch_tiles<2, true, true, false, true>(dev, a, tp, st) : launch_tiles<2, false, true, false, true>(dev, a, tp, st);
+      if (pb == 1)
+        return ints ? launch_tiles<1, true, true, false, true, 0, SUM>(dev, a, tp, st)
+                    : launch_tiles<1, false, true, false, true, 0, SUM>(dev, a, tp, st);
+      return ints ? launch_tiles<2, true, true, false, true, 0, SUM>(dev, a, tp, st)
+                  : launch_tiles<2, false, true, false, true, 0, SUM>(dev, a, tp, st);
     }
     // the headline shape (u8 priorities streamed, one node, table in shared memory): address arithmetic on the FMA
     // pipe unless the test hook 0x02000000 asks for the plain form
     if (pb == 1 && stream && !multi && !(c.flags & 0x02000000u))
-      return ints ? launch_tiles<1, true, true, false, false, 1>(dev, a, tp, st) : launch_tiles<1, false, true, false, false, 1>(dev, a, tp, st);
-    if (pb == 1) return ints ? dispatch_tiles<1, true>(dev, a, tp, stream, multi, st) : dispatch_tiles<1, false>(dev, a, tp, stream, multi, st);
-    return ints ? dispatch_tiles<2, true>(dev, a, tp, stream, multi, st) : dispatch_tiles<2, false>(dev, a, tp, stream, multi, st);
+      return ints ? launch_tiles<1, true, true, false, false, 1, SUM>(dev, a, tp, st)
+                  : launch_tiles<1, false, true, false, false, 1, SUM>(dev, a, tp, st);
+    if (pb == 1)
+      return ints ? dispatch_tiles<1, true, SUM>(dev, a, tp, stream, multi, st)
+                  : dispatch_tiles<1, false, SUM>(dev, a, tp, stream, multi, st);
+    return ints ? dispatch_tiles<2, true, SUM>(dev, a, tp, stream, multi, st)
+                : dispatch_tiles<2, false, SUM>(dev, a, tp, stream, multi, st);
   }
   GenericArgs g;
   g.tab = c.tab; g.J = c.J; g.SG = c.SG; g.opt = c.opt; g.prio = c.prio; g.B = c.B;
@@ -805,17 +819,23 @@ cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, i
   g.id_base = c.id_base; g.tab_in_smem = 0; g.nodes = c.nodes; g.one = 1;
   if (path_used) *path_used = 0;
   if (multi) {
-    if (pb == 1) return ints ? launch_generic<1, true, true>(dev, g, st) : launch_generic<1, false, true>(dev, g, st);
-    return ints ? launch_generic<2, true, true>(dev, g, st) : launch_generic<2, false, true>(dev, g, st);
+    if (pb == 1) return ints ? launch_generic<1, true, true, SUM>(dev, g, st) : launch_generic<1, false, true, SUM>(dev, g, st);
+    return ints ? launch_generic<2, true, true, SUM>(dev, g, st) : launch_generic<2, false, true, SUM>(dev, g, st);
   }
-  if (pb == 1) return ints ? launch_generic<1, true, false>(dev, g, st) : launch_generic<1, false, false>(dev, g, st);
-  return ints ? launch_generic<2, true, false>(dev, g, st) : launch_generic<2, false, false>(dev, g, st);
+  if (pb == 1) return ints ? launch_generic<1, true, false, SUM>(dev, g, st) : launch_generic<1, false, false, SUM>(dev, g, st);
+  return ints ? launch_generic<2, true, false, SUM>(dev, g, st) : launch_generic<2, false, false, SUM>(dev, g, st);
+}
+
+cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, int* path_used) {
+  if (c.B <= 0) return cudaSuccess;
+  return (c.flags & SB_FLAG_SUM_COMPLETION) ? eval_launch_obj<true>(dev, c, st, path_used)
+                                            : eval_launch_obj<false>(dev, c, st, path_used);
 }
 
 // One fused search round over `c.B` chains whose current candidates are (c.opt, c.prio).  Returns
 // cudaErrorNotSupported when the shared-memory tiles (both rows resident, >= 4 warps) do not fit;
 // the caller then runs the unfused propose / evaluate / accept round.
-template <int PB, bool INT>
+template <int PB, bool INT, bool SUM>
 static cudaError_t dispatch_search(const Device& dev, const TileArgs& a, const TilePlan& tp, bool multi,
                                    cudaStream_t st) {
   auto launch = [&](auto kern) {
@@ -826,8 +846,8 @@ static cudaError_t dispatch_search(const Device& dev, const TileArgs& a, const T
     kern<<<grid, tp.warps * 32, tp.smem, st>>>(a);
     return cudaGetLastError();
   };
-  if (multi) return launch(k_eval_tiles<PB, INT, false, true, true>);
-  return launch(k_eval_tiles<PB, INT, false, false, true>);
+  if (multi) return launch(k_eval_tiles<PB, INT, false, true, true, false, 0, SUM>);
+  return launch(k_eval_tiles<PB, INT, false, false, true, false, 0, SUM>);
 }
 
 // 2 = both rows of a candidate fit in shared memory for at least 8 warps: the tile kernel runs the fused
@@ -859,11 +879,18 @@ cudaError_t search_round_launch(const Device& dev, const EvalCall& c, const Sear
   a.ntiles = (c.B + 31) / 32;
   a.one = 1;
   a.sf = sf;
+  if (c.flags & SB_FLAG_SUM_COMPLETION) {
+    if (pb == 1)
+      return ints ? dispatch_search<1, true, true>(dev, a, tp, c.nodes > 1, st)
+                  : dispatch_search<1, false, true>(dev, a, tp, c.nodes > 1, st);
+    return ints ? dispatch_search<2, true, true>(dev, a, tp, c.nodes > 1, st)
+                : dispatch_search<2, false, true>(dev, a, tp, c.nodes > 1, st);
+  }
   if (pb == 1)
-    return ints ? dispatch_search<1, true>(dev, a, tp, c.nodes > 1, st)
-                : dispatch_search<1, false>(dev, a, tp, c.nodes > 1, st);
-  return ints ? dispatch_search<2, true>(dev, a, tp, c.nodes > 1, st)
-              : dispatch_search<2, false>(dev, a, tp, c.nodes > 1, st);
+    return ints ? dispatch_search<1, true, false>(dev, a, tp, c.nodes > 1, st)
+                : dispatch_search<1, false, false>(dev, a, tp, c.nodes > 1, st);
+  return ints ? dispatch_search<2, true, false>(dev, a, tp, c.nodes > 1, st)
+              : dispatch_search<2, false, false>(dev, a, tp, c.nodes > 1, st);
 }
 
 cudaError_t eval_full_launch(const Device& dev, const EvalCall& c, float* start, uint32_t* slotmask, cudaStream_t st) {
@@ -877,12 +904,14 @@ cudaError_t eval_full_launch(const Device& dev, const EvalCall& c, float* start,
   long long blocks = (c.B + 127) / 128;
   long long cap = static_cast<long long>(dev.sm_count) * 16;
   int grid = static_cast<int>(blocks < cap ? blocks : cap);
+  const bool sum = (c.flags & SB_FLAG_SUM_COMPLETION) != 0;
+  auto launch = [&](auto kern) { kern<<<grid, 128, 0, st>>>(a); };
   if (pb == 1) {
-    if (ints) k_eval_full<1, true><<<grid, 128, 0, st>>>(a);
-    else k_eval_full<1, false><<<grid, 128, 0, st>>>(a);
+    if (sum) ints ? launch(k_eval_full<1, true, true>) : launch(k_eval_full<1, false, true>);
+    else ints ? launch(k_eval_full<1, true>) : launch(k_eval_full<1, false>);
   } else {
-    if (ints) k_eval_full<2, true><<<grid, 128, 0, st>>>(a);
-    else k_eval_full<2, false><<<grid, 128, 0, st>>>(a);
+    if (sum) ints ? launch(k_eval_full<2, true, true>) : launch(k_eval_full<2, false, true>);
+    else ints ? launch(k_eval_full<2, true>) : launch(k_eval_full<2, false>);
   }
   return cudaGetLastError();
 }

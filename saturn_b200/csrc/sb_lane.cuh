@@ -36,11 +36,12 @@ __device__ __forceinline__ PrioChunk ld_prio32(const uint8_t* p) {
 // `mad.lo` on run-time multipliers, which ptxas must issue as IMAD on the FMA pipe instead of IADD3 / LEA on
 // the ALU pipe — the step is bound by the ALU pipe (half rate) and by issue together, so the same instruction
 // count with two fewer ALU instructions is the cheaper mix.
-template <bool INT, bool MULTI, int ADDR = 0>
+// SUM: score = sum of completion times (SB_FLAG_SUM_COMPLETION) instead of the makespan; mk holds the running sum.
+template <bool INT, bool MULTI, int ADDR = 0, bool SUM = false>
 struct LaneState {
   float f[8];
   float mk;
-  float pend;  // a completion time parked by an even step (see ls_step)
+  float pend;  // a completion time parked by an even step (see ls_step; never used with SUM)
   const uint8_t* orow;  // this candidate's opt bytes (shared memory or global)
   const float* tab;     // runtime table (shared memory or global)
   int SG;
@@ -83,10 +84,10 @@ struct LaneState {
   // ph: t & 1 inside fully unrolled loops, -1 elsewhere (see ls_step)
   __device__ __forceinline__ void step_resolved(int o, float rt, int ph = -1) {
     if (!MULTI) {
-      ls_step<INT>(f, mk, pend, rt, o & 7, one, ph);
+      ls_step<INT, INT, SUM>(f, mk, pend, rt, o & 7, one, ph);
     } else {
       switch_node(o >> 3);
-      ls_step<INT, true>(f, mk, pend, rt, o & 7, one, ph);
+      ls_step<INT, true, SUM>(f, mk, pend, rt, o & 7, one, ph);
     }
   }
   // ADDR = 1: the two look-ups as separate gathers, so that the streamed loop of k_eval_tiles can issue a whole
@@ -108,21 +109,24 @@ struct LaneState {
   __device__ __forceinline__ void step(int j, int ph = -1) {
     if (!MULTI && ADDR == 1) {
       const uint32_t o = gather_opt(j);
-      ls_step<INT>(f, mk, pend, gather_rt(j, o), static_cast<int>(o & 7u), one, ph);
+      ls_step<INT, INT, SUM>(f, mk, pend, gather_rt(j, o), static_cast<int>(o & 7u), one, ph);
       return;
     }
     const int o = orow[j];
     if (!MULTI) {
       const float rt = tab[j * SG + o];
-      ls_step<INT>(f, mk, pend, rt, o & 7, one, ph);
+      ls_step<INT, INT, SUM>(f, mk, pend, rt, o & 7, one, ph);
     } else {
       const int col = o & 7;  // reduced table only: opt = (node << 3) | (k - 1)
       const float rt = tab[j * 8 + col];
       switch_node(o >> 3);
-      ls_step<INT, true>(f, mk, pend, rt, col, one, ph);
+      ls_step<INT, true, SUM>(f, mk, pend, rt, col, one, ph);
     }
   }
-  __device__ __forceinline__ float result() const { return (INT || MULTI) ? fmaxf(mk, pend) : f[7]; }
+  __device__ __forceinline__ float result() const { return SUM ? mk : ((INT || MULTI) ? fmaxf(mk, pend) : f[7]); }
+  // the running score a snapshot of the incremental rounds stores (SearchFuse::snap): with SUM nothing is parked,
+  // so a snapshot is exact at any step, not only after an even number of steps
+  __device__ __forceinline__ float running() const { return SUM ? mk : fmaxf(mk, pend); }
 };
 
 template <int PB>

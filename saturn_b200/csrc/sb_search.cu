@@ -419,7 +419,8 @@ __device__ __forceinline__ PosMove make_pos_move_win(const SearchFuse& sf, int r
 // 2 = split over the shared memory of a CTA PAIR (cluster of 2): each CTA loads one half with TMA and every
 // look-up is a `ld.shared::cluster` to whichever CTA owns the entry (distributed shared memory) — the
 // alternative to 1, kept behind a test hook.
-template <int PB, bool INT, bool MULTI, bool EVAL = false, int TAB = 0>
+// SUM: score the sum of completion times instead of the makespan (SB_FLAG_SUM_COMPLETION, see ls_step).
+template <int PB, bool INT, bool MULTI, bool EVAL = false, int TAB = 0, bool SUM = false>
 __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
   static_assert(TAB == 0 || (EVAL && !MULTI), "tables outside the CTA's shared memory: scoring only, one node");
   extern __shared__ __align__(128) uint8_t smem[];
@@ -448,7 +449,7 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
       for (uint32_t off = 0; off < tab_bytes; off += 32768u) tma_bulk_g2s(smem + off, src + off, min(32768u, tab_bytes - off), bar_tab);
     }
   }
-  LaneState<INT, MULTI> st;
+  LaneState<INT, MULTI, 0, SUM> st;
   st.tab = tab_s;
   st.SG = a.SG;
   st.one = a.one;
@@ -515,7 +516,7 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
           float* sp = snap_t + ((b * 2 + (((par >> b) & 1u) ^ 1u)) * 9) * 32 + lane;
 #pragma unroll
           for (int i = 0; i < 8; ++i) __stcg(sp + i * 32, st.f[i]);
-          __stcg(sp + 8 * 32, fmaxf(st.mk, st.pend));
+          __stcg(sp + 8 * 32, st.running());
         }
         PrioChunk no = qo, np[PCH];
 #pragma unroll
@@ -752,7 +753,7 @@ size_t search_pos_smem(int J, int SG, int nodes, int warps) {
 }
 
 // Scoring-only launches with the table outside the CTA's own shared memory (TAB = 1 / 2 of k_search_pos).
-template <int TAB>
+template <int TAB, bool SUM>
 static cudaError_t eval_pos_far_launch(const Device& dev, const PosArgs& a, int pb, bool ints, cudaStream_t st) {
   const int warps = 16;
   const size_t smem = TAB == 2 ? static_cast<size_t>(pos_tab_half(a.J, a.SG)) * 4 + 16 : 16;
@@ -787,16 +788,17 @@ static cudaError_t eval_pos_far_launch(const Device& dev, const PosArgs& a, int 
     }
     return cudaLaunchKernelEx(&cfg, kern, a);
   };
-  if (pb == 1) return ints ? launch(k_search_pos<1, true, false, true, TAB>) : launch(k_search_pos<1, false, false, true, TAB>);
-  return ints ? launch(k_search_pos<2, true, false, true, TAB>) : launch(k_search_pos<2, false, false, true, TAB>);
+  if (pb == 1)
+    return ints ? launch(k_search_pos<1, true, false, true, TAB, SUM>) : launch(k_search_pos<1, false, false, true, TAB, SUM>);
+  return ints ? launch(k_search_pos<2, true, false, true, TAB, SUM>) : launch(k_search_pos<2, false, false, true, TAB, SUM>);
 }
 
 // tab_home: 0 = the table in every CTA's shared memory (cudaErrorNotSupported when it does not fit);
 // scoring only, one node: 2 = split over CTA pairs, 1 = global memory
-cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float* tab, int SG, unsigned flags,
-                              long long first, long long count, bool eval_only, const SearchFuse& sf,
-                              cudaStream_t st, int tab_home) {
-  if (count <= 0) return cudaSuccess;
+template <bool SUM>
+static cudaError_t search_pos_launch_obj(const Device& dev, const SearchDev& s, const float* tab, int SG, unsigned flags,
+                                         long long first, long long count, bool eval_only, const SearchFuse& sf,
+                                         cudaStream_t st, int tab_home) {
   PosArgs a;
   a.tab = tab; a.J = s.J; a.SG = SG; a.nodes = s.nodes;
   a.opt = s.cur_o; a.prio = s.cur_p;
@@ -811,7 +813,7 @@ cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float
   const bool multi = s.nodes > 1;
   if (tab_home != 0) {
     if (!eval_only || multi) return cudaErrorNotSupported;
-    return tab_home == 2 ? eval_pos_far_launch<2>(dev, a, s.pb, ints, st) : eval_pos_far_launch<1>(dev, a, s.pb, ints, st);
+    return tab_home == 2 ? eval_pos_far_launch<2, SUM>(dev, a, s.pb, ints, st) : eval_pos_far_launch<1, SUM>(dev, a, s.pb, ints, st);
   }
   const int warps = 16;
   const size_t smem = search_pos_smem(s.J, SG, s.nodes, warps);
@@ -827,18 +829,27 @@ cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float
   };
   if (eval_only) {
     if (s.pb == 1) {
-      if (multi) return ints ? launch(k_search_pos<1, true, true, true>) : launch(k_search_pos<1, false, true, true>);
-      return ints ? launch(k_search_pos<1, true, false, true>) : launch(k_search_pos<1, false, false, true>);
+      if (multi) return ints ? launch(k_search_pos<1, true, true, true, 0, SUM>) : launch(k_search_pos<1, false, true, true, 0, SUM>);
+      return ints ? launch(k_search_pos<1, true, false, true, 0, SUM>) : launch(k_search_pos<1, false, false, true, 0, SUM>);
     }
-    if (multi) return ints ? launch(k_search_pos<2, true, true, true>) : launch(k_search_pos<2, false, true, true>);
-    return ints ? launch(k_search_pos<2, true, false, true>) : launch(k_search_pos<2, false, false, true>);
+    if (multi) return ints ? launch(k_search_pos<2, true, true, true, 0, SUM>) : launch(k_search_pos<2, false, true, true, 0, SUM>);
+    return ints ? launch(k_search_pos<2, true, false, true, 0, SUM>) : launch(k_search_pos<2, false, false, true, 0, SUM>);
   }
   if (s.pb == 1) {
-    if (multi) return ints ? launch(k_search_pos<1, true, true>) : launch(k_search_pos<1, false, true>);
-    return ints ? launch(k_search_pos<1, true, false>) : launch(k_search_pos<1, false, false>);
+    if (multi) return ints ? launch(k_search_pos<1, true, true, false, 0, SUM>) : launch(k_search_pos<1, false, true, false, 0, SUM>);
+    return ints ? launch(k_search_pos<1, true, false, false, 0, SUM>) : launch(k_search_pos<1, false, false, false, 0, SUM>);
   }
-  if (multi) return ints ? launch(k_search_pos<2, true, true>) : launch(k_search_pos<2, false, true>);
-  return ints ? launch(k_search_pos<2, true, false>) : launch(k_search_pos<2, false, false>);
+  if (multi) return ints ? launch(k_search_pos<2, true, true, false, 0, SUM>) : launch(k_search_pos<2, false, true, false, 0, SUM>);
+  return ints ? launch(k_search_pos<2, true, false, false, 0, SUM>) : launch(k_search_pos<2, false, false, false, 0, SUM>);
+}
+
+cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float* tab, int SG, unsigned flags,
+                              long long first, long long count, bool eval_only, const SearchFuse& sf,
+                              cudaStream_t st, int tab_home) {
+  if (count <= 0) return cudaSuccess;
+  return (flags & SB_FLAG_SUM_COMPLETION)
+             ? search_pos_launch_obj<true>(dev, s, tab, SG, flags, first, count, eval_only, sf, st, tab_home)
+             : search_pos_launch_obj<false>(dev, s, tab, SG, flags, first, count, eval_only, sf, st, tab_home);
 }
 
 // Where the position-major scoring kernel keeps a table of J x SG entries: 0 = every CTA's shared memory;

@@ -18,8 +18,19 @@ from ._lib import FLAG_INTEGER_STARTS, FLAG_REDUCED, SaturnB200Error, SearchPara
 NSLOT = 8
 
 
-def _flags(integer_starts: bool, reduced: bool) -> int:
-    return (FLAG_INTEGER_STARTS if integer_starts else 0) | (FLAG_REDUCED if reduced else 0)
+OBJECTIVES = ("makespan", "completion")
+
+
+def objective_flag(objective: str) -> int:
+    """SB_FLAG_SUM_COMPLETION for objective="completion" (score = sum of completion times), 0 for "makespan"."""
+    if objective not in OBJECTIVES:
+        from .solver import SolverError
+        raise SolverError("objective must be 'makespan' or 'completion', not %r" % (objective,))
+    return _lib.FLAG_SUM_COMPLETION if objective == "completion" else 0
+
+
+def _flags(integer_starts: bool, reduced: bool, objective: str = "makespan") -> int:
+    return (FLAG_INTEGER_STARTS if integer_starts else 0) | (FLAG_REDUCED if reduced else 0) | objective_flag(objective)
 
 
 class Engine:
@@ -124,8 +135,9 @@ class Engine:
              out: Optional[torch.Tensor] = None, best_key: Optional[torch.Tensor] = None, id_base: int = 0,
              _force_generic: bool = False, _no_stream: bool = False, post_key: bool = False, fold_prev: bool = False,
              by_position: bool = False, _plain_addr: bool = False, alt_shape: bool = False,
-             _table_home: int = 0, _reorder: Optional[bool] = None) -> torch.Tensor:
+             _table_home: int = 0, _reorder: Optional[bool] = None, objective: str = "makespan") -> torch.Tensor:
         """Makespan of every candidate (device tensors).  Asynchronous on the handle's stream.
+        objective="completion": the sum of completion times instead (SB_FLAG_SUM_COMPLETION), in `out` and `best_key`.
         by_position: opt[b][i] is the option of the job scheduled i-th (see `opt_by_position`).
         alt_shape: the alternate warp-shuffle kernel (SB_FLAG_ALT_WARPSCAN; a measurement, not a fast path).
         Test hooks: _table_home 2 / 1 puts the position-major kernel's table in a CTA pair's shared memory / in
@@ -134,7 +146,7 @@ class Engine:
         B, stride = self._check_cands(opt, prio, True)
         if out is None:
             out = torch.empty(B, dtype=torch.float32, device=self.device)
-        fl = _flags(integer_starts, reduced) | (_lib._FLAG_FORCE_GENERIC if _force_generic else 0) | (
+        fl = _flags(integer_starts, reduced, objective) | (_lib._FLAG_FORCE_GENERIC if _force_generic else 0) | (
             0x40000000 if _no_stream else 0) | (0x02000000 if _plain_addr else 0) | (
             _lib.FLAG_POST_KEY if post_key else 0) | (
             _lib.FLAG_FOLD_PREV if (post_key and fold_prev) else 0) | (
@@ -157,28 +169,32 @@ class Engine:
         return int(bad.value)
 
     def eval_host(self, opt: torch.Tensor, prio: torch.Tensor, integer_starts: bool = True, reduced: bool = False,
-                  out: Optional[torch.Tensor] = None) -> torch.Tensor:
+                  out: Optional[torch.Tensor] = None, objective: str = "makespan") -> torch.Tensor:
         """Same through HOST tensors (pinned for full PCIe speed): H2D + kernel + D2H, synchronous."""
         B, stride = self._check_cands(opt, prio, False)
         if out is None:
             out = torch.empty(B, dtype=torch.float32, pin_memory=True)
         check(self._lib.sb_eval_host(self._h, C.c_void_p(opt.data_ptr()), C.c_void_p(prio.data_ptr()), B, stride,
-                                     _flags(integer_starts, reduced), C.c_void_p(out.data_ptr())))
+                                     _flags(integer_starts, reduced, objective), C.c_void_p(out.data_ptr())))
         return out
 
-    def eval_full(self, opt: torch.Tensor, prio: torch.Tensor, integer_starts: bool = True, reduced: bool = False):
-        """(makespan[B], start[B][J], slotmask[B][J]) — slot-exact plan of every candidate."""
+    def eval_full(self, opt: torch.Tensor, prio: torch.Tensor, integer_starts: bool = True, reduced: bool = False,
+                  objective: str = "makespan"):
+        """(makespan[B], start[B][J], slotmask[B][J]) — slot-exact plan of every candidate (the first element is the
+        sum of completion times with objective="completion"; starts and masks do not depend on the objective)."""
         B, stride = self._check_cands(opt, prio, True)
         mk = torch.empty(B, dtype=torch.float32, device=self.device)
         start = torch.empty((B, self.J), dtype=torch.float32, device=self.device)
         mask = torch.empty((B, self.J), dtype=torch.int32, device=self.device)
         check(self._lib.sb_eval_full(self._h, C.c_void_p(opt.data_ptr()), C.c_void_p(prio.data_ptr()), B, stride,
-                                     _flags(integer_starts, reduced), C.c_void_p(mk.data_ptr()),
+                                     _flags(integer_starts, reduced, objective), C.c_void_p(mk.data_ptr()),
                                      C.c_void_p(start.data_ptr()), C.c_void_p(mask.data_ptr())))
         return mk, start, mask
 
-    def decode(self, opt: np.ndarray, prio: np.ndarray, integer_starts: bool = True, reduced: bool = False):
-        """One candidate (host arrays) -> dict(start, slotmask, strategy, gpus, makespan)."""
+    def decode(self, opt: np.ndarray, prio: np.ndarray, integer_starts: bool = True, reduced: bool = False,
+               objective: str = "makespan"):
+        """One candidate (host arrays) -> dict(start, slotmask, strategy, gpus, makespan); with
+        objective="completion" the "makespan" entry holds the sum of completion times."""
         J = self.J
         opt = np.ascontiguousarray(opt, dtype=np.uint8)
         prio = np.ascontiguousarray(prio, dtype=np.uint8 if J <= 256 else np.uint16)
@@ -191,7 +207,7 @@ class Engine:
         node = np.empty(J, dtype=np.uint8)
         mk = C.c_float(0)
         check(self._lib.sb_decode(self._h, C.c_void_p(opt.ctypes.data), C.c_void_p(prio.ctypes.data),
-                                  _flags(integer_starts, reduced), C.c_void_p(start.ctypes.data),
+                                  _flags(integer_starts, reduced, objective), C.c_void_p(start.ctypes.data),
                                   C.c_void_p(mask.ctypes.data), C.c_void_p(strat.ctypes.data),
                                   C.c_void_p(gpus.ctypes.data), C.c_void_p(node.ctypes.data), C.byref(mk)))
         return {"start": start, "slotmask": mask, "strategy": strat, "gpus": gpus, "node": node,
@@ -241,11 +257,12 @@ class Engine:
     def search_init(self, chains: int, seed: int = 0, chain_base: int = 0, integer_starts: bool = True,
                     reduced: bool = False, t_start: float = 0.02, t_end: float = 1e-4, total_rounds: int = 200,
                     warm: Optional[Tuple[np.ndarray, np.ndarray]] = None, resample_every: int = 0,
-                    _no_fused: bool = False, _extra_flags: int = 0):
+                    _no_fused: bool = False, _extra_flags: int = 0, objective: str = "makespan"):
         """resample_every > 0: search_round resamples the population by tournament on that cadence itself.
+        objective="completion": minimise the sum of completion times (every score and key holds that sum).
         _extra_flags: test hooks of sb_search_params.flags (see sb_search_verify_count in the header)."""
         p = SearchParams(seed=seed, chains=chains, chain_base=chain_base, resample_every=int(resample_every or 0),
-                         flags=_flags(integer_starts, reduced) | (0x20000000 if _no_fused else 0) | int(_extra_flags),
+                         flags=_flags(integer_starts, reduced, objective) | (0x20000000 if _no_fused else 0) | int(_extra_flags),
                          t_start=t_start, t_end=t_end, total_rounds=total_rounds)
         wo = wp = None
         keep = None
@@ -260,7 +277,8 @@ class Engine:
         self._search_base = chain_base
 
     def search_seed_lpt(self):
-        """Plant the three longest-processing-time seeds into an eighth of the population each."""
+        """Plant the three longest-processing-time seeds into an eighth of the population each (shortest-processing-time
+        orders when the search minimises the sum of completion times)."""
         check(self._lib.sb_search_seed_lpt(self._h))
 
     def search_run(self, chains: int, rounds: int, seed: int = 0, chain_base: int = 0, integer_starts: bool = True,
@@ -268,12 +286,13 @@ class Engine:
                    warm: Optional[Tuple[np.ndarray, np.ndarray]] = None, resample_every: int = -1, sync_every: int = 16,
                    patience: int = 0, time_budget_s: float = 0.0, target_makespan: float = 0.0,
                    heuristic_seeds: bool = True, record_history: bool = False, _no_fused: bool = False,
-                   _extra_flags: int = 0):
+                   _extra_flags: int = 0, objective: str = "makespan"):
         """The whole single-GPU search in one C call (sb_search_run).  Returns a dict: opt, prio, makespan, key,
-        evaluated, rounds, stop_reason, wall_s, history [(wall s, evaluated, makespan)]."""
+        evaluated, rounds, stop_reason, wall_s, history [(wall s, evaluated, makespan)].  With
+        objective="completion" every "makespan" there is the sum of completion times, and target_makespan targets it."""
         return _search_run(self._lib, [self._h], self.J, chains, rounds, seed, chain_base, integer_starts, reduced,
                            t_start, t_end, warm, resample_every, sync_every, patience, time_budget_s, target_makespan,
-                           heuristic_seeds, record_history, _no_fused, _extra_flags)
+                           heuristic_seeds, record_history, _no_fused, _extra_flags, objective)
 
     def search_wave(self, reduced: bool = False) -> int:
         """Chains that fill the device exactly once with the round kernel of the current table; populations
@@ -333,11 +352,11 @@ class Engine:
 
 def _search_run(lib, handles, J, chains, rounds, seed, chain_base, integer_starts, reduced, t_start, t_end, warm,
                 resample_every, sync_every, patience, time_budget_s, target_makespan, heuristic_seeds,
-                record_history, _no_fused, _extra_flags=0):
+                record_history, _no_fused, _extra_flags=0, objective="makespan"):
     """sb_search_run (one handle) / sb_search_run_multi (one handle per device of this process)."""
     pdt = np.uint8 if J <= 256 else np.uint16
     p = SearchParams(seed=seed, chains=chains, chain_base=chain_base,
-                     flags=_flags(integer_starts, reduced) | (0x20000000 if _no_fused else 0) | int(_extra_flags),
+                     flags=_flags(integer_starts, reduced, objective) | (0x20000000 if _no_fused else 0) | int(_extra_flags),
                      t_start=t_start, t_end=t_end, total_rounds=max(rounds, 1))
     cap = (max(rounds, 1) // max(1, sync_every) + 3) if record_history else 0
     hw, he, hm = np.zeros(cap, np.float64), np.zeros(cap, np.int64), np.zeros(cap, np.float32)
@@ -427,11 +446,12 @@ class MultiEngine:
                    reduced: bool = False, t_start: float = 5e-4, t_end: float = 1e-6, warm=None,
                    resample_every: int = -1, sync_every: int = 16, patience: int = 0, time_budget_s: float = 0.0,
                    target_makespan: float = 0.0, heuristic_seeds: bool = True, record_history: bool = False,
-                   _no_fused: bool = False, _extra_flags: int = 0):
+                   _no_fused: bool = False, _extra_flags: int = 0, objective: str = "makespan"):
         """`chains` is per device; the result's `evaluated` counts every device."""
         return _search_run(self._lib, [e._h for e in self.engines], self.J, chains, rounds, seed, chain_base,
                            integer_starts, reduced, t_start, t_end, warm, resample_every, sync_every, patience,
-                           time_budget_s, target_makespan, heuristic_seeds, record_history, _no_fused, _extra_flags)
+                           time_budget_s, target_makespan, heuristic_seeds, record_history, _no_fused, _extra_flags,
+                           objective)
 
 
 class _CudaArrayView:

@@ -17,7 +17,7 @@ from typing import List, Optional, Tuple
 import numpy as np
 import torch
 
-from .engine import Engine
+from .engine import Engine, objective_flag
 
 
 @dataclass
@@ -43,11 +43,14 @@ def key_makespan(key: int) -> float:
     return float(np.array([(key >> 32) & 0xffffffff], dtype=np.uint32).view(np.float32)[0])
 
 
-def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1):
+def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objective: str = "makespan"):
     """Heuristic warm candidates in the reduced encoding (opt byte = k-1, plus node << 3 when there
     are several nodes), longest-processing-time order: (a) every job on its fastest option,
     (b) every job on its least GPU-seconds option, (c) in between.  Nodes are filled greedily by
-    accumulated GPU-seconds."""
+    accumulated GPU-seconds.  objective="completion": shortest-processing-time order instead (ascending
+    runtime of the chosen option), the order that favours the sum of completion times; same options and
+    node fill (sb_search_seed_lpt plants the same seeds)."""
+    objective_flag(objective)
     J = tmin.shape[0]
     usable = np.where(tmin < sentinel, tmin, np.inf)
     if not np.isfinite(usable).any(axis=1).all():
@@ -58,7 +61,10 @@ def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1):
         cost = usable.astype(np.float64) * (k ** area_weight)
         col = np.argmin(cost, axis=1)
         rt = usable[np.arange(J), col]
-        order = np.argsort(-rt * (col + 1) ** 0.5, kind="stable")
+        if objective == "completion":
+            order = np.argsort(rt, kind="stable")
+        else:
+            order = np.argsort(-rt * (col + 1) ** 0.5, kind="stable")
         ob = col.astype(np.uint8)
         if nodes > 1:
             load = np.zeros(nodes)
@@ -78,13 +84,16 @@ def run_search(engine: Engine, chains: int = 1 << 16, rounds: int = 200, seed: i
                target_makespan: Optional[float] = None, reseed_every: int = 0, resample_every: Optional[int] = None,
                record_history: bool = False, heuristic_seeds: bool = True,
                exchange_every: int = 16, _no_fused: bool = False, _python_driver: bool = False,
-               _extra_flags: int = 0) -> SearchResult:
+               _extra_flags: int = 0, objective: str = "makespan") -> SearchResult:
     """Run the search on `engine` (table already set).  Returns the best candidate found by any rank.
+    objective="completion" minimises the sum of completion times; the result's `makespan`, the history and
+    `target_makespan` then hold / target that sum.
 
     `rounds` device rounds are issued in groups of `exchange_every` (tournament resampling every
     `resample_every` rounds inside a group is only another launch); after each group the ranks exchange
     their best key (one MIN) and the stopping rules are evaluated, so the host synchronises once per
     group rather than once per round."""
+    objective_flag(objective)
     if resample_every is None:
         resample_every = -1          # the library's choice: 2 inside the tile kernel, 4 where it costs a copy
     dist = _dist() if use_dist else None
@@ -94,7 +103,8 @@ def run_search(engine: Engine, chains: int = 1 << 16, rounds: int = 200, seed: i
                               t_start=t_start, t_end=t_end, warm=warm, resample_every=resample_every,
                               sync_every=exchange_every, patience=patience or 0, time_budget_s=time_budget_s or 0.0,
                               target_makespan=target_makespan or 0.0, heuristic_seeds=heuristic_seeds,
-                              record_history=record_history, _no_fused=_no_fused, _extra_flags=_extra_flags)
+                              record_history=record_history, _no_fused=_no_fused, _extra_flags=_extra_flags,
+                              **({"objective": objective} if objective != "makespan" else {}))
         return SearchResult(opt=r["opt"], prio=r["prio"], makespan=r["makespan"], evaluated=r["evaluated"],
                             rounds=r["rounds"], wall_s=r["wall_s"], history=r["history"], owner_rank=0)
     rank = dist.get_rank() if dist else 0
@@ -105,14 +115,15 @@ def run_search(engine: Engine, chains: int = 1 << 16, rounds: int = 200, seed: i
     engine.search_init(chains, seed=seed, chain_base=rank * chains, integer_starts=integer_starts,
                        reduced=reduced, t_start=t_start, t_end=t_end, total_rounds=max(rounds, 1), warm=warm,
                        resample_every=resample_every, **({"_no_fused": True} if _no_fused else {}),
-                       **({"_extra_flags": _extra_flags} if _extra_flags else {}))
+                       **({"_extra_flags": _extra_flags} if _extra_flags else {}),
+                       **({"objective": objective} if objective != "makespan" else {}))
     if heuristic_seeds:
         # every rank plants the longest-processing-time seeds in an eighth of its population each;
         # the rest stays random (diversity), tournament resampling then concentrates the population
         tmin, args = engine.reduced_table()
         per = max(1, chains // 8)
         nodes = getattr(engine, "nodes", 1)
-        for i, (col, order) in enumerate(lpt_seeds(tmin, nodes=nodes)):
+        for i, (col, order) in enumerate(lpt_seeds(tmin, nodes=nodes, objective=objective)):
             opt = col if reduced else ((args[np.arange(J), col & 7].astype(np.uint8) << 3) | col)
             first = min(i * per, max(0, chains - per))
             engine.search_inject(opt.astype(np.uint8), order.astype(pdt), copies=min(per, chains), first=first)

@@ -212,6 +212,21 @@ def _check_horizon(T, found_makespan=None):
                           "fp32 at that horizon; express runtimes in coarser units (e.g. minutes) or drop sentinel "
                           "options" % lower)
 
+def _check_objective(objective, hysteresis=False):
+    if objective not in ("makespan", "completion"):
+        raise SolverError("objective must be 'makespan' or 'completion', not %r" % (objective,))
+    if objective == "completion" and hysteresis:
+        raise SolverError("hysteresis=True compares plans by makespan (milp.py:363-442); it is not defined for "
+                          "objective='completion'")
+
+
+def _plan_horizon(start, rt):
+    """max(start + rt) of a decoded plan: the latest time the device's fp32 schedule holds.  With the
+    sum-of-completion-times objective the device's score is a sum that may exceed 2^24 while every start is
+    exact, so the horizon guard checks the plan itself."""
+    return max((float(s) + float(r) for s, r in zip(start, rt)), default=0.0)
+
+
 def _default_nodes() -> int:
     env = os.environ.get("SATURN_B200_NODES")
     if env:
@@ -228,8 +243,16 @@ def _default_nodes() -> int:
 def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count() or 4) // 4), interval=1000,
           timeout=500, *, chains: Optional[int] = None, rounds: Optional[int] = None, seed: int = 0,
           integer_starts: bool = True, engine=None, hysteresis: Optional[bool] = None,
-          nodes: Optional[int] = None, devices=None):
+          nodes: Optional[int] = None, devices=None, objective: str = "makespan"):
     """Drop-in for saturn.solver.solve (milp.py:23).
+
+    Objective.  "makespan" (the default, the reference's) or "completion": minimise the sum of the tasks'
+    completion times sum_t (start_t + runtime_t) — equivalently the mean time a job waits for its result —
+    which a makespan-optimal plan can leave poor (long jobs first, every short job finishes late).  The
+    6th element returned is the plan's makespan under both objectives; last_stats["objective"] names the
+    objective and last_stats["total_completion"] holds the plan's sum of completion times, recomputed in
+    float64 from the emitted plan and the tasks' own runtimes; last_stats["device_makespan"] is the device's
+    fp32 score of the plan (the sum, under "completion").  Anything else raises SolverError.
 
     Returns (sta, tga, bss, bna, boa, makespan) — milp.py:445 — with a real float makespan
     (the reference returns None on a cold start, milp.py:394-399; callers only thread it back in
@@ -250,9 +273,12 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     (milp.py:394-399 never assigns it), so the swap / keep branches are unreachable (SURVEY §3.2).
     That observable behaviour is the default here.  `hysteresis=True` (or SATURN_B200_HYSTERESIS=1)
     enables the documented intent instead: keep the current plan, shifted by one interval, unless
-    the new one is better by more than interval + 500 s (milp.py:363,377,429-442).
+    the new one is better by more than interval + 500 s (milp.py:363,377,429-442).  The rule is stated
+    in makespans: hysteresis=True with objective="completion" raises SolverError, and
+    SATURN_B200_HYSTERESIS applies to the makespan objective only.
     """
     from .search import run_search
+    _check_objective(objective, bool(hysteresis))
     t_wall = time.perf_counter()
     task_list = list(task_list)
     J = len(task_list)
@@ -286,10 +312,14 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
         pass
     warm = candidate_from_arrays(task_list, presolved, nodes)
     res = run_search(eng, chains=chains, rounds=rounds, seed=seed, integer_starts=integer_starts, reduced=True,
-                     time_budget_s=budget, patience=max(40, rounds // 4), warm=warm)
-    _check_horizon(Tdev, res.makespan)
+                     time_budget_s=budget, patience=max(40, rounds // 4), warm=warm,
+                     **({"objective": objective} if objective != "makespan" else {}))
+    if objective == "makespan":
+        _check_horizon(Tdev, res.makespan)
     dec = eng.decode(res.opt, res.prio, integer_starts=integer_starts, reduced=True)
     gpus = dec["gpus"].astype(np.int64)
+    if objective != "makespan":
+        _check_horizon(Tdev, _plan_horizon(dec["start"], Tdev[np.arange(J), 0, gpus - 1]))
     chosen = optindex[np.arange(J), gpus - 1]
     if (chosen < 0).any():
         raise SolverError("search returned an option a task does not have")
@@ -307,12 +337,14 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     last_stats = {"candidates": res.evaluated, "rounds": res.rounds, "search_wall_s": res.wall_s,
                   "device_makespan": res.makespan, "makespan": prop_makespan, "J": J, "chains": chains,
                   "nodes": nodes, "devices": len(getattr(eng, "engines", [eng])),
-                  "total_wall_s": None, "adopted": True}
+                  "total_wall_s": None, "adopted": True, "objective": objective,
+                  "total_completion": sum(float(dec["start"][i]) + float(rts[i]) for i in range(J))}
 
     # ---- introspection hysteresis (opt-in): the documented intent of milp.py:363-442
     out = prop + (prop_makespan,)
     if hysteresis is None:
-        hysteresis = os.environ.get("SATURN_B200_HYSTERESIS", "0") not in ("", "0", "false", "False")
+        hysteresis = objective == "makespan" and os.environ.get("SATURN_B200_HYSTERESIS", "0") not in (
+            "", "0", "false", "False")
     if presolved is not None and hysteresis:
         p_sta, p_tga, p_bss, p_bna, p_boa, saved = presolved
         same_tasks = p_tga is not None and len(p_tga) == J
@@ -401,8 +433,10 @@ def strategies_from_table(T, mask, executors=None, params=None, gcount=None):
 
 def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeout=500, *,
                 chains: Optional[int] = None, rounds: Optional[int] = None, seed: int = 0,
-                integer_starts: bool = True, engine=None, nodes: Optional[int] = None, devices=None):
+                integer_starts: bool = True, engine=None, nodes: Optional[int] = None, devices=None,
+                objective: str = "makespan"):
     """solve() on the dense profiler tensor T[J][S][G] (+ mask of usable cells, + gcount[G] GPU counts).
+    `objective` as for solve(): "makespan" or "completion" (sum of completion times).
 
     The table goes to the device un-reduced (sb_set_table: min over strategies with the first-minimum rule
     and its arg-min on the device, PerformanceEvaluator.py:101-115); the search runs on the reduced view
@@ -412,6 +446,7 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     each task's chosen cell.  For the same seed and population the plan equals solve() on the
     `strategies_from_table` view."""
     from .search import run_search
+    _check_objective(objective)
     T = np.ascontiguousarray(T, dtype=np.float32)
     if T.ndim != 3:
         raise SolverError("T must be [J][S][G]")
@@ -448,8 +483,10 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
             strategies = {g: None for g in gcount}
         warm = candidate_from_arrays([_Opt] * J, presolved, nodes)
     res = run_search(eng, chains=chains, rounds=rounds, seed=seed, integer_starts=integer_starts, reduced=True,
-                     time_budget_s=budget, patience=max(40, rounds // 4), warm=warm)
-    _check_horizon(Tdev, res.makespan)
+                     time_budget_s=budget, patience=max(40, rounds // 4), warm=warm,
+                     **({"objective": objective} if objective != "makespan" else {}))
+    if objective == "makespan":
+        _check_horizon(Tdev, res.makespan)
     dec = eng.decode(res.opt, res.prio, integer_starts=integer_starts, reduced=True)
     gpus = dec["gpus"].astype(np.int64)
     chosen = np.array([col_of_k[int(k)] for k in gpus], dtype=np.int64)
@@ -457,11 +494,15 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     position[res.prio.astype(np.int64)] = np.arange(J)
     arrays = plan_to_arrays([G] * J, chosen, dec["start"], dec["slotmask"], position, nodes=nodes, node_of=dec["node"])
     strategy = dec["strategy"].astype(np.int64)
-    makespan = max(float(dec["start"][j]) + float(T[j, strategy[j], chosen[j]]) for j in range(J))
+    rts = [float(T[j, strategy[j], chosen[j]]) for j in range(J)]
+    if objective != "makespan":
+        _check_horizon(Tdev, _plan_horizon(dec["start"], rts))
+    makespan = max(float(dec["start"][j]) + rts[j] for j in range(J))
     global last_stats
     last_stats = {"candidates": res.evaluated, "rounds": res.rounds, "search_wall_s": res.wall_s,
                   "device_makespan": res.makespan, "makespan": makespan, "J": J, "chains": chains, "nodes": nodes,
-                  "devices": len(getattr(eng, "engines", [eng])), "total_wall_s": None, "adopted": True}
+                  "devices": len(getattr(eng, "engines", [eng])), "total_wall_s": None, "adopted": True,
+                  "objective": objective, "total_completion": sum(float(dec["start"][j]) + rts[j] for j in range(J))}
     return arrays + (makespan, strategy)
 
 

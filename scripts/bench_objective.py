@@ -1,0 +1,106 @@
+"""Cost and effect of the sum-of-completion-times objective on one GPU; prints one JSON line.
+
+    python scripts/bench_objective.py [--steps 200] [--warmup 20] [--solve-chains 0] [--solve-rounds 400]
+
+kernel: sb_eval on bench.py's C4 batch (J = 256, S = 8, 946,176 candidates, the same seeded inputs, integer
+        starts), scored for the makespan and for the sum of completion times, the two launches alternated in one
+        process and timed with CUDA events; median of --steps launches each.
+solve:  solve() wall time on a 256-task set (synthetic table, seed 3, 4 strategies) for both objectives, each plan
+        scored on both objectives (float64, the tasks' own runtimes).
+The card's name and power limit are read in the same run (nvidia-smi, read-only queries).
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
+
+
+def card(index):
+    q = "name,power.limit,clocks.max.sm"
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=" + q, "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=20).stdout.strip().split(",")
+        return {"name": out[0].strip(), "power_limit_w": float(out[1]), "sm_max_mhz": float(out[2])}
+    except Exception as e:  # noqa: BLE001 - the measurement still stands, the card is then named by torch only
+        import torch
+        return {"name": torch.cuda.get_device_name(index), "power_limit_w": None, "error": str(e)}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=200)
+    ap.add_argument("--warmup", type=int, default=20)
+    ap.add_argument("--solve-chains", type=int, default=0, help="0 = solve()'s default population")
+    ap.add_argument("--solve-rounds", type=int, default=400)
+    args = ap.parse_args()
+    import numpy as np
+    import torch
+    from saturn_b200 import solver as S
+    from saturn_b200.engine import Engine, random_candidates
+    from saturn_b200.synth import synth_table
+    torch.cuda.set_device(0)
+    eng = Engine(0)
+    J, Sx, G = 256, 8, 8
+    B = 132 * 8 * 32 * 28                                   # bench.py's B_PER_GPU
+    T, valid = synth_table(J, Sx, G, seed=0)
+    eng.set_table(T)
+    opt, prio = random_candidates(eng, B, valid, seed=1)
+    out = torch.empty(B, dtype=torch.float32, device=eng.device)
+    key = torch.full((1,), 2 ** 63 - 1, dtype=torch.int64, device=eng.device)
+    times = {"makespan": [], "completion": []}
+    for i in range(args.warmup + args.steps):
+        for obj in ("makespan", "completion") if i % 2 == 0 else ("completion", "makespan"):
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record()
+            eng.eval(opt, prio, out=out, best_key=key, objective=obj)
+            b.record()
+            b.synchronize()
+            if i >= args.warmup:
+                times[obj].append(a.elapsed_time(b))
+    path = eng.last_eval_path()
+    kernel = {o: {"median_ms": float(np.median(t)), "p10_ms": float(np.percentile(t, 10)),
+                  "p90_ms": float(np.percentile(t, 90)), "candidates_per_s": B / (float(np.median(t)) * 1e-3)}
+              for o, t in times.items()}
+    kernel["completion_over_makespan"] = kernel["completion"]["median_ms"] / kernel["makespan"]["median_ms"]
+    kernel.update(B=B, J=J, S=Sx, path=path, steps=args.steps)
+    del opt, prio, out
+    torch.cuda.empty_cache()
+
+    from saturn_b200.solver import strategies_from_table
+
+    class _Task:
+        def __init__(self, name, strategies):
+            self.name, self.strategies, self.selected_strategy = name, strategies, None
+
+        def select_strategy(self, s):
+            self.selected_strategy = s
+
+    T2, valid2 = synth_table(256, 4, 8, seed=3)
+    strategies = strategies_from_table(T2, valid2)
+    tasks = [_Task("t%d" % j, strategies[j]) for j in range(256)]
+    kw = dict(rounds=args.solve_rounds, seed=1, engine=eng)
+    if args.solve_chains:
+        kw["chains"] = args.solve_chains
+    S.solve(tasks, None, rounds=4, engine=eng)               # first launches load the kernels
+    S.solve(tasks, None, rounds=4, engine=eng, objective="completion")
+    solve = {}
+    for obj in ("makespan", "completion"):
+        t0 = time.perf_counter()
+        res = S.solve(tasks, None, objective=obj, **kw)
+        wall = time.perf_counter() - t0
+        st = S.last_stats
+        solve[obj] = {"wall_s": wall, "makespan": res[5], "total_completion": st["total_completion"],
+                      "mean_completion": st["total_completion"] / len(tasks), "rounds": st["rounds"],
+                      "candidates": st["candidates"]}
+    print(json.dumps({"card": card(0), "kernel": kernel, "solve": solve}))
+    eng.close()
+
+
+if __name__ == "__main__":
+    main()
