@@ -14,7 +14,19 @@ FLAG_FOLD_PREV = 16
 FLAG_ALT_WARPSCAN = 32
 FLAG_SUM_COMPLETION = 64
 IPC_HANDLE_BYTES = 64
-_FLAG_FORCE_GENERIC = 0x80000000
+# test hooks in the top bits of the same flags word: the enum in csrc/sb_internal.h says what each one forces
+HOOK_FORCE_GENERIC = 0x80000000
+HOOK_NO_STREAM = 0x40000000
+HOOK_NO_FUSED = 0x20000000
+HOOK_NO_INCREMENTAL = 0x10000000
+HOOK_VERIFY_INCREMENTAL = 0x08000000
+HOOK_ROUND1_MOVES = 0x04000000
+HOOK_PLAIN_ADDR = 0x02000000
+HOOK_WINDOW_BIAS = 0x01000000
+HOOK_TABLE_GLOBAL = 0x00800000
+HOOK_TABLE_PAIR = 0x00400000
+HOOK_REORDER = 0x00200000
+HOOK_NO_REORDER = 0x00100000
 
 # every symbol include/saturn_b200.h declares (tests check that the library exports them all)
 SYMBOLS = [

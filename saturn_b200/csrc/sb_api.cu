@@ -356,14 +356,14 @@ int sb_eval(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, int64
   // tiles (C5 with all strategies: 256 KB, tile kernel path 4) or J >= 1024 (33 KB of opt tile per warp: 5 warps
   // per SM): re-order the opt bytes into schedule order on the device (h->by_pos, B x row_stride bytes, grow-only)
   // and score them with the position-major kernel, which keeps no tile and streams both rows.
-  // Test hooks: 0x00200000 takes this route at any size, 0x00100000 never.
+  // HOOK_REORDER takes this route at any size.
   {
-    const bool hooks = (flags & (0x80000000u | 0x40000000u | 0x00100000u | SB_FLAG_POST_KEY | SB_FLAG_FOLD_PREV |
-                                 SB_FLAG_ALT_WARPSCAN)) != 0;
+    const bool hooks = (flags & (HOOK_FORCE_GENERIC | HOOK_NO_STREAM | HOOK_NO_REORDER | SB_FLAG_POST_KEY |
+                                 SB_FLAG_FOLD_PREV | SB_FLAG_ALT_WARPSCAN)) != 0;
     const bool aligned = row_stride % 32 == 0 && reinterpret_cast<uintptr_t>(opt) % 32 == 0 &&
                          reinterpret_cast<uintptr_t>(prio) % 32 == 0;
     const int home = eval_pos_home(h->dev, c.J, c.SG, c.nodes, flags);
-    if (!hooks && aligned && B > 0 && c.J <= 6144 && home >= 0 && (home != 0 || c.J >= 1024 || (flags & 0x00200000u))) {
+    if (!hooks && aligned && B > 0 && c.J <= 6144 && home >= 0 && (home != 0 || c.J >= 1024 || (flags & HOOK_REORDER))) {
       const size_t need = static_cast<size_t>(B) * static_cast<size_t>(row_stride);
       if (need > h->by_pos_bytes) {
         if (h->by_pos) CK(cudaFree(h->by_pos));
@@ -396,7 +396,7 @@ int sb_eval(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, int64
     h->last_path = 6;
     return SB_OK;
   }
-  c.force_generic = (flags & 0x80000000u) ? 1 : 0;  // test hooks: 0x80000000 generic kernel, 0x40000000 no streaming
+  c.force_generic = (flags & HOOK_FORCE_GENERIC) ? 1 : 0;
   const bool post = (flags & SB_FLAG_POST_KEY) != 0;
   if (post) {
     if (!h->xchg_ready) return fail(SB_ERR_STATE, "SB_FLAG_POST_KEY needs sb_xchg_connect first");
@@ -551,12 +551,8 @@ int sb_decode(sb_handle* h, const uint8_t* opt, const void* prio, unsigned flags
 }
 
 // ------------------------------------------------------------------------------------------ exchange
-int sb_xchg_create(sb_handle* h, int rank, int world, void* handle_out) {
-  int rc = use_device(h);
-  if (rc) return rc;
-  if (world < 1 || world > kMaxRanks || rank < 0 || rank >= world)
-    return fail(SB_ERR_ARG, "rank %d / world %d outside 0..%d", rank, world, kMaxRanks);
-  if (!handle_out) return fail(SB_ERR_ARG, "handle_out is null");
+// a fresh, zeroed mailbox, completion counter and error flag on the handle's device, for rank `rank` of `world`
+static int create_mailbox(sb_handle* h, int rank, int world) {
   free_xchg(h);
   const size_t bytes = 2 * kMaxRanks * 2 * sizeof(unsigned long long);
   CK(cudaMalloc(&h->xd.local, bytes));
@@ -567,6 +563,16 @@ int sb_xchg_create(sb_handle* h, int rank, int world, void* handle_out) {
   CK(cudaMemset(h->d_xerr, 0, sizeof(int)));
   h->xd.rank = rank;
   h->xd.world = world;
+  return SB_OK;
+}
+
+int sb_xchg_create(sb_handle* h, int rank, int world, void* handle_out) {
+  int rc = use_device(h);
+  if (rc) return rc;
+  if (world < 1 || world > kMaxRanks || rank < 0 || rank >= world)
+    return fail(SB_ERR_ARG, "rank %d / world %d outside 0..%d", rank, world, kMaxRanks);
+  if (!handle_out) return fail(SB_ERR_ARG, "handle_out is null");
+  if ((rc = create_mailbox(h, rank, world))) return rc;
   cudaIpcMemHandle_t hdl;
   CK(cudaIpcGetMemHandle(&hdl, h->xd.local));
   static_assert(sizeof(hdl) == SB_IPC_HANDLE_BYTES, "cudaIpcMemHandle_t is 64 bytes");
@@ -615,16 +621,7 @@ int sb_xchg_connect_local(sb_handle** hs, int n) {
     int rc = use_device(h);
     if (rc) return rc;
     CK(cudaStreamSynchronize(h->stream));
-    free_xchg(h);
-    const size_t bytes = 2 * kMaxRanks * 2 * sizeof(unsigned long long);
-    CK(cudaMalloc(&h->xd.local, bytes));
-    CK(cudaMemset(h->xd.local, 0, bytes));
-    CK(cudaMalloc(&h->d_xcounter, sizeof(unsigned)));
-    CK(cudaMemset(h->d_xcounter, 0, sizeof(unsigned)));
-    CK(cudaMalloc(&h->d_xerr, sizeof(int)));
-    CK(cudaMemset(h->d_xerr, 0, sizeof(int)));
-    h->xd.rank = i;
-    h->xd.world = n;
+    if ((rc = create_mailbox(h, i, n))) return rc;
     h->xchg_created = true;
   }
   // same address space: a peer's mailbox is reachable as soon as peer access is on (no IPC handles)
@@ -789,7 +786,7 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
   // (the initialisation kernels write whole rows, padding included: no memset of the population)
   // Rows that do not fit in shared memory: keep the population in schedule order and stream both rows.
   const int SGs = (reduced ? 1 : h->S) * kSlots;
-  const bool no_fused = (p->flags & 0x20000000u) != 0;  // test hook
+  const bool no_fused = (p->flags & HOOK_NO_FUSED) != 0;
   const int mode = search_round_mode(h->dev, J, SGs, h->nodes);
   d.pos = (!no_fused && mode != 2 && search_pos_smem(J, SGs, h->nodes, 16) <= h->dev.smem_optin) ? 1 : 0;
   if (d.pos) CK(search_init_population_pos(d, h->stream));
@@ -823,17 +820,15 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
   s.launches = 0;
   s.fused_ok = d.pos || (!no_fused && mode != 0);
   // incremental rounds: fused kernels, one node, at least two windows (tile kernel: windows of kSnapPos
-  // positions; position-major kernel: windows of whole 32-position blocks, at most 32 windows).  Test hooks in
-  // the flags: 0x04000000 = round-1 move generator (no windows), 0x10000000 = windowed moves scored from
-  // position 0, 0x08000000 = verify
+  // positions; position-major kernel: windows of whole 32-position blocks, at most 32 windows)
   int nwin = (J + kSnapPos - 1) / kSnapPos;
   if (d.pos) {
     const int nout = (J + 31) / 32, wblk = (nout + 31) / 32;
     nwin = (nout + wblk - 1) / wblk;
   }
-  s.win = s.fused_ok && h->nodes == 1 && nwin >= 2 && nwin <= 32 && !(p->flags & 0x04000000u);
-  s.inc = s.win && !(p->flags & 0x10000000u);
-  s.verify = s.inc && (p->flags & 0x08000000u);
+  s.win = s.fused_ok && h->nodes == 1 && nwin >= 2 && nwin <= 32 && !(p->flags & HOOK_ROUND1_MOVES);
+  s.inc = s.win && !(p->flags & HOOK_NO_INCREMENTAL);
+  s.verify = s.inc && (p->flags & HOOK_VERIFY_INCREMENTAL);
   // automatic cadence: resampling is nearly free inside the tile kernel; elsewhere it is a full copy of the
   // population and ends a launch (an incremental launch starts with one unmodified pass, so longer is better)
   if (s.p.resample_every < 0) s.p.resample_every = (s.fused_ok && !d.pos) ? 2 : (s.inc ? 8 : 4);
@@ -879,7 +874,7 @@ static SearchFuse make_fuse(const SearchState& s, int round, int n) {
   sf.resample_every = s.p.resample_every > 0 ? s.p.resample_every : 0;
   sf.deal = static_cast<int>(s.launches & 1);
   sf.win = s.win ? 1 : 0;
-  sf.win_bias = (s.p.flags & 0x01000000u) ? 1 : 0;
+  sf.win_bias = (s.p.flags & HOOK_WINDOW_BIAS) ? 1 : 0;
   sf.snap = s.inc ? s.snap : nullptr;
   sf.verify_bad = s.verify ? s.verify_bad : nullptr;
   sf.keep.counter = s.tail_counter;
@@ -887,6 +882,17 @@ static SearchFuse make_fuse(const SearchState& s, int round, int n) {
   sf.keep.best_o = s.d.best_o; sf.keep.best_p = s.d.best_p;
   sf.keep.chains = s.d.chains; sf.keep.stride_o = s.d.stride_o; sf.keep.stride_p = s.d.stride_p;
   return sf;
+}
+
+// tournament resampling of the whole population: the kernel writes the result to the proposal buffers, which then
+// become the current ones
+static int resample_population(sb_handle* h) {
+  SearchDev& d = h->search.d;
+  CK(search_resample(d, h->search.rounds_done, h->stream));
+  std::swap(d.cur_o, d.prop_o);
+  std::swap(d.cur_p, d.prop_p);
+  std::swap(d.cur_mk, d.prop_mk);
+  return SB_OK;
 }
 
 int sb_search_round(sb_handle* h, int rounds) {
@@ -903,8 +909,7 @@ int sb_search_round(sb_handle* h, int rounds) {
     const bool due = re > 0 && round > 1 && (round - 1) % re == 0;  // the population is resampled before this round
     if (s.d.pos) {
       if (due) {
-        CK(search_resample(s.d, s.rounds_done, h->stream));
-        std::swap(s.d.cur_o, s.d.prop_o); std::swap(s.d.cur_p, s.d.prop_p); std::swap(s.d.cur_mk, s.d.prop_mk);
+        if ((rc = resample_population(h))) return rc;
       }
       n = std::min(left, kMaxFusedRounds);
       if (re > 0) n = std::min(n, re - (round - 1) % re);  // up to the next resampling point
@@ -935,8 +940,7 @@ int sb_search_round(sb_handle* h, int rounds) {
     }
     if (!fused) {
       if (due) {
-        CK(search_resample(s.d, s.rounds_done, h->stream));
-        std::swap(s.d.cur_o, s.d.prop_o); std::swap(s.d.cur_p, s.d.prop_p); std::swap(s.d.cur_mk, s.d.prop_mk);
+        if ((rc = resample_population(h))) return rc;
       }
       CK(search_propose(s.d, round, h->stream));
       if ((rc = search_eval(h, false, 0, s.d.chains))) return rc;
@@ -990,12 +994,7 @@ int sb_search_resample(sb_handle* h) {
   if (rc) return rc;
   SearchState& s = h->search;
   if (!s.ready) return fail(SB_ERR_STATE, "sb_search_init has not been called");
-  CK(search_resample(s.d, s.rounds_done, h->stream));
-  // the resampled population was written to the proposal buffers: swap roles
-  std::swap(s.d.cur_o, s.d.prop_o);
-  std::swap(s.d.cur_p, s.d.prop_p);
-  std::swap(s.d.cur_mk, s.d.prop_mk);
-  return SB_OK;
+  return resample_population(h);
 }
 
 int sb_search_inject(sb_handle* h, const uint8_t* opt, const void* prio, int64_t first_chain, int copies) {

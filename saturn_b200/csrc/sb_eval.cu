@@ -714,60 +714,41 @@ int plan_tiles(const Device& dev, int J, int SG, int pb, bool stream, int nodes,
   return nw;
 }
 
-template <int PB, bool INT, bool STREAM, bool MULTI, bool TABG = false, int ADDR = 0, bool SUM = false>
-static cudaError_t launch_tiles(const Device& dev, const TileArgs& a, const TilePlan& tp, cudaStream_t st) {
-  auto kern = k_eval_tiles<PB, INT, STREAM, MULTI, false, TABG, ADDR, SUM>;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(tp.smem));
-  if (e != cudaSuccess) return e;
+using TileKernel = void (*)(TileArgs);
+
+// both row buffers start on 16-byte boundaries and stay on them from row to row: TMA bulk copies can fetch the rows
+static bool bulk_aligned(const EvalCall& c) {
+  return (c.stride_o % 16 == 0) && (c.stride_p % 16 == 0) && (reinterpret_cast<uintptr_t>(c.opt) % 16 == 0) &&
+         (reinterpret_cast<uintptr_t>(c.prio) % 16 == 0);
+}
+
+// the fields of TileArgs that the call and the tile plan fix
+static TileArgs tile_args(const EvalCall& c, const TilePlan& tp) {
+  TileArgs a;
+  a.tab = c.tab; a.J = c.J; a.SG = c.SG; a.opt = c.opt; a.prio = c.prio; a.B = c.B;
+  a.stride_o = c.stride_o; a.stride_p = c.stride_p;
+  a.row_o = tp.row_o; a.row_p = tp.row_p; a.copy_o = tp.copy_o; a.copy_p = tp.copy_p;
+  a.nodes = c.nodes;
+  a.out = c.out; a.best_key = c.best_key; a.id_base = c.id_base;
+  a.ntiles = (c.B + 31) / 32;
+  a.one = 1;
+  return a;
+}
+
+static cudaError_t launch_tiles(const Device& dev, TileKernel kern, const TileArgs& a, const TilePlan& tp,
+                                cudaStream_t st) {
   long long ctas = (a.ntiles + tp.warps - 1) / tp.warps;
   int grid = static_cast<int>(ctas < dev.sm_count ? ctas : dev.sm_count);
-  kern<<<grid, tp.warps * 32, tp.smem, st>>>(a);
-  return cudaGetLastError();
+  return launch(kern, grid, tp.warps * 32, tp.smem, st, a);
 }
 
-template <int PB, bool INT, bool SUM>
-static cudaError_t dispatch_tiles(const Device& dev, const TileArgs& a, const TilePlan& tp, bool stream, bool multi,
-                                  cudaStream_t st) {
-  if (stream) {
-    return multi ? launch_tiles<PB, INT, true, true, false, 0, SUM>(dev, a, tp, st)
-                 : launch_tiles<PB, INT, true, false, false, 0, SUM>(dev, a, tp, st);
-  }
-  return multi ? launch_tiles<PB, INT, false, true, false, 0, SUM>(dev, a, tp, st)
-               : launch_tiles<PB, INT, false, false, false, 0, SUM>(dev, a, tp, st);
-}
-
-template <int PB, bool INT, bool MULTI, bool SUM>
-static cudaError_t launch_generic(const Device& dev, const GenericArgs& a0, cudaStream_t st) {
-  GenericArgs a = a0;
-  auto kern = k_eval_generic<PB, INT, MULTI, SUM>;
-  const size_t tab_bytes = static_cast<size_t>(a.J) * a.SG * 4;
-  size_t smem = MULTI ? static_cast<size_t>(4) * a.nodes * 1024u : 0u;  // 4 warps per CTA
-  a.tab_in_smem = 0;
-  if (tab_bytes <= dev.smem_optin / 2) {
-    a.tab_in_smem = 1;
-    smem += tab_bytes;
-  }
-  if (smem > 0) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-    if (e != cudaSuccess) return e;
-  }
-  long long blocks = (a.B + 127) / 128;
-  long long cap = static_cast<long long>(dev.sm_count) * 8;
-  int grid = static_cast<int>(blocks < cap ? blocks : cap);
-  if (grid < 1) grid = 1;
-  kern<<<grid, 128, smem, st>>>(a);
-  return cudaGetLastError();
-}
-
-template <bool SUM>
-static cudaError_t eval_launch_obj(const Device& dev, const EvalCall& c, cudaStream_t st, int* path_used) {
+cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, int* path_used) {
+  if (c.B <= 0) return cudaSuccess;
   const int pb = c.J <= 256 ? 1 : 2;
-  const bool ints = (c.flags & SB_FLAG_INTEGER_STARTS) != 0;
   const bool multi = c.nodes > 1;
-  const bool bulk_ok = (c.stride_o % 16 == 0) && (c.stride_p % 16 == 0) &&
-                       (reinterpret_cast<uintptr_t>(c.opt) % 16 == 0) && (reinterpret_cast<uintptr_t>(c.prio) % 16 == 0);
+  const bool bulk_ok = bulk_aligned(c);
   const bool stream_ok = bulk_ok && (c.stride_p % 32 == 0) && (reinterpret_cast<uintptr_t>(c.prio) % 32 == 0) &&
-                         !(c.flags & 0x40000000u);
+                         !(c.flags & HOOK_NO_STREAM);
   TilePlan tp;
   int nw = 0;
   bool stream = false, tabg = false;
@@ -784,70 +765,45 @@ static cudaError_t eval_launch_obj(const Device& dev, const EvalCall& c, cudaStr
     if (!stream) nw = plan_tiles(dev, c.J, c.SG, pb, false, c.nodes, &tp);
   }
   if (nw >= 2) {
-    TileArgs a;
-    a.tab = c.tab; a.J = c.J; a.SG = c.SG; a.opt = c.opt; a.prio = c.prio; a.B = c.B;
-    a.stride_o = c.stride_o; a.stride_p = c.stride_p;
-    a.row_o = tp.row_o; a.row_p = tp.row_p; a.copy_o = tp.copy_o; a.copy_p = tp.copy_p;
+    TileArgs a = tile_args(c, tp);
     a.use_bulk = stream || (bulk_ok && (c.stride_o >= tp.copy_o) && (c.stride_p >= tp.copy_p));
-    a.nodes = c.nodes;
-    a.out = c.out; a.best_key = c.best_key; a.id_base = c.id_base;
-    a.ntiles = (c.B + 31) / 32;
-    a.one = 1;
     a.xp = c.xp;
     if (path_used) *path_used = tabg ? 4 : (stream ? 3 : (a.use_bulk ? 2 : 1));
-    if (tabg) {
-      if (pb == 1)
-        return ints ? launch_tiles<1, true, true, false, true, 0, SUM>(dev, a, tp, st)
-                    : launch_tiles<1, false, true, false, true, 0, SUM>(dev, a, tp, st);
-      return ints ? launch_tiles<2, true, true, false, true, 0, SUM>(dev, a, tp, st)
-                  : launch_tiles<2, false, true, false, true, 0, SUM>(dev, a, tp, st);
-    }
     // the headline shape (u8 priorities streamed, one node, table in shared memory): address arithmetic on the FMA
-    // pipe unless the test hook 0x02000000 asks for the plain form
-    if (pb == 1 && stream && !multi && !(c.flags & 0x02000000u))
-      return ints ? launch_tiles<1, true, true, false, false, 1, SUM>(dev, a, tp, st)
-                  : launch_tiles<1, false, true, false, false, 1, SUM>(dev, a, tp, st);
-    if (pb == 1)
-      return ints ? dispatch_tiles<1, true, SUM>(dev, a, tp, stream, multi, st)
-                  : dispatch_tiles<1, false, SUM>(dev, a, tp, stream, multi, st);
-    return ints ? dispatch_tiles<2, true, SUM>(dev, a, tp, stream, multi, st)
-                : dispatch_tiles<2, false, SUM>(dev, a, tp, stream, multi, st);
+    // pipe unless HOOK_PLAIN_ADDR asks for the plain form
+    const bool fma_addr = pb == 1 && stream && !tabg && !multi && !(c.flags & HOOK_PLAIN_ADDR);
+    const TileKernel kern = with_eval_types(pb, c.flags, [&](auto PB, auto INT, auto SUM) -> TileKernel {
+      if (tabg) return k_eval_tiles<PB, INT, true, false, false, true, 0, SUM>;
+      if constexpr (PB == 1) {
+        if (fma_addr) return k_eval_tiles<1, INT, true, false, false, false, 1, SUM>;
+      }
+      return with_bool(stream, [&](auto STREAM) {
+        return with_bool(multi, [&](auto MULTI) -> TileKernel {
+          return k_eval_tiles<PB, INT, STREAM, MULTI, false, false, 0, SUM>;
+        });
+      });
+    });
+    return launch_tiles(dev, kern, a, tp, st);
   }
   GenericArgs g;
   g.tab = c.tab; g.J = c.J; g.SG = c.SG; g.opt = c.opt; g.prio = c.prio; g.B = c.B;
   g.stride_o = c.stride_o; g.stride_p = c.stride_p; g.out = c.out; g.best_key = c.best_key;
   g.id_base = c.id_base; g.tab_in_smem = 0; g.nodes = c.nodes; g.one = 1;
   if (path_used) *path_used = 0;
-  if (multi) {
-    if (pb == 1) return ints ? launch_generic<1, true, true, SUM>(dev, g, st) : launch_generic<1, false, true, SUM>(dev, g, st);
-    return ints ? launch_generic<2, true, true, SUM>(dev, g, st) : launch_generic<2, false, true, SUM>(dev, g, st);
+  const size_t tab_bytes = static_cast<size_t>(c.J) * c.SG * 4;
+  size_t smem = multi ? static_cast<size_t>(4) * c.nodes * 1024u : 0u;  // 4 warps per CTA
+  if (tab_bytes <= dev.smem_optin / 2) {
+    g.tab_in_smem = 1;
+    smem += tab_bytes;
   }
-  if (pb == 1) return ints ? launch_generic<1, true, false, SUM>(dev, g, st) : launch_generic<1, false, false, SUM>(dev, g, st);
-  return ints ? launch_generic<2, true, false, SUM>(dev, g, st) : launch_generic<2, false, false, SUM>(dev, g, st);
-}
-
-cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, int* path_used) {
-  if (c.B <= 0) return cudaSuccess;
-  return (c.flags & SB_FLAG_SUM_COMPLETION) ? eval_launch_obj<true>(dev, c, st, path_used)
-                                            : eval_launch_obj<false>(dev, c, st, path_used);
-}
-
-// One fused search round over `c.B` chains whose current candidates are (c.opt, c.prio).  Returns
-// cudaErrorNotSupported when the shared-memory tiles (both rows resident, >= 4 warps) do not fit;
-// the caller then runs the unfused propose / evaluate / accept round.
-template <int PB, bool INT, bool SUM>
-static cudaError_t dispatch_search(const Device& dev, const TileArgs& a, const TilePlan& tp, bool multi,
-                                   cudaStream_t st) {
-  auto launch = [&](auto kern) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(tp.smem));
-    if (e != cudaSuccess) return e;
-    long long ctas = (a.ntiles + tp.warps - 1) / tp.warps;
-    int grid = static_cast<int>(ctas < dev.sm_count ? ctas : dev.sm_count);
-    kern<<<grid, tp.warps * 32, tp.smem, st>>>(a);
-    return cudaGetLastError();
-  };
-  if (multi) return launch(k_eval_tiles<PB, INT, false, true, true, false, 0, SUM>);
-  return launch(k_eval_tiles<PB, INT, false, false, true, false, 0, SUM>);
+  long long blocks = (c.B + 127) / 128;
+  long long cap = static_cast<long long>(dev.sm_count) * 8;
+  int grid = static_cast<int>(blocks < cap ? blocks : cap);
+  if (grid < 1) grid = 1;
+  const auto kern = with_eval_types(pb, c.flags, [&](auto PB, auto INT, auto SUM) {
+    return with_bool(multi, [&](auto MULTI) { return k_eval_generic<PB, INT, MULTI, SUM>; });
+  });
+  return launch(kern, grid, 128, smem, st, g);
 }
 
 // 2 = both rows of a candidate fit in shared memory for at least 8 warps: the tile kernel runs the fused
@@ -859,44 +815,30 @@ int search_round_mode(const Device& dev, int J, int SG, int nodes) {
   return plan_tiles(dev, J, SG, pb, false, nodes, &tp) >= 8 ? 2 : 0;
 }
 
+// One fused search round over `c.B` chains whose current candidates are (c.opt, c.prio).  Returns
+// cudaErrorNotSupported when the shared-memory tiles (both rows resident, >= 4 warps) do not fit;
+// the caller then runs the unfused propose / evaluate / accept round.
 cudaError_t search_round_launch(const Device& dev, const EvalCall& c, const SearchFuse& sf, cudaStream_t st) {
   if (c.B <= 0) return cudaSuccess;
   const int pb = c.J <= 256 ? 1 : 2;
-  const bool ints = (c.flags & SB_FLAG_INTEGER_STARTS) != 0;
-  const bool bulk_ok = (c.stride_o % 16 == 0) && (c.stride_p % 16 == 0) &&
-                       (reinterpret_cast<uintptr_t>(c.opt) % 16 == 0) && (reinterpret_cast<uintptr_t>(c.prio) % 16 == 0);
   TilePlan tp;
-  if (search_round_mode(dev, c.J, c.SG, c.nodes) == 0 || !bulk_ok) return cudaErrorNotSupported;
+  if (search_round_mode(dev, c.J, c.SG, c.nodes) == 0 || !bulk_aligned(c)) return cudaErrorNotSupported;
   plan_tiles(dev, c.J, c.SG, pb, false, c.nodes, &tp);
   if (c.stride_o < tp.copy_o || c.stride_p < tp.copy_p) return cudaErrorNotSupported;
-  TileArgs a;
-  a.tab = c.tab; a.J = c.J; a.SG = c.SG; a.opt = c.opt; a.prio = c.prio; a.B = c.B;
-  a.stride_o = c.stride_o; a.stride_p = c.stride_p;
-  a.row_o = tp.row_o; a.row_p = tp.row_p; a.copy_o = tp.copy_o; a.copy_p = tp.copy_p;
+  TileArgs a = tile_args(c, tp);
   a.use_bulk = 1;
-  a.nodes = c.nodes;
-  a.out = nullptr; a.best_key = c.best_key; a.id_base = c.id_base;
-  a.ntiles = (c.B + 31) / 32;
-  a.one = 1;
   a.sf = sf;
-  if (c.flags & SB_FLAG_SUM_COMPLETION) {
-    if (pb == 1)
-      return ints ? dispatch_search<1, true, true>(dev, a, tp, c.nodes > 1, st)
-                  : dispatch_search<1, false, true>(dev, a, tp, c.nodes > 1, st);
-    return ints ? dispatch_search<2, true, true>(dev, a, tp, c.nodes > 1, st)
-                : dispatch_search<2, false, true>(dev, a, tp, c.nodes > 1, st);
-  }
-  if (pb == 1)
-    return ints ? dispatch_search<1, true, false>(dev, a, tp, c.nodes > 1, st)
-                : dispatch_search<1, false, false>(dev, a, tp, c.nodes > 1, st);
-  return ints ? dispatch_search<2, true, false>(dev, a, tp, c.nodes > 1, st)
-              : dispatch_search<2, false, false>(dev, a, tp, c.nodes > 1, st);
+  const TileKernel kern = with_eval_types(pb, c.flags, [&](auto PB, auto INT, auto SUM) {
+    return with_bool(c.nodes > 1, [&](auto MULTI) -> TileKernel {
+      return k_eval_tiles<PB, INT, false, MULTI, true, false, 0, SUM>;
+    });
+  });
+  return launch_tiles(dev, kern, a, tp, st);
 }
 
 cudaError_t eval_full_launch(const Device& dev, const EvalCall& c, float* start, uint32_t* slotmask, cudaStream_t st) {
   if (c.B <= 0) return cudaSuccess;
   const int pb = c.J <= 256 ? 1 : 2;
-  const bool ints = (c.flags & SB_FLAG_INTEGER_STARTS) != 0;
   FullArgs a;
   a.tab = c.tab; a.J = c.J; a.SG = c.SG; a.opt = c.opt; a.prio = c.prio; a.B = c.B;
   a.stride_o = c.stride_o; a.stride_p = c.stride_p; a.nodes = c.nodes < 1 ? 1 : c.nodes;
@@ -904,16 +846,8 @@ cudaError_t eval_full_launch(const Device& dev, const EvalCall& c, float* start,
   long long blocks = (c.B + 127) / 128;
   long long cap = static_cast<long long>(dev.sm_count) * 16;
   int grid = static_cast<int>(blocks < cap ? blocks : cap);
-  const bool sum = (c.flags & SB_FLAG_SUM_COMPLETION) != 0;
-  auto launch = [&](auto kern) { kern<<<grid, 128, 0, st>>>(a); };
-  if (pb == 1) {
-    if (sum) ints ? launch(k_eval_full<1, true, true>) : launch(k_eval_full<1, false, true>);
-    else ints ? launch(k_eval_full<1, true>) : launch(k_eval_full<1, false>);
-  } else {
-    if (sum) ints ? launch(k_eval_full<2, true, true>) : launch(k_eval_full<2, false, true>);
-    else ints ? launch(k_eval_full<2, true>) : launch(k_eval_full<2, false>);
-  }
-  return cudaGetLastError();
+  const auto kern = with_eval_types(pb, c.flags, [](auto PB, auto INT, auto SUM) { return k_eval_full<PB, INT, SUM>; });
+  return launch(kern, grid, 128, 0, st, a);
 }
 
 cudaError_t validate_launch(const Device& dev, const EvalCall& c, unsigned long long* bad, cudaStream_t st, bool by_pos) {

@@ -93,8 +93,6 @@ cudaError_t eval_alt_launch(const Device& dev, const EvalCall& c, cudaStream_t s
   AltArgs a;
   a.tab = c.tab; a.J = c.J; a.SG = c.SG; a.opt = c.opt; a.prio = c.prio; a.B = c.B;
   a.stride_o = c.stride_o; a.stride_p = c.stride_p; a.out = c.out; a.best_key = c.best_key; a.id_base = c.id_base;
-  const bool ints = (c.flags & SB_FLAG_INTEGER_STARTS) != 0;
-  const int pb = c.J <= 256 ? 1 : 2;
   // resident CTAs per SM are bounded by the table copy each of them holds
   const int threads = 512;
   int per_sm = static_cast<int>(dev.smem_optin / (smem + 1024));
@@ -102,14 +100,10 @@ cudaError_t eval_alt_launch(const Device& dev, const EvalCall& c, cudaStream_t s
   const long long need = (c.B + 4 * (threads / 32) - 1) / (4 * (threads / 32));
   const long long cap = static_cast<long long>(dev.sm_count) * per_sm;
   const int grid = static_cast<int>(need < cap ? need : cap);
-  auto launch = [&](auto kern) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-    if (e != cudaSuccess) return e;
-    kern<<<grid, threads, smem, st>>>(a);
-    return cudaGetLastError();
-  };
-  if (pb == 1) return ints ? launch(k_eval_groups<1, true>) : launch(k_eval_groups<1, false>);
-  return ints ? launch(k_eval_groups<2, true>) : launch(k_eval_groups<2, false>);
+  const auto kern = with_pb(c.J <= 256 ? 1 : 2, [&](auto PB) {
+    return with_bool(c.flags & SB_FLAG_INTEGER_STARTS, [&](auto INT) { return k_eval_groups<PB, INT>; });
+  });
+  return launch(kern, grid, threads, smem, st, a);
 }
 
 }  // namespace sb

@@ -3,9 +3,69 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "sb_common.cuh"
 
 namespace sb {
+
+// Test hooks: the top twelve bits of the flags word of sb_eval / sb_search_params force a kernel path or a
+// search mode that the automatic choice would not take, so that the tests can pin every path and compare the
+// forms of the search.  They are not part of the ABI; saturn_b200/_lib.py mirrors the names.
+enum : unsigned {
+  HOOK_FORCE_GENERIC = 0x80000000u,       // sb_eval: the generic kernel (path 0)
+  HOOK_NO_STREAM = 0x40000000u,           // sb_eval: prio rows staged in shared memory, never streamed (tile paths 2 / 1)
+  HOOK_NO_FUSED = 0x20000000u,            // search: unfused propose / evaluate / accept rounds
+  HOOK_NO_INCREMENTAL = 0x10000000u,      // search: windowed moves, always scored from position 0
+  HOOK_VERIFY_INCREMENTAL = 0x08000000u,  // search: also score every incremental proposal from position 0 and count
+                                          // the mismatches (sb_search_verify_count)
+  HOOK_ROUND1_MOVES = 0x04000000u,        // search: the round-1 move generator (no windows)
+  HOOK_PLAIN_ADDR = 0x02000000u,          // sb_eval: plain C++ addressing in the headline tile kernel (ADDR = 0)
+  HOOK_WINDOW_BIAS = 0x01000000u,         // search: windows drawn with P(w) ~ w + 1 (experiment, see draw_window)
+  HOOK_TABLE_GLOBAL = 0x00800000u,        // position-major scoring: the table in global memory (path 8)
+  HOOK_TABLE_PAIR = 0x00400000u,          // position-major scoring: the table split over a CTA pair (path 7)
+  HOOK_REORDER = 0x00200000u,             // sb_eval: re-order job-indexed rows into schedule order at any size (path 9)
+  HOOK_NO_REORDER = 0x00100000u,          // sb_eval: never re-order job-indexed rows
+};
+static_assert(((HOOK_FORCE_GENERIC | HOOK_NO_STREAM | HOOK_NO_FUSED | HOOK_NO_INCREMENTAL | HOOK_VERIFY_INCREMENTAL |
+                HOOK_ROUND1_MOVES | HOOK_PLAIN_ADDR | HOOK_WINDOW_BIAS | HOOK_TABLE_GLOBAL | HOOK_TABLE_PAIR |
+                HOOK_REORDER | HOOK_NO_REORDER) &
+               (SB_FLAG_INTEGER_STARTS | SB_FLAG_REDUCED | SB_FLAG_OPT_BY_POSITION | SB_FLAG_POST_KEY |
+                SB_FLAG_FOLD_PREV | SB_FLAG_ALT_WARPSCAN | SB_FLAG_SUM_COMPLETION)) == 0,
+              "the test hooks share no bit with the SB_FLAG_* flags");
+
+// Compile-time dispatch: f is called with the run-time value as a type (std::true_type / std::false_type, or the
+// prio width as std::integral_constant), so that a launch site names its kernel's template arguments once.
+template <class F>
+decltype(auto) with_bool(bool b, F&& f) {
+  return b ? f(std::true_type{}) : f(std::false_type{});
+}
+template <class F>
+decltype(auto) with_pb(int pb, F&& f) {
+  return pb == 1 ? f(std::integral_constant<int, 1>{}) : f(std::integral_constant<int, 2>{});
+}
+// f(PB, INT, SUM): the prio width, SB_FLAG_INTEGER_STARTS and SB_FLAG_SUM_COMPLETION, the template arguments that
+// every evaluation and search kernel takes
+template <class F>
+decltype(auto) with_eval_types(int pb, unsigned flags, F&& f) {
+  return with_pb(pb, [&](auto PB) {
+    return with_bool(flags & SB_FLAG_INTEGER_STARTS, [&](auto INT) {
+      return with_bool(flags & SB_FLAG_SUM_COMPLETION, [&](auto SUM) { return f(PB, INT, SUM); });
+    });
+  });
+}
+
+// One kernel launch: raise the kernel's dynamic shared-memory limit to what the launch uses (when it uses any),
+// launch, and return the launch error.
+template <class... P, class... A>
+cudaError_t launch(void (*kern)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, const A&... args) {
+  if (smem > 0) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    if (e != cudaSuccess) return e;
+  }
+  kern<<<grid, block, smem, st>>>(args...);
+  return cudaGetLastError();
+}
 
 struct Device {
   int ordinal = 0;

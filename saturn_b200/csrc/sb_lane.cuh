@@ -280,7 +280,7 @@ __device__ __forceinline__ Move apply_move(const SearchFuse& sf, int round, int 
 }
 
 // The window of a round, from one 64-bit draw shared by the warp.  bias 0: uniform over the nwin windows.
-// bias 1 (experiment, sb_search_params.flags 0x01000000): P(w) proportional to w + 1 — later windows skip more
+// bias 1 (experiment, test hook HOOK_WINDOW_BIAS): P(w) proportional to w + 1 — later windows skip more
 // of the schedule (mean resume point 0.58 instead of 0.44 of the way in at 8 windows) at the price of fewer
 // moves near the front of the schedule.
 __device__ __forceinline__ int draw_window(uint64_t r, int nwin, int bias) {

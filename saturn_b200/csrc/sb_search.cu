@@ -674,13 +674,8 @@ static cudaError_t init_population_smem(const SearchDev& s, cudaStream_t st) {
   }
   const size_t smem = static_cast<size_t>(threads) * row_p + lists;
   const int grid = static_cast<int>((s.chains + threads - 1) / threads);
-  auto launch = [&](auto kern) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-    if (e != cudaSuccess) return e;
-    kern<<<grid, threads, smem, st>>>(s, row_p);
-    return cudaGetLastError();
-  };
-  return s.pb == 1 ? launch(k_init_population_smem<1, POS>) : launch(k_init_population_smem<2, POS>);
+  return launch(with_pb(s.pb, [](auto PB) { return k_init_population_smem<PB, POS>; }), grid, threads, smem, st, s,
+                row_p);
 }
 
 static cudaError_t zero_rows(const SearchDev& s, cudaStream_t st) {
@@ -696,17 +691,13 @@ cudaError_t search_init_population(const SearchDev& s, cudaStream_t st) {
   if ((e = zero_rows(s, st)) != cudaSuccess) return e;
   const int threads = 128;
   const int grid = static_cast<int>((s.chains + threads - 1) / threads);
-  if (s.pb == 1) k_init_population<1><<<grid, threads, 0, st>>>(s);
-  else k_init_population<2><<<grid, threads, 0, st>>>(s);
-  return cudaGetLastError();
+  return launch(with_pb(s.pb, [](auto PB) { return k_init_population<PB>; }), grid, threads, 0, st, s);
 }
 
 cudaError_t search_propose(const SearchDev& s, int round, cudaStream_t st) {
   const int threads = 256;
-  const int grid = warp_grid(s.chains, threads);
-  if (s.pb == 1) k_propose<1><<<grid, threads, 0, st>>>(s, round);
-  else k_propose<2><<<grid, threads, 0, st>>>(s, round);
-  return cudaGetLastError();
+  return launch(with_pb(s.pb, [](auto PB) { return k_propose<PB>; }), warp_grid(s.chains, threads), threads, 0, st, s,
+                round);
 }
 
 cudaError_t search_keep_best(const SearchDev& s, bool from_cur, cudaStream_t st) {
@@ -722,9 +713,8 @@ cudaError_t search_accept(const SearchDev& s, int round, float temperature, cuda
 
 cudaError_t search_resample(const SearchDev& s, int round, cudaStream_t st) {
   const int threads = 256;
-  if (s.pb == 1) k_resample<1><<<warp_grid(s.chains, threads), threads, 0, st>>>(s, round);
-  else k_resample<2><<<warp_grid(s.chains, threads), threads, 0, st>>>(s, round);
-  return cudaGetLastError();
+  return launch(with_pb(s.pb, [](auto PB) { return k_resample<PB>; }), warp_grid(s.chains, threads), threads, 0, st, s,
+                round);
 }
 
 cudaError_t search_inject(const SearchDev& s, const uint8_t* cand_o, const uint8_t* cand_p, long long first,
@@ -741,9 +731,7 @@ cudaError_t search_init_population_pos(const SearchDev& s, cudaStream_t st) {
   if ((e = zero_rows(s, st)) != cudaSuccess) return e;
   const int threads = 128;
   const int grid = static_cast<int>((s.chains + threads - 1) / threads);
-  if (s.pb == 1) k_init_population_pos<1><<<grid, threads, 0, st>>>(s);
-  else k_init_population_pos<2><<<grid, threads, 0, st>>>(s);
-  return cudaGetLastError();
+  return launch(with_pb(s.pb, [](auto PB) { return k_init_population_pos<PB>; }), grid, threads, 0, st, s);
 }
 
 // smem: table + mbarrier + per-warp node states (MULTI)
@@ -752,53 +740,53 @@ size_t search_pos_smem(int J, int SG, int nodes, int warps) {
   return tab_bytes + 16 + static_cast<size_t>(warps) * (nodes > 1 ? nodes * 1024u : 0u);
 }
 
-// Scoring-only launches with the table outside the CTA's own shared memory (TAB = 1 / 2 of k_search_pos).
-template <int TAB, bool SUM>
-static cudaError_t eval_pos_far_launch(const Device& dev, const PosArgs& a, int pb, bool ints, cudaStream_t st) {
+using PosKernel = void (*)(PosArgs);
+
+// Scoring-only launches with the table outside the CTA's own shared memory (TAB = tab_home = 1 / 2 of k_search_pos).
+static cudaError_t eval_pos_far_launch(const Device& dev, const PosArgs& a, int tab_home, int pb, unsigned flags,
+                                       cudaStream_t st) {
   const int warps = 16;
-  const size_t smem = TAB == 2 ? static_cast<size_t>(pos_tab_half(a.J, a.SG)) * 4 + 16 : 16;
+  const size_t smem = tab_home == 2 ? static_cast<size_t>(pos_tab_half(a.J, a.SG)) * 4 + 16 : 16;
   if (smem > dev.smem_optin) return cudaErrorNotSupported;
   const long long ntiles = (a.chains + 31) / 32;
   const long long ctas = (ntiles + warps - 1) / warps;
-  auto launch = [&](auto kern) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  const PosKernel kern = with_eval_types(pb, flags, [&](auto PB, auto INT, auto SUM) {
+    return tab_home == 2 ? k_search_pos<PB, INT, false, true, 2, SUM> : k_search_pos<PB, INT, false, true, 1, SUM>;
+  });
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  if (e != cudaSuccess) return e;
+  cudaLaunchConfig_t cfg = {};
+  cfg.blockDim = dim3(warps * 32);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cudaLaunchAttribute attr;
+  if (tab_home == 2) {
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = 2; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    cfg.gridDim = dim3(2);
+    int pairs = 0;
+    e = cudaOccupancyMaxActiveClusters(&pairs, kern, &cfg);
     if (e != cudaSuccess) return e;
-    cudaLaunchConfig_t cfg = {};
-    cfg.blockDim = dim3(warps * 32);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr;
-    if (TAB == 2) {
-      attr.id = cudaLaunchAttributeClusterDimension;
-      attr.val.clusterDim.x = 2; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
-      cfg.attrs = &attr;
-      cfg.numAttrs = 1;
-      cfg.gridDim = dim3(2);
-      int pairs = 0;
-      e = cudaOccupancyMaxActiveClusters(&pairs, kern, &cfg);
-      if (e != cudaSuccess) return e;
-      if (pairs < 1) return cudaErrorNotSupported;
-      const long long want = (ctas + 1) / 2;
-      cfg.gridDim = dim3(static_cast<unsigned>(2 * (want < pairs ? want : pairs)));
-    } else {
-      // nothing but an mbarrier in shared memory: leave the SM's array to L1, which caches the table
-      e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, 0);
-      if (e != cudaSuccess) return e;
-      cfg.gridDim = dim3(static_cast<unsigned>(ctas < dev.sm_count ? ctas : dev.sm_count));
-    }
-    return cudaLaunchKernelEx(&cfg, kern, a);
-  };
-  if (pb == 1)
-    return ints ? launch(k_search_pos<1, true, false, true, TAB, SUM>) : launch(k_search_pos<1, false, false, true, TAB, SUM>);
-  return ints ? launch(k_search_pos<2, true, false, true, TAB, SUM>) : launch(k_search_pos<2, false, false, true, TAB, SUM>);
+    if (pairs < 1) return cudaErrorNotSupported;
+    const long long want = (ctas + 1) / 2;
+    cfg.gridDim = dim3(static_cast<unsigned>(2 * (want < pairs ? want : pairs)));
+  } else {
+    // nothing but an mbarrier in shared memory: leave the SM's array to L1, which caches the table
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, 0);
+    if (e != cudaSuccess) return e;
+    cfg.gridDim = dim3(static_cast<unsigned>(ctas < dev.sm_count ? ctas : dev.sm_count));
+  }
+  return cudaLaunchKernelEx(&cfg, kern, a);
 }
 
 // tab_home: 0 = the table in every CTA's shared memory (cudaErrorNotSupported when it does not fit);
 // scoring only, one node: 2 = split over CTA pairs, 1 = global memory
-template <bool SUM>
-static cudaError_t search_pos_launch_obj(const Device& dev, const SearchDev& s, const float* tab, int SG, unsigned flags,
-                                         long long first, long long count, bool eval_only, const SearchFuse& sf,
-                                         cudaStream_t st, int tab_home) {
+cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float* tab, int SG, unsigned flags,
+                              long long first, long long count, bool eval_only, const SearchFuse& sf,
+                              cudaStream_t st, int tab_home) {
+  if (count <= 0) return cudaSuccess;
   PosArgs a;
   a.tab = tab; a.J = s.J; a.SG = SG; a.nodes = s.nodes;
   a.opt = s.cur_o; a.prio = s.cur_p;
@@ -809,11 +797,10 @@ static cudaError_t search_pos_launch_obj(const Device& dev, const SearchDev& s, 
   a.eval_only = eval_only ? 1 : 0;
   a.one = 1;
   a.sf = sf;
-  const bool ints = (flags & SB_FLAG_INTEGER_STARTS) != 0;
   const bool multi = s.nodes > 1;
   if (tab_home != 0) {
     if (!eval_only || multi) return cudaErrorNotSupported;
-    return tab_home == 2 ? eval_pos_far_launch<2, SUM>(dev, a, s.pb, ints, st) : eval_pos_far_launch<1, SUM>(dev, a, s.pb, ints, st);
+    return eval_pos_far_launch(dev, a, tab_home, s.pb, flags, st);
   }
   const int warps = 16;
   const size_t smem = search_pos_smem(s.J, SG, s.nodes, warps);
@@ -821,46 +808,22 @@ static cudaError_t search_pos_launch_obj(const Device& dev, const SearchDev& s, 
   const long long ntiles = (count + 31) / 32;
   const long long ctas = (ntiles + warps - 1) / warps;
   const int grid = static_cast<int>(ctas < dev.sm_count ? ctas : dev.sm_count);
-  auto launch = [&](auto kern) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-    if (e != cudaSuccess) return e;
-    kern<<<grid, warps * 32, smem, st>>>(a);
-    return cudaGetLastError();
-  };
-  if (eval_only) {
-    if (s.pb == 1) {
-      if (multi) return ints ? launch(k_search_pos<1, true, true, true, 0, SUM>) : launch(k_search_pos<1, false, true, true, 0, SUM>);
-      return ints ? launch(k_search_pos<1, true, false, true, 0, SUM>) : launch(k_search_pos<1, false, false, true, 0, SUM>);
-    }
-    if (multi) return ints ? launch(k_search_pos<2, true, true, true, 0, SUM>) : launch(k_search_pos<2, false, true, true, 0, SUM>);
-    return ints ? launch(k_search_pos<2, true, false, true, 0, SUM>) : launch(k_search_pos<2, false, false, true, 0, SUM>);
-  }
-  if (s.pb == 1) {
-    if (multi) return ints ? launch(k_search_pos<1, true, true, false, 0, SUM>) : launch(k_search_pos<1, false, true, false, 0, SUM>);
-    return ints ? launch(k_search_pos<1, true, false, false, 0, SUM>) : launch(k_search_pos<1, false, false, false, 0, SUM>);
-  }
-  if (multi) return ints ? launch(k_search_pos<2, true, true, false, 0, SUM>) : launch(k_search_pos<2, false, true, false, 0, SUM>);
-  return ints ? launch(k_search_pos<2, true, false, false, 0, SUM>) : launch(k_search_pos<2, false, false, false, 0, SUM>);
-}
-
-cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float* tab, int SG, unsigned flags,
-                              long long first, long long count, bool eval_only, const SearchFuse& sf,
-                              cudaStream_t st, int tab_home) {
-  if (count <= 0) return cudaSuccess;
-  return (flags & SB_FLAG_SUM_COMPLETION)
-             ? search_pos_launch_obj<true>(dev, s, tab, SG, flags, first, count, eval_only, sf, st, tab_home)
-             : search_pos_launch_obj<false>(dev, s, tab, SG, flags, first, count, eval_only, sf, st, tab_home);
+  const PosKernel kern = with_eval_types(s.pb, flags, [&](auto PB, auto INT, auto SUM) {
+    return with_bool(multi, [&](auto MULTI) {
+      return with_bool(eval_only, [&](auto EVAL) -> PosKernel { return k_search_pos<PB, INT, MULTI, EVAL, 0, SUM>; });
+    });
+  });
+  return launch(kern, grid, warps * 32, smem, st, a);
 }
 
 // Where the position-major scoring kernel keeps a table of J x SG entries: 0 = every CTA's shared memory;
 // a one-node table that does not fit there: 1 = global memory, read through L1 / L2 (with no tile in shared
 // memory the SM's whole array is L1); -1 = nowhere (multi-node table beyond shared memory).
-// Test hooks in flags: 0x00400000 forces 2 (split over CTA pairs: scattered 4-byte ld.shared::cluster),
-// 0x00800000 forces 1.
+// HOOK_TABLE_PAIR forces 2 (split over CTA pairs: scattered 4-byte ld.shared::cluster), HOOK_TABLE_GLOBAL forces 1.
 int eval_pos_home(const Device& dev, int J, int SG, int nodes, unsigned flags) {
   const bool pair_ok = nodes == 1 && static_cast<size_t>(pos_tab_half(J, SG)) * 4 + 16 <= dev.smem_optin;
-  if (flags & 0x00400000u) return pair_ok ? 2 : -1;
-  if (flags & 0x00800000u) return nodes == 1 ? 1 : -1;
+  if (flags & HOOK_TABLE_PAIR) return pair_ok ? 2 : -1;
+  if (flags & HOOK_TABLE_GLOBAL) return nodes == 1 ? 1 : -1;
   if (search_pos_smem(J, SG, nodes, 16) <= dev.smem_optin) return 0;
   return nodes == 1 ? 1 : -1;
 }
@@ -932,9 +895,8 @@ cudaError_t opt_by_position_launch(const Device& dev, const EvalCall& c, uint8_t
   const long long need = (c.B + threads / 32 - 1) / (threads / 32);
   const long long cap = static_cast<long long>(dev.sm_count) * 8;
   const int grid = static_cast<int>(need < cap ? need : cap);
-  if (c.J <= 256) k_opt_by_position<1><<<grid, threads, smem, st>>>(c.opt, c.prio, out, c.B, c.J, c.stride_o, c.stride_p, row_s);
-  else k_opt_by_position<2><<<grid, threads, smem, st>>>(c.opt, c.prio, out, c.B, c.J, c.stride_o, c.stride_p, row_s);
-  return cudaGetLastError();
+  return launch(with_pb(c.J <= 256 ? 1 : 2, [](auto PB) { return k_opt_by_position<PB>; }), grid, threads, smem, st,
+                c.opt, c.prio, out, c.B, c.J, c.stride_o, c.stride_p, row_s);
 }
 
 }  // namespace sb

@@ -146,13 +146,13 @@ class Engine:
         B, stride = self._check_cands(opt, prio, True)
         if out is None:
             out = torch.empty(B, dtype=torch.float32, device=self.device)
-        fl = _flags(integer_starts, reduced, objective) | (_lib._FLAG_FORCE_GENERIC if _force_generic else 0) | (
-            0x40000000 if _no_stream else 0) | (0x02000000 if _plain_addr else 0) | (
+        fl = _flags(integer_starts, reduced, objective) | (_lib.HOOK_FORCE_GENERIC if _force_generic else 0) | (
+            _lib.HOOK_NO_STREAM if _no_stream else 0) | (_lib.HOOK_PLAIN_ADDR if _plain_addr else 0) | (
             _lib.FLAG_POST_KEY if post_key else 0) | (
             _lib.FLAG_FOLD_PREV if (post_key and fold_prev) else 0) | (
             _lib.FLAG_OPT_BY_POSITION if by_position else 0) | (_lib.FLAG_ALT_WARPSCAN if alt_shape else 0) | (
-            {0: 0, 1: 0x00800000, 2: 0x00400000}[_table_home]) | (
-            0 if _reorder is None else (0x00200000 if _reorder else 0x00100000))
+            {0: 0, 1: _lib.HOOK_TABLE_GLOBAL, 2: _lib.HOOK_TABLE_PAIR}[_table_home]) | (
+            0 if _reorder is None else (_lib.HOOK_REORDER if _reorder else _lib.HOOK_NO_REORDER))
         kp = C.c_void_p(best_key.data_ptr()) if best_key is not None else None
         check(self._lib.sb_eval(self._h, C.c_void_p(opt.data_ptr()), C.c_void_p(prio.data_ptr()), B, stride, fl,
                                 C.c_void_p(out.data_ptr()), kp, id_base & 0xffffffff))
@@ -260,9 +260,10 @@ class Engine:
                     _no_fused: bool = False, _extra_flags: int = 0, objective: str = "makespan"):
         """resample_every > 0: search_round resamples the population by tournament on that cadence itself.
         objective="completion": minimise the sum of completion times (every score and key holds that sum).
-        _extra_flags: test hooks of sb_search_params.flags (see sb_search_verify_count in the header)."""
+        _extra_flags: test hooks of sb_search_params.flags (_lib.HOOK_*)."""
         p = SearchParams(seed=seed, chains=chains, chain_base=chain_base, resample_every=int(resample_every or 0),
-                         flags=_flags(integer_starts, reduced, objective) | (0x20000000 if _no_fused else 0) | int(_extra_flags),
+                         flags=_flags(integer_starts, reduced, objective) | (_lib.HOOK_NO_FUSED if _no_fused else 0) |
+                         int(_extra_flags),
                          t_start=t_start, t_end=t_end, total_rounds=total_rounds)
         wo = wp = None
         keep = None
@@ -333,7 +334,8 @@ class Engine:
         check(self._lib.sb_search_resample(self._h))
 
     def search_verify_count(self) -> int:
-        """Incremental scores that differed from a from-scratch score (test hook, needs _extra_flags 0x08000000)."""
+        """Incremental scores that differed from a from-scratch score (test hook: needs
+        _extra_flags=_lib.HOOK_VERIFY_INCREMENTAL)."""
         n = C.c_uint64(0)
         check(self._lib.sb_search_verify_count(self._h, C.byref(n)))
         return int(n.value)
@@ -356,7 +358,8 @@ def _search_run(lib, handles, J, chains, rounds, seed, chain_base, integer_start
     """sb_search_run (one handle) / sb_search_run_multi (one handle per device of this process)."""
     pdt = np.uint8 if J <= 256 else np.uint16
     p = SearchParams(seed=seed, chains=chains, chain_base=chain_base,
-                     flags=_flags(integer_starts, reduced, objective) | (0x20000000 if _no_fused else 0) | int(_extra_flags),
+                     flags=_flags(integer_starts, reduced, objective) | (_lib.HOOK_NO_FUSED if _no_fused else 0) |
+                     int(_extra_flags),
                      t_start=t_start, t_end=t_end, total_rounds=max(rounds, 1))
     cap = (max(rounds, 1) // max(1, sync_every) + 3) if record_history else 0
     hw, he, hm = np.zeros(cap, np.float64), np.zeros(cap, np.int64), np.zeros(cap, np.float32)

@@ -5,6 +5,7 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch  # noqa: E402
 
+from saturn_b200 import _lib  # noqa: E402
 from saturn_b200.engine import Engine  # noqa: E402
 from saturn_b200.synth import synth_table  # noqa: E402
 
@@ -16,7 +17,7 @@ for J in (256, 1024):
     wave = eng.search_wave(reduced=True)
     for chains in (2 * wave, wave * round((1 << 20) / wave) if J == 256 else 4 * wave):
         for rs in ((0, 2) if J == 256 else (0, 8)):
-            for name, fl in (("full", 0x10000000), ("incremental", 0)):
+            for name, fl in (("full", _lib.HOOK_NO_INCREMENTAL), ("incremental", 0)):
                 eng.search_init(chains, seed=1, reduced=True, t_start=5e-4, t_end=1e-6, total_rounds=64, resample_every=rs,
                                 _extra_flags=fl)
                 eng.search_round(8)

@@ -12,13 +12,15 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from saturn_b200 import _lib  # noqa: E402
 from saturn_b200.engine import Engine  # noqa: E402
 from saturn_b200.search import run_search  # noqa: E402
 from saturn_b200.synth import synth_table  # noqa: E402
 
-MODES = [("round-1 moves, scored from position 0", 0x04000000), ("windowed moves, scored from position 0", 0x10000000),
+MODES = [("round-1 moves, scored from position 0", _lib.HOOK_ROUND1_MOVES),
+         ("windowed moves, scored from position 0", _lib.HOOK_NO_INCREMENTAL),
          ("windowed moves, incremental (shipped)", 0),
-         ("windowed moves, incremental, windows drawn with P(w) ~ w + 1 (experiment)", 0x01000000)]
+         ("windowed moves, incremental, windows drawn with P(w) ~ w + 1 (experiment)", _lib.HOOK_WINDOW_BIAS)]
 
 
 def main():

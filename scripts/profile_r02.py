@@ -9,6 +9,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from saturn_b200 import _lib  # noqa: E402
 from saturn_b200.engine import Engine, random_candidates  # noqa: E402
 from saturn_b200.synth import synth_table  # noqa: E402
 
@@ -29,7 +30,7 @@ if which in ("search", "search_full"):
     eng.set_table(T)
     wave = eng.search_wave(reduced=True)
     eng.search_init(wave * round((1 << 20) / wave), seed=0, reduced=True, t_start=5e-4, t_end=1e-6, total_rounds=64,
-                    resample_every=-1, _extra_flags=(0x10000000 if which == "search_full" else 0))
+                    resample_every=-1, _extra_flags=(_lib.HOOK_NO_INCREMENTAL if which == "search_full" else 0))
     eng.search_round(24)
     torch.cuda.synchronize()
 if which == "pos":

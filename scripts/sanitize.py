@@ -2,6 +2,7 @@
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
+from saturn_b200 import _lib
 from saturn_b200.engine import Engine, random_candidates, opt_by_position
 from saturn_b200.search import run_search
 from saturn_b200.synth import synth_table
@@ -32,14 +33,14 @@ for (J, S, G, B) in [(64, 6, 8, 2000), (100, 3, 8, 777), (300, 2, 8, 500)]:
     r = run_search(eng, chains=2048, rounds=6, use_dist=False)
     eng.decode(r.opt, r.prio)
     # round 2: incremental rounds with the verify hook (snapshots, windowed moves, in-kernel tournament)
-    r = run_search(eng, chains=2048, rounds=20, reduced=True, use_dist=False, _extra_flags=0x08000000)
+    r = run_search(eng, chains=2048, rounds=20, reduced=True, use_dist=False, _extra_flags=_lib.HOOK_VERIFY_INCREMENTAL)
     assert eng.search_verify_count() == 0 and eng.search_validate() == 0
 # large J: position-major search populations (k_search_pos), ragged tails, one and two nodes
 for (J, nodes, chains) in [(1030, 1, 300), (777, 2, 130), (513, 1, 64)]:
     T, valid = synth_table(J, 1, 8, seed=3)
     eng.set_table(T, nodes=nodes)
     r = run_search(eng, chains=chains, rounds=6, reduced=True, use_dist=False)
-    r = run_search(eng, chains=chains, rounds=18, reduced=True, use_dist=False, _extra_flags=0x08000000, resample_every=4)
+    r = run_search(eng, chains=chains, rounds=18, reduced=True, use_dist=False, _extra_flags=_lib.HOOK_VERIFY_INCREMENTAL, resample_every=4)
     assert eng.search_verify_count() == 0 and eng.search_validate() == 0
     eng.search_inject(r.opt, r.prio, copies=3)
     eng.search_resample()

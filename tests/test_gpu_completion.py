@@ -207,13 +207,14 @@ def test_solve_reaches_the_exhaustive_optimum_on_random_small_instances():
 def test_incremental_rounds_in_completion_mode(engine, J):
     """The verify hook recomputes every incremental score from position 0: no mismatch with the running sum stored in
     the snapshots.  Fused and unfused rounds both return valid plans that re-score to the reported sum."""
+    from saturn_b200 import _lib
     from saturn_b200.search import run_search
     T, valid = R.synth_table(J, 3, 8, seed=100 + J)
     engine.set_table(T)
     tmin = R.reduce_table(R.canon_table(T, range(1, 9)))[0][:, None, :]
     kw = dict(chains=9472, rounds=48, seed=11, reduced=True, use_dist=False, record_history=True, exchange_every=8,
               resample_every=4, objective="completion")
-    a = run_search(engine, _extra_flags=0x08000000, **kw)
+    a = run_search(engine, _extra_flags=_lib.HOOK_VERIFY_INCREMENTAL, **kw)
     assert engine.search_verify_count() == 0
     b = run_search(engine, **kw)
     assert b.makespan == a.makespan and np.array_equal(b.opt, a.opt) and np.array_equal(b.prio, a.prio)

@@ -376,15 +376,16 @@ def test_incremental_rounds_equal_full_evaluation(engine, J):
         the same chains: identical incumbent key, rows and history under a fixed seed;
     (c) the incumbent re-scores to its makespan in the oracle.
     J = 700 and up run the position-major kernel (both rows streamed; windows of whole 32-position blocks)."""
+    from saturn_b200 import _lib
     from saturn_b200.search import run_search
     T, valid = R.synth_table(J, 3, 8, seed=100 + J)
     engine.set_table(T)
     # an explicit tournament cadence: the automatic one differs between the modes for position-major populations
     kw = dict(chains=9472, rounds=48, seed=11, reduced=True, use_dist=False, record_history=True, exchange_every=8,
               resample_every=4)
-    a = run_search(engine, _extra_flags=0x08000000, **kw)
+    a = run_search(engine, _extra_flags=_lib.HOOK_VERIFY_INCREMENTAL, **kw)
     assert engine.search_verify_count() == 0
-    b = run_search(engine, _extra_flags=0x10000000, **kw)
+    b = run_search(engine, _extra_flags=_lib.HOOK_NO_INCREMENTAL, **kw)
     c = run_search(engine, **kw)
     for x in (b, c):
         assert x.makespan == a.makespan and np.array_equal(x.opt, a.opt) and np.array_equal(x.prio, a.prio)
@@ -394,5 +395,5 @@ def test_incremental_rounds_equal_full_evaluation(engine, J):
     assert float(R.list_schedule(tmin[:, None, :], c.opt, c.prio, True, np.float32)[0]) == c.makespan
     assert c.history[-1][2] < c.history[0][2] or J <= 40
     # the round-1 move generator (no windows) reaches a comparable plan: the windows cost no quality
-    d = run_search(engine, _extra_flags=0x04000000, **kw)
+    d = run_search(engine, _extra_flags=_lib.HOOK_ROUND1_MOVES, **kw)
     assert c.makespan <= d.makespan * 1.01

@@ -59,6 +59,23 @@ def test_ctypes_structs_match_the_header_layout(tmp_path):
             assert int(got["%s.%s" % (cname, fname)]) == getattr(cls, fname).offset, (cname, fname)
 
 
+def test_test_hook_names_match_the_library():
+    """The HOOK_* constants of _lib.py have the names and bits of the hook enum in csrc/sb_internal.h, and no hook
+    shares a bit with a FLAG_* flag."""
+    src = open(os.path.join(ROOT, "saturn_b200", "csrc", "sb_internal.h")).read()
+    enum = re.search(r"enum : unsigned \{(.*?)\};", src, flags=re.S).group(1)
+    in_c = {name: int(value, 16) for name, value in re.findall(r"^\s*(HOOK_\w+)\s*=\s*(0x[0-9a-fA-F]+)u,", enum, flags=re.M)}
+    in_py = {name: value for name, value in vars(_lib).items() if name.startswith("HOOK_")}
+    assert len(in_c) == 12 and in_c == in_py, set(in_c.items()) ^ set(in_py.items())
+    flags = 0
+    for name, value in vars(_lib).items():
+        if name.startswith("FLAG_"):
+            flags |= value
+    for value in in_py.values():
+        assert bin(value).count("1") == 1 and value & flags == 0
+    assert len(set(in_py.values())) == len(in_py)
+
+
 def test_no_cpu_fallback_fails_loudly():
     import torch
     if torch.cuda.is_available():
