@@ -44,7 +44,11 @@
  * With SB_FLAG_SUM_COMPLETION the score is the sum of completion times instead:
  *   total = sum_j (start_j + rt_j), in fp32 a left fold in schedule order, acc = acc + (start + rt) from +0
  * (one add per job, never paired or reassociated; the oracle folds the same way and agrees bit for bit).
- * The schedule, every start and every slot mask are the same under both objectives.
+ * With SB_FLAG_WEIGHTED as well (per-job weights w_j > 0, sb_set_weights) it is the weighted sum:
+ *   total = sum_j w_j (start_j + rt_j), acc = acc + (w_j * (start_j + rt_j)) from +0 in schedule order, with TWO
+ * fp32 roundings per job (the product, then the sum; never one fused multiply-add).  w = 1 gives exactly the
+ * unweighted fold, w = 2 exactly twice it (barring overflow).
+ * The schedule, every start and every slot mask are the same under every objective.
  * With integer_starts the slot state is the integer time a slot becomes usable, start + ceil(rt);
  * SURVEY.md §8a writes the same rule as `start = ceil(max ready)` over real-valued ready times.  Starts,
  * makespans and the set of k slots taken are identical (ceil is monotone); the one observable difference
@@ -105,6 +109,14 @@ typedef enum sb_status {
                                      temperature unit becomes the incumbent's MEAN completion (sum / J), and
                                      sb_search_seed_lpt plants shortest-processing-time orders.  Not available with
                                      SB_FLAG_ALT_WARPSCAN (SB_ERR_UNSUPPORTED). */
+#define SB_FLAG_WEIGHTED 128u      /* with SB_FLAG_SUM_COMPLETION only (else SB_ERR_ARG), after sb_set_weights (else
+                                     SB_ERR_STATE): the objective is the WEIGHTED sum of completion times
+                                     sum_j w_j (start_j + rt_j) (see the evaluation rule above).  Accepted wherever
+                                     SB_FLAG_SUM_COMPLETION is, sb_search_run_multi included (every handle must hold
+                                     weights); every score the library emits then holds the weighted sum.  The
+                                     search's temperature unit becomes the incumbent's weighted sum / sum_j w_j, and
+                                     sb_search_seed_lpt plants WSPT orders (Smith's rule: ascending rt / w, ties by
+                                     job index).  Not available with SB_FLAG_ALT_WARPSCAN (SB_ERR_UNSUPPORTED). */
 #define SB_IPC_HANDLE_BYTES 64
 
 typedef struct sb_handle sb_handle;
@@ -134,6 +146,10 @@ int sb_set_table(sb_handle* h, const float* T, const uint8_t* gcount, int J, int
  * search (it is still evaluated like any number if a caller's candidate selects it).  Default 1e6;
  * pass +inf to treat every finite cell as usable.  Takes effect at the next sb_set_table. */
 int sb_set_sentinel(sb_handle* h, float threshold);
+/* Per-job weights for SB_FLAG_WEIGHTED: w host fp32 [J], every value finite and > 0 (else SB_ERR_ARG, as is a J
+ * that differs from the table's); w = NULL clears them.  SB_ERR_STATE before sb_set_table.  sb_set_table clears
+ * the weights; setting or clearing them ends the current search (sb_search_init again). */
+int sb_set_weights(sb_handle* h, const float* w, int J);
 /* copy the reduced table back (host pointers, either may be NULL): tmin fp32 [J][8], args u8 [J][8].
  * This is the table the reference solver is actually given: Task.strategies[g] after the profiler's
  * min over executors (PerformanceEvaluator.py:101-115), read at milp.py:77-81. */
@@ -228,7 +244,8 @@ typedef struct sb_search_params {
   uint64_t chain_base;  /* global id of chain 0 (rank * chains) */
   unsigned flags;       /* SB_FLAG_* */
   float t_start;        /* initial temperature as a fraction of the incumbent makespan (SB_FLAG_SUM_COMPLETION:
-                         * of the incumbent's mean completion time, its sum / J) */
+                         * of the incumbent's mean completion time, its sum / J; with SB_FLAG_WEIGHTED its
+                         * weighted sum / the sum of the weights) */
   float t_end;          /* final temperature fraction */
   int total_rounds;     /* cooling horizon */
   int resample_every;   /* > 0: sb_search_round itself resamples the population by tournament before every round r
@@ -260,7 +277,8 @@ int sb_search_resample(sb_handle* h);
  * sb_search_seed_lpt plants three longest-processing-time candidates (every job on its fastest option / on its
  * least GPU-seconds option / in between; nodes filled greedily by GPU-seconds) into an eighth of the
  * population each and scores them; with SB_FLAG_SUM_COMPLETION the orders are shortest-processing-time
- * instead (ascending runtime of the chosen option), same options and node fill.  sb_search_run = sb_search_init + seeds + `rounds` rounds in groups of
+ * instead (ascending runtime of the chosen option), with SB_FLAG_WEIGHTED as well WSPT orders (ascending runtime / weight,
+ * ties by job index), same options and node fill.  sb_search_run = sb_search_init + seeds + `rounds` rounds in groups of
  * `sync_every` (tournament resampling every `resample_every` rounds inside a group is only another launch;
  * the host reads the incumbent key once per group and applies the stopping rules) + sb_search_best.
  * The multi-GPU driver (saturn_b200/search.py) runs the same steps with a key exchange per group. */

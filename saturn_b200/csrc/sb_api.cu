@@ -40,7 +40,8 @@ struct SearchState {
   bool ready = false;
   SearchDev d;
   sb_search_params p;
-  float scale = 0.f;  // temperature unit: incumbent makespan after initialisation (SB_FLAG_SUM_COMPLETION: sum / J)
+  float scale = 0.f;  // temperature unit: incumbent makespan after initialisation (SB_FLAG_SUM_COMPLETION: sum / J;
+                      // with SB_FLAG_WEIGHTED: weighted sum / sum of the weights)
   long long evaluated = 0;
   int rounds_done = 0;
   bool fused_ok = true;  // run rounds with the fused kernel while its tiles fit
@@ -58,6 +59,7 @@ struct SearchState {
   unsigned long long* verify_bad = nullptr;
   bool win = false, inc = false, verify = false;
   SearchDev alloc;  // the pointers as allocated (s.d's cur / prop pairs trade places when resampling)
+  const float* w = nullptr;  // SB_FLAG_WEIGHTED: the handle's job weights (position-major kernels)
 };
 
 struct sb_handle {
@@ -90,6 +92,13 @@ struct sb_handle {
   size_t dec_cap = 0;
   float* stage_T = nullptr;  // device staging of a host table (kept across sb_set_table calls)
   size_t stage_T_bytes = 0;
+  // job weights (sb_set_weights): device copy zero-padded to a multiple of 4 floats (16-byte TMA copies), host copy
+  // (WSPT seeds) and their sum in double (the temperature unit); has_w is cleared by sb_set_table
+  float* d_w = nullptr;
+  size_t d_w_cap = 0;
+  std::vector<float> h_w;
+  double w_sum = 0.0;
+  bool has_w = false;
   SearchState search;
   int last_path = -1;
   // peer-memory exchange
@@ -200,6 +209,7 @@ int sb_destroy(sb_handle* h) {
   cudaFree(h->by_pos);
   cudaFree(h->dec_buf);
   cudaFree(h->stage_T);
+  cudaFree(h->d_w);
   for (int i = 0; i < 2; ++i)
     if (h->hs[i]) cudaStreamDestroy(h->hs[i]);
   if (h->own_stream && h->stream) cudaStreamDestroy(h->stream);
@@ -229,6 +239,7 @@ int sb_set_table(sb_handle* h, const float* T, const uint8_t* gcount, int J, int
   }
   CK(cudaStreamSynchronize(h->stream));
   h->search.ready = false;  // its buffers are reused by the next sb_search_init if the shape is unchanged
+  h->has_w = false;         // weights belong to a task set: a new table needs new ones
   const size_t nT = static_cast<size_t>(J) * S * G;
   const size_t ntab = static_cast<size_t>(J) * S * kSlots;
   // a re-planning loop sets a table of the same shape every interval: keep the allocations (cudaFree /
@@ -292,6 +303,49 @@ int sb_set_sentinel(sb_handle* h, float threshold) {
   return SB_OK;
 }
 
+int sb_set_weights(sb_handle* h, const float* w, int J) {
+  int rc = use_device(h);
+  if (rc) return rc;
+  if (h->J == 0) return fail(SB_ERR_STATE, "sb_set_table has not been called");
+  CK(cudaStreamSynchronize(h->stream));  // no queued kernel may still read the old weights
+  h->search.ready = false;               // the running search was set up for the old weights (scale, seeds)
+  if (!w) {
+    h->has_w = false;
+    return SB_OK;
+  }
+  if (J != h->J) return fail(SB_ERR_ARG, "J=%d differs from the table's J=%d", J, h->J);
+  double sum = 0.0;
+  for (int j = 0; j < J; ++j) {
+    if (!isfinite(w[j]) || !(w[j] > 0.f)) return fail(SB_ERR_ARG, "weight %d (%g) is not finite and > 0", j, w[j]);
+    sum += static_cast<double>(w[j]);
+  }
+  h->has_w = false;
+  const size_t cap = static_cast<size_t>((J + 3) & ~3);
+  if (h->d_w_cap < cap) {
+    cudaFree(h->d_w);
+    h->d_w = nullptr;
+    h->d_w_cap = 0;
+    CK(cudaMalloc(&h->d_w, cap * sizeof(float)));
+    h->d_w_cap = cap;
+  }
+  h->h_w.assign(w, w + J);
+  h->h_w.resize(cap, 0.f);
+  CK(cudaMemcpyAsync(h->d_w, h->h_w.data(), cap * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  h->w_sum = sum;
+  h->has_w = true;
+  return SB_OK;
+}
+
+// SB_FLAG_WEIGHTED is valid with SB_FLAG_SUM_COMPLETION and after sb_set_weights only
+static int check_weighted(const sb_handle* h, unsigned flags) {
+  if (!(flags & SB_FLAG_WEIGHTED)) return SB_OK;
+  if (!(flags & SB_FLAG_SUM_COMPLETION))
+    return fail(SB_ERR_ARG, "SB_FLAG_WEIGHTED weights the sum of completion times: it needs SB_FLAG_SUM_COMPLETION");
+  if (!h->has_w) return fail(SB_ERR_STATE, "SB_FLAG_WEIGHTED needs sb_set_weights (sb_set_table clears the weights)");
+  return SB_OK;
+}
+
 int sb_get_reduced(sb_handle* h, float* tmin, uint8_t* args) {
   if (!h) return fail(SB_ERR_ARG, "null handle");
   if (h->J == 0) return fail(SB_ERR_STATE, "sb_set_table has not been called");
@@ -308,6 +362,7 @@ static int make_call(sb_handle* h, const uint8_t* opt, const void* prio, int64_t
   if (B < 0) return fail(SB_ERR_ARG, "B=%lld is negative", static_cast<long long>(B));
   if (B > 0 && (!opt || !prio)) return fail(SB_ERR_ARG, "opt / prio is null");
   if (row_stride < h->J) return fail(SB_ERR_ARG, "row_stride=%lld < J=%d", static_cast<long long>(row_stride), h->J);
+  if (int rc = check_weighted(h, flags)) return rc;
   if (B > 0xffffffffll) return fail(SB_ERR_ARG, "B=%lld exceeds 2^32-1 candidates per call", static_cast<long long>(B));
   const int pb = h->J <= 256 ? 1 : 2;
   const bool reduced = (flags & SB_FLAG_REDUCED) != 0;
@@ -324,6 +379,7 @@ static int make_call(sb_handle* h, const uint8_t* opt, const void* prio, int64_t
   c->stride_o = row_stride;
   c->stride_p = row_stride * pb;
   c->flags = flags;
+  c->w = (flags & SB_FLAG_WEIGHTED) ? h->d_w : nullptr;
   return SB_OK;
 }
 
@@ -382,9 +438,9 @@ int sb_eval(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, int64
     }
   }
   if (flags & SB_FLAG_ALT_WARPSCAN) {
-    if (flags & SB_FLAG_SUM_COMPLETION)
+    if (flags & (SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED))
       return fail(SB_ERR_UNSUPPORTED, "SB_FLAG_ALT_WARPSCAN scores the makespan only: it cannot be combined with "
-                  "SB_FLAG_SUM_COMPLETION");
+                  "SB_FLAG_SUM_COMPLETION or SB_FLAG_WEIGHTED");
     if (flags & (SB_FLAG_POST_KEY | SB_FLAG_FOLD_PREV))
       return fail(SB_ERR_UNSUPPORTED, "SB_FLAG_ALT_WARPSCAN cannot be combined with the fused key exchange");
     cudaError_t e = eval_alt_launch(h->dev, c, h->stream);
@@ -712,7 +768,7 @@ static int search_eval(sb_handle* h, bool cur_rows, long long first, long long c
     SearchFuse sf = {};
     sf.cur_mk = s.d.cur_mk;
     const bool reduced = (s.p.flags & SB_FLAG_REDUCED) != 0;
-    CK(search_pos_launch(h->dev, s.d, reduced ? h->tmin : h->tab, (reduced ? 1 : h->S) * kSlots, s.p.flags, first,
+    CK(search_pos_launch(h->dev, s.d, reduced ? h->tmin : h->tab, s.w, (reduced ? 1 : h->S) * kSlots, s.p.flags, first,
                          count, true, sf, h->stream));
     return SB_OK;
   }
@@ -734,6 +790,7 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
   if (h->J == 0) return fail(SB_ERR_STATE, "sb_set_table has not been called");
   if (!p) return fail(SB_ERR_ARG, "params is null");
   if (p->chains < 1 || p->chains > (1ll << 31)) return fail(SB_ERR_ARG, "chains=%lld out of range", (long long)p->chains);
+  if ((rc = check_weighted(h, p->flags))) return rc;
   CK(cudaStreamSynchronize(h->stream));
   SearchState& s = h->search;
   s.ready = false;
@@ -748,6 +805,8 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
   d.chains = p->chains;
   d.chain_base = p->chain_base;
   d.seed = p->seed;
+  const bool weighted = (p->flags & SB_FLAG_WEIGHTED) != 0;
+  s.w = weighted ? h->d_w : nullptr;
   d.stride_o = (J + 31) & ~31;  // 32-byte rows: TMA bulk copies for opt, 256-bit streaming loads for prio
   // make stride_p == stride_o * pb so that one element stride describes both (sb_eval contract)
   d.stride_p = d.stride_o * pb;
@@ -787,8 +846,8 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
   // Rows that do not fit in shared memory: keep the population in schedule order and stream both rows.
   const int SGs = (reduced ? 1 : h->S) * kSlots;
   const bool no_fused = (p->flags & HOOK_NO_FUSED) != 0;
-  const int mode = search_round_mode(h->dev, J, SGs, h->nodes);
-  d.pos = (!no_fused && mode != 2 && search_pos_smem(J, SGs, h->nodes, 16) <= h->dev.smem_optin) ? 1 : 0;
+  const int mode = search_round_mode(h->dev, J, SGs, h->nodes, weighted);
+  d.pos = (!no_fused && mode != 2 && search_pos_smem(J, SGs, h->nodes, 16, weighted) <= h->dev.smem_optin) ? 1 : 0;
   if (d.pos) CK(search_init_population_pos(d, h->stream));
   else CK(search_init_population(d, h->stream));
   s.ready = true;
@@ -812,9 +871,11 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
   uint32_t bits = static_cast<uint32_t>(key >> 32);
   float mk;
   memcpy(&mk, &bits, 4);
-  // the temperature unit: the incumbent's makespan, or its mean completion time (the sum / J), so that t_start /
-  // t_end mean the same fraction of a typical score difference under both objectives
-  s.scale = isfinite(mk) ? ((p->flags & SB_FLAG_SUM_COMPLETION) ? mk / static_cast<float>(J) : mk) : 1.0f;
+  // the temperature unit: the incumbent's makespan, or its mean completion time (the sum / J; weighted: the weighted
+  // sum / the sum of the weights, the same fp32 value for unit weights), so that t_start / t_end mean the same
+  // fraction of a typical score difference under every objective
+  const float per = weighted ? static_cast<float>(h->w_sum) : static_cast<float>(J);
+  s.scale = isfinite(mk) ? ((p->flags & SB_FLAG_SUM_COMPLETION) ? mk / per : mk) : 1.0f;
   s.evaluated = d.chains;
   s.rounds_done = 0;
   s.launches = 0;
@@ -916,7 +977,7 @@ int sb_search_round(sb_handle* h, int rounds) {
       SearchFuse sf = make_fuse(s, round, n);
       sf.resample_every = 0;
       const bool reduced = (s.p.flags & SB_FLAG_REDUCED) != 0;
-      CK(search_pos_launch(h->dev, s.d, reduced ? h->tmin : h->tab, (reduced ? 1 : h->S) * kSlots, s.p.flags, 0,
+      CK(search_pos_launch(h->dev, s.d, reduced ? h->tmin : h->tab, s.w, (reduced ? 1 : h->S) * kSlots, s.p.flags, 0,
                            s.d.chains, false, sf, h->stream));  // keeps the incumbent in its tail
       fused = true;
     } else if (s.fused_ok) {
@@ -1033,6 +1094,8 @@ int sb_search_seed_lpt(sb_handle* h) {
   const bool reduced = (s.p.flags & SB_FLAG_REDUCED) != 0;
   const float* tmin = h->h_tmin.data();
   const bool spt = (s.p.flags & SB_FLAG_SUM_COMPLETION) != 0;  // shortest first: the order that favours the sum
+  // weighted sum: Smith's rule (WSPT), ascending rt / w; with unit weights exactly the SPT order
+  const bool wspt = spt && (s.p.flags & SB_FLAG_WEIGHTED) != 0;
   const double INF = HUGE_VAL;
   // usable cells: below the sentinel threshold; a job with none falls back to any finite cell
   std::vector<double> usable(static_cast<size_t>(J) * kSlots);
@@ -1069,7 +1132,10 @@ int sb_search_seed_lpt(sb_handle* h) {
       weight[j] = rt[j] * sqrt(best + 1.0);
       order[j] = j;
     }
-    if (spt) std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return rt[a] < rt[b]; });
+    if (wspt) {
+      for (int j = 0; j < J; ++j) weight[j] = rt[j] / static_cast<double>(h->h_w[j]);
+      std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return weight[a] < weight[b]; });
+    } else if (spt) std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return rt[a] < rt[b]; });
     else std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return weight[a] > weight[b]; });
     std::vector<double> load(nodes, 0.0);
     for (int j = 0; j < J; ++j) opt[j] = static_cast<uint8_t>(col[j]);
@@ -1280,15 +1346,16 @@ int sb_search_wave(sb_handle* h, unsigned flags, int64_t* chains) {
   const bool reduced = (flags & SB_FLAG_REDUCED) != 0;
   const int SG = (reduced ? 1 : h->S) * kSlots;
   const int pb = h->J <= 256 ? 1 : 2;
+  const bool weighted = (flags & SB_FLAG_WEIGHTED) != 0;
   int warps = 0;
   TilePlan tp;
-  if (search_round_mode(h->dev, h->J, SG, h->nodes) == 2) {
-    plan_tiles(h->dev, h->J, SG, pb, false, h->nodes, &tp);
+  if (search_round_mode(h->dev, h->J, SG, h->nodes, weighted) == 2) {
+    plan_tiles(h->dev, h->J, SG, pb, false, h->nodes, &tp, false, weighted);
     warps = tp.warps;
-  } else if (search_pos_smem(h->J, SG, h->nodes, 16) <= h->dev.smem_optin) {
+  } else if (search_pos_smem(h->J, SG, h->nodes, 16, weighted) <= h->dev.smem_optin) {
     warps = 16;
   } else {  // unfused rounds: the evaluation kernel's own plan (1 warp stands for the generic kernel's 128-thread CTAs)
-    warps = plan_tiles(h->dev, h->J, SG, pb, true, h->nodes, &tp);
+    warps = plan_tiles(h->dev, h->J, SG, pb, true, h->nodes, &tp, false, weighted);
     if (warps < 1) warps = 4;
   }
   *chains = static_cast<int64_t>(warps) * 32 * h->dev.sm_count;

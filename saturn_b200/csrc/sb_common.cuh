@@ -145,8 +145,13 @@ __device__ __forceinline__ float fmax3_mk(float mk, float b, float c) {
 // kSum (SB_FLAG_SUM_COMPLETION): mk is the running SUM of completions instead, one add per step in schedule
 // order (acc = acc + (s + rt), the oracle's left fold bit for bit); `ph` and `pend` are unused, and the
 // completion is tracked whatever kTrackMk says.  The slot update is the same: only the score differs.
-template <bool kIntegerStarts, bool kTrackMk = kIntegerStarts, bool kSum = false>
-__device__ __forceinline__ void ls_step(float (&f)[8], float& mk, float& pend, float rt, int km1, int one, int ph) {
+// kWeighted (SB_FLAG_WEIGHTED, with kSum only): the job's weight `w` scales its completion, acc = acc + (w * e) with
+// TWO roundings (__fmul_rn, __fadd_rn: nvcc would otherwise contract them into one FFMA, which the oracle cannot
+// reproduce); w = 1 then gives the unweighted fold bit for bit.
+template <bool kIntegerStarts, bool kTrackMk = kIntegerStarts, bool kSum = false, bool kWeighted = false>
+__device__ __forceinline__ void ls_step(float (&f)[8], float& mk, float& pend, float rt, int km1, int one, int ph,
+                                        float w = 0.f) {
+  static_assert(kSum || !kWeighted, "weights scale the sum of completion times only");
   const float INF = inf_f();
   const int b2 = km1 & 4, b1 = km1 & 2, b0 = km1 & 1;
   // stage "shift by 4"
@@ -169,7 +174,8 @@ __device__ __forceinline__ void ls_step(float (&f)[8], float& mk, float& pend, f
   }
   if (kSum) {
     const float e = kIntegerStarts ? s + rt : v;
-    mk = mk + e;
+    if (kWeighted) mk = __fadd_rn(mk, __fmul_rn(w, e));
+    else mk = mk + e;
   } else if (kTrackMk) {
     const float e = kIntegerStarts ? s + rt : v;
     if (ph < 0) mk = fmaxf(mk, e);

@@ -31,7 +31,7 @@ static_assert(((HOOK_FORCE_GENERIC | HOOK_NO_STREAM | HOOK_NO_FUSED | HOOK_NO_IN
                 HOOK_ROUND1_MOVES | HOOK_PLAIN_ADDR | HOOK_WINDOW_BIAS | HOOK_TABLE_GLOBAL | HOOK_TABLE_PAIR |
                 HOOK_REORDER | HOOK_NO_REORDER) &
                (SB_FLAG_INTEGER_STARTS | SB_FLAG_REDUCED | SB_FLAG_OPT_BY_POSITION | SB_FLAG_POST_KEY |
-                SB_FLAG_FOLD_PREV | SB_FLAG_ALT_WARPSCAN | SB_FLAG_SUM_COMPLETION)) == 0,
+                SB_FLAG_FOLD_PREV | SB_FLAG_ALT_WARPSCAN | SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED)) == 0,
               "the test hooks share no bit with the SB_FLAG_* flags");
 
 // Compile-time dispatch: f is called with the run-time value as a type (std::true_type / std::false_type, or the
@@ -44,13 +44,17 @@ template <class F>
 decltype(auto) with_pb(int pb, F&& f) {
   return pb == 1 ? f(std::integral_constant<int, 1>{}) : f(std::integral_constant<int, 2>{});
 }
-// f(PB, INT, SUM): the prio width, SB_FLAG_INTEGER_STARTS and SB_FLAG_SUM_COMPLETION, the template arguments that
-// every evaluation and search kernel takes
+// f(PB, INT, SUM, W): the prio width, SB_FLAG_INTEGER_STARTS, SB_FLAG_SUM_COMPLETION and SB_FLAG_WEIGHTED, the
+// template arguments that every evaluation and search kernel takes.  W is true only together with SUM: no kernel
+// that weights the makespan is ever instantiated.
 template <class F>
 decltype(auto) with_eval_types(int pb, unsigned flags, F&& f) {
   return with_pb(pb, [&](auto PB) {
     return with_bool(flags & SB_FLAG_INTEGER_STARTS, [&](auto INT) {
-      return with_bool(flags & SB_FLAG_SUM_COMPLETION, [&](auto SUM) { return f(PB, INT, SUM); });
+      return with_bool(flags & SB_FLAG_SUM_COMPLETION, [&](auto SUM) {
+        if constexpr (SUM) return with_bool(flags & SB_FLAG_WEIGHTED, [&](auto W) { return f(PB, INT, SUM, W); });
+        else return f(PB, INT, SUM, std::false_type{});
+      });
     });
   });
 }
@@ -101,6 +105,7 @@ struct TilePlan {
 
 struct EvalCall {
   const float* tab = nullptr;  // canonical table actually used (full or reduced)
+  const float* w = nullptr;    // SB_FLAG_WEIGHTED: the job weights [J], padded with zeros to a multiple of 4
   int J = 0, SG = 0;
   const uint8_t* opt = nullptr;
   const uint8_t* prio = nullptr;
@@ -156,10 +161,12 @@ struct SearchFuse {
   } keep;
 };
 
-int plan_tiles(const Device& dev, int J, int SG, int pb, bool stream, int nodes, TilePlan* tp, bool tab_global = false);
+// weighted: the J weights are staged beside the table (unless tab_global: then both stay in global memory)
+int plan_tiles(const Device& dev, int J, int SG, int pb, bool stream, int nodes, TilePlan* tp, bool tab_global = false,
+               bool weighted = false);
 cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, int* path_used);
 cudaError_t eval_alt_launch(const Device& dev, const EvalCall& c, cudaStream_t st);  // sb_eval_alt.cu
-int search_round_mode(const Device& dev, int J, int SG, int nodes);
+int search_round_mode(const Device& dev, int J, int SG, int nodes, bool weighted = false);
 cudaError_t search_round_launch(const Device& dev, const EvalCall& c, const SearchFuse& sf, cudaStream_t st);
 cudaError_t eval_full_launch(const Device& dev, const EvalCall& c, float* start, uint32_t* slotmask, cudaStream_t st);
 cudaError_t validate_launch(const Device& dev, const EvalCall& c, unsigned long long* bad, cudaStream_t st,

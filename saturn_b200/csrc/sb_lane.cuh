@@ -37,16 +37,20 @@ __device__ __forceinline__ PrioChunk ld_prio32(const uint8_t* p) {
 // the ALU pipe — the step is bound by the ALU pipe (half rate) and by issue together, so the same instruction
 // count with two fewer ALU instructions is the cheaper mix.
 // SUM: score = sum of completion times (SB_FLAG_SUM_COMPLETION) instead of the makespan; mk holds the running sum.
-template <bool INT, bool MULTI, int ADDR = 0, bool SUM = false>
+// WGT (SB_FLAG_WEIGHTED, with SUM only): each completion is scaled by its job's weight, read from `wt` — 1: the
+// weights are in shared memory beside the table, 2: in global memory, read with ld.global.nc.
+template <bool INT, bool MULTI, int ADDR = 0, bool SUM = false, int WGT = 0>
 struct LaneState {
   float f[8];
   float mk;
   float pend;  // a completion time parked by an even step (see ls_step; never used with SUM)
   const uint8_t* orow;  // this candidate's opt bytes (shared memory or global)
   const float* tab;     // runtime table (shared memory or global)
+  const float* wt;      // WGT: the job weights [J]
   int SG;
   int one;
   uint32_t orow_s, tab_s, four;  // ADDR = 1: shared-window addresses of orow / tab, and a run-time 4
+  uint32_t wt_s;                 // ADDR = 1 with WGT: shared-window address of wt
   float4* ns;  // MULTI: lane-private node-state column; node n lives at ns[(2n)*32], ns[(2n+1)*32]
   int cur;     // MULTI: the node whose state is currently in f[] (its shared-memory copy is stale)
 
@@ -81,13 +85,19 @@ struct LaneState {
   __device__ __forceinline__ float lookup_rt(int j, int o) const {
     return MULTI ? tab[j * 8 + (o & 7)] : tab[j * SG + o];
   }
-  // ph: t & 1 inside fully unrolled loops, -1 elsewhere (see ls_step)
-  __device__ __forceinline__ void step_resolved(int o, float rt, int ph = -1) {
+  // the job's weight (WGT only; 0 otherwise, and then unused)
+  __device__ __forceinline__ float lookup_w(int j) const {
+    if constexpr (WGT == 1) return wt[j];
+    else if constexpr (WGT == 2) return __ldg(wt + j);
+    else return 0.f;
+  }
+  // ph: t & 1 inside fully unrolled loops, -1 elsewhere (see ls_step); w: the job's weight (WGT only)
+  __device__ __forceinline__ void step_resolved(int o, float rt, int ph = -1, float w = 0.f) {
     if (!MULTI) {
-      ls_step<INT, INT, SUM>(f, mk, pend, rt, o & 7, one, ph);
+      ls_step<INT, INT, SUM, (WGT != 0)>(f, mk, pend, rt, o & 7, one, ph, w);
     } else {
       switch_node(o >> 3);
-      ls_step<INT, true, SUM>(f, mk, pend, rt, o & 7, one, ph);
+      ls_step<INT, true, SUM, (WGT != 0)>(f, mk, pend, rt, o & 7, one, ph, w);
     }
   }
   // ADDR = 1: the two look-ups as separate gathers, so that the streamed loop of k_eval_tiles can issue a whole
@@ -106,21 +116,34 @@ struct LaneState {
     asm("ld.shared.f32 %0, [%1];" : "=f"(rt) : "r"(ta));
     return rt;
   }
+  // ADDR = 1 with WGT = 1: the weight gather, its address formed on the FMA pipe like the two above
+  __device__ __forceinline__ float gather_w(int j) const {
+    if constexpr (WGT == 0) {
+      return 0.f;
+    } else {
+      uint32_t wa;
+      float w;
+      asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(wa) : "r"(j), "r"(four), "r"(wt_s));
+      asm("ld.shared.f32 %0, [%1];" : "=f"(w) : "r"(wa));
+      return w;
+    }
+  }
   __device__ __forceinline__ void step(int j, int ph = -1) {
+    constexpr bool W = WGT != 0;
     if (!MULTI && ADDR == 1) {
       const uint32_t o = gather_opt(j);
-      ls_step<INT, INT, SUM>(f, mk, pend, gather_rt(j, o), static_cast<int>(o & 7u), one, ph);
+      ls_step<INT, INT, SUM, W>(f, mk, pend, gather_rt(j, o), static_cast<int>(o & 7u), one, ph, gather_w(j));
       return;
     }
     const int o = orow[j];
     if (!MULTI) {
       const float rt = tab[j * SG + o];
-      ls_step<INT, INT, SUM>(f, mk, pend, rt, o & 7, one, ph);
+      ls_step<INT, INT, SUM, W>(f, mk, pend, rt, o & 7, one, ph, lookup_w(j));
     } else {
       const int col = o & 7;  // reduced table only: opt = (node << 3) | (k - 1)
       const float rt = tab[j * 8 + col];
       switch_node(o >> 3);
-      ls_step<INT, true, SUM>(f, mk, pend, rt, col, one, ph);
+      ls_step<INT, true, SUM, W>(f, mk, pend, rt, col, one, ph, lookup_w(j));
     }
   }
   __device__ __forceinline__ float result() const { return SUM ? mk : ((INT || MULTI) ? fmaxf(mk, pend) : f[7]); }

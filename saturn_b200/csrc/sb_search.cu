@@ -328,6 +328,7 @@ struct PosArgs {
   int eval_only;  // 1: score the rows as they are and store cur_mk (initialisation, injected rows)
   int one;
   SearchFuse sf;
+  const float* w;  // W: job weights [J], zero-padded to a multiple of 4 (16 bytes)
 };
 
 struct PosMove {
@@ -420,9 +421,12 @@ __device__ __forceinline__ PosMove make_pos_move_win(const SearchFuse& sf, int r
 // look-up is a `ld.shared::cluster` to whichever CTA owns the entry (distributed shared memory) — the
 // alternative to 1, kept behind a test hook.
 // SUM: score the sum of completion times instead of the makespan (SB_FLAG_SUM_COMPLETION, see ls_step).
-template <int PB, bool INT, bool MULTI, bool EVAL = false, int TAB = 0, bool SUM = false>
+// W: weight each completion by its job's weight (SB_FLAG_WEIGHTED, with SUM only); the weights follow the table in
+// shared memory with TAB = 0 and are read from global memory (ld.global.nc) with TAB = 1 / 2.
+template <int PB, bool INT, bool MULTI, bool EVAL = false, int TAB = 0, bool SUM = false, bool W = false>
 __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
   static_assert(TAB == 0 || (EVAL && !MULTI), "tables outside the CTA's shared memory: scoring only, one node");
+  static_assert(SUM || !W, "weights scale the sum of completion times only");
   extern __shared__ __align__(128) uint8_t smem[];
   const int nw = blockDim.x >> 5;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -433,8 +437,10 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
   const uint32_t tab_off = TAB == 2 ? rank * half * 4u : 0u;
   const uint32_t tab_bytes = TAB == 1 ? 0u : (TAB == 2 ? (rank == 0 ? half * 4u : tab_all - half * 4u) : tab_all);
   const uint32_t tab_room = TAB == 1 ? 0u : (TAB == 2 ? half * 4u : tab_all);
+  const uint32_t w_bytes = (W && TAB == 0) ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u;
   float* tab_s = reinterpret_cast<float*>(smem);
-  uint64_t* bar_tab = reinterpret_cast<uint64_t*>(smem + ((tab_room + 15u) & ~15u));
+  [[maybe_unused]] float* w_s = reinterpret_cast<float*>(smem + ((tab_room + 15u) & ~15u));
+  uint64_t* bar_tab = reinterpret_cast<uint64_t*>(smem + ((tab_room + 15u) & ~15u) + w_bytes);
   const uint32_t node_bytes = MULTI ? static_cast<uint32_t>(a.nodes) * 1024u : 0u;
   float4* node_s = reinterpret_cast<float4*>(reinterpret_cast<uint8_t*>(bar_tab) + 16 + static_cast<size_t>(warp) * node_bytes);
   if (threadIdx.x == 0) {
@@ -444,13 +450,19 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
   __syncthreads();
   if constexpr (TAB != 1) {
     if (threadIdx.x == 0) {
-      mbar_arrive_expect_tx(bar_tab, tab_bytes);
+      mbar_arrive_expect_tx(bar_tab, tab_bytes + w_bytes);
       const uint8_t* src = reinterpret_cast<const uint8_t*>(a.tab) + tab_off;
       for (uint32_t off = 0; off < tab_bytes; off += 32768u) tma_bulk_g2s(smem + off, src + off, min(32768u, tab_bytes - off), bar_tab);
+      if constexpr (W && TAB == 0) {
+        const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(a.w);
+        for (uint32_t off = 0; off < w_bytes; off += 32768u)
+          tma_bulk_g2s(reinterpret_cast<uint8_t*>(w_s) + off, wsrc + off, min(32768u, w_bytes - off), bar_tab);
+      }
     }
   }
-  LaneState<INT, MULTI, 0, SUM> st;
+  LaneState<INT, MULTI, 0, SUM, (W ? (TAB == 0 ? 1 : 2) : 0)> st;
   st.tab = tab_s;
+  if constexpr (W) st.wt = TAB == 0 ? w_s : a.w;
   st.SG = a.SG;
   st.one = a.one;
   st.orow = nullptr;
@@ -544,7 +556,8 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
           for (int t = 0; t < 32; ++t) {
             const int j = prio_at<PB>(qp[(t * PB) / 32].w, t % (32 / PB));
             const int o = prio_at<1>(qo.w, t);
-            st.step_resolved(o, lookup(j, o), t & 1);
+            if constexpr (W) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j));
+            else st.step_resolved(o, lookup(j, o), t & 1);
           }
         } else {
 #pragma unroll
@@ -552,7 +565,8 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
             if (base + t < J) {
               const int j = prio_at<PB>(qp[(t * PB) / 32].w, t % (32 / PB));
               const int o = prio_at<1>(qo.w, t);
-              st.step_resolved(o, lookup(j, o), t & 1);
+              if constexpr (W) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j));
+              else st.step_resolved(o, lookup(j, o), t & 1);
             }
           }
         }
@@ -734,10 +748,11 @@ cudaError_t search_init_population_pos(const SearchDev& s, cudaStream_t st) {
   return launch(with_pb(s.pb, [](auto PB) { return k_init_population_pos<PB>; }), grid, threads, 0, st, s);
 }
 
-// smem: table + mbarrier + per-warp node states (MULTI)
-size_t search_pos_smem(int J, int SG, int nodes, int warps) {
+// smem: table (+ weights) + mbarrier + per-warp node states (MULTI)
+size_t search_pos_smem(int J, int SG, int nodes, int warps, bool weighted) {
   const size_t tab_bytes = (static_cast<size_t>(J) * SG * 4 + 15) & ~size_t(15);
-  return tab_bytes + 16 + static_cast<size_t>(warps) * (nodes > 1 ? nodes * 1024u : 0u);
+  const size_t w_bytes = weighted ? (static_cast<size_t>(J) * 4 + 15) & ~size_t(15) : 0;
+  return tab_bytes + w_bytes + 16 + static_cast<size_t>(warps) * (nodes > 1 ? nodes * 1024u : 0u);
 }
 
 using PosKernel = void (*)(PosArgs);
@@ -750,8 +765,8 @@ static cudaError_t eval_pos_far_launch(const Device& dev, const PosArgs& a, int 
   if (smem > dev.smem_optin) return cudaErrorNotSupported;
   const long long ntiles = (a.chains + 31) / 32;
   const long long ctas = (ntiles + warps - 1) / warps;
-  const PosKernel kern = with_eval_types(pb, flags, [&](auto PB, auto INT, auto SUM) {
-    return tab_home == 2 ? k_search_pos<PB, INT, false, true, 2, SUM> : k_search_pos<PB, INT, false, true, 1, SUM>;
+  const PosKernel kern = with_eval_types(pb, flags, [&](auto PB, auto INT, auto SUM, auto W) {
+    return tab_home == 2 ? k_search_pos<PB, INT, false, true, 2, SUM, W> : k_search_pos<PB, INT, false, true, 1, SUM, W>;
   });
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
   if (e != cudaSuccess) return e;
@@ -783,7 +798,7 @@ static cudaError_t eval_pos_far_launch(const Device& dev, const PosArgs& a, int 
 
 // tab_home: 0 = the table in every CTA's shared memory (cudaErrorNotSupported when it does not fit);
 // scoring only, one node: 2 = split over CTA pairs, 1 = global memory
-cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float* tab, int SG, unsigned flags,
+cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float* tab, const float* w, int SG, unsigned flags,
                               long long first, long long count, bool eval_only, const SearchFuse& sf,
                               cudaStream_t st, int tab_home) {
   if (count <= 0) return cudaSuccess;
@@ -797,20 +812,21 @@ cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float
   a.eval_only = eval_only ? 1 : 0;
   a.one = 1;
   a.sf = sf;
+  a.w = w;
   const bool multi = s.nodes > 1;
   if (tab_home != 0) {
     if (!eval_only || multi) return cudaErrorNotSupported;
     return eval_pos_far_launch(dev, a, tab_home, s.pb, flags, st);
   }
   const int warps = 16;
-  const size_t smem = search_pos_smem(s.J, SG, s.nodes, warps);
+  const size_t smem = search_pos_smem(s.J, SG, s.nodes, warps, (flags & SB_FLAG_WEIGHTED) != 0);
   if (smem > dev.smem_optin) return cudaErrorNotSupported;
   const long long ntiles = (count + 31) / 32;
   const long long ctas = (ntiles + warps - 1) / warps;
   const int grid = static_cast<int>(ctas < dev.sm_count ? ctas : dev.sm_count);
-  const PosKernel kern = with_eval_types(s.pb, flags, [&](auto PB, auto INT, auto SUM) {
+  const PosKernel kern = with_eval_types(s.pb, flags, [&](auto PB, auto INT, auto SUM, auto W) {
     return with_bool(multi, [&](auto MULTI) {
-      return with_bool(eval_only, [&](auto EVAL) -> PosKernel { return k_search_pos<PB, INT, MULTI, EVAL, 0, SUM>; });
+      return with_bool(eval_only, [&](auto EVAL) -> PosKernel { return k_search_pos<PB, INT, MULTI, EVAL, 0, SUM, W>; });
     });
   });
   return launch(kern, grid, warps * 32, smem, st, a);
@@ -824,7 +840,7 @@ int eval_pos_home(const Device& dev, int J, int SG, int nodes, unsigned flags) {
   const bool pair_ok = nodes == 1 && static_cast<size_t>(pos_tab_half(J, SG)) * 4 + 16 <= dev.smem_optin;
   if (flags & HOOK_TABLE_PAIR) return pair_ok ? 2 : -1;
   if (flags & HOOK_TABLE_GLOBAL) return nodes == 1 ? 1 : -1;
-  if (search_pos_smem(J, SG, nodes, 16) <= dev.smem_optin) return 0;
+  if (search_pos_smem(J, SG, nodes, 16, (flags & SB_FLAG_WEIGHTED) != 0) <= dev.smem_optin) return 0;
   return nodes == 1 ? 1 : -1;
 }
 
@@ -846,7 +862,7 @@ cudaError_t eval_pos_launch(const Device& dev, const EvalCall& c, cudaStream_t s
   s.keys = c.best_key;
   SearchFuse sf = {};
   sf.cur_mk = c.out;
-  return search_pos_launch(dev, s, c.tab, c.SG, c.flags, 0, c.B, true, sf, st, home);
+  return search_pos_launch(dev, s, c.tab, c.w, c.SG, c.flags, 0, c.B, true, sf, st, home);
 }
 
 // Job-indexed opt rows -> schedule order (out[i] = opt[prio[i]]), one warp per candidate: the row is staged in

@@ -18,15 +18,37 @@ from ._lib import FLAG_INTEGER_STARTS, FLAG_REDUCED, SaturnB200Error, SearchPara
 NSLOT = 8
 
 
-OBJECTIVES = ("makespan", "completion")
+OBJECTIVES = ("makespan", "completion", "weighted_completion")
 
 
 def objective_flag(objective: str) -> int:
-    """SB_FLAG_SUM_COMPLETION for objective="completion" (score = sum of completion times), 0 for "makespan"."""
+    """SB_FLAG_SUM_COMPLETION for objective="completion" (score = sum of completion times), SB_FLAG_SUM_COMPLETION |
+    SB_FLAG_WEIGHTED for "weighted_completion" (the sum weighted by the engine's set_weights), 0 for "makespan"."""
     if objective not in OBJECTIVES:
         from .solver import SolverError
-        raise SolverError("objective must be 'makespan' or 'completion', not %r" % (objective,))
-    return _lib.FLAG_SUM_COMPLETION if objective == "completion" else 0
+        raise SolverError("objective must be one of %s, not %r" % (", ".join(map(repr, OBJECTIVES)), objective))
+    if objective == "makespan":
+        return 0
+    return _lib.FLAG_SUM_COMPLETION | (_lib.FLAG_WEIGHTED if objective == "weighted_completion" else 0)
+
+
+def weights_f32(w, J: int) -> np.ndarray:
+    """J job weights as fp32 (round to nearest).  Every weight must be finite and > 0, and stay so in fp32 (a
+    value that rounds to 0 or to inf is refused); raises SolverError otherwise."""
+    from .solver import SolverError
+    try:
+        w64 = np.asarray(w, dtype=np.float64)
+    except (TypeError, ValueError) as e:
+        raise SolverError("weights must be numbers: %s" % e)
+    if w64.shape != (J,):
+        raise SolverError("weights must have one value per task (%d), got shape %s" % (J, w64.shape))
+    if not (np.isfinite(w64).all() and (w64 > 0).all()):
+        raise SolverError("every weight must be finite and > 0")
+    with np.errstate(over="ignore", under="ignore"):
+        w32 = w64.astype(np.float32)
+    if not (np.isfinite(w32).all() and (w32 > 0).all()):
+        raise SolverError("every weight must stay finite and > 0 in fp32 (a weight rounds to 0 or to inf)")
+    return w32
 
 
 def _flags(integer_starts: bool, reduced: bool, objective: str = "makespan") -> int:
@@ -56,6 +78,7 @@ class Engine:
         self.G = 0
         self.gcount = None
         self.nodes = 1
+        self.weights = None  # fp32 job weights of objective="weighted_completion" (set_weights)
 
     # ------------------------------------------------------------------ lifecycle
     def close(self):
@@ -99,6 +122,19 @@ class Engine:
         self.J, self.S, self.G = int(J), int(S), int(G)
         self.gcount = [int(x) for x in gc]
         self.nodes = int(nodes)
+        self.weights = None  # sb_set_table clears them
+        return self
+
+    def set_weights(self, w) -> "Engine":
+        """Per-job weights (J values, finite and > 0, converted to fp32) for objective="weighted_completion", which
+        scores sum_j w_j (start_j + rt_j).  None clears them; set_table clears them too."""
+        if w is None:
+            check(self._lib.sb_set_weights(self._h, None, 0))
+            self.weights = None
+            return self
+        w32 = np.ascontiguousarray(weights_f32(w, self.J))
+        check(self._lib.sb_set_weights(self._h, C.c_void_p(w32.ctypes.data), int(self.J)))
+        self.weights = w32
         return self
 
     def reduced_table(self) -> Tuple[np.ndarray, np.ndarray]:
@@ -437,6 +473,14 @@ class MultiEngine:
 
     def reduced_table(self):
         return self.engines[0].reduced_table()
+
+    def set_weights(self, w):
+        """Engine.set_weights on every device."""
+        for e in self.engines:
+            e.set_weights(w)
+        return self
+
+    weights = property(lambda self: self.engines[0].weights)
 
     def decode(self, *a, **kw):
         return self.engines[0].decode(*a, **kw)

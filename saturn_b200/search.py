@@ -43,14 +43,21 @@ def key_makespan(key: int) -> float:
     return float(np.array([(key >> 32) & 0xffffffff], dtype=np.uint32).view(np.float32)[0])
 
 
-def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objective: str = "makespan"):
+def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objective: str = "makespan",
+              weights: Optional[np.ndarray] = None):
     """Heuristic warm candidates in the reduced encoding (opt byte = k-1, plus node << 3 when there
     are several nodes), longest-processing-time order: (a) every job on its fastest option,
     (b) every job on its least GPU-seconds option, (c) in between.  Nodes are filled greedily by
     accumulated GPU-seconds.  objective="completion": shortest-processing-time order instead (ascending
     runtime of the chosen option), the order that favours the sum of completion times; same options and
-    node fill (sb_search_seed_lpt plants the same seeds)."""
+    node fill (sb_search_seed_lpt plants the same seeds).  objective="weighted_completion" with the fp32 job
+    `weights`: WSPT order (Smith's rule), ascending runtime / weight in float64, ties by job index — for unit
+    weights exactly the shortest-processing-time order."""
     objective_flag(objective)
+    if objective == "weighted_completion":
+        if weights is None:
+            raise ValueError("objective='weighted_completion' needs the job weights")
+        w64 = np.asarray(weights, dtype=np.float32).astype(np.float64)
     J = tmin.shape[0]
     usable = np.where(tmin < sentinel, tmin, np.inf)
     if not np.isfinite(usable).any(axis=1).all():
@@ -61,7 +68,9 @@ def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objecti
         cost = usable.astype(np.float64) * (k ** area_weight)
         col = np.argmin(cost, axis=1)
         rt = usable[np.arange(J), col]
-        if objective == "completion":
+        if objective == "weighted_completion":
+            order = np.argsort(rt.astype(np.float64) / w64, kind="stable")
+        elif objective == "completion":
             order = np.argsort(rt, kind="stable")
         else:
             order = np.argsort(-rt * (col + 1) ** 0.5, kind="stable")
@@ -87,7 +96,8 @@ def run_search(engine: Engine, chains: int = 1 << 16, rounds: int = 200, seed: i
                _extra_flags: int = 0, objective: str = "makespan") -> SearchResult:
     """Run the search on `engine` (table already set).  Returns the best candidate found by any rank.
     objective="completion" minimises the sum of completion times; the result's `makespan`, the history and
-    `target_makespan` then hold / target that sum.
+    `target_makespan` then hold / target that sum.  objective="weighted_completion" minimises the sum weighted by
+    the engine's set_weights.
 
     `rounds` device rounds are issued in groups of `exchange_every` (tournament resampling every
     `resample_every` rounds inside a group is only another launch); after each group the ranks exchange
@@ -123,7 +133,8 @@ def run_search(engine: Engine, chains: int = 1 << 16, rounds: int = 200, seed: i
         tmin, args = engine.reduced_table()
         per = max(1, chains // 8)
         nodes = getattr(engine, "nodes", 1)
-        for i, (col, order) in enumerate(lpt_seeds(tmin, nodes=nodes, objective=objective)):
+        for i, (col, order) in enumerate(lpt_seeds(tmin, nodes=nodes, objective=objective,
+                                                   weights=getattr(engine, "weights", None))):
             opt = col if reduced else ((args[np.arange(J), col & 7].astype(np.uint8) << 3) | col)
             first = min(i * per, max(0, chains - per))
             engine.search_inject(opt.astype(np.uint8), order.astype(pdt), copies=min(per, chains), first=first)

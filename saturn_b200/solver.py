@@ -23,6 +23,7 @@ import math
 import os
 import time
 from collections import defaultdict
+from collections.abc import Mapping
 from typing import List, Optional, Sequence
 
 import numpy as np
@@ -220,6 +221,30 @@ def _check_objective(objective, hysteresis=False):
                           "objective='completion'")
 
 
+def _resolve_weights(weights, objective, J, task_list=None):
+    """The caller's per-task weights as (float64 values in task order, fp32 array for the device), or (None, None).
+    A sequence is aligned with the tasks (or T's rows); with `task_list`, a mapping keyed by Task is accepted too —
+    what an orchestrate() loop needs, since its task list shrinks every interval.  Raises SolverError before any
+    device call."""
+    if weights is None:
+        return None, None
+    if objective != "completion":
+        raise SolverError("weights apply to objective='completion' only (the weighted sum of completion times), "
+                          "not to %r" % (objective,))
+    if isinstance(weights, Mapping):
+        if task_list is None:
+            raise SolverError("weights must be a sequence aligned with T's rows")
+        missing = [getattr(t, "name", repr(t)) for t in task_list if t not in weights]
+        if missing:
+            raise SolverError("weights has no entry for task(s) %s" % ", ".join(map(str, missing[:5])))
+        weights = [weights[t] for t in task_list]
+    elif isinstance(weights, (str, bytes)) or not hasattr(weights, "__len__"):
+        raise SolverError("weights must be a sequence of J numbers or a mapping Task -> number")
+    from .engine import weights_f32
+    w32 = weights_f32(weights, J)
+    return [float(x) for x in weights], w32
+
+
 def _plan_horizon(start, rt):
     """max(start + rt) of a decoded plan: the latest time the device's fp32 schedule holds.  With the
     sum-of-completion-times objective the device's score is a sum that may exceed 2^24 while every start is
@@ -243,7 +268,7 @@ def _default_nodes() -> int:
 def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count() or 4) // 4), interval=1000,
           timeout=500, *, chains: Optional[int] = None, rounds: Optional[int] = None, seed: int = 0,
           integer_starts: bool = True, engine=None, hysteresis: Optional[bool] = None,
-          nodes: Optional[int] = None, devices=None, objective: str = "makespan"):
+          nodes: Optional[int] = None, devices=None, objective: str = "makespan", weights=None):
     """Drop-in for saturn.solver.solve (milp.py:23).
 
     Objective.  "makespan" (the default, the reference's) or "completion": minimise the sum of the tasks'
@@ -253,6 +278,14 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     objective and last_stats["total_completion"] holds the plan's sum of completion times, recomputed in
     float64 from the emitted plan and the tasks' own runtimes; last_stats["device_makespan"] is the device's
     fp32 score of the plan (the sum, under "completion").  Anything else raises SolverError.
+
+    Weights.  With objective="completion", `weights` (a sequence aligned with task_list, or a mapping keyed by
+    Task, which survives orchestrate()'s shrinking task list) makes the objective the weighted sum
+    sum_t w_t (start_t + runtime_t): a job's priority.  Every weight must be finite and > 0, and stay so in fp32;
+    anything else, weights under objective="makespan", a wrong length or a task missing from the mapping raises
+    SolverError before any device call.  last_stats["weighted_completion"] then holds the plan's weighted sum in
+    float64 (the caller's weights, the tasks' own runtimes) and last_stats["device_makespan"] the device's fp32
+    weighted sum; "total_completion" and the 6th element keep their meaning.
 
     Returns (sta, tga, bss, bna, boa, makespan) — milp.py:445 — with a real float makespan
     (the reference returns None on a cold start, milp.py:394-399; callers only thread it back in
@@ -282,6 +315,7 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     t_wall = time.perf_counter()
     task_list = list(task_list)
     J = len(task_list)
+    w64, w32 = _resolve_weights(weights, objective, J, task_list)
     if J == 0:
         return [[[] for _ in range(NSLOT)]], [], [], [], [], 0.0
     eng = engine if engine is not None else _engine(devices)
@@ -297,6 +331,10 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
         nodes = _default_nodes()
     nodes = int(nodes)
     eng.set_table(Tdev, list(range(1, NSLOT + 1)), sentinel=float("inf"), nodes=nodes)
+    search_objective = objective
+    if w32 is not None:
+        eng.set_weights(w32)
+        search_objective = "weighted_completion"
     if chains is None:
         chains = int(os.environ.get("SATURN_B200_CHAINS", 0))
         if chains <= 0:
@@ -313,7 +351,7 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     warm = candidate_from_arrays(task_list, presolved, nodes)
     res = run_search(eng, chains=chains, rounds=rounds, seed=seed, integer_starts=integer_starts, reduced=True,
                      time_budget_s=budget, patience=max(40, rounds // 4), warm=warm,
-                     **({"objective": objective} if objective != "makespan" else {}))
+                     **({"objective": search_objective} if search_objective != "makespan" else {}))
     if objective == "makespan":
         _check_horizon(Tdev, res.makespan)
     dec = eng.decode(res.opt, res.prio, integer_starts=integer_starts, reduced=True)
@@ -339,6 +377,8 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
                   "nodes": nodes, "devices": len(getattr(eng, "engines", [eng])),
                   "total_wall_s": None, "adopted": True, "objective": objective,
                   "total_completion": sum(float(dec["start"][i]) + float(rts[i]) for i in range(J))}
+    if w64 is not None:
+        last_stats["weighted_completion"] = sum(w64[i] * (float(dec["start"][i]) + float(rts[i])) for i in range(J))
 
     # ---- introspection hysteresis (opt-in): the documented intent of milp.py:363-442
     out = prop + (prop_makespan,)
@@ -434,9 +474,10 @@ def strategies_from_table(T, mask, executors=None, params=None, gcount=None):
 def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeout=500, *,
                 chains: Optional[int] = None, rounds: Optional[int] = None, seed: int = 0,
                 integer_starts: bool = True, engine=None, nodes: Optional[int] = None, devices=None,
-                objective: str = "makespan"):
+                objective: str = "makespan", weights=None):
     """solve() on the dense profiler tensor T[J][S][G] (+ mask of usable cells, + gcount[G] GPU counts).
-    `objective` as for solve(): "makespan" or "completion" (sum of completion times).
+    `objective` as for solve(): "makespan" or "completion" (sum of completion times); `weights` as for solve(),
+    a sequence aligned with T's rows (the weighted sum of completion times, last_stats["weighted_completion"]).
 
     The table goes to the device un-reduced (sb_set_table: min over strategies with the first-minimum rule
     and its arg-min on the device, PerformanceEvaluator.py:101-115); the search runs on the reduced view
@@ -451,6 +492,7 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     if T.ndim != 3:
         raise SolverError("T must be [J][S][G]")
     J, S, G = T.shape
+    w64, w32 = _resolve_weights(weights, objective, J)
     if J == 0:
         return [[[] for _ in range(NSLOT)]], [], [], [], [], 0.0, np.zeros(0, dtype=np.int64)
     gcount = list(range(1, G + 1)) if gcount is None else [int(g) for g in gcount]
@@ -468,6 +510,10 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     eng = engine if engine is not None else _engine(devices)
     nodes = int(_default_nodes() if nodes is None else nodes)
     eng.set_table(Tdev, gcount, sentinel=float("inf"), nodes=nodes)
+    search_objective = objective
+    if w32 is not None:
+        eng.set_weights(w32)
+        search_objective = "weighted_completion"
     if chains is None:
         chains = int(os.environ.get("SATURN_B200_CHAINS", 0))
         if chains <= 0:
@@ -484,7 +530,7 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
         warm = candidate_from_arrays([_Opt] * J, presolved, nodes)
     res = run_search(eng, chains=chains, rounds=rounds, seed=seed, integer_starts=integer_starts, reduced=True,
                      time_budget_s=budget, patience=max(40, rounds // 4), warm=warm,
-                     **({"objective": objective} if objective != "makespan" else {}))
+                     **({"objective": search_objective} if search_objective != "makespan" else {}))
     if objective == "makespan":
         _check_horizon(Tdev, res.makespan)
     dec = eng.decode(res.opt, res.prio, integer_starts=integer_starts, reduced=True)
@@ -503,6 +549,8 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
                   "device_makespan": res.makespan, "makespan": makespan, "J": J, "chains": chains, "nodes": nodes,
                   "devices": len(getattr(eng, "engines", [eng])), "total_wall_s": None, "adopted": True,
                   "objective": objective, "total_completion": sum(float(dec["start"][j]) + rts[j] for j in range(J))}
+    if w64 is not None:
+        last_stats["weighted_completion"] = sum(w64[j] * (float(dec["start"][j]) + rts[j]) for j in range(J))
     return arrays + (makespan, strategy)
 
 

@@ -1,12 +1,14 @@
-"""Cost and effect of the sum-of-completion-times objective on one GPU; prints one JSON line.
+"""Cost and effect of the sum-of-completion-times objectives (plain and weighted) on one GPU; prints one JSON line.
 
     python scripts/bench_objective.py [--steps 200] [--warmup 20] [--solve-chains 0] [--solve-rounds 400]
 
 kernel: sb_eval on bench.py's C4 batch (J = 256, S = 8, 946,176 candidates, the same seeded inputs, integer
-        starts), scored for the makespan and for the sum of completion times, the two launches alternated in one
-        process and timed with CUDA events; median of --steps launches each.
-solve:  solve() wall time on a 256-task set (synthetic table, seed 3, 4 strategies) for both objectives, each plan
-        scored on both objectives (float64, the tasks' own runtimes).
+        starts), scored for the makespan, the sum of completion times and the weighted sum (seeded weights), the
+        three launches alternated in one process (the order rotates every step) and timed with CUDA events; median
+        of --steps launches each.
+solve:  solve() wall time on a 256-task set (synthetic table, seed 3, 4 strategies) for the makespan, the sum of
+        completion times and the weighted sum (seeded weights: 32 tasks of weight 8, the rest 1), each plan scored
+        on all three measures (float64, the tasks' own runtimes).
 The card's name and power limit are read in the same run (nvidia-smi, read-only queries).
 """
 import argparse
@@ -41,6 +43,7 @@ def main():
     args = ap.parse_args()
     import numpy as np
     import torch
+    from oracle import ref_eval as R
     from saturn_b200 import solver as S
     from saturn_b200.engine import Engine, random_candidates
     from saturn_b200.synth import synth_table
@@ -51,11 +54,13 @@ def main():
     T, valid = synth_table(J, Sx, G, seed=0)
     eng.set_table(T)
     opt, prio = random_candidates(eng, B, valid, seed=1)
+    eng.set_weights(np.random.default_rng(2).choice([1.0, 2.0, 3.0, 5.0, 8.0, 0.25, 0.5, 1.5], size=J))
     out = torch.empty(B, dtype=torch.float32, device=eng.device)
     key = torch.full((1,), 2 ** 63 - 1, dtype=torch.int64, device=eng.device)
-    times = {"makespan": [], "completion": []}
+    objs = ("makespan", "completion", "weighted_completion")
+    times = {o: [] for o in objs}
     for i in range(args.warmup + args.steps):
-        for obj in ("makespan", "completion") if i % 2 == 0 else ("completion", "makespan"):
+        for obj in objs[i % 3:] + objs[:i % 3]:
             a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             a.record()
             eng.eval(opt, prio, out=out, best_key=key, objective=obj)
@@ -68,6 +73,7 @@ def main():
                   "p90_ms": float(np.percentile(t, 90)), "candidates_per_s": B / (float(np.median(t)) * 1e-3)}
               for o, t in times.items()}
     kernel["completion_over_makespan"] = kernel["completion"]["median_ms"] / kernel["makespan"]["median_ms"]
+    kernel["weighted_over_completion"] = kernel["weighted_completion"]["median_ms"] / kernel["completion"]["median_ms"]
     kernel.update(B=B, J=J, S=Sx, path=path, steps=args.steps)
     del opt, prio, out
     torch.cuda.empty_cache()
@@ -89,15 +95,23 @@ def main():
         kw["chains"] = args.solve_chains
     S.solve(tasks, None, rounds=4, engine=eng)               # first launches load the kernels
     S.solve(tasks, None, rounds=4, engine=eng, objective="completion")
+    w = [8.0 if j % 8 == 0 else 1.0 for j in range(len(tasks))]
+    S.solve(tasks, None, rounds=4, engine=eng, objective="completion", weights=w)
     solve = {}
-    for obj in ("makespan", "completion"):
+    for name, obj, weights in (("makespan", "makespan", None), ("completion", "completion", None),
+                               ("weighted_completion", "completion", w)):
         t0 = time.perf_counter()
-        res = S.solve(tasks, None, objective=obj, **kw)
+        res = S.solve(tasks, None, objective=obj, weights=weights, **kw)
         wall = time.perf_counter() - t0
         st = S.last_stats
-        solve[obj] = {"wall_s": wall, "makespan": res[5], "total_completion": st["total_completion"],
-                      "mean_completion": st["total_completion"] / len(tasks), "rounds": st["rounds"],
-                      "candidates": st["candidates"]}
+        # the plan scored on all three measures, in float64 from its starts and the tasks' own runtimes
+        tuples = [[(g, s.runtime) for g, s in t.strategies.items()] for t in tasks]
+        comp = [p[0] + p[2] for p in R.plan_from_arrays(tuples, res[0], res[1], res[2], res[3])]
+        solve[name] = {"wall_s": wall, "makespan": res[5], "total_completion": st["total_completion"],
+                       "mean_completion": st["total_completion"] / len(tasks),
+                       "weighted_completion": sum(wi * c for wi, c in zip(w, comp)),
+                       "heavy_mean_completion": float(np.mean([c for wi, c in zip(w, comp) if wi > 1])),
+                       "rounds": st["rounds"], "candidates": st["candidates"]}
     print(json.dumps({"card": card(0), "kernel": kernel, "solve": solve}))
     eng.close()
 
