@@ -48,6 +48,12 @@
  *   total = sum_j w_j (start_j + rt_j), acc = acc + (w_j * (start_j + rt_j)) from +0 in schedule order, with TWO
  * fp32 roundings per job (the product, then the sum; never one fused multiply-add).  w = 1 gives exactly the
  * unweighted fold, w = 2 exactly twice it (barring overflow).
+ * With SB_FLAG_DUE as well (per-job due dates d_j, sb_set_due; unit weights unless SB_FLAG_WEIGHTED) it is the
+ * weighted tardiness:
+ *   total = sum_j w_j max(0, start_j + rt_j - d_j), from +0 in schedule order per job: e = start + rt (as above),
+ *   l = e - d, t = max(l, +0), acc = acc + (w * t), every step rounded on its own (no fused or reassociated step).
+ * d = 0 gives exactly the weighted fold, due dates at or past every completion give +0, w = 2 exactly twice w = 1.
+ * The score is >= +0, so the (bits << 32) | id key still orders by it.
  * The schedule, every start and every slot mask are the same under every objective.
  * With integer_starts the slot state is the integer time a slot becomes usable, start + ceil(rt);
  * SURVEY.md §8a writes the same rule as `start = ceil(max ready)` over real-valued ready times.  Starts,
@@ -117,6 +123,17 @@ typedef enum sb_status {
                                      search's temperature unit becomes the incumbent's weighted sum / sum_j w_j, and
                                      sb_search_seed_lpt plants WSPT orders (Smith's rule: ascending rt / w, ties by
                                      job index).  Not available with SB_FLAG_ALT_WARPSCAN (SB_ERR_UNSUPPORTED). */
+#define SB_FLAG_DUE 256u           /* with SB_FLAG_SUM_COMPLETION only (else SB_ERR_ARG), after sb_set_due (else
+                                     SB_ERR_STATE): the objective is the total tardiness against the due dates,
+                                     weighted by the weights with SB_FLAG_WEIGHTED as well (see the evaluation rule
+                                     above).  Accepted wherever SB_FLAG_WEIGHTED is, sb_search_run_multi included
+                                     (every handle must hold due dates); every score the library emits then holds
+                                     the tardiness.  The search's temperature unit becomes max(incumbent / sum_j w_j,
+                                     sum_j w_j min_k rt_jk / sum_j w_j) (the second term: the weighted mean of each
+                                     job's smallest proposable runtime), sb_search_run stops as soon as the
+                                     incumbent is +0 (stop_reason 3), and sb_search_seed_lpt plants EDD orders
+                                     (ascending due date, ties by runtime / weight, then job index).  Not available
+                                     with SB_FLAG_ALT_WARPSCAN (SB_ERR_UNSUPPORTED). */
 #define SB_IPC_HANDLE_BYTES 64
 
 typedef struct sb_handle sb_handle;
@@ -150,6 +167,11 @@ int sb_set_sentinel(sb_handle* h, float threshold);
  * that differs from the table's); w = NULL clears them.  SB_ERR_STATE before sb_set_table.  sb_set_table clears
  * the weights; setting or clearing them ends the current search (sb_search_init again). */
 int sb_set_weights(sb_handle* h, const float* w, int J);
+/* Per-job due dates for SB_FLAG_DUE: d host fp32 [J] in the runtimes' units from the plan's t = 0, every value
+ * finite with |d| < 2^24 (negative: already overdue) (else SB_ERR_ARG, as is a J that differs from the table's);
+ * d = NULL clears them.  SB_ERR_STATE before sb_set_table.  sb_set_table clears the due dates; setting or clearing
+ * them ends the current search (sb_search_init again). */
+int sb_set_due(sb_handle* h, const float* d, int J);
 /* copy the reduced table back (host pointers, either may be NULL): tmin fp32 [J][8], args u8 [J][8].
  * This is the table the reference solver is actually given: Task.strategies[g] after the profiler's
  * min over executors (PerformanceEvaluator.py:101-115), read at milp.py:77-81. */
@@ -245,7 +267,7 @@ typedef struct sb_search_params {
   unsigned flags;       /* SB_FLAG_* */
   float t_start;        /* initial temperature as a fraction of the incumbent makespan (SB_FLAG_SUM_COMPLETION:
                          * of the incumbent's mean completion time, its sum / J; with SB_FLAG_WEIGHTED its
-                         * weighted sum / the sum of the weights) */
+                         * weighted sum / the sum of the weights; with SB_FLAG_DUE the unit of SB_FLAG_DUE) */
   float t_end;          /* final temperature fraction */
   int total_rounds;     /* cooling horizon */
   int resample_every;   /* > 0: sb_search_round itself resamples the population by tournament before every round r
@@ -278,7 +300,8 @@ int sb_search_resample(sb_handle* h);
  * least GPU-seconds option / in between; nodes filled greedily by GPU-seconds) into an eighth of the
  * population each and scores them; with SB_FLAG_SUM_COMPLETION the orders are shortest-processing-time
  * instead (ascending runtime of the chosen option), with SB_FLAG_WEIGHTED as well WSPT orders (ascending runtime / weight,
- * ties by job index), same options and node fill.  sb_search_run = sb_search_init + seeds + `rounds` rounds in groups of
+ * ties by job index), with SB_FLAG_DUE EDD orders (ascending due date, ties by runtime / weight, then job index),
+ * same options and node fill.  sb_search_run = sb_search_init + seeds + `rounds` rounds in groups of
  * `sync_every` (tournament resampling every `resample_every` rounds inside a group is only another launch;
  * the host reads the incumbent key once per group and applies the stopping rules) + sb_search_best.
  * The multi-GPU driver (saturn_b200/search.py) runs the same steps with a key exchange per group. */
@@ -302,7 +325,8 @@ typedef struct sb_search_result {
   uint64_t key;        /* (float bits << 32) | global chain id of the incumbent */
   int64_t evaluated;   /* candidates scored */
   int rounds;          /* rounds run */
-  int stop_reason;     /* 0 rounds exhausted, 1 time budget, 2 patience, 3 target reached */
+  int stop_reason;     /* 0 rounds exhausted, 1 time budget, 2 patience, 3 target reached (SB_FLAG_DUE: also a
+                        * score of +0, which no plan can beat) */
   double wall_s;
 } sb_search_result;
 int sb_search_seed_lpt(sb_handle* h);

@@ -41,7 +41,7 @@ struct SearchState {
   SearchDev d;
   sb_search_params p;
   float scale = 0.f;  // temperature unit: incumbent makespan after initialisation (SB_FLAG_SUM_COMPLETION: sum / J;
-                      // with SB_FLAG_WEIGHTED: weighted sum / sum of the weights)
+                      // with SB_FLAG_WEIGHTED: weighted sum / sum of the weights; SB_FLAG_DUE: see sb_search_init)
   long long evaluated = 0;
   int rounds_done = 0;
   bool fused_ok = true;  // run rounds with the fused kernel while its tiles fit
@@ -59,7 +59,8 @@ struct SearchState {
   unsigned long long* verify_bad = nullptr;
   bool win = false, inc = false, verify = false;
   SearchDev alloc;  // the pointers as allocated (s.d's cur / prop pairs trade places when resampling)
-  const float* w = nullptr;  // SB_FLAG_WEIGHTED: the handle's job weights (position-major kernels)
+  const float* w = nullptr;    // SB_FLAG_WEIGHTED: the handle's job weights (SB_FLAG_DUE alone: its unit weights)
+  const float* due = nullptr;  // SB_FLAG_DUE: the handle's due dates (position-major kernels)
 };
 
 struct sb_handle {
@@ -99,6 +100,13 @@ struct sb_handle {
   std::vector<float> h_w;
   double w_sum = 0.0;
   bool has_w = false;
+  // due dates (sb_set_due): device copy padded like d_w, J unit weights for SB_FLAG_DUE without SB_FLAG_WEIGHTED,
+  // and the host copy (EDD seeds); has_d is cleared by sb_set_table
+  float* d_d = nullptr;
+  float* d_one = nullptr;
+  size_t d_d_cap = 0;
+  std::vector<float> h_d;
+  bool has_d = false;
   SearchState search;
   int last_path = -1;
   // peer-memory exchange
@@ -210,6 +218,8 @@ int sb_destroy(sb_handle* h) {
   cudaFree(h->dec_buf);
   cudaFree(h->stage_T);
   cudaFree(h->d_w);
+  cudaFree(h->d_d);
+  cudaFree(h->d_one);
   for (int i = 0; i < 2; ++i)
     if (h->hs[i]) cudaStreamDestroy(h->hs[i]);
   if (h->own_stream && h->stream) cudaStreamDestroy(h->stream);
@@ -240,6 +250,7 @@ int sb_set_table(sb_handle* h, const float* T, const uint8_t* gcount, int J, int
   CK(cudaStreamSynchronize(h->stream));
   h->search.ready = false;  // its buffers are reused by the next sb_search_init if the shape is unchanged
   h->has_w = false;         // weights belong to a task set: a new table needs new ones
+  h->has_d = false;         // so do due dates
   const size_t nT = static_cast<size_t>(J) * S * G;
   const size_t ntab = static_cast<size_t>(J) * S * kSlots;
   // a re-planning loop sets a table of the same shape every interval: keep the allocations (cudaFree /
@@ -337,13 +348,59 @@ int sb_set_weights(sb_handle* h, const float* w, int J) {
   return SB_OK;
 }
 
-// SB_FLAG_WEIGHTED is valid with SB_FLAG_SUM_COMPLETION and after sb_set_weights only
-static int check_weighted(const sb_handle* h, unsigned flags) {
-  if (!(flags & SB_FLAG_WEIGHTED)) return SB_OK;
-  if (!(flags & SB_FLAG_SUM_COMPLETION))
-    return fail(SB_ERR_ARG, "SB_FLAG_WEIGHTED weights the sum of completion times: it needs SB_FLAG_SUM_COMPLETION");
-  if (!h->has_w) return fail(SB_ERR_STATE, "SB_FLAG_WEIGHTED needs sb_set_weights (sb_set_table clears the weights)");
+int sb_set_due(sb_handle* h, const float* d, int J) {
+  int rc = use_device(h);
+  if (rc) return rc;
+  if (h->J == 0) return fail(SB_ERR_STATE, "sb_set_table has not been called");
+  CK(cudaStreamSynchronize(h->stream));  // no queued kernel may still read the old due dates
+  h->search.ready = false;               // the running search was set up for the old due dates (scale, seeds)
+  if (!d) {
+    h->has_d = false;
+    return SB_OK;
+  }
+  if (J != h->J) return fail(SB_ERR_ARG, "J=%d differs from the table's J=%d", J, h->J);
+  for (int j = 0; j < J; ++j)
+    if (!isfinite(d[j]) || !(fabsf(d[j]) < 16777216.f))
+      return fail(SB_ERR_ARG, "due date %d (%g) is not finite with |d| < 2^24", j, d[j]);
+  h->has_d = false;
+  const size_t cap = static_cast<size_t>((J + 3) & ~3);
+  if (h->d_d_cap < cap) {
+    cudaFree(h->d_d);
+    cudaFree(h->d_one);
+    h->d_d = h->d_one = nullptr;
+    h->d_d_cap = 0;
+    CK(cudaMalloc(&h->d_d, cap * sizeof(float)));
+    CK(cudaMalloc(&h->d_one, cap * sizeof(float)));
+    h->d_d_cap = cap;
+  }
+  std::vector<float> one(cap, 0.f);
+  std::fill(one.begin(), one.begin() + J, 1.f);
+  h->h_d.assign(d, d + J);
+  h->h_d.resize(cap, 0.f);
+  CK(cudaMemcpyAsync(h->d_d, h->h_d.data(), cap * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+  CK(cudaMemcpyAsync(h->d_one, one.data(), cap * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  h->has_d = true;
   return SB_OK;
+}
+
+// SB_FLAG_WEIGHTED and SB_FLAG_DUE are valid with SB_FLAG_SUM_COMPLETION only, and after sb_set_weights /
+// sb_set_due respectively
+static int check_per_job(const sb_handle* h, unsigned flags) {
+  if ((flags & SB_FLAG_WEIGHTED) && !(flags & SB_FLAG_SUM_COMPLETION))
+    return fail(SB_ERR_ARG, "SB_FLAG_WEIGHTED weights the sum of completion times: it needs SB_FLAG_SUM_COMPLETION");
+  if ((flags & SB_FLAG_DUE) && !(flags & SB_FLAG_SUM_COMPLETION))
+    return fail(SB_ERR_ARG, "SB_FLAG_DUE scores the tardiness of the completion times: it needs SB_FLAG_SUM_COMPLETION");
+  if ((flags & SB_FLAG_WEIGHTED) && !h->has_w)
+    return fail(SB_ERR_STATE, "SB_FLAG_WEIGHTED needs sb_set_weights (sb_set_table clears the weights)");
+  if ((flags & SB_FLAG_DUE) && !h->has_d)
+    return fail(SB_ERR_STATE, "SB_FLAG_DUE needs sb_set_due (sb_set_table clears the due dates)");
+  return SB_OK;
+}
+// the weights the kernels read: the caller's, the unit weights of SB_FLAG_DUE alone, or none
+static const float* job_weights(const sb_handle* h, unsigned flags) {
+  if (flags & SB_FLAG_WEIGHTED) return h->d_w;
+  return (flags & SB_FLAG_DUE) ? h->d_one : nullptr;
 }
 
 int sb_get_reduced(sb_handle* h, float* tmin, uint8_t* args) {
@@ -362,7 +419,7 @@ static int make_call(sb_handle* h, const uint8_t* opt, const void* prio, int64_t
   if (B < 0) return fail(SB_ERR_ARG, "B=%lld is negative", static_cast<long long>(B));
   if (B > 0 && (!opt || !prio)) return fail(SB_ERR_ARG, "opt / prio is null");
   if (row_stride < h->J) return fail(SB_ERR_ARG, "row_stride=%lld < J=%d", static_cast<long long>(row_stride), h->J);
-  if (int rc = check_weighted(h, flags)) return rc;
+  if (int rc = check_per_job(h, flags)) return rc;
   if (B > 0xffffffffll) return fail(SB_ERR_ARG, "B=%lld exceeds 2^32-1 candidates per call", static_cast<long long>(B));
   const int pb = h->J <= 256 ? 1 : 2;
   const bool reduced = (flags & SB_FLAG_REDUCED) != 0;
@@ -379,7 +436,8 @@ static int make_call(sb_handle* h, const uint8_t* opt, const void* prio, int64_t
   c->stride_o = row_stride;
   c->stride_p = row_stride * pb;
   c->flags = flags;
-  c->w = (flags & SB_FLAG_WEIGHTED) ? h->d_w : nullptr;
+  c->w = job_weights(h, flags);
+  c->d = (flags & SB_FLAG_DUE) ? h->d_d : nullptr;
   return SB_OK;
 }
 
@@ -438,9 +496,9 @@ int sb_eval(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, int64
     }
   }
   if (flags & SB_FLAG_ALT_WARPSCAN) {
-    if (flags & (SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED))
+    if (flags & (SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED | SB_FLAG_DUE))
       return fail(SB_ERR_UNSUPPORTED, "SB_FLAG_ALT_WARPSCAN scores the makespan only: it cannot be combined with "
-                  "SB_FLAG_SUM_COMPLETION or SB_FLAG_WEIGHTED");
+                  "SB_FLAG_SUM_COMPLETION, SB_FLAG_WEIGHTED or SB_FLAG_DUE");
     if (flags & (SB_FLAG_POST_KEY | SB_FLAG_FOLD_PREV))
       return fail(SB_ERR_UNSUPPORTED, "SB_FLAG_ALT_WARPSCAN cannot be combined with the fused key exchange");
     cudaError_t e = eval_alt_launch(h->dev, c, h->stream);
@@ -768,7 +826,7 @@ static int search_eval(sb_handle* h, bool cur_rows, long long first, long long c
     SearchFuse sf = {};
     sf.cur_mk = s.d.cur_mk;
     const bool reduced = (s.p.flags & SB_FLAG_REDUCED) != 0;
-    CK(search_pos_launch(h->dev, s.d, reduced ? h->tmin : h->tab, s.w, (reduced ? 1 : h->S) * kSlots, s.p.flags, first,
+    CK(search_pos_launch(h->dev, s.d, reduced ? h->tmin : h->tab, s.w, s.due, (reduced ? 1 : h->S) * kSlots, s.p.flags, first,
                          count, true, sf, h->stream));
     return SB_OK;
   }
@@ -790,7 +848,7 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
   if (h->J == 0) return fail(SB_ERR_STATE, "sb_set_table has not been called");
   if (!p) return fail(SB_ERR_ARG, "params is null");
   if (p->chains < 1 || p->chains > (1ll << 31)) return fail(SB_ERR_ARG, "chains=%lld out of range", (long long)p->chains);
-  if ((rc = check_weighted(h, p->flags))) return rc;
+  if ((rc = check_per_job(h, p->flags))) return rc;
   CK(cudaStreamSynchronize(h->stream));
   SearchState& s = h->search;
   s.ready = false;
@@ -806,7 +864,10 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
   d.chain_base = p->chain_base;
   d.seed = p->seed;
   const bool weighted = (p->flags & SB_FLAG_WEIGHTED) != 0;
-  s.w = weighted ? h->d_w : nullptr;
+  const bool due = (p->flags & SB_FLAG_DUE) != 0;
+  const int arrays = job_arrays(p->flags);
+  s.w = job_weights(h, p->flags);
+  s.due = due ? h->d_d : nullptr;
   d.stride_o = (J + 31) & ~31;  // 32-byte rows: TMA bulk copies for opt, 256-bit streaming loads for prio
   // make stride_p == stride_o * pb so that one element stride describes both (sb_eval contract)
   d.stride_p = d.stride_o * pb;
@@ -846,8 +907,8 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
   // Rows that do not fit in shared memory: keep the population in schedule order and stream both rows.
   const int SGs = (reduced ? 1 : h->S) * kSlots;
   const bool no_fused = (p->flags & HOOK_NO_FUSED) != 0;
-  const int mode = search_round_mode(h->dev, J, SGs, h->nodes, weighted);
-  d.pos = (!no_fused && mode != 2 && search_pos_smem(J, SGs, h->nodes, 16, weighted) <= h->dev.smem_optin) ? 1 : 0;
+  const int mode = search_round_mode(h->dev, J, SGs, h->nodes, arrays);
+  d.pos = (!no_fused && mode != 2 && search_pos_smem(J, SGs, h->nodes, 16, arrays) <= h->dev.smem_optin) ? 1 : 0;
   if (d.pos) CK(search_init_population_pos(d, h->stream));
   else CK(search_init_population(d, h->stream));
   s.ready = true;
@@ -876,6 +937,23 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
   // fraction of a typical score difference under every objective
   const float per = weighted ? static_cast<float>(h->w_sum) : static_cast<float>(J);
   s.scale = isfinite(mk) ? ((p->flags & SB_FLAG_SUM_COMPLETION) ? mk / per : mk) : 1.0f;
+  if (due && isfinite(mk)) {
+    // tardiness can be 0 or tiny at the incumbent: the unit is at least the weighted mean of each job's smallest
+    // proposable runtime, the size of the score change one move makes
+    const float* tmin = h->h_tmin.data();
+    double move = 0.0;
+    for (int j = 0; j < J; ++j) {
+      double lo = HUGE_VAL, lo_any = HUGE_VAL;
+      for (int k = 0; k < kSlots; ++k) {
+        const float v = tmin[j * kSlots + k];
+        if (v < h->sentinel) lo = std::min(lo, static_cast<double>(v));
+        if (isfinite(v)) lo_any = std::min(lo_any, static_cast<double>(v));
+      }
+      if (!isfinite(lo)) lo = lo_any;
+      if (isfinite(lo)) move += (weighted ? static_cast<double>(h->h_w[j]) : 1.0) * lo;
+    }
+    s.scale = std::max(s.scale, static_cast<float>(move / (weighted ? h->w_sum : static_cast<double>(J))));
+  }
   s.evaluated = d.chains;
   s.rounds_done = 0;
   s.launches = 0;
@@ -977,7 +1055,7 @@ int sb_search_round(sb_handle* h, int rounds) {
       SearchFuse sf = make_fuse(s, round, n);
       sf.resample_every = 0;
       const bool reduced = (s.p.flags & SB_FLAG_REDUCED) != 0;
-      CK(search_pos_launch(h->dev, s.d, reduced ? h->tmin : h->tab, s.w, (reduced ? 1 : h->S) * kSlots, s.p.flags, 0,
+      CK(search_pos_launch(h->dev, s.d, reduced ? h->tmin : h->tab, s.w, s.due, (reduced ? 1 : h->S) * kSlots, s.p.flags, 0,
                            s.d.chains, false, sf, h->stream));  // keeps the incumbent in its tail
       fused = true;
     } else if (s.fused_ok) {
@@ -1096,6 +1174,8 @@ int sb_search_seed_lpt(sb_handle* h) {
   const bool spt = (s.p.flags & SB_FLAG_SUM_COMPLETION) != 0;  // shortest first: the order that favours the sum
   // weighted sum: Smith's rule (WSPT), ascending rt / w; with unit weights exactly the SPT order
   const bool wspt = spt && (s.p.flags & SB_FLAG_WEIGHTED) != 0;
+  // tardiness: earliest due date first (EDD), ties by rt / w (rt with unit weights), then by job index
+  const bool edd = spt && (s.p.flags & SB_FLAG_DUE) != 0;
   const double INF = HUGE_VAL;
   // usable cells: below the sentinel threshold; a job with none falls back to any finite cell
   std::vector<double> usable(static_cast<size_t>(J) * kSlots);
@@ -1132,7 +1212,13 @@ int sb_search_seed_lpt(sb_handle* h) {
       weight[j] = rt[j] * sqrt(best + 1.0);
       order[j] = j;
     }
-    if (wspt) {
+    if (edd) {
+      for (int j = 0; j < J; ++j) weight[j] = wspt ? rt[j] / static_cast<double>(h->h_w[j]) : rt[j];
+      std::stable_sort(order.begin(), order.end(), [&](int a, int b) {
+        if (h->h_d[a] != h->h_d[b]) return h->h_d[a] < h->h_d[b];
+        return weight[a] < weight[b];
+      });
+    } else if (wspt) {
       for (int j = 0; j < J; ++j) weight[j] = rt[j] / static_cast<double>(h->h_w[j]);
       std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return weight[a] < weight[b]; });
     } else if (spt) std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return rt[a] < rt[b]; });
@@ -1277,9 +1363,11 @@ static int search_run_impl(sb_handle** hs, int n, const sb_search_params* p, con
   unsigned long long best = 0, key = 0;
   if ((rc = exchange(&best))) return rc;
   record(best);
-  int done = 0, stale = 0, reason = 0;
+  // SB_FLAG_DUE: a tardiness of +0 (key bits 0) cannot be beaten
+  const bool stop_at_zero = (p->flags & SB_FLAG_DUE) != 0;
+  int done = 0, stale = 0, reason = (stop_at_zero && (best >> 32) == 0) ? 3 : 0;
   bool first_group = true;
-  while (done < c->rounds) {
+  while (reason == 0 && done < c->rounds) {
     const int step = std::min(c->sync_every, c->rounds - done);
     for (int i = 0; i < n; ++i)
       if ((rc = sb_search_round(hs[i], step))) return rc;  // asynchronous; resamples on its own cadence
@@ -1300,6 +1388,7 @@ static int search_run_impl(sb_handle** hs, int n, const sb_search_params* p, con
     if (c->time_budget_s > 0 && elapsed() > c->time_budget_s) { reason = 1; break; }
     if (c->patience > 0 && stale >= c->patience) { reason = 2; break; }
     if (c->target_makespan > 0 && mk <= c->target_makespan) { reason = 3; break; }
+    if (stop_at_zero && (best >> 32) == 0) { reason = 3; break; }
   }
   // the incumbent lives on the device that owns the chain id in the key
   int owner = 0;
@@ -1346,16 +1435,16 @@ int sb_search_wave(sb_handle* h, unsigned flags, int64_t* chains) {
   const bool reduced = (flags & SB_FLAG_REDUCED) != 0;
   const int SG = (reduced ? 1 : h->S) * kSlots;
   const int pb = h->J <= 256 ? 1 : 2;
-  const bool weighted = (flags & SB_FLAG_WEIGHTED) != 0;
+  const int arrays = job_arrays(flags);
   int warps = 0;
   TilePlan tp;
-  if (search_round_mode(h->dev, h->J, SG, h->nodes, weighted) == 2) {
-    plan_tiles(h->dev, h->J, SG, pb, false, h->nodes, &tp, false, weighted);
+  if (search_round_mode(h->dev, h->J, SG, h->nodes, arrays) == 2) {
+    plan_tiles(h->dev, h->J, SG, pb, false, h->nodes, &tp, false, arrays);
     warps = tp.warps;
-  } else if (search_pos_smem(h->J, SG, h->nodes, 16, weighted) <= h->dev.smem_optin) {
+  } else if (search_pos_smem(h->J, SG, h->nodes, 16, arrays) <= h->dev.smem_optin) {
     warps = 16;
   } else {  // unfused rounds: the evaluation kernel's own plan (1 warp stands for the generic kernel's 128-thread CTAs)
-    warps = plan_tiles(h->dev, h->J, SG, pb, true, h->nodes, &tp, false, weighted);
+    warps = plan_tiles(h->dev, h->J, SG, pb, true, h->nodes, &tp, false, arrays);
     if (warps < 1) warps = 4;
   }
   *chains = static_cast<int64_t>(warps) * 32 * h->dev.sm_count;

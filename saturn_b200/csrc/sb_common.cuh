@@ -148,10 +148,14 @@ __device__ __forceinline__ float fmax3_mk(float mk, float b, float c) {
 // kWeighted (SB_FLAG_WEIGHTED, with kSum only): the job's weight `w` scales its completion, acc = acc + (w * e) with
 // TWO roundings (__fmul_rn, __fadd_rn: nvcc would otherwise contract them into one FFMA, which the oracle cannot
 // reproduce); w = 1 then gives the unweighted fold bit for bit.
-template <bool kIntegerStarts, bool kTrackMk = kIntegerStarts, bool kSum = false, bool kWeighted = false>
+// kDue (SB_FLAG_DUE, with kWeighted only): the job's tardiness max(e - d, +0) against its due date `d` takes the
+// completion's place, acc = acc + (w * max(e - d, +0)), each step rounded on its own; d = 0 gives the weighted fold.
+template <bool kIntegerStarts, bool kTrackMk = kIntegerStarts, bool kSum = false, bool kWeighted = false,
+          bool kDue = false>
 __device__ __forceinline__ void ls_step(float (&f)[8], float& mk, float& pend, float rt, int km1, int one, int ph,
-                                        float w = 0.f) {
+                                        float w = 0.f, float d = 0.f) {
   static_assert(kSum || !kWeighted, "weights scale the sum of completion times only");
+  static_assert(kWeighted || !kDue, "due dates run on the weighted form (unit weights for plain tardiness)");
   const float INF = inf_f();
   const int b2 = km1 & 4, b1 = km1 & 2, b0 = km1 & 1;
   // stage "shift by 4"
@@ -174,7 +178,8 @@ __device__ __forceinline__ void ls_step(float (&f)[8], float& mk, float& pend, f
   }
   if (kSum) {
     const float e = kIntegerStarts ? s + rt : v;
-    if (kWeighted) mk = __fadd_rn(mk, __fmul_rn(w, e));
+    if (kDue) mk = __fadd_rn(mk, __fmul_rn(w, fmaxf(__fsub_rn(e, d), 0.f)));
+    else if (kWeighted) mk = __fadd_rn(mk, __fmul_rn(w, e));
     else mk = mk + e;
   } else if (kTrackMk) {
     const float e = kIntegerStarts ? s + rt : v;

@@ -28,7 +28,9 @@
 //   * SUM (SB_FLAG_SUM_COMPLETION): every kernel here also comes in a form that scores the sum of completion
 //     times instead of the makespan (ls_step<..., kSum>); the schedule, and every start, is the same;
 //   * W (SB_FLAG_WEIGHTED, with SUM only): the sum is weighted per job.  The weights sit beside the table wherever
-//     the table is in shared memory (same TMA phase), and are read from global memory where the table is.
+//     the table is in shared memory (same TMA phase), and are read from global memory where the table is;
+//   * D (SB_FLAG_DUE, with W only): the weighted sum is of tardiness against per-job due dates instead of
+//     completions.  The due dates follow the weights, in the same memory and the same TMA phase.
 #include "sb_lane.cuh"
 
 namespace sb {
@@ -52,25 +54,30 @@ struct TileArgs {
   SearchFuse sf;  // SEARCH variant only
   XchgPost xp;    // xp.counter != nullptr: the last CTA to finish posts *best_key to every peer's mailbox
   const float* w;  // W: job weights [J], zero-padded to a multiple of 4 (16 bytes)
+  const float* d;  // D: job due dates [J], padded the same way
 };
 
 // TABG: the runtime table stays in global memory (read through L1/L2) — for tables larger than the
 // shared memory left beside the opt tiles (e.g. J = 1024 with 8 strategies: 256 KB).
 template <int PB, bool INT, bool STREAM, bool MULTI, bool SEARCH = false, bool TABG = false, int ADDR = 0,
-          bool SUM = false, bool W = false>
+          bool SUM = false, bool W = false, bool D = false>
 __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const TileArgs a) {
   static_assert(!(SEARCH && (STREAM || TABG)), "the fused search round runs on shared-memory tiles only");
   static_assert(ADDR == 0 || (!TABG && !MULTI && !SEARCH), "ADDR = 1 needs the table and the opt rows in shared memory");
   static_assert(SUM || !W, "weights scale the sum of completion times only");
+  static_assert(W || !D, "due dates run on the weighted form");
   extern __shared__ __align__(128) uint8_t smem[];
   const int nw = blockDim.x >> 5;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t tab_bytes = TABG ? 0u : static_cast<uint32_t>(a.J) * a.SG * 4u;  // a multiple of 32 (SG = S * 8)
-  // W: the weights follow the table in the same TMA phase, padded to 16 bytes (TABG: both stay in global memory)
+  // W: the weights follow the table in the same TMA phase, padded to 16 bytes (TABG: both stay in global memory);
+  // D: the due dates follow the weights the same way
   const uint32_t w_bytes = (W && !TABG) ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u;
+  const uint32_t d_bytes = D ? w_bytes : 0u;
   float* tab_s = reinterpret_cast<float*>(smem);
   [[maybe_unused]] float* w_s = reinterpret_cast<float*>(smem + tab_bytes);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + ((tab_bytes + w_bytes + 15u) & ~15u));
+  [[maybe_unused]] float* d_s = reinterpret_cast<float*>(smem + tab_bytes + w_bytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + ((tab_bytes + w_bytes + d_bytes + 15u) & ~15u));
   uint8_t* tiles = reinterpret_cast<uint8_t*>(bars) + (((1 + nw) * 8 + 15) & ~15);
   const uint32_t node_bytes = MULTI ? static_cast<uint32_t>(a.nodes) * 1024u : 0u;
   const uint32_t tile_bytes = 32u * (a.row_o + (STREAM ? 0 : a.row_p)) + node_bytes;
@@ -90,7 +97,7 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
   if constexpr (!TABG) {
     if (threadIdx.x == 0) {
       // stage the runtime table: TMA bulk copies of <= 32 KB each, one mbarrier phase
-      mbar_arrive_expect_tx(bar_tab, tab_bytes + w_bytes);
+      mbar_arrive_expect_tx(bar_tab, tab_bytes + w_bytes + d_bytes);
       const uint8_t* src = reinterpret_cast<const uint8_t*>(a.tab);
       for (uint32_t off = 0; off < tab_bytes; off += 32768u) {
         uint32_t n = min(32768u, tab_bytes - off);
@@ -101,15 +108,24 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
         for (uint32_t off = 0; off < w_bytes; off += 32768u)
           tma_bulk_g2s(smem + tab_bytes + off, wsrc + off, min(32768u, w_bytes - off), bar_tab);
       }
+      if constexpr (D) {
+        const uint8_t* dsrc = reinterpret_cast<const uint8_t*>(a.d);
+        for (uint32_t off = 0; off < d_bytes; off += 32768u)
+          tma_bulk_g2s(smem + tab_bytes + w_bytes + off, dsrc + off, min(32768u, d_bytes - off), bar_tab);
+      }
     }
   }
 
-  LaneState<INT, MULTI, ADDR, SUM, (W ? (TABG ? 2 : 1) : 0)> st;
+  LaneState<INT, MULTI, ADDR, SUM, (W ? (TABG ? 2 : 1) : 0), D> st;
   if (TABG) st.tab = a.tab;
   else st.tab = tab_s;
   if constexpr (W) {
     st.wt = TABG ? a.w : w_s;
     st.wt_s = smem_u32(w_s);
+  }
+  if constexpr (D) {
+    st.dd = TABG ? a.d : d_s;
+    st.dd_s = smem_u32(d_s);
   }
   st.SG = a.SG;
   st.one = a.one;
@@ -234,6 +250,7 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
         uint32_t ob[kBatch];
         float rb[kBatch];
         [[maybe_unused]] float wb[kBatch];  // W: the batch's weights, gathered with its runtimes
+        [[maybe_unused]] float db[kBatch];  // D: the batch's due dates, likewise
         auto resolve = [&](const uint32_t* w) {  // w: the kBatch / 4 words that hold the batch's job ids
           int js[kBatch];
 #pragma unroll
@@ -245,6 +262,10 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
           if constexpr (W) {
 #pragma unroll
             for (int i = 0; i < kBatch; ++i) wb[i] = st.gather_w(js[i]);
+          }
+          if constexpr (D) {
+#pragma unroll
+            for (int i = 0; i < kBatch; ++i) db[i] = st.gather_d(js[i]);
           }
         };
         if (nfull > 0) resolve(q.w);
@@ -262,16 +283,22 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
             uint32_t oc[kBatch];
             float rc[kBatch];
             [[maybe_unused]] float wc[kBatch];
+            [[maybe_unused]] float dc[kBatch];
 #pragma unroll
             for (int i = 0; i < kBatch; ++i) { oc[i] = ob[i]; rc[i] = rb[i]; }
             if constexpr (W) {
 #pragma unroll
               for (int i = 0; i < kBatch; ++i) wc[i] = wb[i];
             }
+            if constexpr (D) {
+#pragma unroll
+              for (int i = 0; i < kBatch; ++i) dc[i] = db[i];
+            }
             resolve(b + 1 < STEPS / kBatch ? q.w + (b + 1) * (kBatch / 4) : head);
 #pragma unroll
             for (int i = 0; i < kBatch; ++i) {
-              if constexpr (W) st.step_resolved(static_cast<int>(oc[i]), rc[i], i & 1, wc[i]);
+              if constexpr (D) st.step_resolved(static_cast<int>(oc[i]), rc[i], i & 1, wc[i], dc[i]);
+              else if constexpr (W) st.step_resolved(static_cast<int>(oc[i]), rc[i], i & 1, wc[i]);
               else st.step_resolved(static_cast<int>(oc[i]), rc[i], i & 1);
             }
           }
@@ -564,11 +591,13 @@ struct GenericArgs {
   int nodes;
   int one;
   const float* w;  // W: job weights [J], read with ld.global.nc
+  const float* d;  // D: job due dates [J], likewise
 };
 
-template <int PB, bool INT, bool MULTI, bool SUM = false, bool W = false>
+template <int PB, bool INT, bool MULTI, bool SUM = false, bool W = false, bool D = false>
 __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
   static_assert(SUM || !W, "weights scale the sum of completion times only");
+  static_assert(W || !D, "due dates run on the weighted form");
   extern __shared__ __align__(128) uint8_t smem[];
   const float* tab = a.tab;
   const uint32_t node_bytes = MULTI ? static_cast<uint32_t>(a.nodes) * 1024u : 0u;  // per warp
@@ -581,9 +610,10 @@ __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
     tab = tab_s;
   }
   const int lane = threadIdx.x & 31;
-  LaneState<INT, MULTI, 0, SUM, (W ? 2 : 0)> st;
+  LaneState<INT, MULTI, 0, SUM, (W ? 2 : 0), D> st;
   st.tab = tab;
   st.wt = a.w;
+  st.dd = a.d;
   st.SG = a.SG;
   st.one = a.one;
   st.ns = node_s + lane;
@@ -609,7 +639,15 @@ __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
         for (int t = 0; t < BATCH; ++t) os[t] = st.lookup_opt(js[t]);
 #pragma unroll
         for (int t = 0; t < BATCH; ++t) rts[t] = st.lookup_rt(js[t], os[t]);
-        if constexpr (W) {
+        if constexpr (D) {
+          float ws[BATCH], ds[BATCH];
+#pragma unroll
+          for (int t = 0; t < BATCH; ++t) ws[t] = st.lookup_w(js[t]);
+#pragma unroll
+          for (int t = 0; t < BATCH; ++t) ds[t] = st.lookup_d(js[t]);
+#pragma unroll
+          for (int t = 0; t < BATCH; ++t) st.step_resolved(os[t], rts[t], t & 1, ws[t], ds[t]);
+        } else if constexpr (W) {
           float ws[BATCH];
 #pragma unroll
           for (int t = 0; t < BATCH; ++t) ws[t] = st.lookup_w(js[t]);
@@ -646,11 +684,13 @@ struct FullArgs {
   float* start;         // [B][J] by job, nullable
   uint32_t* slotmask;   // [B][J] by job, nullable
   const float* w;       // W: job weights [J]
+  const float* d;       // D: job due dates [J]
 };
 
-template <int PB, bool INT, bool SUM = false, bool W = false>
+template <int PB, bool INT, bool SUM = false, bool W = false, bool D = false>
 __global__ void __launch_bounds__(128) k_eval_full(const FullArgs a) {
   static_assert(SUM || !W, "weights scale the sum of completion times only");
+  static_assert(W || !D, "due dates run on the weighted form");
   const long long nthreads = static_cast<long long>(gridDim.x) * blockDim.x;
   const bool multi = a.nodes > 1;
   for (long long b = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; b < a.B; b += nthreads) {
@@ -685,7 +725,9 @@ __global__ void __launch_bounds__(128) k_eval_full(const FullArgs a) {
       const float nxt = s + hold;
       for (int g = 0; g < kSlots; ++g)
         if ((taken >> g) & 1u) rd[g] = nxt;
-      if constexpr (W) mk = __fadd_rn(mk, __fmul_rn(__ldg(a.w + j), s + rt));  // ls_step<..., kSum, kWeighted>
+      if constexpr (D)  // ls_step<..., kSum, kWeighted, kDue>
+        mk = __fadd_rn(mk, __fmul_rn(__ldg(a.w + j), fmaxf(__fsub_rn(s + rt, __ldg(a.d + j)), 0.f)));
+      else if constexpr (W) mk = __fadd_rn(mk, __fmul_rn(__ldg(a.w + j), s + rt));  // ls_step<..., kSum, kWeighted>
       else if (SUM) mk = mk + (s + rt);  // the left fold in schedule order of ls_step<..., kSum>
       else mk = fmaxf(mk, s + rt);
       if (a.start) a.start[b * a.J + j] = s;
@@ -743,13 +785,13 @@ static int round_row(int bytes) {
 }
 
 int plan_tiles(const Device& dev, int J, int SG, int pb, bool stream, int nodes, TilePlan* tp, bool tab_global,
-               bool weighted) {
+               int arrays) {
   tp->row_o = round_row(J);
   tp->row_p = round_row(J * pb);
   tp->copy_o = (J + 15) & ~15;
   tp->copy_p = (J * pb + 15) & ~15;
   size_t tab_bytes = tab_global ? 0 : ((static_cast<size_t>(J) * SG * 4 + 15) & ~size_t(15));
-  if (weighted && !tab_global) tab_bytes += (static_cast<size_t>(J) * 4 + 15) & ~size_t(15);
+  if (!tab_global) tab_bytes += arrays * job_array_bytes(J);
   const size_t per_warp = 32u * static_cast<size_t>(tp->row_o + (stream ? 0 : tp->row_p)) +
                           (nodes > 1 ? static_cast<size_t>(nodes) * 1024u : 0u);
   int nw = stream ? 16 : 12;  // block size limits: 512 / 384 threads (128 registers per thread)
@@ -776,6 +818,7 @@ static TileArgs tile_args(const EvalCall& c, const TilePlan& tp) {
   a.nodes = c.nodes;
   a.out = c.out; a.best_key = c.best_key; a.id_base = c.id_base;
   a.w = c.w;
+  a.d = c.d;
   a.ntiles = (c.B + 31) / 32;
   a.one = 1;
   return a;
@@ -795,13 +838,13 @@ cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, i
   const bool bulk_ok = bulk_aligned(c);
   const bool stream_ok = bulk_ok && (c.stride_p % 32 == 0) && (reinterpret_cast<uintptr_t>(c.prio) % 32 == 0) &&
                          !(c.flags & HOOK_NO_STREAM);
-  const bool weighted = (c.flags & SB_FLAG_WEIGHTED) != 0;
+  const int arrays = job_arrays(c.flags);
   TilePlan tp;
   int nw = 0;
   bool stream = false, tabg = false;
   if (!c.force_generic) {
     if (stream_ok) {
-      nw = plan_tiles(dev, c.J, c.SG, pb, true, c.nodes, &tp, false, weighted);
+      nw = plan_tiles(dev, c.J, c.SG, pb, true, c.nodes, &tp, false, arrays);
       stream = nw >= 2 && c.stride_o >= tp.copy_o && c.stride_p >= ((c.J * pb + 31) & ~31);
       if (!stream && !multi) {
         // the table itself does not fit beside the tiles: keep it in global memory
@@ -809,7 +852,7 @@ cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, i
         stream = tabg = nw >= 2 && c.stride_o >= tp.copy_o && c.stride_p >= ((c.J * pb + 31) & ~31);
       }
     }
-    if (!stream) nw = plan_tiles(dev, c.J, c.SG, pb, false, c.nodes, &tp, false, weighted);
+    if (!stream) nw = plan_tiles(dev, c.J, c.SG, pb, false, c.nodes, &tp, false, arrays);
   }
   if (nw >= 2) {
     TileArgs a = tile_args(c, tp);
@@ -819,14 +862,14 @@ cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, i
     // the headline shape (u8 priorities streamed, one node, table in shared memory): address arithmetic on the FMA
     // pipe unless HOOK_PLAIN_ADDR asks for the plain form
     const bool fma_addr = pb == 1 && stream && !tabg && !multi && !(c.flags & HOOK_PLAIN_ADDR);
-    const TileKernel kern = with_eval_types(pb, c.flags, [&](auto PB, auto INT, auto SUM, auto W) -> TileKernel {
-      if (tabg) return k_eval_tiles<PB, INT, true, false, false, true, 0, SUM, W>;
+    const TileKernel kern = with_eval_types(pb, c.flags, [&](auto PB, auto INT, auto SUM, auto W, auto D) -> TileKernel {
+      if (tabg) return k_eval_tiles<PB, INT, true, false, false, true, 0, SUM, W, D>;
       if constexpr (PB == 1) {
-        if (fma_addr) return k_eval_tiles<1, INT, true, false, false, false, 1, SUM, W>;
+        if (fma_addr) return k_eval_tiles<1, INT, true, false, false, false, 1, SUM, W, D>;
       }
       return with_bool(stream, [&](auto STREAM) {
         return with_bool(multi, [&](auto MULTI) -> TileKernel {
-          return k_eval_tiles<PB, INT, STREAM, MULTI, false, false, 0, SUM, W>;
+          return k_eval_tiles<PB, INT, STREAM, MULTI, false, false, 0, SUM, W, D>;
         });
       });
     });
@@ -835,7 +878,7 @@ cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, i
   GenericArgs g;
   g.tab = c.tab; g.J = c.J; g.SG = c.SG; g.opt = c.opt; g.prio = c.prio; g.B = c.B;
   g.stride_o = c.stride_o; g.stride_p = c.stride_p; g.out = c.out; g.best_key = c.best_key;
-  g.id_base = c.id_base; g.tab_in_smem = 0; g.nodes = c.nodes; g.one = 1; g.w = c.w;
+  g.id_base = c.id_base; g.tab_in_smem = 0; g.nodes = c.nodes; g.one = 1; g.w = c.w; g.d = c.d;
   if (path_used) *path_used = 0;
   const size_t tab_bytes = static_cast<size_t>(c.J) * c.SG * 4;
   size_t smem = multi ? static_cast<size_t>(4) * c.nodes * 1024u : 0u;  // 4 warps per CTA
@@ -847,8 +890,8 @@ cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, i
   long long cap = static_cast<long long>(dev.sm_count) * 8;
   int grid = static_cast<int>(blocks < cap ? blocks : cap);
   if (grid < 1) grid = 1;
-  const auto kern = with_eval_types(pb, c.flags, [&](auto PB, auto INT, auto SUM, auto W) {
-    return with_bool(multi, [&](auto MULTI) { return k_eval_generic<PB, INT, MULTI, SUM, W>; });
+  const auto kern = with_eval_types(pb, c.flags, [&](auto PB, auto INT, auto SUM, auto W, auto D) {
+    return with_bool(multi, [&](auto MULTI) { return k_eval_generic<PB, INT, MULTI, SUM, W, D>; });
   });
   return launch(kern, grid, 128, smem, st, g);
 }
@@ -856,10 +899,10 @@ cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, i
 // 2 = both rows of a candidate fit in shared memory for at least 8 warps: the tile kernel runs the fused
 // round (all moves); 0 = they do not: the search keeps a position-major population (sb_search.cu: 16 warps
 // at any J, where only a few tile warps would fit) or, when even the table does not fit, runs unfused rounds
-int search_round_mode(const Device& dev, int J, int SG, int nodes, bool weighted) {
+int search_round_mode(const Device& dev, int J, int SG, int nodes, int arrays) {
   const int pb = J <= 256 ? 1 : 2;
   TilePlan tp;
-  return plan_tiles(dev, J, SG, pb, false, nodes, &tp, false, weighted) >= 8 ? 2 : 0;
+  return plan_tiles(dev, J, SG, pb, false, nodes, &tp, false, arrays) >= 8 ? 2 : 0;
 }
 
 // One fused search round over `c.B` chains whose current candidates are (c.opt, c.prio).  Returns
@@ -869,16 +912,16 @@ cudaError_t search_round_launch(const Device& dev, const EvalCall& c, const Sear
   if (c.B <= 0) return cudaSuccess;
   const int pb = c.J <= 256 ? 1 : 2;
   TilePlan tp;
-  const bool weighted = (c.flags & SB_FLAG_WEIGHTED) != 0;
-  if (search_round_mode(dev, c.J, c.SG, c.nodes, weighted) == 0 || !bulk_aligned(c)) return cudaErrorNotSupported;
-  plan_tiles(dev, c.J, c.SG, pb, false, c.nodes, &tp, false, weighted);
+  const int arrays = job_arrays(c.flags);
+  if (search_round_mode(dev, c.J, c.SG, c.nodes, arrays) == 0 || !bulk_aligned(c)) return cudaErrorNotSupported;
+  plan_tiles(dev, c.J, c.SG, pb, false, c.nodes, &tp, false, arrays);
   if (c.stride_o < tp.copy_o || c.stride_p < tp.copy_p) return cudaErrorNotSupported;
   TileArgs a = tile_args(c, tp);
   a.use_bulk = 1;
   a.sf = sf;
-  const TileKernel kern = with_eval_types(pb, c.flags, [&](auto PB, auto INT, auto SUM, auto W) {
+  const TileKernel kern = with_eval_types(pb, c.flags, [&](auto PB, auto INT, auto SUM, auto W, auto D) {
     return with_bool(c.nodes > 1, [&](auto MULTI) -> TileKernel {
-      return k_eval_tiles<PB, INT, false, MULTI, true, false, 0, SUM, W>;
+      return k_eval_tiles<PB, INT, false, MULTI, true, false, 0, SUM, W, D>;
     });
   });
   return launch_tiles(dev, kern, a, tp, st);
@@ -890,12 +933,12 @@ cudaError_t eval_full_launch(const Device& dev, const EvalCall& c, float* start,
   FullArgs a;
   a.tab = c.tab; a.J = c.J; a.SG = c.SG; a.opt = c.opt; a.prio = c.prio; a.B = c.B;
   a.stride_o = c.stride_o; a.stride_p = c.stride_p; a.nodes = c.nodes < 1 ? 1 : c.nodes;
-  a.out = c.out; a.start = start; a.slotmask = slotmask; a.w = c.w;
+  a.out = c.out; a.start = start; a.slotmask = slotmask; a.w = c.w; a.d = c.d;
   long long blocks = (c.B + 127) / 128;
   long long cap = static_cast<long long>(dev.sm_count) * 16;
   int grid = static_cast<int>(blocks < cap ? blocks : cap);
-  const auto kern = with_eval_types(pb, c.flags, [](auto PB, auto INT, auto SUM, auto W) {
-    return k_eval_full<PB, INT, SUM, W>;
+  const auto kern = with_eval_types(pb, c.flags, [](auto PB, auto INT, auto SUM, auto W, auto D) {
+    return k_eval_full<PB, INT, SUM, W, D>;
   });
   return launch(kern, grid, 128, 0, st, a);
 }

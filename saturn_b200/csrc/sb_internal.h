@@ -31,7 +31,8 @@ static_assert(((HOOK_FORCE_GENERIC | HOOK_NO_STREAM | HOOK_NO_FUSED | HOOK_NO_IN
                 HOOK_ROUND1_MOVES | HOOK_PLAIN_ADDR | HOOK_WINDOW_BIAS | HOOK_TABLE_GLOBAL | HOOK_TABLE_PAIR |
                 HOOK_REORDER | HOOK_NO_REORDER) &
                (SB_FLAG_INTEGER_STARTS | SB_FLAG_REDUCED | SB_FLAG_OPT_BY_POSITION | SB_FLAG_POST_KEY |
-                SB_FLAG_FOLD_PREV | SB_FLAG_ALT_WARPSCAN | SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED)) == 0,
+                SB_FLAG_FOLD_PREV | SB_FLAG_ALT_WARPSCAN | SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED |
+                SB_FLAG_DUE)) == 0,
               "the test hooks share no bit with the SB_FLAG_* flags");
 
 // Compile-time dispatch: f is called with the run-time value as a type (std::true_type / std::false_type, or the
@@ -44,20 +45,33 @@ template <class F>
 decltype(auto) with_pb(int pb, F&& f) {
   return pb == 1 ? f(std::integral_constant<int, 1>{}) : f(std::integral_constant<int, 2>{});
 }
-// f(PB, INT, SUM, W): the prio width, SB_FLAG_INTEGER_STARTS, SB_FLAG_SUM_COMPLETION and SB_FLAG_WEIGHTED, the
-// template arguments that every evaluation and search kernel takes.  W is true only together with SUM: no kernel
-// that weights the makespan is ever instantiated.
+// f(PB, INT, SUM, W, D): the prio width, SB_FLAG_INTEGER_STARTS, SB_FLAG_SUM_COMPLETION, SB_FLAG_WEIGHTED and
+// SB_FLAG_DUE, the template arguments that every evaluation and search kernel takes.  W is true only together with
+// SUM, and D only together with W: no kernel that weights the makespan, or that scores tardiness without weights, is
+// ever instantiated (SB_FLAG_DUE alone runs the weighted form on unit weights, exact since 1 * x = x).
 template <class F>
 decltype(auto) with_eval_types(int pb, unsigned flags, F&& f) {
   return with_pb(pb, [&](auto PB) {
     return with_bool(flags & SB_FLAG_INTEGER_STARTS, [&](auto INT) {
       return with_bool(flags & SB_FLAG_SUM_COMPLETION, [&](auto SUM) {
-        if constexpr (SUM) return with_bool(flags & SB_FLAG_WEIGHTED, [&](auto W) { return f(PB, INT, SUM, W); });
-        else return f(PB, INT, SUM, std::false_type{});
+        if constexpr (SUM) {
+          return with_bool(flags & (SB_FLAG_WEIGHTED | SB_FLAG_DUE), [&](auto W) {
+            if constexpr (W) return with_bool(flags & SB_FLAG_DUE, [&](auto D) { return f(PB, INT, SUM, W, D); });
+            else return f(PB, INT, SUM, W, std::false_type{});
+          });
+        } else {
+          return f(PB, INT, SUM, std::false_type{}, std::false_type{});
+        }
       });
     });
   });
 }
+// the per-job fp32 arrays a kernel stages beside the table: the weights (SB_FLAG_WEIGHTED, or the unit weights of
+// SB_FLAG_DUE alone), then the due dates (SB_FLAG_DUE); each is padded to 16 bytes
+inline int job_arrays(unsigned flags) {
+  return (flags & SB_FLAG_DUE) ? 2 : ((flags & SB_FLAG_WEIGHTED) ? 1 : 0);
+}
+inline size_t job_array_bytes(int J) { return (static_cast<size_t>(J) * 4 + 15) & ~size_t(15); }
 
 // One kernel launch: raise the kernel's dynamic shared-memory limit to what the launch uses (when it uses any),
 // launch, and return the launch error.
@@ -106,6 +120,8 @@ struct TilePlan {
 struct EvalCall {
   const float* tab = nullptr;  // canonical table actually used (full or reduced)
   const float* w = nullptr;    // SB_FLAG_WEIGHTED: the job weights [J], padded with zeros to a multiple of 4
+                               // (SB_FLAG_DUE alone: J ones, padded the same way)
+  const float* d = nullptr;    // SB_FLAG_DUE: the job due dates [J], padded the same way
   int J = 0, SG = 0;
   const uint8_t* opt = nullptr;
   const uint8_t* prio = nullptr;
@@ -161,12 +177,13 @@ struct SearchFuse {
   } keep;
 };
 
-// weighted: the J weights are staged beside the table (unless tab_global: then both stay in global memory)
+// arrays: job_arrays(flags), the per-job arrays staged beside the table (unless tab_global: then they all stay in
+// global memory)
 int plan_tiles(const Device& dev, int J, int SG, int pb, bool stream, int nodes, TilePlan* tp, bool tab_global = false,
-               bool weighted = false);
+               int arrays = 0);
 cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, int* path_used);
 cudaError_t eval_alt_launch(const Device& dev, const EvalCall& c, cudaStream_t st);  // sb_eval_alt.cu
-int search_round_mode(const Device& dev, int J, int SG, int nodes, bool weighted = false);
+int search_round_mode(const Device& dev, int J, int SG, int nodes, int arrays = 0);
 cudaError_t search_round_launch(const Device& dev, const EvalCall& c, const SearchFuse& sf, cudaStream_t st);
 cudaError_t eval_full_launch(const Device& dev, const EvalCall& c, float* start, uint32_t* slotmask, cudaStream_t st);
 cudaError_t validate_launch(const Device& dev, const EvalCall& c, unsigned long long* bad, cudaStream_t st,

@@ -39,7 +39,9 @@ __device__ __forceinline__ PrioChunk ld_prio32(const uint8_t* p) {
 // SUM: score = sum of completion times (SB_FLAG_SUM_COMPLETION) instead of the makespan; mk holds the running sum.
 // WGT (SB_FLAG_WEIGHTED, with SUM only): each completion is scaled by its job's weight, read from `wt` — 1: the
 // weights are in shared memory beside the table, 2: in global memory, read with ld.global.nc.
-template <bool INT, bool MULTI, int ADDR = 0, bool SUM = false, int WGT = 0>
+// DUE (SB_FLAG_DUE, with WGT only): each job's tardiness against its due date, read from `dd` (in the same memory
+// as the weights) takes its completion's place.
+template <bool INT, bool MULTI, int ADDR = 0, bool SUM = false, int WGT = 0, bool DUE = false>
 struct LaneState {
   float f[8];
   float mk;
@@ -47,10 +49,12 @@ struct LaneState {
   const uint8_t* orow;  // this candidate's opt bytes (shared memory or global)
   const float* tab;     // runtime table (shared memory or global)
   const float* wt;      // WGT: the job weights [J]
+  const float* dd;      // DUE: the job due dates [J]
   int SG;
   int one;
   uint32_t orow_s, tab_s, four;  // ADDR = 1: shared-window addresses of orow / tab, and a run-time 4
   uint32_t wt_s;                 // ADDR = 1 with WGT: shared-window address of wt
+  uint32_t dd_s;                 // ADDR = 1 with DUE: shared-window address of dd
   float4* ns;  // MULTI: lane-private node-state column; node n lives at ns[(2n)*32], ns[(2n+1)*32]
   int cur;     // MULTI: the node whose state is currently in f[] (its shared-memory copy is stale)
 
@@ -91,13 +95,20 @@ struct LaneState {
     else if constexpr (WGT == 2) return __ldg(wt + j);
     else return 0.f;
   }
-  // ph: t & 1 inside fully unrolled loops, -1 elsewhere (see ls_step); w: the job's weight (WGT only)
-  __device__ __forceinline__ void step_resolved(int o, float rt, int ph = -1, float w = 0.f) {
+  // the job's due date (DUE only; 0 otherwise, and then unused)
+  __device__ __forceinline__ float lookup_d(int j) const {
+    if constexpr (!DUE) return 0.f;
+    else if constexpr (WGT == 1) return dd[j];
+    else return __ldg(dd + j);
+  }
+  // ph: t & 1 inside fully unrolled loops, -1 elsewhere (see ls_step); w, d: the job's weight (WGT only) and due
+  // date (DUE only)
+  __device__ __forceinline__ void step_resolved(int o, float rt, int ph = -1, float w = 0.f, float d = 0.f) {
     if (!MULTI) {
-      ls_step<INT, INT, SUM, (WGT != 0)>(f, mk, pend, rt, o & 7, one, ph, w);
+      ls_step<INT, INT, SUM, (WGT != 0), DUE>(f, mk, pend, rt, o & 7, one, ph, w, d);
     } else {
       switch_node(o >> 3);
-      ls_step<INT, true, SUM, (WGT != 0)>(f, mk, pend, rt, o & 7, one, ph, w);
+      ls_step<INT, true, SUM, (WGT != 0), DUE>(f, mk, pend, rt, o & 7, one, ph, w, d);
     }
   }
   // ADDR = 1: the two look-ups as separate gathers, so that the streamed loop of k_eval_tiles can issue a whole
@@ -128,22 +139,35 @@ struct LaneState {
       return w;
     }
   }
+  // ADDR = 1 with DUE: the due-date gather, like gather_w
+  __device__ __forceinline__ float gather_d(int j) const {
+    if constexpr (!DUE) {
+      return 0.f;
+    } else {
+      uint32_t da;
+      float d;
+      asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(da) : "r"(j), "r"(four), "r"(dd_s));
+      asm("ld.shared.f32 %0, [%1];" : "=f"(d) : "r"(da));
+      return d;
+    }
+  }
   __device__ __forceinline__ void step(int j, int ph = -1) {
     constexpr bool W = WGT != 0;
     if (!MULTI && ADDR == 1) {
       const uint32_t o = gather_opt(j);
-      ls_step<INT, INT, SUM, W>(f, mk, pend, gather_rt(j, o), static_cast<int>(o & 7u), one, ph, gather_w(j));
+      ls_step<INT, INT, SUM, W, DUE>(f, mk, pend, gather_rt(j, o), static_cast<int>(o & 7u), one, ph, gather_w(j),
+                                     gather_d(j));
       return;
     }
     const int o = orow[j];
     if (!MULTI) {
       const float rt = tab[j * SG + o];
-      ls_step<INT, INT, SUM, W>(f, mk, pend, rt, o & 7, one, ph, lookup_w(j));
+      ls_step<INT, INT, SUM, W, DUE>(f, mk, pend, rt, o & 7, one, ph, lookup_w(j), lookup_d(j));
     } else {
       const int col = o & 7;  // reduced table only: opt = (node << 3) | (k - 1)
       const float rt = tab[j * 8 + col];
       switch_node(o >> 3);
-      ls_step<INT, true, SUM, W>(f, mk, pend, rt, col, one, ph, lookup_w(j));
+      ls_step<INT, true, SUM, W, DUE>(f, mk, pend, rt, col, one, ph, lookup_w(j), lookup_d(j));
     }
   }
   __device__ __forceinline__ float result() const { return SUM ? mk : ((INT || MULTI) ? fmaxf(mk, pend) : f[7]); }

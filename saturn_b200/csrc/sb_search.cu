@@ -329,6 +329,7 @@ struct PosArgs {
   int one;
   SearchFuse sf;
   const float* w;  // W: job weights [J], zero-padded to a multiple of 4 (16 bytes)
+  const float* d;  // D: job due dates [J], padded the same way
 };
 
 struct PosMove {
@@ -423,10 +424,13 @@ __device__ __forceinline__ PosMove make_pos_move_win(const SearchFuse& sf, int r
 // SUM: score the sum of completion times instead of the makespan (SB_FLAG_SUM_COMPLETION, see ls_step).
 // W: weight each completion by its job's weight (SB_FLAG_WEIGHTED, with SUM only); the weights follow the table in
 // shared memory with TAB = 0 and are read from global memory (ld.global.nc) with TAB = 1 / 2.
-template <int PB, bool INT, bool MULTI, bool EVAL = false, int TAB = 0, bool SUM = false, bool W = false>
+// D: score tardiness against the jobs' due dates (SB_FLAG_DUE, with W only); the due dates follow the weights.
+template <int PB, bool INT, bool MULTI, bool EVAL = false, int TAB = 0, bool SUM = false, bool W = false,
+          bool D = false>
 __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
   static_assert(TAB == 0 || (EVAL && !MULTI), "tables outside the CTA's shared memory: scoring only, one node");
   static_assert(SUM || !W, "weights scale the sum of completion times only");
+  static_assert(W || !D, "due dates run on the weighted form");
   extern __shared__ __align__(128) uint8_t smem[];
   const int nw = blockDim.x >> 5;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -438,9 +442,11 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
   const uint32_t tab_bytes = TAB == 1 ? 0u : (TAB == 2 ? (rank == 0 ? half * 4u : tab_all - half * 4u) : tab_all);
   const uint32_t tab_room = TAB == 1 ? 0u : (TAB == 2 ? half * 4u : tab_all);
   const uint32_t w_bytes = (W && TAB == 0) ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u;
+  const uint32_t d_bytes = D ? w_bytes : 0u;
   float* tab_s = reinterpret_cast<float*>(smem);
   [[maybe_unused]] float* w_s = reinterpret_cast<float*>(smem + ((tab_room + 15u) & ~15u));
-  uint64_t* bar_tab = reinterpret_cast<uint64_t*>(smem + ((tab_room + 15u) & ~15u) + w_bytes);
+  [[maybe_unused]] float* d_s = reinterpret_cast<float*>(smem + ((tab_room + 15u) & ~15u) + w_bytes);
+  uint64_t* bar_tab = reinterpret_cast<uint64_t*>(smem + ((tab_room + 15u) & ~15u) + w_bytes + d_bytes);
   const uint32_t node_bytes = MULTI ? static_cast<uint32_t>(a.nodes) * 1024u : 0u;
   float4* node_s = reinterpret_cast<float4*>(reinterpret_cast<uint8_t*>(bar_tab) + 16 + static_cast<size_t>(warp) * node_bytes);
   if (threadIdx.x == 0) {
@@ -450,7 +456,7 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
   __syncthreads();
   if constexpr (TAB != 1) {
     if (threadIdx.x == 0) {
-      mbar_arrive_expect_tx(bar_tab, tab_bytes + w_bytes);
+      mbar_arrive_expect_tx(bar_tab, tab_bytes + w_bytes + d_bytes);
       const uint8_t* src = reinterpret_cast<const uint8_t*>(a.tab) + tab_off;
       for (uint32_t off = 0; off < tab_bytes; off += 32768u) tma_bulk_g2s(smem + off, src + off, min(32768u, tab_bytes - off), bar_tab);
       if constexpr (W && TAB == 0) {
@@ -458,11 +464,17 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
         for (uint32_t off = 0; off < w_bytes; off += 32768u)
           tma_bulk_g2s(reinterpret_cast<uint8_t*>(w_s) + off, wsrc + off, min(32768u, w_bytes - off), bar_tab);
       }
+      if constexpr (D && TAB == 0) {
+        const uint8_t* dsrc = reinterpret_cast<const uint8_t*>(a.d);
+        for (uint32_t off = 0; off < d_bytes; off += 32768u)
+          tma_bulk_g2s(reinterpret_cast<uint8_t*>(d_s) + off, dsrc + off, min(32768u, d_bytes - off), bar_tab);
+      }
     }
   }
-  LaneState<INT, MULTI, 0, SUM, (W ? (TAB == 0 ? 1 : 2) : 0)> st;
+  LaneState<INT, MULTI, 0, SUM, (W ? (TAB == 0 ? 1 : 2) : 0), D> st;
   st.tab = tab_s;
   if constexpr (W) st.wt = TAB == 0 ? w_s : a.w;
+  if constexpr (D) st.dd = TAB == 0 ? d_s : a.d;
   st.SG = a.SG;
   st.one = a.one;
   st.orow = nullptr;
@@ -556,7 +568,8 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
           for (int t = 0; t < 32; ++t) {
             const int j = prio_at<PB>(qp[(t * PB) / 32].w, t % (32 / PB));
             const int o = prio_at<1>(qo.w, t);
-            if constexpr (W) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j));
+            if constexpr (D) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j), st.lookup_d(j));
+            else if constexpr (W) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j));
             else st.step_resolved(o, lookup(j, o), t & 1);
           }
         } else {
@@ -565,7 +578,8 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
             if (base + t < J) {
               const int j = prio_at<PB>(qp[(t * PB) / 32].w, t % (32 / PB));
               const int o = prio_at<1>(qo.w, t);
-              if constexpr (W) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j));
+              if constexpr (D) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j), st.lookup_d(j));
+              else if constexpr (W) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j));
               else st.step_resolved(o, lookup(j, o), t & 1);
             }
           }
@@ -748,11 +762,10 @@ cudaError_t search_init_population_pos(const SearchDev& s, cudaStream_t st) {
   return launch(with_pb(s.pb, [](auto PB) { return k_init_population_pos<PB>; }), grid, threads, 0, st, s);
 }
 
-// smem: table (+ weights) + mbarrier + per-warp node states (MULTI)
-size_t search_pos_smem(int J, int SG, int nodes, int warps, bool weighted) {
+// smem: table (+ weights, + due dates) + mbarrier + per-warp node states (MULTI)
+size_t search_pos_smem(int J, int SG, int nodes, int warps, int arrays) {
   const size_t tab_bytes = (static_cast<size_t>(J) * SG * 4 + 15) & ~size_t(15);
-  const size_t w_bytes = weighted ? (static_cast<size_t>(J) * 4 + 15) & ~size_t(15) : 0;
-  return tab_bytes + w_bytes + 16 + static_cast<size_t>(warps) * (nodes > 1 ? nodes * 1024u : 0u);
+  return tab_bytes + arrays * job_array_bytes(J) + 16 + static_cast<size_t>(warps) * (nodes > 1 ? nodes * 1024u : 0u);
 }
 
 using PosKernel = void (*)(PosArgs);
@@ -765,8 +778,9 @@ static cudaError_t eval_pos_far_launch(const Device& dev, const PosArgs& a, int 
   if (smem > dev.smem_optin) return cudaErrorNotSupported;
   const long long ntiles = (a.chains + 31) / 32;
   const long long ctas = (ntiles + warps - 1) / warps;
-  const PosKernel kern = with_eval_types(pb, flags, [&](auto PB, auto INT, auto SUM, auto W) {
-    return tab_home == 2 ? k_search_pos<PB, INT, false, true, 2, SUM, W> : k_search_pos<PB, INT, false, true, 1, SUM, W>;
+  const PosKernel kern = with_eval_types(pb, flags, [&](auto PB, auto INT, auto SUM, auto W, auto D) {
+    return tab_home == 2 ? k_search_pos<PB, INT, false, true, 2, SUM, W, D>
+                         : k_search_pos<PB, INT, false, true, 1, SUM, W, D>;
   });
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
   if (e != cudaSuccess) return e;
@@ -798,8 +812,8 @@ static cudaError_t eval_pos_far_launch(const Device& dev, const PosArgs& a, int 
 
 // tab_home: 0 = the table in every CTA's shared memory (cudaErrorNotSupported when it does not fit);
 // scoring only, one node: 2 = split over CTA pairs, 1 = global memory
-cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float* tab, const float* w, int SG, unsigned flags,
-                              long long first, long long count, bool eval_only, const SearchFuse& sf,
+cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float* tab, const float* w, const float* d,
+                              int SG, unsigned flags, long long first, long long count, bool eval_only, const SearchFuse& sf,
                               cudaStream_t st, int tab_home) {
   if (count <= 0) return cudaSuccess;
   PosArgs a;
@@ -813,20 +827,23 @@ cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float
   a.one = 1;
   a.sf = sf;
   a.w = w;
+  a.d = d;
   const bool multi = s.nodes > 1;
   if (tab_home != 0) {
     if (!eval_only || multi) return cudaErrorNotSupported;
     return eval_pos_far_launch(dev, a, tab_home, s.pb, flags, st);
   }
   const int warps = 16;
-  const size_t smem = search_pos_smem(s.J, SG, s.nodes, warps, (flags & SB_FLAG_WEIGHTED) != 0);
+  const size_t smem = search_pos_smem(s.J, SG, s.nodes, warps, job_arrays(flags));
   if (smem > dev.smem_optin) return cudaErrorNotSupported;
   const long long ntiles = (count + 31) / 32;
   const long long ctas = (ntiles + warps - 1) / warps;
   const int grid = static_cast<int>(ctas < dev.sm_count ? ctas : dev.sm_count);
-  const PosKernel kern = with_eval_types(s.pb, flags, [&](auto PB, auto INT, auto SUM, auto W) {
+  const PosKernel kern = with_eval_types(s.pb, flags, [&](auto PB, auto INT, auto SUM, auto W, auto D) {
     return with_bool(multi, [&](auto MULTI) {
-      return with_bool(eval_only, [&](auto EVAL) -> PosKernel { return k_search_pos<PB, INT, MULTI, EVAL, 0, SUM, W>; });
+      return with_bool(eval_only, [&](auto EVAL) -> PosKernel {
+        return k_search_pos<PB, INT, MULTI, EVAL, 0, SUM, W, D>;
+      });
     });
   });
   return launch(kern, grid, warps * 32, smem, st, a);
@@ -840,7 +857,7 @@ int eval_pos_home(const Device& dev, int J, int SG, int nodes, unsigned flags) {
   const bool pair_ok = nodes == 1 && static_cast<size_t>(pos_tab_half(J, SG)) * 4 + 16 <= dev.smem_optin;
   if (flags & HOOK_TABLE_PAIR) return pair_ok ? 2 : -1;
   if (flags & HOOK_TABLE_GLOBAL) return nodes == 1 ? 1 : -1;
-  if (search_pos_smem(J, SG, nodes, 16, (flags & SB_FLAG_WEIGHTED) != 0) <= dev.smem_optin) return 0;
+  if (search_pos_smem(J, SG, nodes, 16, job_arrays(flags)) <= dev.smem_optin) return 0;
   return nodes == 1 ? 1 : -1;
 }
 
@@ -862,7 +879,7 @@ cudaError_t eval_pos_launch(const Device& dev, const EvalCall& c, cudaStream_t s
   s.keys = c.best_key;
   SearchFuse sf = {};
   sf.cur_mk = c.out;
-  return search_pos_launch(dev, s, c.tab, c.w, c.SG, c.flags, 0, c.B, true, sf, st, home);
+  return search_pos_launch(dev, s, c.tab, c.w, c.d, c.SG, c.flags, 0, c.B, true, sf, st, home);
 }
 
 // Job-indexed opt rows -> schedule order (out[i] = opt[prio[i]]), one warp per candidate: the row is staged in

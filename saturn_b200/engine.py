@@ -18,18 +18,21 @@ from ._lib import FLAG_INTEGER_STARTS, FLAG_REDUCED, SaturnB200Error, SearchPara
 NSLOT = 8
 
 
-OBJECTIVES = ("makespan", "completion", "weighted_completion")
+OBJECTIVES = ("makespan", "completion", "weighted_completion", "tardiness", "weighted_tardiness")
 
 
 def objective_flag(objective: str) -> int:
     """SB_FLAG_SUM_COMPLETION for objective="completion" (score = sum of completion times), SB_FLAG_SUM_COMPLETION |
-    SB_FLAG_WEIGHTED for "weighted_completion" (the sum weighted by the engine's set_weights), 0 for "makespan"."""
+    SB_FLAG_WEIGHTED for "weighted_completion" (the sum weighted by the engine's set_weights), SB_FLAG_SUM_COMPLETION |
+    SB_FLAG_DUE for "tardiness" (total tardiness against the engine's set_due) and SB_FLAG_SUM_COMPLETION |
+    SB_FLAG_DUE | SB_FLAG_WEIGHTED for "weighted_tardiness", 0 for "makespan"."""
     if objective not in OBJECTIVES:
         from .solver import SolverError
         raise SolverError("objective must be one of %s, not %r" % (", ".join(map(repr, OBJECTIVES)), objective))
     if objective == "makespan":
         return 0
-    return _lib.FLAG_SUM_COMPLETION | (_lib.FLAG_WEIGHTED if objective == "weighted_completion" else 0)
+    return _lib.FLAG_SUM_COMPLETION | (_lib.FLAG_WEIGHTED if objective.startswith("weighted_") else 0) | (
+        _lib.FLAG_DUE if objective.endswith("tardiness") else 0)
 
 
 def weights_f32(w, J: int) -> np.ndarray:
@@ -51,8 +54,31 @@ def weights_f32(w, J: int) -> np.ndarray:
     return w32
 
 
+def due_f32(d, J: int) -> np.ndarray:
+    """J due dates as fp32 (round to nearest: integers are exact).  Every due date must be finite with |d| < 2^24
+    (negative values are allowed: the job is already overdue); raises SolverError otherwise."""
+    from .solver import SolverError
+    try:
+        d64 = np.asarray(d, dtype=np.float64)
+    except (TypeError, ValueError) as e:
+        raise SolverError("due dates must be numbers: %s" % e)
+    if d64.shape != (J,):
+        raise SolverError("due dates must have one value per task (%d), got shape %s" % (J, d64.shape))
+    if not (np.isfinite(d64).all() and (np.abs(d64) < 2.0 ** 24).all()):
+        raise SolverError("every due date must be finite with |d| < 2^24")
+    return d64.astype(np.float32)
+
+
 def _flags(integer_starts: bool, reduced: bool, objective: str = "makespan") -> int:
     return (FLAG_INTEGER_STARTS if integer_starts else 0) | (FLAG_REDUCED if reduced else 0) | objective_flag(objective)
+
+
+def _require_due(due, objective: str):
+    """The tardiness objectives score against the due dates of set_due: refuse them, before any device call, on an
+    engine that has none (set_table clears them)."""
+    if objective.endswith("tardiness") and due is None:
+        from .solver import SolverError
+        raise SolverError("objective=%r needs due dates: call set_due after set_table" % (objective,))
 
 
 class Engine:
@@ -79,6 +105,7 @@ class Engine:
         self.gcount = None
         self.nodes = 1
         self.weights = None  # fp32 job weights of objective="weighted_completion" (set_weights)
+        self.due = None  # fp32 job due dates of objective="tardiness" / "weighted_tardiness" (set_due)
 
     # ------------------------------------------------------------------ lifecycle
     def close(self):
@@ -123,6 +150,7 @@ class Engine:
         self.gcount = [int(x) for x in gc]
         self.nodes = int(nodes)
         self.weights = None  # sb_set_table clears them
+        self.due = None
         return self
 
     def set_weights(self, w) -> "Engine":
@@ -136,6 +164,23 @@ class Engine:
         check(self._lib.sb_set_weights(self._h, C.c_void_p(w32.ctypes.data), int(self.J)))
         self.weights = w32
         return self
+
+    def set_due(self, d) -> "Engine":
+        """Per-job due dates (J values, finite with |d| < 2^24, converted to fp32) for objective="tardiness", which
+        scores sum_j max(0, start_j + rt_j - d_j), and "weighted_tardiness" (each term times the set_weights
+        weight).  None clears them; set_table clears them too."""
+        if d is None:
+            check(self._lib.sb_set_due(self._h, None, 0))
+            self.due = None
+            return self
+        d32 = np.ascontiguousarray(due_f32(d, self.J))
+        check(self._lib.sb_set_due(self._h, C.c_void_p(d32.ctypes.data), int(self.J)))
+        self.due = d32
+        return self
+
+    def _flags(self, integer_starts: bool, reduced: bool, objective: str) -> int:
+        _require_due(self.due, objective)
+        return _flags(integer_starts, reduced, objective)
 
     def reduced_table(self) -> Tuple[np.ndarray, np.ndarray]:
         tmin = np.empty((self.J, NSLOT), dtype=np.float32)
@@ -182,7 +227,7 @@ class Engine:
         B, stride = self._check_cands(opt, prio, True)
         if out is None:
             out = torch.empty(B, dtype=torch.float32, device=self.device)
-        fl = _flags(integer_starts, reduced, objective) | (_lib.HOOK_FORCE_GENERIC if _force_generic else 0) | (
+        fl = self._flags(integer_starts, reduced, objective) | (_lib.HOOK_FORCE_GENERIC if _force_generic else 0) | (
             _lib.HOOK_NO_STREAM if _no_stream else 0) | (_lib.HOOK_PLAIN_ADDR if _plain_addr else 0) | (
             _lib.FLAG_POST_KEY if post_key else 0) | (
             _lib.FLAG_FOLD_PREV if (post_key and fold_prev) else 0) | (
@@ -211,7 +256,7 @@ class Engine:
         if out is None:
             out = torch.empty(B, dtype=torch.float32, pin_memory=True)
         check(self._lib.sb_eval_host(self._h, C.c_void_p(opt.data_ptr()), C.c_void_p(prio.data_ptr()), B, stride,
-                                     _flags(integer_starts, reduced, objective), C.c_void_p(out.data_ptr())))
+                                     self._flags(integer_starts, reduced, objective), C.c_void_p(out.data_ptr())))
         return out
 
     def eval_full(self, opt: torch.Tensor, prio: torch.Tensor, integer_starts: bool = True, reduced: bool = False,
@@ -223,7 +268,7 @@ class Engine:
         start = torch.empty((B, self.J), dtype=torch.float32, device=self.device)
         mask = torch.empty((B, self.J), dtype=torch.int32, device=self.device)
         check(self._lib.sb_eval_full(self._h, C.c_void_p(opt.data_ptr()), C.c_void_p(prio.data_ptr()), B, stride,
-                                     _flags(integer_starts, reduced, objective), C.c_void_p(mk.data_ptr()),
+                                     self._flags(integer_starts, reduced, objective), C.c_void_p(mk.data_ptr()),
                                      C.c_void_p(start.data_ptr()), C.c_void_p(mask.data_ptr())))
         return mk, start, mask
 
@@ -243,7 +288,7 @@ class Engine:
         node = np.empty(J, dtype=np.uint8)
         mk = C.c_float(0)
         check(self._lib.sb_decode(self._h, C.c_void_p(opt.ctypes.data), C.c_void_p(prio.ctypes.data),
-                                  _flags(integer_starts, reduced, objective), C.c_void_p(start.ctypes.data),
+                                  self._flags(integer_starts, reduced, objective), C.c_void_p(start.ctypes.data),
                                   C.c_void_p(mask.ctypes.data), C.c_void_p(strat.ctypes.data),
                                   C.c_void_p(gpus.ctypes.data), C.c_void_p(node.ctypes.data), C.byref(mk)))
         return {"start": start, "slotmask": mask, "strategy": strat, "gpus": gpus, "node": node,
@@ -298,7 +343,7 @@ class Engine:
         objective="completion": minimise the sum of completion times (every score and key holds that sum).
         _extra_flags: test hooks of sb_search_params.flags (_lib.HOOK_*)."""
         p = SearchParams(seed=seed, chains=chains, chain_base=chain_base, resample_every=int(resample_every or 0),
-                         flags=_flags(integer_starts, reduced, objective) | (_lib.HOOK_NO_FUSED if _no_fused else 0) |
+                         flags=self._flags(integer_starts, reduced, objective) | (_lib.HOOK_NO_FUSED if _no_fused else 0) |
                          int(_extra_flags),
                          t_start=t_start, t_end=t_end, total_rounds=total_rounds)
         wo = wp = None
@@ -327,6 +372,7 @@ class Engine:
         """The whole single-GPU search in one C call (sb_search_run).  Returns a dict: opt, prio, makespan, key,
         evaluated, rounds, stop_reason, wall_s, history [(wall s, evaluated, makespan)].  With
         objective="completion" every "makespan" there is the sum of completion times, and target_makespan targets it."""
+        _require_due(self.due, objective)
         return _search_run(self._lib, [self._h], self.J, chains, rounds, seed, chain_base, integer_starts, reduced,
                            t_start, t_end, warm, resample_every, sync_every, patience, time_budget_s, target_makespan,
                            heuristic_seeds, record_history, _no_fused, _extra_flags, objective)
@@ -482,6 +528,14 @@ class MultiEngine:
 
     weights = property(lambda self: self.engines[0].weights)
 
+    def set_due(self, d):
+        """Engine.set_due on every device."""
+        for e in self.engines:
+            e.set_due(d)
+        return self
+
+    due = property(lambda self: self.engines[0].due)
+
     def decode(self, *a, **kw):
         return self.engines[0].decode(*a, **kw)
 
@@ -495,6 +549,7 @@ class MultiEngine:
                    target_makespan: float = 0.0, heuristic_seeds: bool = True, record_history: bool = False,
                    _no_fused: bool = False, _extra_flags: int = 0, objective: str = "makespan"):
         """`chains` is per device; the result's `evaluated` counts every device."""
+        _require_due(self.due, objective)
         return _search_run(self._lib, [e._h for e in self.engines], self.J, chains, rounds, seed, chain_base,
                            integer_starts, reduced, t_start, t_end, warm, resample_every, sync_every, patience,
                            time_budget_s, target_makespan, heuristic_seeds, record_history, _no_fused, _extra_flags,

@@ -12,9 +12,10 @@ simulated time (useful for what-if planning and for the tests).
 from __future__ import annotations
 
 import logging
+from collections.abc import Mapping
 from typing import Callable, Optional
 
-from .solver import convert_into_comprehensible, solve
+from .solver import SolverError, convert_into_comprehensible, solve
 
 
 def forecast(task_list, interval, interval_sta):
@@ -52,13 +53,24 @@ def orchestrate(task_list, log=False, interval=1000, gurobi=True, *,
     Same positional signature as the reference (orchestrator.py:32).  `execute_fn(relevant_tasks,
     batches_to_run, interval, node_per_task, task_dependency_dict)` stands in for
     saturn.executor.execute; returns the list of per-interval records (plan makespan, tasks run).
+
+    A `due` mapping Task -> due date in `solver_kwargs` (objective="tardiness") is measured from the first plan's
+    t = 0: the solve for interval n plans from n * interval on, so it receives {t: d - n * interval}.  A sequence
+    `due` raises SolverError, since the task list shrinks from interval to interval.
     """
     logging.basicConfig(level=logging.INFO if log else logging.WARNING,
                         format="%(asctime)s %(levelname)-8s %(message)s", datefmt="%Y-%m-%d %H:%M:%S")
     kw = dict(solver_kwargs or {})
+    due = kw.pop("due", None)
+    if due is not None and not isinstance(due, Mapping):
+        raise SolverError("orchestrate() needs due as a mapping Task -> due date: its task list shrinks every interval")
+
+    def kw_at(n):  # the solver arguments of the plan for interval n (whose t = 0 is n * interval)
+        return kw if due is None else dict(kw, due={t: d - n * interval for t, d in due.items()})
+
     task_list = list(task_list)
     records = []
-    presolved = solve(task_list, None, gurobi=gurobi, interval=interval, timeout=max(1, interval // 2), **kw)
+    presolved = solve(task_list, None, gurobi=gurobi, interval=interval, timeout=max(1, interval // 2), **kw_at(0))
     sta, tga, bss, bna, boa, makespan = presolved
     npt, tdd, sta_comp = convert_into_comprehensible(task_list, bss, boa, tga, bna, sta)
     n = 0
@@ -73,7 +85,7 @@ def orchestrate(task_list, log=False, interval=1000, gurobi=True, *,
         if len(task_list) == 0:
             break
         presolved = solve(task_list, presolved, gurobi=gurobi, interval=interval,
-                          timeout=max(1, interval // 2), **kw)
+                          timeout=max(1, interval // 2), **kw_at(n + 1))
         sta, tga, bss, bna, boa, makespan = presolved
         npt, tdd, sta_comp = convert_into_comprehensible(task_list, bss, boa, tga, bna, sta)
         n += 1

@@ -30,6 +30,7 @@ class SearchResult:
     wall_s: float
     history: List[Tuple[float, int, float]] = field(default_factory=list)  # (wall s, evaluated, best makespan)
     owner_rank: int = 0
+    stop_reason: int = 0    # as sb_search_result: 0 rounds, 1 time budget, 2 patience, 3 target (or tardiness 0)
 
 
 def _dist():
@@ -44,7 +45,7 @@ def key_makespan(key: int) -> float:
 
 
 def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objective: str = "makespan",
-              weights: Optional[np.ndarray] = None):
+              weights: Optional[np.ndarray] = None, due: Optional[np.ndarray] = None):
     """Heuristic warm candidates in the reduced encoding (opt byte = k-1, plus node << 3 when there
     are several nodes), longest-processing-time order: (a) every job on its fastest option,
     (b) every job on its least GPU-seconds option, (c) in between.  Nodes are filled greedily by
@@ -52,12 +53,18 @@ def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objecti
     runtime of the chosen option), the order that favours the sum of completion times; same options and
     node fill (sb_search_seed_lpt plants the same seeds).  objective="weighted_completion" with the fp32 job
     `weights`: WSPT order (Smith's rule), ascending runtime / weight in float64, ties by job index — for unit
-    weights exactly the shortest-processing-time order."""
+    weights exactly the shortest-processing-time order.  objective="tardiness" / "weighted_tardiness" with the fp32
+    `due` dates: EDD order (earliest due date first), ties by runtime (by runtime / weight when weighted), then by
+    job index."""
     objective_flag(objective)
-    if objective == "weighted_completion":
+    if objective.startswith("weighted_"):
         if weights is None:
-            raise ValueError("objective='weighted_completion' needs the job weights")
+            raise ValueError("objective=%r needs the job weights" % objective)
         w64 = np.asarray(weights, dtype=np.float32).astype(np.float64)
+    if objective.endswith("tardiness"):
+        if due is None:
+            raise ValueError("objective=%r needs the job due dates" % objective)
+        d32 = np.asarray(due, dtype=np.float32)
     J = tmin.shape[0]
     usable = np.where(tmin < sentinel, tmin, np.inf)
     if not np.isfinite(usable).any(axis=1).all():
@@ -68,7 +75,10 @@ def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objecti
         cost = usable.astype(np.float64) * (k ** area_weight)
         col = np.argmin(cost, axis=1)
         rt = usable[np.arange(J), col]
-        if objective == "weighted_completion":
+        if objective.endswith("tardiness"):
+            tie = rt.astype(np.float64) / w64 if objective == "weighted_tardiness" else rt.astype(np.float64)
+            order = np.lexsort((np.arange(J), tie, d32))
+        elif objective == "weighted_completion":
             order = np.argsort(rt.astype(np.float64) / w64, kind="stable")
         elif objective == "completion":
             order = np.argsort(rt, kind="stable")
@@ -97,7 +107,8 @@ def run_search(engine: Engine, chains: int = 1 << 16, rounds: int = 200, seed: i
     """Run the search on `engine` (table already set).  Returns the best candidate found by any rank.
     objective="completion" minimises the sum of completion times; the result's `makespan`, the history and
     `target_makespan` then hold / target that sum.  objective="weighted_completion" minimises the sum weighted by
-    the engine's set_weights.
+    the engine's set_weights.  objective="tardiness" / "weighted_tardiness" minimises the total (weighted) tardiness
+    against the engine's set_due, and stops as soon as the incumbent's tardiness is 0, which no plan can beat.
 
     `rounds` device rounds are issued in groups of `exchange_every` (tournament resampling every
     `resample_every` rounds inside a group is only another launch); after each group the ranks exchange
@@ -116,7 +127,8 @@ def run_search(engine: Engine, chains: int = 1 << 16, rounds: int = 200, seed: i
                               record_history=record_history, _no_fused=_no_fused, _extra_flags=_extra_flags,
                               **({"objective": objective} if objective != "makespan" else {}))
         return SearchResult(opt=r["opt"], prio=r["prio"], makespan=r["makespan"], evaluated=r["evaluated"],
-                            rounds=r["rounds"], wall_s=r["wall_s"], history=r["history"], owner_rank=0)
+                            rounds=r["rounds"], wall_s=r["wall_s"], history=r["history"], owner_rank=0,
+                            stop_reason=r["stop_reason"])
     rank = dist.get_rank() if dist else 0
     world = dist.get_world_size() if dist else 1
     J = engine.J
@@ -134,7 +146,8 @@ def run_search(engine: Engine, chains: int = 1 << 16, rounds: int = 200, seed: i
         per = max(1, chains // 8)
         nodes = getattr(engine, "nodes", 1)
         for i, (col, order) in enumerate(lpt_seeds(tmin, nodes=nodes, objective=objective,
-                                                   weights=getattr(engine, "weights", None))):
+                                                   weights=getattr(engine, "weights", None),
+                                                   due=getattr(engine, "due", None))):
             opt = col if reduced else ((args[np.arange(J), col & 7].astype(np.uint8) << 3) | col)
             first = min(i * per, max(0, chains - per))
             engine.search_inject(opt.astype(np.uint8), order.astype(pdt), copies=min(per, chains), first=first)
@@ -176,7 +189,9 @@ def run_search(engine: Engine, chains: int = 1 << 16, rounds: int = 200, seed: i
     if record_history:
         history.append((time.perf_counter() - t0, chains * world, key_makespan(key)))
     exchange_every = max(1, int(exchange_every))
-    while done_rounds < rounds:
+    at_zero = objective.endswith("tardiness")  # a tardiness of +0 (key bits 0) cannot be beaten
+    reason = 3 if at_zero and (best_seen >> 32) == 0 else 0
+    while reason == 0 and done_rounds < rounds:
         # one group of rounds, no host synchronisation; the library resamples on its own cadence
         step = min(exchange_every, rounds - done_rounds)
         engine.search_round(step)
@@ -191,18 +206,21 @@ def run_search(engine: Engine, chains: int = 1 << 16, rounds: int = 200, seed: i
         if record_history:
             history.append((time.perf_counter() - t0, chains * world * (done_rounds + 1), key_makespan(key)))
         # stopping decisions must be identical on every rank: derive them from rank 0's clock
-        want_stop = False
+        want_stop = 0
         if time_budget_s is not None and time.perf_counter() - t0 > time_budget_s:
-            want_stop = True
-        if patience is not None and stale >= patience:
-            want_stop = True
-        if target_makespan is not None and key_makespan(best_seen) <= target_makespan:
-            want_stop = True
+            want_stop = 1
+        elif patience is not None and stale >= patience:
+            want_stop = 2
+        elif target_makespan is not None and key_makespan(best_seen) <= target_makespan:
+            want_stop = 3
+        elif at_zero and (best_seen >> 32) == 0:
+            want_stop = 3
         if dist:
-            stop.fill_(1 if want_stop else 0)
+            stop.fill_(want_stop)
             dist.broadcast(stop, src=0)
-            want_stop = bool(stop.item())
+            want_stop = int(stop.item())
         if want_stop:
+            reason = want_stop
             break
         if reseed_every and (r + 1) % reseed_every == 0 and r + 1 < rounds:
             opt, prio = _gather_best(engine, best_seen, chains, dist, rank)
@@ -216,7 +234,7 @@ def run_search(engine: Engine, chains: int = 1 << 16, rounds: int = 200, seed: i
         total_ev = int(evt.item())
     return SearchResult(opt=opt, prio=prio, makespan=key_makespan(best_seen), evaluated=total_ev,
                         rounds=done_rounds, wall_s=time.perf_counter() - t0, history=history,
-                        owner_rank=int((best_seen & 0xffffffff) // chains) if world > 1 else 0)
+                        owner_rank=int((best_seen & 0xffffffff) // chains) if world > 1 else 0, stop_reason=reason)
 
 
 def _gather_best(engine: Engine, key: int, chains: int, dist, rank: int):

@@ -214,35 +214,73 @@ def _check_horizon(T, found_makespan=None):
                           "options" % lower)
 
 def _check_objective(objective, hysteresis=False):
-    if objective not in ("makespan", "completion"):
-        raise SolverError("objective must be 'makespan' or 'completion', not %r" % (objective,))
-    if objective == "completion" and hysteresis:
+    if objective not in ("makespan", "completion", "tardiness"):
+        raise SolverError("objective must be 'makespan', 'completion' or 'tardiness', not %r" % (objective,))
+    if objective != "makespan" and hysteresis:
         raise SolverError("hysteresis=True compares plans by makespan (milp.py:363-442); it is not defined for "
-                          "objective='completion'")
+                          "objective=%r" % (objective,))
+
+
+def _per_task(values, what, task_list):
+    """A per-task argument as a list in task order: a sequence aligned with the tasks (or T's rows), or, with
+    `task_list`, a mapping keyed by Task — what an orchestrate() loop needs, since its task list shrinks every
+    interval."""
+    if isinstance(values, Mapping):
+        if task_list is None:
+            raise SolverError("%s must be a sequence aligned with T's rows" % what)
+        missing = [getattr(t, "name", repr(t)) for t in task_list if t not in values]
+        if missing:
+            raise SolverError("%s has no entry for task(s) %s" % (what, ", ".join(map(str, missing[:5]))))
+        return [values[t] for t in task_list]
+    if isinstance(values, (str, bytes)) or not hasattr(values, "__len__"):
+        raise SolverError("%s must be a sequence of J numbers or a mapping Task -> number" % what)
+    return values
 
 
 def _resolve_weights(weights, objective, J, task_list=None):
     """The caller's per-task weights as (float64 values in task order, fp32 array for the device), or (None, None).
-    A sequence is aligned with the tasks (or T's rows); with `task_list`, a mapping keyed by Task is accepted too —
-    what an orchestrate() loop needs, since its task list shrinks every interval.  Raises SolverError before any
-    device call."""
+    Raises SolverError before any device call."""
     if weights is None:
         return None, None
-    if objective != "completion":
-        raise SolverError("weights apply to objective='completion' only (the weighted sum of completion times), "
-                          "not to %r" % (objective,))
-    if isinstance(weights, Mapping):
-        if task_list is None:
-            raise SolverError("weights must be a sequence aligned with T's rows")
-        missing = [getattr(t, "name", repr(t)) for t in task_list if t not in weights]
-        if missing:
-            raise SolverError("weights has no entry for task(s) %s" % ", ".join(map(str, missing[:5])))
-        weights = [weights[t] for t in task_list]
-    elif isinstance(weights, (str, bytes)) or not hasattr(weights, "__len__"):
-        raise SolverError("weights must be a sequence of J numbers or a mapping Task -> number")
+    if objective not in ("completion", "tardiness"):
+        raise SolverError("weights apply to objective='completion' or 'tardiness' only, not to %r" % (objective,))
+    weights = _per_task(weights, "weights", task_list)
     from .engine import weights_f32
     w32 = weights_f32(weights, J)
     return [float(x) for x in weights], w32
+
+
+def _resolve_due(due, objective, J, task_list=None):
+    """The caller's per-task due dates as (float64 values in task order, fp32 array for the device), or (None, None)
+    without objective="tardiness", which requires them.  Raises SolverError before any device call."""
+    if objective != "tardiness":
+        if due is not None:
+            raise SolverError("due dates apply to objective='tardiness' only, not to %r" % (objective,))
+        return None, None
+    if due is None:
+        raise SolverError("objective='tardiness' needs due dates (due=...)")
+    due = _per_task(due, "due", task_list)
+    from .engine import due_f32
+    d32 = due_f32(due, J)
+    return [float(x) for x in due], d32
+
+
+def _set_objective(eng, objective, w32, d32):
+    """Hand the weights and due dates to the engine; returns the engine objective the search runs."""
+    if w32 is not None:
+        eng.set_weights(w32)
+    if d32 is not None:
+        eng.set_due(d32)
+        return "weighted_tardiness" if w32 is not None else "tardiness"
+    return "weighted_completion" if w32 is not None else objective
+
+
+def _tardiness_stats(start, rts, w64, d64):
+    """weighted_tardiness (unit weights without w64) and late_tasks of a plan, in float64."""
+    late = [float(s) + float(r) - d for s, r, d in zip(start, rts, d64)]
+    w = w64 if w64 is not None else [1.0] * len(late)
+    return {"weighted_tardiness": sum(wi * max(0.0, x) for wi, x in zip(w, late)),
+            "late_tasks": sum(1 for x in late if x > 0)}
 
 
 def _plan_horizon(start, rt):
@@ -268,7 +306,7 @@ def _default_nodes() -> int:
 def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count() or 4) // 4), interval=1000,
           timeout=500, *, chains: Optional[int] = None, rounds: Optional[int] = None, seed: int = 0,
           integer_starts: bool = True, engine=None, hysteresis: Optional[bool] = None,
-          nodes: Optional[int] = None, devices=None, objective: str = "makespan", weights=None):
+          nodes: Optional[int] = None, devices=None, objective: str = "makespan", weights=None, due=None):
     """Drop-in for saturn.solver.solve (milp.py:23).
 
     Objective.  "makespan" (the default, the reference's) or "completion": minimise the sum of the tasks'
@@ -286,6 +324,16 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     SolverError before any device call.  last_stats["weighted_completion"] then holds the plan's weighted sum in
     float64 (the caller's weights, the tasks' own runtimes) and last_stats["device_makespan"] the device's fp32
     weighted sum; "total_completion" and the 6th element keep their meaning.
+
+    Due dates.  objective="tardiness" with `due` (a sequence aligned with task_list, or a mapping keyed by Task,
+    in the runtimes' units from the plan's t = 0) minimises the total tardiness sum_t max(0, C_t - d_t), with
+    C_t = start_t + runtime_t; with `weights` as well, the weighted tardiness sum_t w_t max(0, C_t - d_t).  Every
+    due date must be finite with |d| < 2^24 (negative: already overdue).  A missing `due`, `due` under another
+    objective, a wrong length, a task missing from the mapping or a bad value raises SolverError before any device
+    call, as does hysteresis=True.  The search stops as soon as it finds a plan with no tardiness.
+    last_stats["weighted_tardiness"] (unit weights without `weights`) and last_stats["late_tasks"] (tasks with
+    C_t > d_t) are computed in float64 from the emitted plan, the tasks' own runtimes and the caller's d and w;
+    last_stats["device_makespan"] holds the device's fp32 tardiness.
 
     Returns (sta, tga, bss, bna, boa, makespan) — milp.py:445 — with a real float makespan
     (the reference returns None on a cold start, milp.py:394-399; callers only thread it back in
@@ -307,7 +355,7 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     That observable behaviour is the default here.  `hysteresis=True` (or SATURN_B200_HYSTERESIS=1)
     enables the documented intent instead: keep the current plan, shifted by one interval, unless
     the new one is better by more than interval + 500 s (milp.py:363,377,429-442).  The rule is stated
-    in makespans: hysteresis=True with objective="completion" raises SolverError, and
+    in makespans: hysteresis=True with another objective raises SolverError, and
     SATURN_B200_HYSTERESIS applies to the makespan objective only.
     """
     from .search import run_search
@@ -316,6 +364,7 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     task_list = list(task_list)
     J = len(task_list)
     w64, w32 = _resolve_weights(weights, objective, J, task_list)
+    d64, d32 = _resolve_due(due, objective, J, task_list)
     if J == 0:
         return [[[] for _ in range(NSLOT)]], [], [], [], [], 0.0
     eng = engine if engine is not None else _engine(devices)
@@ -331,10 +380,7 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
         nodes = _default_nodes()
     nodes = int(nodes)
     eng.set_table(Tdev, list(range(1, NSLOT + 1)), sentinel=float("inf"), nodes=nodes)
-    search_objective = objective
-    if w32 is not None:
-        eng.set_weights(w32)
-        search_objective = "weighted_completion"
+    search_objective = _set_objective(eng, objective, w32, d32)
     if chains is None:
         chains = int(os.environ.get("SATURN_B200_CHAINS", 0))
         if chains <= 0:
@@ -379,6 +425,8 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
                   "total_completion": sum(float(dec["start"][i]) + float(rts[i]) for i in range(J))}
     if w64 is not None:
         last_stats["weighted_completion"] = sum(w64[i] * (float(dec["start"][i]) + float(rts[i])) for i in range(J))
+    if d64 is not None:
+        last_stats.update(_tardiness_stats(dec["start"], rts, w64, d64))
 
     # ---- introspection hysteresis (opt-in): the documented intent of milp.py:363-442
     out = prop + (prop_makespan,)
@@ -474,10 +522,11 @@ def strategies_from_table(T, mask, executors=None, params=None, gcount=None):
 def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeout=500, *,
                 chains: Optional[int] = None, rounds: Optional[int] = None, seed: int = 0,
                 integer_starts: bool = True, engine=None, nodes: Optional[int] = None, devices=None,
-                objective: str = "makespan", weights=None):
+                objective: str = "makespan", weights=None, due=None):
     """solve() on the dense profiler tensor T[J][S][G] (+ mask of usable cells, + gcount[G] GPU counts).
     `objective` as for solve(): "makespan" or "completion" (sum of completion times); `weights` as for solve(),
-    a sequence aligned with T's rows (the weighted sum of completion times, last_stats["weighted_completion"]).
+    a sequence aligned with T's rows (the weighted sum of completion times, last_stats["weighted_completion"]);
+    `due` as for solve() with objective="tardiness", a sequence aligned with T's rows.
 
     The table goes to the device un-reduced (sb_set_table: min over strategies with the first-minimum rule
     and its arg-min on the device, PerformanceEvaluator.py:101-115); the search runs on the reduced view
@@ -493,6 +542,7 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
         raise SolverError("T must be [J][S][G]")
     J, S, G = T.shape
     w64, w32 = _resolve_weights(weights, objective, J)
+    d64, d32 = _resolve_due(due, objective, J)
     if J == 0:
         return [[[] for _ in range(NSLOT)]], [], [], [], [], 0.0, np.zeros(0, dtype=np.int64)
     gcount = list(range(1, G + 1)) if gcount is None else [int(g) for g in gcount]
@@ -510,10 +560,7 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     eng = engine if engine is not None else _engine(devices)
     nodes = int(_default_nodes() if nodes is None else nodes)
     eng.set_table(Tdev, gcount, sentinel=float("inf"), nodes=nodes)
-    search_objective = objective
-    if w32 is not None:
-        eng.set_weights(w32)
-        search_objective = "weighted_completion"
+    search_objective = _set_objective(eng, objective, w32, d32)
     if chains is None:
         chains = int(os.environ.get("SATURN_B200_CHAINS", 0))
         if chains <= 0:
@@ -551,6 +598,8 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
                   "objective": objective, "total_completion": sum(float(dec["start"][j]) + rts[j] for j in range(J))}
     if w64 is not None:
         last_stats["weighted_completion"] = sum(w64[j] * (float(dec["start"][j]) + rts[j]) for j in range(J))
+    if d64 is not None:
+        last_stats.update(_tardiness_stats(dec["start"], rts, w64, d64))
     return arrays + (makespan, strategy)
 
 

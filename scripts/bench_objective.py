@@ -1,14 +1,17 @@
-"""Cost and effect of the sum-of-completion-times objectives (plain and weighted) on one GPU; prints one JSON line.
+"""Cost and effect of the sum-of-completion-times objectives (plain and weighted) and of the weighted tardiness on
+one GPU; prints one JSON line.
 
     python scripts/bench_objective.py [--steps 200] [--warmup 20] [--solve-chains 0] [--solve-rounds 400]
 
 kernel: sb_eval on bench.py's C4 batch (J = 256, S = 8, 946,176 candidates, the same seeded inputs, integer
-        starts), scored for the makespan, the sum of completion times and the weighted sum (seeded weights), the
-        three launches alternated in one process (the order rotates every step) and timed with CUDA events; median
-        of --steps launches each.
+        starts), scored for the makespan, the sum of completion times, the weighted sum (seeded weights) and the
+        weighted tardiness (the same weights, seeded due dates), the four launches alternated in one process (the
+        order rotates every step) and timed with CUDA events; median of --steps launches each.
 solve:  solve() wall time on a 256-task set (synthetic table, seed 3, 4 strategies) for the makespan, the sum of
         completion times and the weighted sum (seeded weights: 32 tasks of weight 8, the rest 1), each plan scored
-        on all three measures (float64, the tasks' own runtimes).
+        on all three measures (float64, the tasks' own runtimes); and the total tardiness (unit weights, seeded
+        integer due dates in [0, 200000) s): its tardiness and late tasks against those of the makespan and
+        completion plans.
 The card's name and power limit are read in the same run (nvidia-smi, read-only queries).
 """
 import argparse
@@ -55,12 +58,13 @@ def main():
     eng.set_table(T)
     opt, prio = random_candidates(eng, B, valid, seed=1)
     eng.set_weights(np.random.default_rng(2).choice([1.0, 2.0, 3.0, 5.0, 8.0, 0.25, 0.5, 1.5], size=J))
+    eng.set_due(np.random.default_rng(3).integers(0, 20000, size=J))
     out = torch.empty(B, dtype=torch.float32, device=eng.device)
     key = torch.full((1,), 2 ** 63 - 1, dtype=torch.int64, device=eng.device)
-    objs = ("makespan", "completion", "weighted_completion")
+    objs = ("makespan", "completion", "weighted_completion", "weighted_tardiness")
     times = {o: [] for o in objs}
     for i in range(args.warmup + args.steps):
-        for obj in objs[i % 3:] + objs[:i % 3]:
+        for obj in objs[i % len(objs):] + objs[:i % len(objs)]:
             a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             a.record()
             eng.eval(opt, prio, out=out, best_key=key, objective=obj)
@@ -74,6 +78,7 @@ def main():
               for o, t in times.items()}
     kernel["completion_over_makespan"] = kernel["completion"]["median_ms"] / kernel["makespan"]["median_ms"]
     kernel["weighted_over_completion"] = kernel["weighted_completion"]["median_ms"] / kernel["completion"]["median_ms"]
+    kernel["tardiness_over_weighted"] = kernel["weighted_tardiness"]["median_ms"] / kernel["weighted_completion"]["median_ms"]
     kernel.update(B=B, J=J, S=Sx, path=path, steps=args.steps)
     del opt, prio, out
     torch.cuda.empty_cache()
@@ -97,11 +102,13 @@ def main():
     S.solve(tasks, None, rounds=4, engine=eng, objective="completion")
     w = [8.0 if j % 8 == 0 else 1.0 for j in range(len(tasks))]
     S.solve(tasks, None, rounds=4, engine=eng, objective="completion", weights=w)
+    due = [float(x) for x in np.random.default_rng(4).integers(0, 200000, size=len(tasks))]
+    S.solve(tasks, None, rounds=4, engine=eng, objective="tardiness", due=due)
     solve = {}
     for name, obj, weights in (("makespan", "makespan", None), ("completion", "completion", None),
-                               ("weighted_completion", "completion", w)):
+                               ("weighted_completion", "completion", w), ("tardiness", "tardiness", None)):
         t0 = time.perf_counter()
-        res = S.solve(tasks, None, objective=obj, weights=weights, **kw)
+        res = S.solve(tasks, None, objective=obj, weights=weights, **({"due": due} if obj == "tardiness" else {}), **kw)
         wall = time.perf_counter() - t0
         st = S.last_stats
         # the plan scored on all three measures, in float64 from its starts and the tasks' own runtimes
@@ -111,6 +118,8 @@ def main():
                        "mean_completion": st["total_completion"] / len(tasks),
                        "weighted_completion": sum(wi * c for wi, c in zip(w, comp)),
                        "heavy_mean_completion": float(np.mean([c for wi, c in zip(w, comp) if wi > 1])),
+                       "tardiness": sum(max(0.0, c - d) for c, d in zip(comp, due)),
+                       "late_tasks": sum(1 for c, d in zip(comp, due) if c > d),
                        "rounds": st["rounds"], "candidates": st["candidates"]}
     print(json.dumps({"card": card(0), "kernel": kernel, "solve": solve}))
     eng.close()
