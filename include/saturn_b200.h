@@ -55,6 +55,12 @@
  * d = 0 gives exactly the weighted fold, due dates at or past every completion give +0, w = 2 exactly twice w = 1.
  * The score is >= +0, so the (bits << 32) | id key still orders by it.
  * The schedule, every start and every slot mask are the same under every objective.
+ * With SB_FLAG_RELEASE (per-job release dates r_j, sb_set_release; valid under every objective above) a job may not
+ * start before its release:
+ *       start = max(max(ready[sel]), r_j)
+ * slot selection and everything after the start are unchanged, and so is every score's fold.  r <= 0 means the job
+ * is already released (max(ready, r) = ready, since ready >= +0).  With integer_starts the release enters as
+ * ceil(r_j), so every start stays an integer.  All-zero release dates give exactly the results without the flag.
  * With integer_starts the slot state is the integer time a slot becomes usable, start + ceil(rt);
  * SURVEY.md §8a writes the same rule as `start = ceil(max ready)` over real-valued ready times.  Starts,
  * makespans and the set of k slots taken are identical (ceil is monotone); the one observable difference
@@ -134,6 +140,15 @@ typedef enum sb_status {
                                      incumbent is +0 (stop_reason 3), and sb_search_seed_lpt plants EDD orders
                                      (ascending due date, ties by runtime / weight, then job index).  Not available
                                      with SB_FLAG_ALT_WARPSCAN (SB_ERR_UNSUPPORTED). */
+#define SB_FLAG_RELEASE 512u       /* after sb_set_release (else SB_ERR_STATE): no job starts before its release date
+                                     (see the evaluation rule above).  Valid under every objective (the makespan,
+                                     SB_FLAG_SUM_COMPLETION, SB_FLAG_WEIGHTED and SB_FLAG_DUE), and accepted by
+                                     sb_eval, sb_eval_host, sb_eval_full, sb_decode and the search,
+                                     sb_search_run_multi included (every handle must hold release dates).  The
+                                     search's temperature unit and stopping rules are unchanged; sb_search_seed_lpt
+                                     re-sorts each seed's order stably by ascending release date (ceiled with
+                                     SB_FLAG_INTEGER_STARTS), so jobs released together keep the objective's order.
+                                     Not available with SB_FLAG_ALT_WARPSCAN (SB_ERR_UNSUPPORTED). */
 #define SB_IPC_HANDLE_BYTES 64
 
 typedef struct sb_handle sb_handle;
@@ -172,6 +187,12 @@ int sb_set_weights(sb_handle* h, const float* w, int J);
  * d = NULL clears them.  SB_ERR_STATE before sb_set_table.  sb_set_table clears the due dates; setting or clearing
  * them ends the current search (sb_search_init again). */
 int sb_set_due(sb_handle* h, const float* d, int J);
+/* Per-job release dates for SB_FLAG_RELEASE: r host fp32 [J] in the runtimes' units from the plan's t = 0, every
+ * value finite with |r| < 2^24 (r <= 0: already released) (else SB_ERR_ARG, as is a J that differs from the
+ * table's); r = NULL clears them.  SB_ERR_STATE before sb_set_table.  The ceiled copy that SB_FLAG_INTEGER_STARTS
+ * uses is made here, once.  sb_set_table clears the release dates; setting or clearing them ends the current
+ * search (sb_search_init again). */
+int sb_set_release(sb_handle* h, const float* r, int J);
 /* copy the reduced table back (host pointers, either may be NULL): tmin fp32 [J][8], args u8 [J][8].
  * This is the table the reference solver is actually given: Task.strategies[g] after the profiler's
  * min over executors (PerformanceEvaluator.py:101-115), read at milp.py:77-81. */

@@ -61,6 +61,7 @@ struct SearchState {
   SearchDev alloc;  // the pointers as allocated (s.d's cur / prop pairs trade places when resampling)
   const float* w = nullptr;    // SB_FLAG_WEIGHTED: the handle's job weights (SB_FLAG_DUE alone: its unit weights)
   const float* due = nullptr;  // SB_FLAG_DUE: the handle's due dates (position-major kernels)
+  const float* rel = nullptr;  // SB_FLAG_RELEASE: the handle's release dates as the flags read them (likewise)
 };
 
 struct sb_handle {
@@ -107,6 +108,13 @@ struct sb_handle {
   size_t d_d_cap = 0;
   std::vector<float> h_d;
   bool has_d = false;
+  // release dates (sb_set_release): device copies padded like d_w, as given (d_r) and ceiled for
+  // SB_FLAG_INTEGER_STARTS (d_rc), and the host copies (seed orders); has_r is cleared by sb_set_table
+  float* d_r = nullptr;
+  float* d_rc = nullptr;
+  size_t d_r_cap = 0;
+  std::vector<float> h_r, h_rc;
+  bool has_r = false;
   SearchState search;
   int last_path = -1;
   // peer-memory exchange
@@ -220,6 +228,8 @@ int sb_destroy(sb_handle* h) {
   cudaFree(h->d_w);
   cudaFree(h->d_d);
   cudaFree(h->d_one);
+  cudaFree(h->d_r);
+  cudaFree(h->d_rc);
   for (int i = 0; i < 2; ++i)
     if (h->hs[i]) cudaStreamDestroy(h->hs[i]);
   if (h->own_stream && h->stream) cudaStreamDestroy(h->stream);
@@ -251,6 +261,7 @@ int sb_set_table(sb_handle* h, const float* T, const uint8_t* gcount, int J, int
   h->search.ready = false;  // its buffers are reused by the next sb_search_init if the shape is unchanged
   h->has_w = false;         // weights belong to a task set: a new table needs new ones
   h->has_d = false;         // so do due dates
+  h->has_r = false;         // and release dates
   const size_t nT = static_cast<size_t>(J) * S * G;
   const size_t ntab = static_cast<size_t>(J) * S * kSlots;
   // a re-planning loop sets a table of the same shape every interval: keep the allocations (cudaFree /
@@ -384,8 +395,47 @@ int sb_set_due(sb_handle* h, const float* d, int J) {
   return SB_OK;
 }
 
+int sb_set_release(sb_handle* h, const float* r, int J) {
+  int rc = use_device(h);
+  if (rc) return rc;
+  if (h->J == 0) return fail(SB_ERR_STATE, "sb_set_table has not been called");
+  CK(cudaStreamSynchronize(h->stream));  // no queued kernel may still read the old release dates
+  h->search.ready = false;               // the running search was set up for the old release dates (seeds)
+  if (!r) {
+    h->has_r = false;
+    return SB_OK;
+  }
+  if (J != h->J) return fail(SB_ERR_ARG, "J=%d differs from the table's J=%d", J, h->J);
+  for (int j = 0; j < J; ++j)
+    if (!isfinite(r[j]) || !(fabsf(r[j]) < 16777216.f))
+      return fail(SB_ERR_ARG, "release date %d (%g) is not finite with |r| < 2^24", j, r[j]);
+  h->has_r = false;
+  const size_t cap = static_cast<size_t>((J + 3) & ~3);
+  if (h->d_r_cap < cap) {
+    cudaFree(h->d_r);
+    cudaFree(h->d_rc);
+    h->d_r = h->d_rc = nullptr;
+    h->d_r_cap = 0;
+    CK(cudaMalloc(&h->d_r, cap * sizeof(float)));
+    CK(cudaMalloc(&h->d_rc, cap * sizeof(float)));
+    h->d_r_cap = cap;
+  }
+  // -0 is stored as +0 (x + 0 = x otherwise), so that max(ready, r) with ready = +0 is +0 whatever max does with
+  // zeros of both signs: a released job's start keeps its bits
+  h->h_r.assign(cap, 0.f);
+  for (int j = 0; j < J; ++j) h->h_r[j] = r[j] + 0.f;
+  // integer starts: a start >= r is a start >= ceil(r) (exact in fp32 below 2^24), so the step needs no rounding
+  h->h_rc.resize(cap);
+  for (size_t j = 0; j < cap; ++j) h->h_rc[j] = ceilf(h->h_r[j]) + 0.f;
+  CK(cudaMemcpyAsync(h->d_r, h->h_r.data(), cap * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+  CK(cudaMemcpyAsync(h->d_rc, h->h_rc.data(), cap * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  h->has_r = true;
+  return SB_OK;
+}
+
 // SB_FLAG_WEIGHTED and SB_FLAG_DUE are valid with SB_FLAG_SUM_COMPLETION only, and after sb_set_weights /
-// sb_set_due respectively
+// sb_set_due respectively; SB_FLAG_RELEASE under any objective, after sb_set_release
 static int check_per_job(const sb_handle* h, unsigned flags) {
   if ((flags & SB_FLAG_WEIGHTED) && !(flags & SB_FLAG_SUM_COMPLETION))
     return fail(SB_ERR_ARG, "SB_FLAG_WEIGHTED weights the sum of completion times: it needs SB_FLAG_SUM_COMPLETION");
@@ -395,7 +445,14 @@ static int check_per_job(const sb_handle* h, unsigned flags) {
     return fail(SB_ERR_STATE, "SB_FLAG_WEIGHTED needs sb_set_weights (sb_set_table clears the weights)");
   if ((flags & SB_FLAG_DUE) && !h->has_d)
     return fail(SB_ERR_STATE, "SB_FLAG_DUE needs sb_set_due (sb_set_table clears the due dates)");
+  if ((flags & SB_FLAG_RELEASE) && !h->has_r)
+    return fail(SB_ERR_STATE, "SB_FLAG_RELEASE needs sb_set_release (sb_set_table clears the release dates)");
   return SB_OK;
+}
+// the release dates the kernels read: ceiled under SB_FLAG_INTEGER_STARTS, as given otherwise, or none
+static const float* job_release(const sb_handle* h, unsigned flags) {
+  if (!(flags & SB_FLAG_RELEASE)) return nullptr;
+  return (flags & SB_FLAG_INTEGER_STARTS) ? h->d_rc : h->d_r;
 }
 // the weights the kernels read: the caller's, the unit weights of SB_FLAG_DUE alone, or none
 static const float* job_weights(const sb_handle* h, unsigned flags) {
@@ -438,6 +495,7 @@ static int make_call(sb_handle* h, const uint8_t* opt, const void* prio, int64_t
   c->flags = flags;
   c->w = job_weights(h, flags);
   c->d = (flags & SB_FLAG_DUE) ? h->d_d : nullptr;
+  c->r = job_release(h, flags);
   return SB_OK;
 }
 
@@ -496,9 +554,9 @@ int sb_eval(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, int64
     }
   }
   if (flags & SB_FLAG_ALT_WARPSCAN) {
-    if (flags & (SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED | SB_FLAG_DUE))
-      return fail(SB_ERR_UNSUPPORTED, "SB_FLAG_ALT_WARPSCAN scores the makespan only: it cannot be combined with "
-                  "SB_FLAG_SUM_COMPLETION, SB_FLAG_WEIGHTED or SB_FLAG_DUE");
+    if (flags & (SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED | SB_FLAG_DUE | SB_FLAG_RELEASE))
+      return fail(SB_ERR_UNSUPPORTED, "SB_FLAG_ALT_WARPSCAN scores the makespan without release dates only: it "
+                  "cannot be combined with SB_FLAG_SUM_COMPLETION, SB_FLAG_WEIGHTED, SB_FLAG_DUE or SB_FLAG_RELEASE");
     if (flags & (SB_FLAG_POST_KEY | SB_FLAG_FOLD_PREV))
       return fail(SB_ERR_UNSUPPORTED, "SB_FLAG_ALT_WARPSCAN cannot be combined with the fused key exchange");
     cudaError_t e = eval_alt_launch(h->dev, c, h->stream);
@@ -826,7 +884,7 @@ static int search_eval(sb_handle* h, bool cur_rows, long long first, long long c
     SearchFuse sf = {};
     sf.cur_mk = s.d.cur_mk;
     const bool reduced = (s.p.flags & SB_FLAG_REDUCED) != 0;
-    CK(search_pos_launch(h->dev, s.d, reduced ? h->tmin : h->tab, s.w, s.due, (reduced ? 1 : h->S) * kSlots, s.p.flags, first,
+    CK(search_pos_launch(h->dev, s.d, reduced ? h->tmin : h->tab, s.w, s.due, s.rel, (reduced ? 1 : h->S) * kSlots, s.p.flags, first,
                          count, true, sf, h->stream));
     return SB_OK;
   }
@@ -868,6 +926,7 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
   const int arrays = job_arrays(p->flags);
   s.w = job_weights(h, p->flags);
   s.due = due ? h->d_d : nullptr;
+  s.rel = job_release(h, p->flags);
   d.stride_o = (J + 31) & ~31;  // 32-byte rows: TMA bulk copies for opt, 256-bit streaming loads for prio
   // make stride_p == stride_o * pb so that one element stride describes both (sb_eval contract)
   d.stride_p = d.stride_o * pb;
@@ -1055,7 +1114,7 @@ int sb_search_round(sb_handle* h, int rounds) {
       SearchFuse sf = make_fuse(s, round, n);
       sf.resample_every = 0;
       const bool reduced = (s.p.flags & SB_FLAG_REDUCED) != 0;
-      CK(search_pos_launch(h->dev, s.d, reduced ? h->tmin : h->tab, s.w, s.due, (reduced ? 1 : h->S) * kSlots, s.p.flags, 0,
+      CK(search_pos_launch(h->dev, s.d, reduced ? h->tmin : h->tab, s.w, s.due, s.rel, (reduced ? 1 : h->S) * kSlots, s.p.flags, 0,
                            s.d.chains, false, sf, h->stream));  // keeps the incumbent in its tail
       fused = true;
     } else if (s.fused_ok) {
@@ -1176,6 +1235,7 @@ int sb_search_seed_lpt(sb_handle* h) {
   const bool wspt = spt && (s.p.flags & SB_FLAG_WEIGHTED) != 0;
   // tardiness: earliest due date first (EDD), ties by rt / w (rt with unit weights), then by job index
   const bool edd = spt && (s.p.flags & SB_FLAG_DUE) != 0;
+  const bool rel = (s.p.flags & SB_FLAG_RELEASE) != 0;
   const double INF = HUGE_VAL;
   // usable cells: below the sentinel threshold; a job with none falls back to any finite cell
   std::vector<double> usable(static_cast<size_t>(J) * kSlots);
@@ -1223,6 +1283,10 @@ int sb_search_seed_lpt(sb_handle* h) {
       std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return weight[a] < weight[b]; });
     } else if (spt) std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return rt[a] < rt[b]; });
     else std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return weight[a] > weight[b]; });
+    if (rel) {  // release dates: ascending release first, the objective's order among jobs released together
+      const std::vector<float>& r = (s.p.flags & SB_FLAG_INTEGER_STARTS) ? h->h_rc : h->h_r;
+      std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return r[a] < r[b]; });
+    }
     std::vector<double> load(nodes, 0.0);
     for (int j = 0; j < J; ++j) opt[j] = static_cast<uint8_t>(col[j]);
     if (nodes > 1) {

@@ -150,10 +150,13 @@ __device__ __forceinline__ float fmax3_mk(float mk, float b, float c) {
 // reproduce); w = 1 then gives the unweighted fold bit for bit.
 // kDue (SB_FLAG_DUE, with kWeighted only): the job's tardiness max(e - d, +0) against its due date `d` takes the
 // completion's place, acc = acc + (w * max(e - d, +0)), each step rounded on its own; d = 0 gives the weighted fold.
+// kRelease (SB_FLAG_RELEASE, with any of the above): the job starts no earlier than its release date `r`,
+// s = max(f[km1], r) (ceil(r) under integer starts, made once by sb_set_release, so s stays an integer).  The slot
+// update below stays valid because it only needs v >= f[km1]; r <= 0 gives s = f[km1] exactly.
 template <bool kIntegerStarts, bool kTrackMk = kIntegerStarts, bool kSum = false, bool kWeighted = false,
-          bool kDue = false>
+          bool kDue = false, bool kRelease = false>
 __device__ __forceinline__ void ls_step(float (&f)[8], float& mk, float& pend, float rt, int km1, int one, int ph,
-                                        float w = 0.f, float d = 0.f) {
+                                        float w = 0.f, float d = 0.f, float r = 0.f) {
   static_assert(kSum || !kWeighted, "weights scale the sum of completion times only");
   static_assert(kWeighted || !kDue, "due dates run on the weighted form (unit weights for plain tardiness)");
   const float INF = inf_f();
@@ -168,7 +171,7 @@ __device__ __forceinline__ void ls_step(float (&f)[8], float& mk, float& pend, f
   // stage "shift by 1"
   pmov_fma(x0, x1, b0, one); pmov_fma(x1, x2, b0, one); pmov_fma(x2, x3, b0, one); pmov_fma(x3, x4, b0, one);
   pmov_fma(x4, x5, b0, one); pmov_fma(x5, x6, b0, one); pmov_fma(x6, x7, b0, one); pinf_fma(x7, b0);
-  const float s = x0;  // = f[km1]
+  const float s = kRelease ? fmaxf(x0, r) : x0;  // = f[km1], or the release if later
   float v;
   if (kIntegerStarts) {
     // every entry of f is an integer here, so s is; the slot is usable again at s + ceil(rt)

@@ -30,7 +30,9 @@
 //   * W (SB_FLAG_WEIGHTED, with SUM only): the sum is weighted per job.  The weights sit beside the table wherever
 //     the table is in shared memory (same TMA phase), and are read from global memory where the table is;
 //   * D (SB_FLAG_DUE, with W only): the weighted sum is of tardiness against per-job due dates instead of
-//     completions.  The due dates follow the weights, in the same memory and the same TMA phase.
+//     completions.  The due dates follow the weights, in the same memory and the same TMA phase;
+//   * R (SB_FLAG_RELEASE, with any of the above): no job starts before its release date.  Every objective form has
+//     a release twin; the release dates follow the other per-job arrays, in the same memory and TMA phase.
 #include "sb_lane.cuh"
 
 namespace sb {
@@ -55,12 +57,13 @@ struct TileArgs {
   XchgPost xp;    // xp.counter != nullptr: the last CTA to finish posts *best_key to every peer's mailbox
   const float* w;  // W: job weights [J], zero-padded to a multiple of 4 (16 bytes)
   const float* d;  // D: job due dates [J], padded the same way
+  const float* r;  // R: job release dates [J], padded the same way
 };
 
 // TABG: the runtime table stays in global memory (read through L1/L2) — for tables larger than the
 // shared memory left beside the opt tiles (e.g. J = 1024 with 8 strategies: 256 KB).
 template <int PB, bool INT, bool STREAM, bool MULTI, bool SEARCH = false, bool TABG = false, int ADDR = 0,
-          bool SUM = false, bool W = false, bool D = false>
+          bool SUM = false, bool W = false, bool D = false, bool R = false>
 __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const TileArgs a) {
   static_assert(!(SEARCH && (STREAM || TABG)), "the fused search round runs on shared-memory tiles only");
   static_assert(ADDR == 0 || (!TABG && !MULTI && !SEARCH), "ADDR = 1 needs the table and the opt rows in shared memory");
@@ -71,13 +74,15 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t tab_bytes = TABG ? 0u : static_cast<uint32_t>(a.J) * a.SG * 4u;  // a multiple of 32 (SG = S * 8)
   // W: the weights follow the table in the same TMA phase, padded to 16 bytes (TABG: both stay in global memory);
-  // D: the due dates follow the weights the same way
+  // D: the due dates follow the weights the same way; R: the release dates follow them
   const uint32_t w_bytes = (W && !TABG) ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u;
   const uint32_t d_bytes = D ? w_bytes : 0u;
+  const uint32_t r_bytes = (R && !TABG) ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u;
   float* tab_s = reinterpret_cast<float*>(smem);
   [[maybe_unused]] float* w_s = reinterpret_cast<float*>(smem + tab_bytes);
   [[maybe_unused]] float* d_s = reinterpret_cast<float*>(smem + tab_bytes + w_bytes);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + ((tab_bytes + w_bytes + d_bytes + 15u) & ~15u));
+  [[maybe_unused]] float* r_s = reinterpret_cast<float*>(smem + tab_bytes + w_bytes + d_bytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + ((tab_bytes + w_bytes + d_bytes + r_bytes + 15u) & ~15u));
   uint8_t* tiles = reinterpret_cast<uint8_t*>(bars) + (((1 + nw) * 8 + 15) & ~15);
   const uint32_t node_bytes = MULTI ? static_cast<uint32_t>(a.nodes) * 1024u : 0u;
   const uint32_t tile_bytes = 32u * (a.row_o + (STREAM ? 0 : a.row_p)) + node_bytes;
@@ -97,7 +102,7 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
   if constexpr (!TABG) {
     if (threadIdx.x == 0) {
       // stage the runtime table: TMA bulk copies of <= 32 KB each, one mbarrier phase
-      mbar_arrive_expect_tx(bar_tab, tab_bytes + w_bytes + d_bytes);
+      mbar_arrive_expect_tx(bar_tab, tab_bytes + w_bytes + d_bytes + r_bytes);
       const uint8_t* src = reinterpret_cast<const uint8_t*>(a.tab);
       for (uint32_t off = 0; off < tab_bytes; off += 32768u) {
         uint32_t n = min(32768u, tab_bytes - off);
@@ -113,10 +118,15 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
         for (uint32_t off = 0; off < d_bytes; off += 32768u)
           tma_bulk_g2s(smem + tab_bytes + w_bytes + off, dsrc + off, min(32768u, d_bytes - off), bar_tab);
       }
+      if constexpr (R) {
+        const uint8_t* rsrc = reinterpret_cast<const uint8_t*>(a.r);
+        for (uint32_t off = 0; off < r_bytes; off += 32768u)
+          tma_bulk_g2s(smem + tab_bytes + w_bytes + d_bytes + off, rsrc + off, min(32768u, r_bytes - off), bar_tab);
+      }
     }
   }
 
-  LaneState<INT, MULTI, ADDR, SUM, (W ? (TABG ? 2 : 1) : 0), D> st;
+  LaneState<INT, MULTI, ADDR, SUM, (W ? (TABG ? 2 : 1) : 0), D, (R ? (TABG ? 2 : 1) : 0)> st;
   if (TABG) st.tab = a.tab;
   else st.tab = tab_s;
   if constexpr (W) {
@@ -126,6 +136,10 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
   if constexpr (D) {
     st.dd = TABG ? a.d : d_s;
     st.dd_s = smem_u32(d_s);
+  }
+  if constexpr (R) {
+    st.rr = TABG ? a.r : r_s;
+    st.rr_s = smem_u32(r_s);
   }
   st.SG = a.SG;
   st.one = a.one;
@@ -251,6 +265,7 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
         float rb[kBatch];
         [[maybe_unused]] float wb[kBatch];  // W: the batch's weights, gathered with its runtimes
         [[maybe_unused]] float db[kBatch];  // D: the batch's due dates, likewise
+        [[maybe_unused]] float xb[kBatch];  // R: the batch's release dates, likewise
         auto resolve = [&](const uint32_t* w) {  // w: the kBatch / 4 words that hold the batch's job ids
           int js[kBatch];
 #pragma unroll
@@ -266,6 +281,10 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
           if constexpr (D) {
 #pragma unroll
             for (int i = 0; i < kBatch; ++i) db[i] = st.gather_d(js[i]);
+          }
+          if constexpr (R) {
+#pragma unroll
+            for (int i = 0; i < kBatch; ++i) xb[i] = st.gather_r(js[i]);
           }
         };
         if (nfull > 0) resolve(q.w);
@@ -284,6 +303,7 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
             float rc[kBatch];
             [[maybe_unused]] float wc[kBatch];
             [[maybe_unused]] float dc[kBatch];
+            [[maybe_unused]] float xc[kBatch];
 #pragma unroll
             for (int i = 0; i < kBatch; ++i) { oc[i] = ob[i]; rc[i] = rb[i]; }
             if constexpr (W) {
@@ -294,12 +314,17 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
 #pragma unroll
               for (int i = 0; i < kBatch; ++i) dc[i] = db[i];
             }
+            if constexpr (R) {
+#pragma unroll
+              for (int i = 0; i < kBatch; ++i) xc[i] = xb[i];
+            }
             resolve(b + 1 < STEPS / kBatch ? q.w + (b + 1) * (kBatch / 4) : head);
 #pragma unroll
             for (int i = 0; i < kBatch; ++i) {
-              if constexpr (D) st.step_resolved(static_cast<int>(oc[i]), rc[i], i & 1, wc[i], dc[i]);
-              else if constexpr (W) st.step_resolved(static_cast<int>(oc[i]), rc[i], i & 1, wc[i]);
-              else st.step_resolved(static_cast<int>(oc[i]), rc[i], i & 1);
+              const float x = R ? xc[i] : 0.f;
+              if constexpr (D) st.step_resolved(static_cast<int>(oc[i]), rc[i], i & 1, wc[i], dc[i], x);
+              else if constexpr (W) st.step_resolved(static_cast<int>(oc[i]), rc[i], i & 1, wc[i], 0.f, x);
+              else st.step_resolved(static_cast<int>(oc[i]), rc[i], i & 1, 0.f, 0.f, x);
             }
           }
           q = nxt;
@@ -592,9 +617,10 @@ struct GenericArgs {
   int one;
   const float* w;  // W: job weights [J], read with ld.global.nc
   const float* d;  // D: job due dates [J], likewise
+  const float* r;  // R: job release dates [J], likewise
 };
 
-template <int PB, bool INT, bool MULTI, bool SUM = false, bool W = false, bool D = false>
+template <int PB, bool INT, bool MULTI, bool SUM = false, bool W = false, bool D = false, bool R = false>
 __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
   static_assert(SUM || !W, "weights scale the sum of completion times only");
   static_assert(W || !D, "due dates run on the weighted form");
@@ -610,10 +636,11 @@ __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
     tab = tab_s;
   }
   const int lane = threadIdx.x & 31;
-  LaneState<INT, MULTI, 0, SUM, (W ? 2 : 0), D> st;
+  LaneState<INT, MULTI, 0, SUM, (W ? 2 : 0), D, (R ? 2 : 0)> st;
   st.tab = tab;
   st.wt = a.w;
   st.dd = a.d;
+  st.rr = a.r;
   st.SG = a.SG;
   st.one = a.one;
   st.ns = node_s + lane;
@@ -639,6 +666,11 @@ __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
         for (int t = 0; t < BATCH; ++t) os[t] = st.lookup_opt(js[t]);
 #pragma unroll
         for (int t = 0; t < BATCH; ++t) rts[t] = st.lookup_rt(js[t], os[t]);
+        [[maybe_unused]] float xs[BATCH];  // R: the batch's release dates, gathered with its runtimes
+        if constexpr (R) {
+#pragma unroll
+          for (int t = 0; t < BATCH; ++t) xs[t] = st.lookup_r(js[t]);
+        }
         if constexpr (D) {
           float ws[BATCH], ds[BATCH];
 #pragma unroll
@@ -646,16 +678,16 @@ __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
 #pragma unroll
           for (int t = 0; t < BATCH; ++t) ds[t] = st.lookup_d(js[t]);
 #pragma unroll
-          for (int t = 0; t < BATCH; ++t) st.step_resolved(os[t], rts[t], t & 1, ws[t], ds[t]);
+          for (int t = 0; t < BATCH; ++t) st.step_resolved(os[t], rts[t], t & 1, ws[t], ds[t], R ? xs[t] : 0.f);
         } else if constexpr (W) {
           float ws[BATCH];
 #pragma unroll
           for (int t = 0; t < BATCH; ++t) ws[t] = st.lookup_w(js[t]);
 #pragma unroll
-          for (int t = 0; t < BATCH; ++t) st.step_resolved(os[t], rts[t], t & 1, ws[t]);
+          for (int t = 0; t < BATCH; ++t) st.step_resolved(os[t], rts[t], t & 1, ws[t], 0.f, R ? xs[t] : 0.f);
         } else {
 #pragma unroll
-          for (int t = 0; t < BATCH; ++t) st.step_resolved(os[t], rts[t], t & 1);
+          for (int t = 0; t < BATCH; ++t) st.step_resolved(os[t], rts[t], t & 1, 0.f, 0.f, R ? xs[t] : 0.f);
         }
       }
       for (; i < a.J; ++i) st.step(PB == 1 ? prow[i] : reinterpret_cast<const uint16_t*>(prow)[i]);
@@ -685,9 +717,10 @@ struct FullArgs {
   uint32_t* slotmask;   // [B][J] by job, nullable
   const float* w;       // W: job weights [J]
   const float* d;       // D: job due dates [J]
+  const float* r;       // R: job release dates [J] (ceiled with INT)
 };
 
-template <int PB, bool INT, bool SUM = false, bool W = false, bool D = false>
+template <int PB, bool INT, bool SUM = false, bool W = false, bool D = false, bool R = false>
 __global__ void __launch_bounds__(128) k_eval_full(const FullArgs a) {
   static_assert(SUM || !W, "weights scale the sum of completion times only");
   static_assert(W || !D, "due dates run on the weighted form");
@@ -721,6 +754,7 @@ __global__ void __launch_bounds__(128) k_eval_full(const FullArgs a) {
         taken |= 1u << best;
         s = bv;  // scans return non-decreasing values: the last one is the k-th smallest
       }
+      if constexpr (R) s = fmaxf(s, __ldg(a.r + j));  // ls_step<..., kRelease>: not before the release
       const float hold = (INT && isfinite(rt)) ? ceilf(rt) : rt;
       const float nxt = s + hold;
       for (int g = 0; g < kSlots; ++g)
@@ -819,6 +853,7 @@ static TileArgs tile_args(const EvalCall& c, const TilePlan& tp) {
   a.out = c.out; a.best_key = c.best_key; a.id_base = c.id_base;
   a.w = c.w;
   a.d = c.d;
+  a.r = c.r;
   a.ntiles = (c.B + 31) / 32;
   a.one = 1;
   return a;
@@ -862,14 +897,14 @@ cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, i
     // the headline shape (u8 priorities streamed, one node, table in shared memory): address arithmetic on the FMA
     // pipe unless HOOK_PLAIN_ADDR asks for the plain form
     const bool fma_addr = pb == 1 && stream && !tabg && !multi && !(c.flags & HOOK_PLAIN_ADDR);
-    const TileKernel kern = with_eval_types(pb, c.flags, [&](auto PB, auto INT, auto SUM, auto W, auto D) -> TileKernel {
-      if (tabg) return k_eval_tiles<PB, INT, true, false, false, true, 0, SUM, W, D>;
+    const TileKernel kern = with_eval_types(pb, c.flags, [&](auto PB, auto INT, auto SUM, auto W, auto D, auto R) -> TileKernel {
+      if (tabg) return k_eval_tiles<PB, INT, true, false, false, true, 0, SUM, W, D, R>;
       if constexpr (PB == 1) {
-        if (fma_addr) return k_eval_tiles<1, INT, true, false, false, false, 1, SUM, W, D>;
+        if (fma_addr) return k_eval_tiles<1, INT, true, false, false, false, 1, SUM, W, D, R>;
       }
       return with_bool(stream, [&](auto STREAM) {
         return with_bool(multi, [&](auto MULTI) -> TileKernel {
-          return k_eval_tiles<PB, INT, STREAM, MULTI, false, false, 0, SUM, W, D>;
+          return k_eval_tiles<PB, INT, STREAM, MULTI, false, false, 0, SUM, W, D, R>;
         });
       });
     });
@@ -878,7 +913,7 @@ cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, i
   GenericArgs g;
   g.tab = c.tab; g.J = c.J; g.SG = c.SG; g.opt = c.opt; g.prio = c.prio; g.B = c.B;
   g.stride_o = c.stride_o; g.stride_p = c.stride_p; g.out = c.out; g.best_key = c.best_key;
-  g.id_base = c.id_base; g.tab_in_smem = 0; g.nodes = c.nodes; g.one = 1; g.w = c.w; g.d = c.d;
+  g.id_base = c.id_base; g.tab_in_smem = 0; g.nodes = c.nodes; g.one = 1; g.w = c.w; g.d = c.d; g.r = c.r;
   if (path_used) *path_used = 0;
   const size_t tab_bytes = static_cast<size_t>(c.J) * c.SG * 4;
   size_t smem = multi ? static_cast<size_t>(4) * c.nodes * 1024u : 0u;  // 4 warps per CTA
@@ -890,8 +925,8 @@ cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, i
   long long cap = static_cast<long long>(dev.sm_count) * 8;
   int grid = static_cast<int>(blocks < cap ? blocks : cap);
   if (grid < 1) grid = 1;
-  const auto kern = with_eval_types(pb, c.flags, [&](auto PB, auto INT, auto SUM, auto W, auto D) {
-    return with_bool(multi, [&](auto MULTI) { return k_eval_generic<PB, INT, MULTI, SUM, W, D>; });
+  const auto kern = with_eval_types(pb, c.flags, [&](auto PB, auto INT, auto SUM, auto W, auto D, auto R) {
+    return with_bool(multi, [&](auto MULTI) { return k_eval_generic<PB, INT, MULTI, SUM, W, D, R>; });
   });
   return launch(kern, grid, 128, smem, st, g);
 }
@@ -919,9 +954,9 @@ cudaError_t search_round_launch(const Device& dev, const EvalCall& c, const Sear
   TileArgs a = tile_args(c, tp);
   a.use_bulk = 1;
   a.sf = sf;
-  const TileKernel kern = with_eval_types(pb, c.flags, [&](auto PB, auto INT, auto SUM, auto W, auto D) {
+  const TileKernel kern = with_eval_types(pb, c.flags, [&](auto PB, auto INT, auto SUM, auto W, auto D, auto R) {
     return with_bool(c.nodes > 1, [&](auto MULTI) -> TileKernel {
-      return k_eval_tiles<PB, INT, false, MULTI, true, false, 0, SUM, W, D>;
+      return k_eval_tiles<PB, INT, false, MULTI, true, false, 0, SUM, W, D, R>;
     });
   });
   return launch_tiles(dev, kern, a, tp, st);
@@ -933,12 +968,12 @@ cudaError_t eval_full_launch(const Device& dev, const EvalCall& c, float* start,
   FullArgs a;
   a.tab = c.tab; a.J = c.J; a.SG = c.SG; a.opt = c.opt; a.prio = c.prio; a.B = c.B;
   a.stride_o = c.stride_o; a.stride_p = c.stride_p; a.nodes = c.nodes < 1 ? 1 : c.nodes;
-  a.out = c.out; a.start = start; a.slotmask = slotmask; a.w = c.w; a.d = c.d;
+  a.out = c.out; a.start = start; a.slotmask = slotmask; a.w = c.w; a.d = c.d; a.r = c.r;
   long long blocks = (c.B + 127) / 128;
   long long cap = static_cast<long long>(dev.sm_count) * 16;
   int grid = static_cast<int>(blocks < cap ? blocks : cap);
-  const auto kern = with_eval_types(pb, c.flags, [](auto PB, auto INT, auto SUM, auto W, auto D) {
-    return k_eval_full<PB, INT, SUM, W, D>;
+  const auto kern = with_eval_types(pb, c.flags, [](auto PB, auto INT, auto SUM, auto W, auto D, auto R) {
+    return k_eval_full<PB, INT, SUM, W, D, R>;
   });
   return launch(kern, grid, 128, 0, st, a);
 }

@@ -41,7 +41,9 @@ __device__ __forceinline__ PrioChunk ld_prio32(const uint8_t* p) {
 // weights are in shared memory beside the table, 2: in global memory, read with ld.global.nc.
 // DUE (SB_FLAG_DUE, with WGT only): each job's tardiness against its due date, read from `dd` (in the same memory
 // as the weights) takes its completion's place.
-template <bool INT, bool MULTI, int ADDR = 0, bool SUM = false, int WGT = 0, bool DUE = false>
+// REL (SB_FLAG_RELEASE, with any objective): no job starts before its release date, read from `rr` — 1: in shared
+// memory beside the table, 2: in global memory, read with ld.global.nc.
+template <bool INT, bool MULTI, int ADDR = 0, bool SUM = false, int WGT = 0, bool DUE = false, int REL = 0>
 struct LaneState {
   float f[8];
   float mk;
@@ -50,11 +52,13 @@ struct LaneState {
   const float* tab;     // runtime table (shared memory or global)
   const float* wt;      // WGT: the job weights [J]
   const float* dd;      // DUE: the job due dates [J]
+  const float* rr;      // REL: the job release dates [J]
   int SG;
   int one;
   uint32_t orow_s, tab_s, four;  // ADDR = 1: shared-window addresses of orow / tab, and a run-time 4
   uint32_t wt_s;                 // ADDR = 1 with WGT: shared-window address of wt
   uint32_t dd_s;                 // ADDR = 1 with DUE: shared-window address of dd
+  uint32_t rr_s;                 // ADDR = 1 with REL: shared-window address of rr
   float4* ns;  // MULTI: lane-private node-state column; node n lives at ns[(2n)*32], ns[(2n+1)*32]
   int cur;     // MULTI: the node whose state is currently in f[] (its shared-memory copy is stale)
 
@@ -101,14 +105,21 @@ struct LaneState {
     else if constexpr (WGT == 1) return dd[j];
     else return __ldg(dd + j);
   }
-  // ph: t & 1 inside fully unrolled loops, -1 elsewhere (see ls_step); w, d: the job's weight (WGT only) and due
-  // date (DUE only)
-  __device__ __forceinline__ void step_resolved(int o, float rt, int ph = -1, float w = 0.f, float d = 0.f) {
+  // the job's release date (REL only; 0 otherwise, and then unused)
+  __device__ __forceinline__ float lookup_r(int j) const {
+    if constexpr (REL == 1) return rr[j];
+    else if constexpr (REL == 2) return __ldg(rr + j);
+    else return 0.f;
+  }
+  // ph: t & 1 inside fully unrolled loops, -1 elsewhere (see ls_step); w, d, r: the job's weight (WGT only), due
+  // date (DUE only) and release date (REL only)
+  __device__ __forceinline__ void step_resolved(int o, float rt, int ph = -1, float w = 0.f, float d = 0.f,
+                                                float r = 0.f) {
     if (!MULTI) {
-      ls_step<INT, INT, SUM, (WGT != 0), DUE>(f, mk, pend, rt, o & 7, one, ph, w, d);
+      ls_step<INT, INT, SUM, (WGT != 0), DUE, (REL != 0)>(f, mk, pend, rt, o & 7, one, ph, w, d, r);
     } else {
       switch_node(o >> 3);
-      ls_step<INT, true, SUM, (WGT != 0), DUE>(f, mk, pend, rt, o & 7, one, ph, w, d);
+      ls_step<INT, true, SUM, (WGT != 0), DUE, (REL != 0)>(f, mk, pend, rt, o & 7, one, ph, w, d, r);
     }
   }
   // ADDR = 1: the two look-ups as separate gathers, so that the streamed loop of k_eval_tiles can issue a whole
@@ -151,23 +162,36 @@ struct LaneState {
       return d;
     }
   }
+  // ADDR = 1 with REL = 1: the release-date gather, like gather_w
+  __device__ __forceinline__ float gather_r(int j) const {
+    if constexpr (REL == 0) {
+      return 0.f;
+    } else {
+      uint32_t ra;
+      float r;
+      asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(ra) : "r"(j), "r"(four), "r"(rr_s));
+      asm("ld.shared.f32 %0, [%1];" : "=f"(r) : "r"(ra));
+      return r;
+    }
+  }
   __device__ __forceinline__ void step(int j, int ph = -1) {
     constexpr bool W = WGT != 0;
+    constexpr bool R = REL != 0;
     if (!MULTI && ADDR == 1) {
       const uint32_t o = gather_opt(j);
-      ls_step<INT, INT, SUM, W, DUE>(f, mk, pend, gather_rt(j, o), static_cast<int>(o & 7u), one, ph, gather_w(j),
-                                     gather_d(j));
+      ls_step<INT, INT, SUM, W, DUE, R>(f, mk, pend, gather_rt(j, o), static_cast<int>(o & 7u), one, ph, gather_w(j),
+                                        gather_d(j), gather_r(j));
       return;
     }
     const int o = orow[j];
     if (!MULTI) {
       const float rt = tab[j * SG + o];
-      ls_step<INT, INT, SUM, W, DUE>(f, mk, pend, rt, o & 7, one, ph, lookup_w(j), lookup_d(j));
+      ls_step<INT, INT, SUM, W, DUE, R>(f, mk, pend, rt, o & 7, one, ph, lookup_w(j), lookup_d(j), lookup_r(j));
     } else {
       const int col = o & 7;  // reduced table only: opt = (node << 3) | (k - 1)
       const float rt = tab[j * 8 + col];
       switch_node(o >> 3);
-      ls_step<INT, true, SUM, W, DUE>(f, mk, pend, rt, col, one, ph, lookup_w(j), lookup_d(j));
+      ls_step<INT, true, SUM, W, DUE, R>(f, mk, pend, rt, col, one, ph, lookup_w(j), lookup_d(j), lookup_r(j));
     }
   }
   __device__ __forceinline__ float result() const { return SUM ? mk : ((INT || MULTI) ? fmaxf(mk, pend) : f[7]); }

@@ -330,6 +330,7 @@ struct PosArgs {
   SearchFuse sf;
   const float* w;  // W: job weights [J], zero-padded to a multiple of 4 (16 bytes)
   const float* d;  // D: job due dates [J], padded the same way
+  const float* r;  // R: job release dates [J], padded the same way
 };
 
 struct PosMove {
@@ -425,8 +426,10 @@ __device__ __forceinline__ PosMove make_pos_move_win(const SearchFuse& sf, int r
 // W: weight each completion by its job's weight (SB_FLAG_WEIGHTED, with SUM only); the weights follow the table in
 // shared memory with TAB = 0 and are read from global memory (ld.global.nc) with TAB = 1 / 2.
 // D: score tardiness against the jobs' due dates (SB_FLAG_DUE, with W only); the due dates follow the weights.
+// R: no job starts before its release date (SB_FLAG_RELEASE, any objective); the release dates follow the other
+// per-job arrays in shared memory with TAB = 0 and are read from global memory with TAB = 1 / 2.
 template <int PB, bool INT, bool MULTI, bool EVAL = false, int TAB = 0, bool SUM = false, bool W = false,
-          bool D = false>
+          bool D = false, bool R = false>
 __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
   static_assert(TAB == 0 || (EVAL && !MULTI), "tables outside the CTA's shared memory: scoring only, one node");
   static_assert(SUM || !W, "weights scale the sum of completion times only");
@@ -443,10 +446,12 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
   const uint32_t tab_room = TAB == 1 ? 0u : (TAB == 2 ? half * 4u : tab_all);
   const uint32_t w_bytes = (W && TAB == 0) ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u;
   const uint32_t d_bytes = D ? w_bytes : 0u;
+  const uint32_t r_bytes = (R && TAB == 0) ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u;
   float* tab_s = reinterpret_cast<float*>(smem);
   [[maybe_unused]] float* w_s = reinterpret_cast<float*>(smem + ((tab_room + 15u) & ~15u));
   [[maybe_unused]] float* d_s = reinterpret_cast<float*>(smem + ((tab_room + 15u) & ~15u) + w_bytes);
-  uint64_t* bar_tab = reinterpret_cast<uint64_t*>(smem + ((tab_room + 15u) & ~15u) + w_bytes + d_bytes);
+  [[maybe_unused]] float* r_s = reinterpret_cast<float*>(smem + ((tab_room + 15u) & ~15u) + w_bytes + d_bytes);
+  uint64_t* bar_tab = reinterpret_cast<uint64_t*>(smem + ((tab_room + 15u) & ~15u) + w_bytes + d_bytes + r_bytes);
   const uint32_t node_bytes = MULTI ? static_cast<uint32_t>(a.nodes) * 1024u : 0u;
   float4* node_s = reinterpret_cast<float4*>(reinterpret_cast<uint8_t*>(bar_tab) + 16 + static_cast<size_t>(warp) * node_bytes);
   if (threadIdx.x == 0) {
@@ -456,7 +461,7 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
   __syncthreads();
   if constexpr (TAB != 1) {
     if (threadIdx.x == 0) {
-      mbar_arrive_expect_tx(bar_tab, tab_bytes + w_bytes + d_bytes);
+      mbar_arrive_expect_tx(bar_tab, tab_bytes + w_bytes + d_bytes + r_bytes);
       const uint8_t* src = reinterpret_cast<const uint8_t*>(a.tab) + tab_off;
       for (uint32_t off = 0; off < tab_bytes; off += 32768u) tma_bulk_g2s(smem + off, src + off, min(32768u, tab_bytes - off), bar_tab);
       if constexpr (W && TAB == 0) {
@@ -469,12 +474,18 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
         for (uint32_t off = 0; off < d_bytes; off += 32768u)
           tma_bulk_g2s(reinterpret_cast<uint8_t*>(d_s) + off, dsrc + off, min(32768u, d_bytes - off), bar_tab);
       }
+      if constexpr (R && TAB == 0) {
+        const uint8_t* rsrc = reinterpret_cast<const uint8_t*>(a.r);
+        for (uint32_t off = 0; off < r_bytes; off += 32768u)
+          tma_bulk_g2s(reinterpret_cast<uint8_t*>(r_s) + off, rsrc + off, min(32768u, r_bytes - off), bar_tab);
+      }
     }
   }
-  LaneState<INT, MULTI, 0, SUM, (W ? (TAB == 0 ? 1 : 2) : 0), D> st;
+  LaneState<INT, MULTI, 0, SUM, (W ? (TAB == 0 ? 1 : 2) : 0), D, (R ? (TAB == 0 ? 1 : 2) : 0)> st;
   st.tab = tab_s;
   if constexpr (W) st.wt = TAB == 0 ? w_s : a.w;
   if constexpr (D) st.dd = TAB == 0 ? d_s : a.d;
+  if constexpr (R) st.rr = TAB == 0 ? r_s : a.r;
   st.SG = a.SG;
   st.one = a.one;
   st.orow = nullptr;
@@ -568,9 +579,9 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
           for (int t = 0; t < 32; ++t) {
             const int j = prio_at<PB>(qp[(t * PB) / 32].w, t % (32 / PB));
             const int o = prio_at<1>(qo.w, t);
-            if constexpr (D) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j), st.lookup_d(j));
-            else if constexpr (W) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j));
-            else st.step_resolved(o, lookup(j, o), t & 1);
+            if constexpr (D) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j), st.lookup_d(j), st.lookup_r(j));
+            else if constexpr (W) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j), 0.f, st.lookup_r(j));
+            else st.step_resolved(o, lookup(j, o), t & 1, 0.f, 0.f, st.lookup_r(j));
           }
         } else {
 #pragma unroll
@@ -578,9 +589,9 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
             if (base + t < J) {
               const int j = prio_at<PB>(qp[(t * PB) / 32].w, t % (32 / PB));
               const int o = prio_at<1>(qo.w, t);
-              if constexpr (D) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j), st.lookup_d(j));
-              else if constexpr (W) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j));
-              else st.step_resolved(o, lookup(j, o), t & 1);
+              if constexpr (D) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j), st.lookup_d(j), st.lookup_r(j));
+              else if constexpr (W) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j), 0.f, st.lookup_r(j));
+              else st.step_resolved(o, lookup(j, o), t & 1, 0.f, 0.f, st.lookup_r(j));
             }
           }
         }
@@ -762,7 +773,7 @@ cudaError_t search_init_population_pos(const SearchDev& s, cudaStream_t st) {
   return launch(with_pb(s.pb, [](auto PB) { return k_init_population_pos<PB>; }), grid, threads, 0, st, s);
 }
 
-// smem: table (+ weights, + due dates) + mbarrier + per-warp node states (MULTI)
+// smem: table (+ weights, + due dates, + release dates) + mbarrier + per-warp node states (MULTI)
 size_t search_pos_smem(int J, int SG, int nodes, int warps, int arrays) {
   const size_t tab_bytes = (static_cast<size_t>(J) * SG * 4 + 15) & ~size_t(15);
   return tab_bytes + arrays * job_array_bytes(J) + 16 + static_cast<size_t>(warps) * (nodes > 1 ? nodes * 1024u : 0u);
@@ -778,9 +789,9 @@ static cudaError_t eval_pos_far_launch(const Device& dev, const PosArgs& a, int 
   if (smem > dev.smem_optin) return cudaErrorNotSupported;
   const long long ntiles = (a.chains + 31) / 32;
   const long long ctas = (ntiles + warps - 1) / warps;
-  const PosKernel kern = with_eval_types(pb, flags, [&](auto PB, auto INT, auto SUM, auto W, auto D) {
-    return tab_home == 2 ? k_search_pos<PB, INT, false, true, 2, SUM, W, D>
-                         : k_search_pos<PB, INT, false, true, 1, SUM, W, D>;
+  const PosKernel kern = with_eval_types(pb, flags, [&](auto PB, auto INT, auto SUM, auto W, auto D, auto R) {
+    return tab_home == 2 ? k_search_pos<PB, INT, false, true, 2, SUM, W, D, R>
+                         : k_search_pos<PB, INT, false, true, 1, SUM, W, D, R>;
   });
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
   if (e != cudaSuccess) return e;
@@ -813,7 +824,7 @@ static cudaError_t eval_pos_far_launch(const Device& dev, const PosArgs& a, int 
 // tab_home: 0 = the table in every CTA's shared memory (cudaErrorNotSupported when it does not fit);
 // scoring only, one node: 2 = split over CTA pairs, 1 = global memory
 cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float* tab, const float* w, const float* d,
-                              int SG, unsigned flags, long long first, long long count, bool eval_only, const SearchFuse& sf,
+                              const float* r, int SG, unsigned flags, long long first, long long count, bool eval_only, const SearchFuse& sf,
                               cudaStream_t st, int tab_home) {
   if (count <= 0) return cudaSuccess;
   PosArgs a;
@@ -828,6 +839,7 @@ cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float
   a.sf = sf;
   a.w = w;
   a.d = d;
+  a.r = r;
   const bool multi = s.nodes > 1;
   if (tab_home != 0) {
     if (!eval_only || multi) return cudaErrorNotSupported;
@@ -839,10 +851,10 @@ cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float
   const long long ntiles = (count + 31) / 32;
   const long long ctas = (ntiles + warps - 1) / warps;
   const int grid = static_cast<int>(ctas < dev.sm_count ? ctas : dev.sm_count);
-  const PosKernel kern = with_eval_types(s.pb, flags, [&](auto PB, auto INT, auto SUM, auto W, auto D) {
+  const PosKernel kern = with_eval_types(s.pb, flags, [&](auto PB, auto INT, auto SUM, auto W, auto D, auto R) {
     return with_bool(multi, [&](auto MULTI) {
       return with_bool(eval_only, [&](auto EVAL) -> PosKernel {
-        return k_search_pos<PB, INT, MULTI, EVAL, 0, SUM, W, D>;
+        return k_search_pos<PB, INT, MULTI, EVAL, 0, SUM, W, D, R>;
       });
     });
   });
@@ -879,7 +891,7 @@ cudaError_t eval_pos_launch(const Device& dev, const EvalCall& c, cudaStream_t s
   s.keys = c.best_key;
   SearchFuse sf = {};
   sf.cur_mk = c.out;
-  return search_pos_launch(dev, s, c.tab, c.w, c.d, c.SG, c.flags, 0, c.B, true, sf, st, home);
+  return search_pos_launch(dev, s, c.tab, c.w, c.d, c.r, c.SG, c.flags, 0, c.B, true, sf, st, home);
 }
 
 // Job-indexed opt rows -> schedule order (out[i] = opt[prio[i]]), one warp per candidate: the row is staged in

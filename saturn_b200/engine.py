@@ -69,6 +69,27 @@ def due_f32(d, J: int) -> np.ndarray:
     return d64.astype(np.float32)
 
 
+def release_f32(r, J: int) -> np.ndarray:
+    """J release dates as fp32, rounded UP (like build_table's runtimes), so that a start >= the fp32 value is
+    >= the caller's value in float64 too.  Every release date must be finite with |r| < 2^24, in fp32 as well
+    (r <= 0: the job is already released); raises SolverError otherwise."""
+    from .solver import SolverError
+    try:
+        r64 = np.asarray(r, dtype=np.float64)
+    except (TypeError, ValueError) as e:
+        raise SolverError("release dates must be numbers: %s" % e)
+    if r64.shape != (J,):
+        raise SolverError("release dates must have one value per task (%d), got shape %s" % (J, r64.shape))
+    if not (np.isfinite(r64).all() and (np.abs(r64) < 2.0 ** 24).all()):
+        raise SolverError("every release date must be finite with |r| < 2^24")
+    r32 = r64.astype(np.float32)
+    low = r32.astype(np.float64) < r64
+    r32[low] = np.nextafter(r32[low], np.float32(np.inf))
+    if not (np.abs(r32) < np.float32(2.0 ** 24)).all():
+        raise SolverError("every release date must stay below 2^24 in magnitude once rounded up to fp32")
+    return r32
+
+
 def _flags(integer_starts: bool, reduced: bool, objective: str = "makespan") -> int:
     return (FLAG_INTEGER_STARTS if integer_starts else 0) | (FLAG_REDUCED if reduced else 0) | objective_flag(objective)
 
@@ -106,6 +127,7 @@ class Engine:
         self.nodes = 1
         self.weights = None  # fp32 job weights of objective="weighted_completion" (set_weights)
         self.due = None  # fp32 job due dates of objective="tardiness" / "weighted_tardiness" (set_due)
+        self.release = None  # fp32 job release dates, under every objective (set_release)
 
     # ------------------------------------------------------------------ lifecycle
     def close(self):
@@ -151,6 +173,7 @@ class Engine:
         self.nodes = int(nodes)
         self.weights = None  # sb_set_table clears them
         self.due = None
+        self.release = None
         return self
 
     def set_weights(self, w) -> "Engine":
@@ -178,9 +201,26 @@ class Engine:
         self.due = d32
         return self
 
+    def set_release(self, r) -> "Engine":
+        """Per-job release dates (J values, finite with |r| < 2^24, rounded up to fp32) in the runtimes' units from
+        the plan's t = 0: no job starts before its release date, under every objective (ceil(r) with integer
+        starts).  While they are set, every evaluation and search call of this engine passes SB_FLAG_RELEASE.
+        None clears them; set_table clears them too."""
+        if r is None:
+            check(self._lib.sb_set_release(self._h, None, 0))
+            self.release = None
+            return self
+        r32 = np.ascontiguousarray(release_f32(r, self.J))
+        check(self._lib.sb_set_release(self._h, C.c_void_p(r32.ctypes.data), int(self.J)))
+        self.release = r32
+        return self
+
+    def _release_flag(self) -> int:
+        return _lib.FLAG_RELEASE if self.release is not None else 0
+
     def _flags(self, integer_starts: bool, reduced: bool, objective: str) -> int:
         _require_due(self.due, objective)
-        return _flags(integer_starts, reduced, objective)
+        return _flags(integer_starts, reduced, objective) | self._release_flag()
 
     def reduced_table(self) -> Tuple[np.ndarray, np.ndarray]:
         tmin = np.empty((self.J, NSLOT), dtype=np.float32)
@@ -375,13 +415,14 @@ class Engine:
         _require_due(self.due, objective)
         return _search_run(self._lib, [self._h], self.J, chains, rounds, seed, chain_base, integer_starts, reduced,
                            t_start, t_end, warm, resample_every, sync_every, patience, time_budget_s, target_makespan,
-                           heuristic_seeds, record_history, _no_fused, _extra_flags, objective)
+                           heuristic_seeds, record_history, _no_fused, int(_extra_flags) | self._release_flag(),
+                           objective)
 
     def search_wave(self, reduced: bool = False) -> int:
         """Chains that fill the device exactly once with the round kernel of the current table; populations
         that are whole multiples of it leave no partially filled last wave."""
         n = C.c_int64(0)
-        check(self._lib.sb_search_wave(self._h, _flags(False, reduced), C.byref(n)))
+        check(self._lib.sb_search_wave(self._h, _flags(False, reduced) | self._release_flag(), C.byref(n)))
         return int(n.value)
 
     def search_is_fused(self) -> bool:
@@ -536,6 +577,14 @@ class MultiEngine:
 
     due = property(lambda self: self.engines[0].due)
 
+    def set_release(self, r):
+        """Engine.set_release on every device."""
+        for e in self.engines:
+            e.set_release(r)
+        return self
+
+    release = property(lambda self: self.engines[0].release)
+
     def decode(self, *a, **kw):
         return self.engines[0].decode(*a, **kw)
 
@@ -552,8 +601,8 @@ class MultiEngine:
         _require_due(self.due, objective)
         return _search_run(self._lib, [e._h for e in self.engines], self.J, chains, rounds, seed, chain_base,
                            integer_starts, reduced, t_start, t_end, warm, resample_every, sync_every, patience,
-                           time_budget_s, target_makespan, heuristic_seeds, record_history, _no_fused, _extra_flags,
-                           objective)
+                           time_budget_s, target_makespan, heuristic_seeds, record_history, _no_fused,
+                           int(_extra_flags) | self.engines[0]._release_flag(), objective)
 
 
 class _CudaArrayView:

@@ -56,7 +56,8 @@ def orchestrate(task_list, log=False, interval=1000, gurobi=True, *,
 
     A `due` mapping Task -> due date in `solver_kwargs` (objective="tardiness") is measured from the first plan's
     t = 0: the solve for interval n plans from n * interval on, so it receives {t: d - n * interval}.  A sequence
-    `due` raises SolverError, since the task list shrinks from interval to interval.
+    `due` raises SolverError, since the task list shrinks from interval to interval.  A `release` mapping
+    Task -> release date is shifted the same way, {t: r - n * interval}; a sequence `release` raises SolverError.
     """
     logging.basicConfig(level=logging.INFO if log else logging.WARNING,
                         format="%(asctime)s %(levelname)-8s %(message)s", datefmt="%Y-%m-%d %H:%M:%S")
@@ -64,9 +65,18 @@ def orchestrate(task_list, log=False, interval=1000, gurobi=True, *,
     due = kw.pop("due", None)
     if due is not None and not isinstance(due, Mapping):
         raise SolverError("orchestrate() needs due as a mapping Task -> due date: its task list shrinks every interval")
+    release = kw.pop("release", None)
+    if release is not None and not isinstance(release, Mapping):
+        raise SolverError("orchestrate() needs release as a mapping Task -> release date: its task list shrinks "
+                          "every interval")
 
     def kw_at(n):  # the solver arguments of the plan for interval n (whose t = 0 is n * interval)
-        return kw if due is None else dict(kw, due={t: d - n * interval for t, d in due.items()})
+        out = dict(kw)
+        if due is not None:
+            out["due"] = {t: d - n * interval for t, d in due.items()}
+        if release is not None:
+            out["release"] = {t: r - n * interval for t, r in release.items()}
+        return out
 
     task_list = list(task_list)
     records = []

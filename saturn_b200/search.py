@@ -45,7 +45,8 @@ def key_makespan(key: int) -> float:
 
 
 def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objective: str = "makespan",
-              weights: Optional[np.ndarray] = None, due: Optional[np.ndarray] = None):
+              weights: Optional[np.ndarray] = None, due: Optional[np.ndarray] = None,
+              release: Optional[np.ndarray] = None, integer_starts: bool = True):
     """Heuristic warm candidates in the reduced encoding (opt byte = k-1, plus node << 3 when there
     are several nodes), longest-processing-time order: (a) every job on its fastest option,
     (b) every job on its least GPU-seconds option, (c) in between.  Nodes are filled greedily by
@@ -55,7 +56,9 @@ def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objecti
     `weights`: WSPT order (Smith's rule), ascending runtime / weight in float64, ties by job index — for unit
     weights exactly the shortest-processing-time order.  objective="tardiness" / "weighted_tardiness" with the fp32
     `due` dates: EDD order (earliest due date first), ties by runtime (by runtime / weight when weighted), then by
-    job index."""
+    job index.  With the fp32 `release` dates (any objective) each order is then re-sorted stably by ascending
+    release date (ceiled when `integer_starts`, as the device schedules them), so jobs released together keep the
+    objective's order."""
     objective_flag(objective)
     if objective.startswith("weighted_"):
         if weights is None:
@@ -65,6 +68,10 @@ def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objecti
         if due is None:
             raise ValueError("objective=%r needs the job due dates" % objective)
         d32 = np.asarray(due, dtype=np.float32)
+    if release is not None:
+        rel = np.asarray(release, dtype=np.float32)
+        if integer_starts:
+            rel = np.ceil(rel)
     J = tmin.shape[0]
     usable = np.where(tmin < sentinel, tmin, np.inf)
     if not np.isfinite(usable).any(axis=1).all():
@@ -84,6 +91,8 @@ def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objecti
             order = np.argsort(rt, kind="stable")
         else:
             order = np.argsort(-rt * (col + 1) ** 0.5, kind="stable")
+        if release is not None:
+            order = order[np.argsort(rel[order], kind="stable")]
         ob = col.astype(np.uint8)
         if nodes > 1:
             load = np.zeros(nodes)
@@ -147,7 +156,9 @@ def run_search(engine: Engine, chains: int = 1 << 16, rounds: int = 200, seed: i
         nodes = getattr(engine, "nodes", 1)
         for i, (col, order) in enumerate(lpt_seeds(tmin, nodes=nodes, objective=objective,
                                                    weights=getattr(engine, "weights", None),
-                                                   due=getattr(engine, "due", None))):
+                                                   due=getattr(engine, "due", None),
+                                                   release=getattr(engine, "release", None),
+                                                   integer_starts=integer_starts)):
             opt = col if reduced else ((args[np.arange(J), col & 7].astype(np.uint8) << 3) | col)
             first = min(i * per, max(0, chains - per))
             engine.search_inject(opt.astype(np.uint8), order.astype(pdt), copies=min(per, chains), first=first)

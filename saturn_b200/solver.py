@@ -193,10 +193,11 @@ def _engine(devices=None):
     return _MULTI[devices]
 
 
-def _check_horizon(T, found_makespan=None):
+def _check_horizon(T, found_makespan=None, release=None):
     """The kernels keep schedule times in fp32: `start + ceil(rt)` is exact only below 2^24 s (194 days).
-    Before the search: a table whose area lower bound (sum_j min_k k * rt_jk / 8) already reaches that bound
-    cannot have an exactly representable plan and is refused.  After the search (`found_makespan`, the
+    Before the search: a table whose lower bound of the makespan — the area bound sum_j min_k k * rt_jk / 8, and
+    with `release` (per-task release dates) also max_j (r_j + min_k rt_jk) — already reaches that bound cannot
+    have an exactly representable plan and is refused.  After the search (`found_makespan`, the
     device's value): every time inside the winning schedule is <= its makespan, and fp32 addition rounds
     monotonically, so a makespan below 2^24 proves that all of its starts were computed exactly; anything
     else is refused instead of returned with silently rounded starts (rescale to coarser time units)."""
@@ -208,17 +209,23 @@ def _check_horizon(T, found_makespan=None):
     k = np.arange(1, T.shape[-1] + 1, dtype=np.float64)
     area = np.where(np.isfinite(T), T.astype(np.float64) * k, np.inf).reshape(T.shape[0], -1).min(axis=1)
     lower = float(area.sum()) / NSLOT
+    if release is not None:
+        shortest = np.where(np.isfinite(T), T.astype(np.float64), np.inf).reshape(T.shape[0], -1).min(axis=1)
+        lower = max(lower, float(np.max(np.asarray(release, dtype=np.float64) + shortest)))
     if lower >= FP32_EXACT_HORIZON:
         raise SolverError("area lower bound of the makespan is %.3g s >= 2^24 s: schedule times are not exact in "
                           "fp32 at that horizon; express runtimes in coarser units (e.g. minutes) or drop sentinel "
                           "options" % lower)
 
-def _check_objective(objective, hysteresis=False):
+def _check_objective(objective, hysteresis=False, release=None):
     if objective not in ("makespan", "completion", "tardiness"):
         raise SolverError("objective must be 'makespan', 'completion' or 'tardiness', not %r" % (objective,))
     if objective != "makespan" and hysteresis:
         raise SolverError("hysteresis=True compares plans by makespan (milp.py:363-442); it is not defined for "
                           "objective=%r" % (objective,))
+    if release is not None and hysteresis:
+        raise SolverError("hysteresis=True compares plans by a makespan that knows nothing of release dates "
+                          "(milp.py:363-442); it cannot be combined with release")
 
 
 def _per_task(values, what, task_list):
@@ -265,8 +272,21 @@ def _resolve_due(due, objective, J, task_list=None):
     return [float(x) for x in due], d32
 
 
-def _set_objective(eng, objective, w32, d32):
-    """Hand the weights and due dates to the engine; returns the engine objective the search runs."""
+def _resolve_release(release, J, task_list=None):
+    """The caller's per-task release dates as (float64 values in task order, fp32 array for the device, rounded up),
+    or (None, None).  Valid under every objective.  Raises SolverError before any device call."""
+    if release is None:
+        return None, None
+    release = _per_task(release, "release", task_list)
+    from .engine import release_f32
+    r32 = release_f32(release, J)
+    return [float(x) for x in release], r32
+
+
+def _set_objective(eng, objective, w32, d32, r32=None):
+    """Hand the weights, due dates and release dates to the engine; returns the engine objective the search runs."""
+    if r32 is not None:
+        eng.set_release(r32)
     if w32 is not None:
         eng.set_weights(w32)
     if d32 is not None:
@@ -281,6 +301,11 @@ def _tardiness_stats(start, rts, w64, d64):
     w = w64 if w64 is not None else [1.0] * len(late)
     return {"weighted_tardiness": sum(wi * max(0.0, x) for wi, x in zip(w, late)),
             "late_tasks": sum(1 for x in late if x > 0)}
+
+
+def _flow_stats(start, rts, r64):
+    """total_flow_time of a plan, sum_t (C_t - max(r_t, 0)): the time from release to result, in float64."""
+    return {"total_flow_time": sum(float(s) + float(r) - max(x, 0.0) for s, r, x in zip(start, rts, r64))}
 
 
 def _plan_horizon(start, rt):
@@ -306,7 +331,8 @@ def _default_nodes() -> int:
 def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count() or 4) // 4), interval=1000,
           timeout=500, *, chains: Optional[int] = None, rounds: Optional[int] = None, seed: int = 0,
           integer_starts: bool = True, engine=None, hysteresis: Optional[bool] = None,
-          nodes: Optional[int] = None, devices=None, objective: str = "makespan", weights=None, due=None):
+          nodes: Optional[int] = None, devices=None, objective: str = "makespan", weights=None, due=None,
+          release=None):
     """Drop-in for saturn.solver.solve (milp.py:23).
 
     Objective.  "makespan" (the default, the reference's) or "completion": minimise the sum of the tasks'
@@ -335,6 +361,16 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     C_t > d_t) are computed in float64 from the emitted plan, the tasks' own runtimes and the caller's d and w;
     last_stats["device_makespan"] holds the device's fp32 tardiness.
 
+    Release dates.  `release` (a sequence aligned with task_list, or a mapping keyed by Task, in the runtimes' units
+    from the plan's t = 0) keeps every task from starting before its release date, under every objective: a
+    dataset or a parent checkpoint that is only ready later, a job that arrives tomorrow.  r <= 0 means already
+    released.  Every value must be finite with |r| < 2^24; it is rounded up to fp32, and with integer_starts a task
+    starts no earlier than ceil(r), so every emitted start is >= the caller's r.  A wrong length, a task missing
+    from the mapping, a bad value, or hysteresis=True together with `release` raises SolverError before any device
+    call.  The 6th element and last_stats["makespan"] then count from t = 0, releases included;
+    last_stats["total_flow_time"] holds sum_t (C_t - max(r_t, 0)), the time from release to result, in float64
+    (for fixed release dates, minimising it is minimising the sum of completion times).
+
     Returns (sta, tga, bss, bna, boa, makespan) — milp.py:445 — with a real float makespan
     (the reference returns None on a cold start, milp.py:394-399; callers only thread it back in
     as `presolved`).  Keyword-only extras tune the GPU search; environment overrides:
@@ -359,12 +395,13 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     SATURN_B200_HYSTERESIS applies to the makespan objective only.
     """
     from .search import run_search
-    _check_objective(objective, bool(hysteresis))
+    _check_objective(objective, bool(hysteresis), release)
     t_wall = time.perf_counter()
     task_list = list(task_list)
     J = len(task_list)
     w64, w32 = _resolve_weights(weights, objective, J, task_list)
     d64, d32 = _resolve_due(due, objective, J, task_list)
+    r64, r32 = _resolve_release(release, J, task_list)
     if J == 0:
         return [[[] for _ in range(NSLOT)]], [], [], [], [], 0.0
     eng = engine if engine is not None else _engine(devices)
@@ -375,12 +412,12 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     for j in range(J):
         if usable[j].any():
             Tdev[j, 0, ~usable[j]] = np.inf
-    _check_horizon(Tdev)
+    _check_horizon(Tdev, release=r64)
     if nodes is None:
         nodes = _default_nodes()
     nodes = int(nodes)
     eng.set_table(Tdev, list(range(1, NSLOT + 1)), sentinel=float("inf"), nodes=nodes)
-    search_objective = _set_objective(eng, objective, w32, d32)
+    search_objective = _set_objective(eng, objective, w32, d32, r32)
     if chains is None:
         chains = int(os.environ.get("SATURN_B200_CHAINS", 0))
         if chains <= 0:
@@ -427,11 +464,13 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
         last_stats["weighted_completion"] = sum(w64[i] * (float(dec["start"][i]) + float(rts[i])) for i in range(J))
     if d64 is not None:
         last_stats.update(_tardiness_stats(dec["start"], rts, w64, d64))
+    if r64 is not None:
+        last_stats.update(_flow_stats(dec["start"], rts, r64))
 
     # ---- introspection hysteresis (opt-in): the documented intent of milp.py:363-442
     out = prop + (prop_makespan,)
     if hysteresis is None:
-        hysteresis = objective == "makespan" and os.environ.get("SATURN_B200_HYSTERESIS", "0") not in (
+        hysteresis = objective == "makespan" and release is None and os.environ.get("SATURN_B200_HYSTERESIS", "0") not in (
             "", "0", "false", "False")
     if presolved is not None and hysteresis:
         p_sta, p_tga, p_bss, p_bna, p_boa, saved = presolved
@@ -522,11 +561,12 @@ def strategies_from_table(T, mask, executors=None, params=None, gcount=None):
 def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeout=500, *,
                 chains: Optional[int] = None, rounds: Optional[int] = None, seed: int = 0,
                 integer_starts: bool = True, engine=None, nodes: Optional[int] = None, devices=None,
-                objective: str = "makespan", weights=None, due=None):
+                objective: str = "makespan", weights=None, due=None, release=None):
     """solve() on the dense profiler tensor T[J][S][G] (+ mask of usable cells, + gcount[G] GPU counts).
     `objective` as for solve(): "makespan" or "completion" (sum of completion times); `weights` as for solve(),
     a sequence aligned with T's rows (the weighted sum of completion times, last_stats["weighted_completion"]);
-    `due` as for solve() with objective="tardiness", a sequence aligned with T's rows.
+    `due` as for solve() with objective="tardiness", a sequence aligned with T's rows; `release` as for solve(),
+    under every objective, a sequence aligned with T's rows (last_stats["total_flow_time"]).
 
     The table goes to the device un-reduced (sb_set_table: min over strategies with the first-minimum rule
     and its arg-min on the device, PerformanceEvaluator.py:101-115); the search runs on the reduced view
@@ -543,6 +583,7 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     J, S, G = T.shape
     w64, w32 = _resolve_weights(weights, objective, J)
     d64, d32 = _resolve_due(due, objective, J)
+    r64, r32 = _resolve_release(release, J)
     if J == 0:
         return [[[] for _ in range(NSLOT)]], [], [], [], [], 0.0, np.zeros(0, dtype=np.int64)
     gcount = list(range(1, G + 1)) if gcount is None else [int(g) for g in gcount]
@@ -556,11 +597,11 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
         Tdev[j] = np.where(np.isfinite(T[j]), T[j], np.inf)      # nothing usable: the sentinels are all it has
     if not np.isfinite(Tdev.reshape(J, -1)).any(axis=1).all():
         raise SolverError("a task has no finite cell in T")
-    _check_horizon(Tdev)
+    _check_horizon(Tdev, release=r64)
     eng = engine if engine is not None else _engine(devices)
     nodes = int(_default_nodes() if nodes is None else nodes)
     eng.set_table(Tdev, gcount, sentinel=float("inf"), nodes=nodes)
-    search_objective = _set_objective(eng, objective, w32, d32)
+    search_objective = _set_objective(eng, objective, w32, d32, r32)
     if chains is None:
         chains = int(os.environ.get("SATURN_B200_CHAINS", 0))
         if chains <= 0:
@@ -600,6 +641,8 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
         last_stats["weighted_completion"] = sum(w64[j] * (float(dec["start"][j]) + rts[j]) for j in range(J))
     if d64 is not None:
         last_stats.update(_tardiness_stats(dec["start"], rts, w64, d64))
+    if r64 is not None:
+        last_stats.update(_flow_stats(dec["start"], rts, r64))
     return arrays + (makespan, strategy)
 
 

@@ -1,17 +1,23 @@
-"""Cost and effect of the sum-of-completion-times objectives (plain and weighted) and of the weighted tardiness on
-one GPU; prints one JSON line.
+"""Cost and effect of the sum-of-completion-times objectives (plain and weighted), of the weighted tardiness and of
+release dates on one GPU; prints one JSON line.
 
     python scripts/bench_objective.py [--steps 200] [--warmup 20] [--solve-chains 0] [--solve-rounds 400]
 
 kernel: sb_eval on bench.py's C4 batch (J = 256, S = 8, 946,176 candidates, the same seeded inputs, integer
         starts), scored for the makespan, the sum of completion times, the weighted sum (seeded weights) and the
-        weighted tardiness (the same weights, seeded due dates), the four launches alternated in one process (the
-        order rotates every step) and timed with CUDA events; median of --steps launches each.
+        weighted tardiness (the same weights, seeded due dates), and the release twins of the makespan and the
+        weighted tardiness (seeded integer release dates in [0, 20000) s, SB_FLAG_RELEASE, a second handle on the
+        same device), the six launches alternated in one process (the order rotates every step) and timed with CUDA
+        events; median of --steps launches each.
 solve:  solve() wall time on a 256-task set (synthetic table, seed 3, 4 strategies) for the makespan, the sum of
         completion times and the weighted sum (seeded weights: 32 tasks of weight 8, the rest 1), each plan scored
         on all three measures (float64, the tasks' own runtimes); and the total tardiness (unit weights, seeded
         integer due dates in [0, 200000) s): its tardiness and late tasks against those of the makespan and
         completion plans.
+release: the same 256-task set with seeded release dates in [0, 0.5 x the makespan plan's makespan): per objective
+        (makespan, completion, tardiness) the release-aware plan (solve(release=...)) against the release-blind plan
+        (solve() without them, its options and list order rescored under the release rule), on makespan, total flow
+        time sum_t (C_t - max(r_t, 0)) and, for the tardiness objective, the tardiness; all in float64.
 The card's name and power limit are read in the same run (nvidia-smi, read-only queries).
 """
 import argparse
@@ -59,28 +65,40 @@ def main():
     opt, prio = random_candidates(eng, B, valid, seed=1)
     eng.set_weights(np.random.default_rng(2).choice([1.0, 2.0, 3.0, 5.0, 8.0, 0.25, 0.5, 1.5], size=J))
     eng.set_due(np.random.default_rng(3).integers(0, 20000, size=J))
+    eng_r = Engine(0)                                       # the same inputs, plus release dates
+    eng_r.set_table(T)
+    eng_r.set_weights(eng.weights)
+    eng_r.set_due(eng.due)
+    eng_r.set_release(np.random.default_rng(5).integers(0, 20000, size=J))
     out = torch.empty(B, dtype=torch.float32, device=eng.device)
     key = torch.full((1,), 2 ** 63 - 1, dtype=torch.int64, device=eng.device)
-    objs = ("makespan", "completion", "weighted_completion", "weighted_tardiness")
+    objs = ("makespan", "completion", "weighted_completion", "weighted_tardiness", "release_makespan",
+            "release_weighted_tardiness")
     times = {o: [] for o in objs}
     for i in range(args.warmup + args.steps):
         for obj in objs[i % len(objs):] + objs[:i % len(objs)]:
+            e = eng_r if obj.startswith("release_") else eng
             a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             a.record()
-            eng.eval(opt, prio, out=out, best_key=key, objective=obj)
+            e.eval(opt, prio, out=out, best_key=key, objective=obj.replace("release_", ""))
             b.record()
             b.synchronize()
             if i >= args.warmup:
                 times[obj].append(a.elapsed_time(b))
     path = eng.last_eval_path()
+    assert eng_r.last_eval_path() == path
     kernel = {o: {"median_ms": float(np.median(t)), "p10_ms": float(np.percentile(t, 10)),
                   "p90_ms": float(np.percentile(t, 90)), "candidates_per_s": B / (float(np.median(t)) * 1e-3)}
               for o, t in times.items()}
     kernel["completion_over_makespan"] = kernel["completion"]["median_ms"] / kernel["makespan"]["median_ms"]
     kernel["weighted_over_completion"] = kernel["weighted_completion"]["median_ms"] / kernel["completion"]["median_ms"]
     kernel["tardiness_over_weighted"] = kernel["weighted_tardiness"]["median_ms"] / kernel["weighted_completion"]["median_ms"]
+    kernel["release_over_makespan"] = kernel["release_makespan"]["median_ms"] / kernel["makespan"]["median_ms"]
+    kernel["release_over_tardiness"] = (kernel["release_weighted_tardiness"]["median_ms"] /
+                                        kernel["weighted_tardiness"]["median_ms"])
     kernel.update(B=B, J=J, S=Sx, path=path, steps=args.steps)
     del opt, prio, out
+    eng_r.close()
     torch.cuda.empty_cache()
 
     from saturn_b200.solver import strategies_from_table
@@ -121,8 +139,41 @@ def main():
                        "tardiness": sum(max(0.0, c - d) for c, d in zip(comp, due)),
                        "late_tasks": sum(1 for c, d in zip(comp, due) if c > d),
                        "rounds": st["rounds"], "candidates": st["candidates"]}
-    print(json.dumps({"card": card(0), "kernel": kernel, "solve": solve}))
+    print(json.dumps({"card": card(0), "kernel": kernel, "solve": solve,
+                      "release": release_effect(S, R, tasks, due, solve["makespan"]["makespan"], kw)}))
     eng.close()
+
+
+def release_effect(S, R, tasks, due, makespan, kw):
+    """Release-aware against release-blind plans on the 256-task set (see the module doc)."""
+    import numpy as np
+    from oracle import ref_release as RR
+    tuples = [[(g, s.runtime) for g, s in t.strategies.items()] for t in tasks]
+    tab, optmap = R.table_from_tuples(tuples)
+    r = [float(x) for x in np.random.default_rng(6).integers(0, int(0.5 * makespan), size=len(tasks))]
+    J = len(tasks)
+
+    def measures(start, comp):
+        return {"makespan": max(comp), "total_flow_time": sum(c - max(x, 0.0) for c, x in zip(comp, r)),
+                "tardiness": sum(max(0.0, c - d) for c, d in zip(comp, due)),
+                "earliest_slack": min(s - x for s, x in zip(start, r))}
+    out = {}
+    for obj in ("makespan", "completion", "tardiness"):
+        extra = {"due": due} if obj == "tardiness" else {}
+        t0 = time.perf_counter()
+        aware = S.solve(tasks, None, objective=obj, release=r, **extra, **kw)
+        wall = time.perf_counter() - t0
+        plan = R.plan_from_arrays(tuples, *aware[:4])
+        aware_m = measures([p[0] for p in plan], [p[0] + p[2] for p in plan])
+        blind = S.solve(tasks, None, objective=obj, **extra, **kw)
+        plan = R.plan_from_arrays(tuples, *blind[:4])
+        opt = [optmap[t][plan[t][4]] for t in range(J)]
+        order = sorted(range(J), key=lambda t: (plan[t][0], t))
+        _score, start, _m, _rd = RR.list_schedule(tab, opt, order, r, True, np.float64)
+        rt = [plan[t][2] for t in range(J)]
+        out[obj] = {"aware": aware_m, "blind_rescored": measures(list(start), [start[t] + rt[t] for t in range(J)]),
+                    "aware_wall_s": wall}
+    return out
 
 
 if __name__ == "__main__":
