@@ -386,6 +386,15 @@ int sb_search_validate(sb_handle* h, int64_t* bad_rows);
  * windowed moves, always scored from position 0) and 0x04000000 (round-1 move generator) select the
  * reference behaviours the tests and profiles compare against. */
 int sb_search_verify_count(sb_handle* h, uint64_t* mismatches);
+/* Test hooks of the streamed tile kernel (sb_eval path 3), kept on the handle for every later sb_eval until changed
+ * (0 = none, the default).  Bit 1: every warp adds up the %globaltimer nanoseconds from issuing each tile's row
+ * fetch to the fetch's completion, and its whole time in the tile loop, into two counters of the handle.  Bit 2:
+ * one bulk copy per opt row even where the rows of a tile could be fetched with one.  Bit 4: every warp of a CTA
+ * starts at once (no staggered phases).  None of them changes a result. */
+int sb_debug_tile_options(sb_handle* h, unsigned options);
+/* out[0] = the summed fetch waits, out[1] = the summed tile-loop times (ns) of every launch under option bit 1
+ * since the last call; the call resets both.  Synchronous. */
+int sb_debug_tile_wait(sb_handle* h, uint64_t* out);
 /* candidates evaluated so far by this handle's searches */
 int sb_search_stats(sb_handle* h, int64_t* evaluated, int64_t* rounds_done);
 

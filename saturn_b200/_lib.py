@@ -30,6 +30,10 @@ HOOK_TABLE_GLOBAL = 0x00800000
 HOOK_TABLE_PAIR = 0x00400000
 HOOK_REORDER = 0x00200000
 HOOK_NO_REORDER = 0x00100000
+# debug options of the streamed tile kernel, set on the handle (sb_debug_tile_options; TileDebug in csrc/sb_internal.h)
+TILE_DEBUG_TIMING = 1
+TILE_DEBUG_ROW_COPIES = 2
+TILE_DEBUG_NO_STAGGER = 4
 
 # every symbol include/saturn_b200.h declares (tests check that the library exports them all)
 SYMBOLS = [
@@ -38,6 +42,7 @@ SYMBOLS = [
     "sb_decode", "sb_xchg_create", "sb_xchg_connect", "sb_xchg_connect_local", "sb_xchg_post", "sb_xchg_reduce", "sb_xchg_check",
     "sb_search_init", "sb_search_round", "sb_search_best_key_ptr", "sb_search_best",
     "sb_search_inject", "sb_search_resample", "sb_search_seed_lpt", "sb_search_run", "sb_search_run_multi", "sb_search_wave", "sb_search_is_fused", "sb_search_stats", "sb_search_validate", "sb_search_verify_count",
+    "sb_debug_tile_options", "sb_debug_tile_wait",
 ]
 
 
@@ -118,6 +123,8 @@ def load():
         "sb_search_stats": [vp, C.POINTER(i64), C.POINTER(i64)],
         "sb_search_validate": [vp, C.POINTER(i64)],
         "sb_search_verify_count": [vp, C.POINTER(C.c_uint64)],
+        "sb_debug_tile_options": [vp, C.c_uint],
+        "sb_debug_tile_wait": [vp, C.POINTER(C.c_uint64)],
     }
     for name, args in sigs.items():
         fn = getattr(lib, name)

@@ -80,6 +80,8 @@ struct sb_handle {
   std::vector<float> h_tmin;
   std::vector<uint8_t> h_args;
   unsigned long long* d_scratch = nullptr;  // 4 x u64
+  unsigned tile_debug = 0;  // TileDebug options (sb_debug_tile_options)
+  unsigned long long* d_tile_wait = nullptr;  // TILE_DEBUG_TIMING: 2 x u64 (sb_debug_tile_wait), allocated on first use
   uint8_t* by_pos = nullptr;  // sb_eval: opt rows re-ordered by schedule position (path 9), grow-only
   size_t by_pos_bytes = 0;
   // staging for sb_eval_host
@@ -222,6 +224,7 @@ int sb_destroy(sb_handle* h) {
   free_staging(h);
   free_xchg(h);
   cudaFree(h->d_scratch);
+  cudaFree(h->d_tile_wait);
   cudaFree(h->by_pos);
   cudaFree(h->dec_buf);
   cudaFree(h->stage_T);
@@ -569,6 +572,14 @@ int sb_eval(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, int64
     return SB_OK;
   }
   c.force_generic = (flags & HOOK_FORCE_GENERIC) ? 1 : 0;
+  c.tile_debug = h->tile_debug;
+  if (h->tile_debug & TILE_DEBUG_TIMING) {
+    if (!h->d_tile_wait) {
+      CK(cudaMalloc(&h->d_tile_wait, 2 * sizeof(unsigned long long)));
+      CK(cudaMemsetAsync(h->d_tile_wait, 0, 2 * sizeof(unsigned long long), h->stream));
+    }
+    c.tile_wait = h->d_tile_wait;
+  }
   const bool post = (flags & SB_FLAG_POST_KEY) != 0;
   if (post) {
     if (!h->xchg_ready) return fail(SB_ERR_STATE, "SB_FLAG_POST_KEY needs sb_xchg_connect first");
@@ -1545,6 +1556,29 @@ int sb_search_verify_count(sb_handle* h, uint64_t* mismatches) {
   CK(cudaMemcpyAsync(&v, s.verify_bad, sizeof(v), cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   *mismatches = v;
+  return SB_OK;
+}
+
+int sb_debug_tile_options(sb_handle* h, unsigned options) {
+  if (!h) return fail(SB_ERR_ARG, "null handle");
+  if (options & ~(TILE_DEBUG_TIMING | TILE_DEBUG_ROW_COPIES | TILE_DEBUG_NO_STAGGER))
+    return fail(SB_ERR_ARG, "unknown tile debug option 0x%x", options);
+  h->tile_debug = options;
+  return SB_OK;
+}
+
+int sb_debug_tile_wait(sb_handle* h, uint64_t* out) {
+  int rc = use_device(h);
+  if (rc) return rc;
+  if (!out) return fail(SB_ERR_ARG, "out is null");
+  unsigned long long v[2] = {0ull, 0ull};
+  if (h->d_tile_wait) {
+    CK(cudaMemcpyAsync(v, h->d_tile_wait, sizeof(v), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemsetAsync(h->d_tile_wait, 0, sizeof(v), h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+  }
+  out[0] = v[0];
+  out[1] = v[1];
   return SB_OK;
 }
 

@@ -83,6 +83,19 @@ __device__ __forceinline__ void tma_bulk_g2s(void* dst_smem, const void* src_gme
       "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar))
       : "memory");
 }
+// named barriers (id 1..15; 0 is __syncthreads): `count` threads, a multiple of 32, take part in each phase.  Not the
+// .aligned forms: a warp may reach them from inside a lane-divergent branch.
+__device__ __forceinline__ void named_arrive(uint32_t id, uint32_t count) {
+  asm volatile("barrier.cta.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+__device__ __forceinline__ void named_sync(uint32_t id, uint32_t count) {
+  asm volatile("barrier.cta.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+__device__ __forceinline__ unsigned long long globaltimer_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
 
 // ---------------------------------------------------------------- the list-scheduling step
 // State: the 8 slot ready-times kept SORTED ascending in registers (f[0] <= ... <= f[7]).  Which

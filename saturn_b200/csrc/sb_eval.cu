@@ -9,8 +9,9 @@
 //   * persistent grid, one CTA per SM, NW warps per CTA; the J x S x 8 runtime table is staged
 //     once per CTA into shared memory with TMA bulk copies (cp.async.bulk + mbarrier);
 //   * each warp owns a tile of 32 candidates: every lane fetches ITS candidate's opt row with one
-//     TMA bulk copy into a padded shared-memory row (the opt bytes are gathered by job id, so
-//     they must be resident), completion on a per-warp mbarrier — no CTA-wide barrier after
+//     TMA bulk copy into a padded shared-memory row, or (streamed kernel, rows back to back) lane 0
+//     fetches the whole tile with one copy (the opt bytes are gathered by job id, so they must be
+//     resident), completion on a per-warp mbarrier — no CTA-wide barrier after
 //     start-up.  The prio row is consumed in order, so in the STREAM variant (rows 32-byte
 //     aligned) each lane streams it straight from HBM, one full 32-byte sector per lane (two
 //     128-bit loads, prefetched 32 steps ahead), and it never touches shared memory: 8.7 KB of smem
@@ -58,6 +59,10 @@ struct TileArgs {
   const float* w;  // W: job weights [J], zero-padded to a multiple of 4 (16 bytes)
   const float* d;  // D: job due dates [J], padded the same way
   const float* r;  // R: job release dates [J], padded the same way
+  // the streamed tile kernel (STREAM, one node, table in shared memory) only; see "Tile boundaries" below
+  int packed;    // consecutive candidates' rows lie back to back (stride_o == copy_o == row_o, stride_p == copy_p)
+  int stagger;   // start the warps of a CTA at staggered phases
+  unsigned long long* tile_wait;  // TILE_DEBUG_TIMING: [0] += fetch-to-wait ns, [1] += tile-loop ns, per warp
 };
 
 // TABG: the runtime table stays in global memory (read through L1/L2) — for tables larger than the
@@ -205,10 +210,37 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
   };
   if (fold_pending) look_issue();
 
+  // Tile boundaries of the streamed kernel (kFetch).  Every warp has the same work per tile, so warps that start
+  // together reach every tile boundary together, and a whole GPU's row fetches then land on HBM at once while no
+  // warp can issue.  Two things shorten and spread that wait:
+  //   * packed rows: lane 0 fetches the tile's 32 opt rows with ONE bulk copy into an unpadded tile (row stride
+  //     copy_o; the opt bytes are gathered by job id, on random banks at either stride);
+  //   * staggered phases: when every warp of the CTA has >= 2 tiles (uniform per CTA), warp w waits before its
+  //     first tile, on named barrier p = w % nph, until warp 0 has scored p chunks of its first tile (warp 0 arrives
+  //     after chunk p).  Offsets stay under half a tile; the warps then keep them, since they run the same work.
+  //     Warp 0 — in CTA 0 the one that folds the peers' keys — is never gated.
+  constexpr bool kFetch = STREAM && !MULTI && !TABG && !SEARCH;
+  const long long tstride = static_cast<long long>(gridDim.x) * nw;
+  const int nfull_ch = a.J / (32 / PB);  // full chunks (32 / PB schedule positions each) of a candidate
+  int nph = 1;
+  if (kFetch && a.stagger && static_cast<long long>(blockIdx.x) * nw + tstride + nw - 1 < a.ntiles)
+    nph = min(min(4, nw), (nfull_ch + 1) / 2);
+  // threads of barrier p: warp 0 and the warps w = p, p + nph, ... below nw
+  auto gate_count = [&](int p) { return 32u * (1u + static_cast<uint32_t>((nw - 1 - p) / nph + 1)); };
+  int arrive_at = nfull_ch + 1;  // the chunk after which warp 0 next arrives (never, unless it gates)
+  if (nph > 1) {
+    if (warp == 0) {
+      arrive_at = 1;
+    } else if (warp % nph != 0) {
+      named_sync(warp % nph, gate_count(warp % nph));
+    }
+  }
+  unsigned long long t_wait = 0ull, t_loop = 0ull;
+  if (kFetch && a.tile_wait != nullptr) t_loop = globaltimer_ns();
+
   uint32_t phase = 0;
   bool tab_ready = TABG;
-  for (long long tile = static_cast<long long>(blockIdx.x) * nw + warp; tile < a.ntiles;
-       tile += static_cast<long long>(gridDim.x) * nw) {
+  for (long long tile = static_cast<long long>(blockIdx.x) * nw + warp; tile < a.ntiles; tile += tstride) {
     const long long b0 = tile * 32;
     if (!SEARCH && fold_pending) {
       look_consume();
@@ -224,17 +256,22 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
     __syncwarp();
     PrioChunk q;
     if (a.use_bulk) {
+      unsigned long long t_fetch = 0ull;
+      if (kFetch && a.tile_wait != nullptr) t_fetch = globaltimer_ns();
       fence_proxy_async();  // order the previous tile's generic-proxy reads before async writes
       if (lane == 0)
         mbar_arrive_expect_tx(bar_w, static_cast<uint32_t>(nb) * (a.copy_o + (STREAM ? 0 : a.copy_p)));
       __syncwarp();
-      if (active) {
+      if (kFetch && a.packed) {
+        if (lane == 0) tma_bulk_g2s(tile_o, a.opt + b0 * a.stride_o, static_cast<uint32_t>(nb) * a.copy_o, bar_w);
+      } else if (active) {
         tma_bulk_g2s(tile_o + lane * a.row_o, a.opt + cand * a.stride_o, a.copy_o, bar_w);
         if (!STREAM) tma_bulk_g2s(tile_p + lane * a.row_p, pg, a.copy_p, bar_w);
       }
       if (STREAM && active) q = ld_prio32<true>(pg);  // overlaps the TMA wait
       mbar_wait(bar_w, phase);
       phase ^= 1;
+      if (kFetch && a.tile_wait != nullptr) t_wait += globaltimer_ns() - t_fetch;
     } else {
       for (int r = 0; r < nb; ++r) {
         const uint8_t* so = a.opt + (b0 + r) * a.stride_o;
@@ -288,7 +325,10 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
           }
         };
         if (nfull > 0) resolve(q.w);
-        for (int c = 0; c < nfull; ++c) {
+        // one copy of the chunk loop: it stops early only where warp 0 opens a stagger barrier (first tile)
+        int c = 0, stop = min(arrive_at, nfull);
+        for (;;) {
+        for (; c < stop; ++c) {
           PrioChunk nxt = q;
           if (c + 1 < nch) nxt = ld_prio32<true>(pg + (c + 1) * 32);
           // a partial next chunk is not resolved ahead (its bytes past J are not job ids): the last batch then
@@ -329,6 +369,10 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
           }
           q = nxt;
         }
+        if (stop >= nfull) break;
+        named_arrive(stop, gate_count(stop));
+        stop = stop + 1 < nph ? stop + 1 : nfull;
+        }
         if (nfull < nch) {
           const int rem = J - nfull * STEPS;
 #pragma unroll
@@ -338,7 +382,9 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
       } else if (STREAM) {
         constexpr int STEPS = 32 / PB;  // schedule positions per 256-bit load
         const int nch = (J + STEPS - 1) / STEPS;
-        for (int c = 0; c < nch; ++c) {
+        int c = 0, stop = min(arrive_at, nch);  // as above
+        for (;;) {
+        for (; c < stop; ++c) {
           PrioChunk nxt = q;
           if (c + 1 < nch) nxt = ld_prio32<true>(pg + (c + 1) * 32);
           if ((c + 1) * STEPS <= J) {
@@ -351,6 +397,10 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
               if (t < rem) st.step(prio_at<PB>(q.w, t), t & 1);
           }
           q = nxt;
+        }
+        if (stop >= nch) break;
+        named_arrive(stop, gate_count(stop));
+        stop = stop + 1 < nph ? stop + 1 : nch;
         }
       } else {
         const uint4* prow = reinterpret_cast<const uint4*>(prio_row_s);
@@ -426,6 +476,7 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
         a.out[b0 + lane] = mk;
       }
       if (a.best_key != nullptr) fold_best(a.best_key, active, mk, a.id_base + static_cast<uint32_t>(b0 + lane), lane);
+      arrive_at = nfull_ch + 1;  // warp 0 opens the stagger barriers in its first tile only
     } else {
       // ---- sf.nrounds Metropolis rounds on the rows of this tile, which stay in shared memory: a rejected
       // move is undone in place, an accepted one writes its few changed bytes through to HBM.  The lane
@@ -573,6 +624,10 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
     }
   }
   if (!tab_ready && threadIdx.x == 0) mbar_wait(bar_tab, 0);  // never leave a bulk copy in flight
+  if (kFetch && a.tile_wait != nullptr && lane == 0) {
+    atomicAdd(a.tile_wait, t_wait);
+    atomicAdd(a.tile_wait + 1, globaltimer_ns() - t_loop);
+  }
   if (!SEARCH && fold_pending) try_fold(true);  // before the tail: the publish of this round follows the fold
   if (SEARCH) {
     if (a.sf.keep.counter != nullptr) keep_best_tail(a.sf);
@@ -856,6 +911,8 @@ static TileArgs tile_args(const EvalCall& c, const TilePlan& tp) {
   a.r = c.r;
   a.ntiles = (c.B + 31) / 32;
   a.one = 1;
+  a.packed = a.stagger = 0;
+  a.tile_wait = nullptr;
   return a;
 }
 
@@ -897,6 +954,12 @@ cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, i
     // the headline shape (u8 priorities streamed, one node, table in shared memory): address arithmetic on the FMA
     // pipe unless HOOK_PLAIN_ADDR asks for the plain form
     const bool fma_addr = pb == 1 && stream && !tabg && !multi && !(c.flags & HOOK_PLAIN_ADDR);
+    if (stream && !tabg && !multi) {  // the tile-boundary measures of k_eval_tiles (kFetch)
+      a.packed = c.stride_o == tp.copy_o && c.stride_p == tp.copy_p && !(c.tile_debug & TILE_DEBUG_ROW_COPIES);
+      if (a.packed) a.row_o = tp.copy_o;
+      a.stagger = !(c.tile_debug & TILE_DEBUG_NO_STAGGER);
+      a.tile_wait = c.tile_wait;
+    }
     const TileKernel kern = with_eval_types(pb, c.flags, [&](auto PB, auto INT, auto SUM, auto W, auto D, auto R) -> TileKernel {
       if (tabg) return k_eval_tiles<PB, INT, true, false, false, true, 0, SUM, W, D, R>;
       if constexpr (PB == 1) {

@@ -35,6 +35,14 @@ static_assert(((HOOK_FORCE_GENERIC | HOOK_NO_STREAM | HOOK_NO_FUSED | HOOK_NO_IN
                 SB_FLAG_DUE | SB_FLAG_RELEASE)) == 0,
               "the test hooks share no bit with the SB_FLAG_* flags");
 
+// Debug options of the streamed tile kernel (sb_debug_tile_options): kept on the handle, not in the flags word, and
+// read by sb_eval only.  saturn_b200/_lib.py mirrors the names.
+enum TileDebug : unsigned {
+  TILE_DEBUG_TIMING = 1u,      // time every tile fetch and the tile loop per warp (sb_debug_tile_wait)
+  TILE_DEBUG_ROW_COPIES = 2u,  // one bulk copy per opt row, never one per tile
+  TILE_DEBUG_NO_STAGGER = 4u,  // every warp starts at once
+};
+
 // Compile-time dispatch: f is called with the run-time value as a type (std::true_type / std::false_type, or the
 // prio width as std::integral_constant), so that a launch site names its kernel's template arguments once.
 template <class F>
@@ -140,6 +148,8 @@ struct EvalCall {
   uint32_t id_base = 0;
   int force_generic = 0;
   XchgPost xp;  // fused post of best_key at the end of the tile kernel (tile paths only)
+  unsigned tile_debug = 0;                  // the handle's TileDebug options
+  unsigned long long* tile_wait = nullptr;  // TILE_DEBUG_TIMING: the handle's two counters (sb_debug_tile_wait)
 };
 
 // what the fused search round needs besides an EvalCall (see k_eval_tiles<..., SEARCH = true>)

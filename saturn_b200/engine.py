@@ -256,14 +256,16 @@ class Engine:
              out: Optional[torch.Tensor] = None, best_key: Optional[torch.Tensor] = None, id_base: int = 0,
              _force_generic: bool = False, _no_stream: bool = False, post_key: bool = False, fold_prev: bool = False,
              by_position: bool = False, _plain_addr: bool = False, alt_shape: bool = False,
-             _table_home: int = 0, _reorder: Optional[bool] = None, objective: str = "makespan") -> torch.Tensor:
+             _table_home: int = 0, _reorder: Optional[bool] = None, objective: str = "makespan",
+             _tile_debug: int = 0) -> torch.Tensor:
         """Makespan of every candidate (device tensors).  Asynchronous on the handle's stream.
         objective="completion": the sum of completion times instead (SB_FLAG_SUM_COMPLETION), in `out` and `best_key`.
         by_position: opt[b][i] is the option of the job scheduled i-th (see `opt_by_position`).
         alt_shape: the alternate warp-shuffle kernel (SB_FLAG_ALT_WARPSCAN; a measurement, not a fast path).
         Test hooks: _table_home 2 / 1 puts the position-major kernel's table in a CTA pair's shared memory / in
         global memory whatever its size; _reorder True / False forces / forbids the route that re-orders
-        job-indexed opt rows on the device (path 9)."""
+        job-indexed opt rows on the device (path 9); _tile_debug: the streamed tile kernel's debug options
+        (_lib.TILE_DEBUG_*, sb_debug_tile_options), for this call only."""
         B, stride = self._check_cands(opt, prio, True)
         if out is None:
             out = torch.empty(B, dtype=torch.float32, device=self.device)
@@ -275,9 +277,22 @@ class Engine:
             {0: 0, 1: _lib.HOOK_TABLE_GLOBAL, 2: _lib.HOOK_TABLE_PAIR}[_table_home]) | (
             0 if _reorder is None else (_lib.HOOK_REORDER if _reorder else _lib.HOOK_NO_REORDER))
         kp = C.c_void_p(best_key.data_ptr()) if best_key is not None else None
-        check(self._lib.sb_eval(self._h, C.c_void_p(opt.data_ptr()), C.c_void_p(prio.data_ptr()), B, stride, fl,
-                                C.c_void_p(out.data_ptr()), kp, id_base & 0xffffffff))
+        if _tile_debug:
+            check(self._lib.sb_debug_tile_options(self._h, int(_tile_debug)))
+        try:
+            check(self._lib.sb_eval(self._h, C.c_void_p(opt.data_ptr()), C.c_void_p(prio.data_ptr()), B, stride, fl,
+                                    C.c_void_p(out.data_ptr()), kp, id_base & 0xffffffff))
+        finally:
+            if _tile_debug:
+                check(self._lib.sb_debug_tile_options(self._h, 0))
         return out
+
+    def debug_tile_wait(self):
+        """(fetch-wait ns, tile-loop ns) summed over the warps of every streamed tile launch since the last call that
+        ran with _tile_debug=_lib.TILE_DEBUG_TIMING; resets both (sb_debug_tile_wait)."""
+        v = (C.c_uint64 * 2)()
+        check(self._lib.sb_debug_tile_wait(self._h, v))
+        return int(v[0]), int(v[1])
 
     def last_eval_path(self) -> int:
         return int(self._lib.sb_last_eval_path(self._h))
