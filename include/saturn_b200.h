@@ -171,7 +171,11 @@ int sb_sync(sb_handle* h);
  * With nodes > 1 candidates are evaluated on the reduced table only (SB_FLAG_REDUCED) and the opt
  * byte reads (node << 3) | (k - 1).  Builds on the device: the canonical table
  * tab[J][S][8] (column k-1, +inf where no option), and the min-over-strategies table
- * tmin[J][8] with argS[J][8] (first minimum wins, PerformanceEvaluator.py:105-110). */
+ * tmin[J][8] with argS[J][8] (first minimum wins, PerformanceEvaluator.py:105-110).
+ * Every cell must be >= 0 (-0.0 counts as zero), +inf or a sentinel: a negative or NaN cell returns SB_ERR_ARG (the
+ * list-scheduling step cannot score a negative hold, and a NaN would read as an absent option).  T may be device
+ * memory, so the cells are checked on the device while the table is built.  After that refusal, as after a failed
+ * build, the handle has no table (sb_eval and the rest return SB_ERR_STATE until a table is set). */
 int sb_set_table(sb_handle* h, const float* T, const uint8_t* gcount, int J, int S, int G, int nodes);
 /* Runtime threshold at and above which a table cell counts as one of the profiler's sentinels
  * (1e6 "not profiled", 1e8 "failed", PerformanceEvaluator.py:99,106) and is never PROPOSED by the

@@ -301,7 +301,10 @@ int sb_set_table(sb_handle* h, const float* T, const uint8_t* gcount, int J, int
     if (e == cudaSuccess) e = cudaMemcpyAsync(tmp, T, nT * sizeof(float), cudaMemcpyHostToDevice, h->stream);
     Tdev = tmp;
   }
-  if (e == cudaSuccess) e = build_table_launch(Tdev, J, S, G, packed, h->tab, h->tmin, h->args, h->stream);
+  // d_scratch[0]: set by k_canon_table when a cell is negative or NaN (T may be device memory, so it is checked there)
+  unsigned long long bad_cells = 0;
+  if (e == cudaSuccess) e = cudaMemsetAsync(h->d_scratch, 0, sizeof(unsigned long long), h->stream);
+  if (e == cudaSuccess) e = build_table_launch(Tdev, J, S, G, packed, h->tab, h->tmin, h->args, h->d_scratch, h->stream);
   if (e == cudaSuccess) e = build_valid_launch(h->tmin, h->args, J, 0, h->sentinel, h->vopt[0], h->nvalid[0], h->stream);
   if (e == cudaSuccess) e = build_valid_launch(h->tmin, h->args, J, 1, h->sentinel, h->vopt[1], h->nvalid[1], h->stream);
   h->h_tmin.assign(static_cast<size_t>(J) * kSlots, 0.f);
@@ -310,10 +313,16 @@ int sb_set_table(sb_handle* h, const float* T, const uint8_t* gcount, int J, int
     e = cudaMemcpyAsync(h->h_tmin.data(), h->tmin, h->h_tmin.size() * sizeof(float), cudaMemcpyDeviceToHost, h->stream);
   if (e == cudaSuccess)
     e = cudaMemcpyAsync(h->h_args.data(), h->args, h->h_args.size(), cudaMemcpyDeviceToHost, h->stream);
+  if (e == cudaSuccess)
+    e = cudaMemcpyAsync(&bad_cells, h->d_scratch, sizeof(bad_cells), cudaMemcpyDeviceToHost, h->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
   if (e != cudaSuccess) {
     free_table(h);
     return fail(SB_ERR_CUDA, "building the table failed: %s", cudaGetErrorString(e));
+  }
+  if (bad_cells) {
+    free_table(h);
+    return fail(SB_ERR_ARG, "T holds a negative or NaN runtime (every cell must be >= 0, +inf or a sentinel)");
   }
   h->J = J;
   h->S = S;

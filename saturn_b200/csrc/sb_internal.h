@@ -205,9 +205,9 @@ cudaError_t eval_full_launch(const Device& dev, const EvalCall& c, float* start,
 cudaError_t validate_launch(const Device& dev, const EvalCall& c, unsigned long long* bad, cudaStream_t st,
                             bool by_pos = false);
 
-// table construction (sb_table.cu)
+// table construction (sb_table.cu); *bad (device) is set to 1 when a cell of T is negative or NaN
 cudaError_t build_table_launch(const float* T, int J, int S, int G, uint64_t gcount_packed, float* tab, float* tmin,
-                               uint8_t* args, cudaStream_t st);
+                               uint8_t* args, unsigned long long* bad, cudaStream_t st);
 // valid (non-dominated, non-sentinel) option lists for the search: vopt[J][8] opt bytes, nvalid[J]
 cudaError_t build_valid_launch(const float* tmin, const uint8_t* args, int J, int reduced, float sentinel, uint8_t* vopt,
                                int* nvalid, cudaStream_t st);

@@ -10,9 +10,11 @@
 
 namespace sb {
 
-// one thread per (j, s): scatter the G input columns to their gpu-count column
+// one thread per (j, s): scatter the G input columns to their gpu-count column.  A negative or NaN cell sets
+// *bad: the list-scheduling step needs every hold >= 0 (-0.0 counts as zero; +inf and sentinels are legal), and
+// fminf would turn a NaN into an absent option where the oracle keeps it.
 __global__ void k_canon_table(const float* __restrict__ T, int J, int S, int G, uint64_t gcount_packed,
-                              float* __restrict__ tab) {
+                              float* __restrict__ tab, unsigned long long* __restrict__ bad) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= J * S) return;
   float col[kSlots];
@@ -21,6 +23,7 @@ __global__ void k_canon_table(const float* __restrict__ T, int J, int S, int G, 
   for (int g = 0; g < G; ++g) {
     const int k = static_cast<int>((gcount_packed >> (8 * g)) & 0xff);
     const float v = T[static_cast<size_t>(idx) * G + g];
+    if (!(v >= 0.f)) *bad = 1ull;
 #pragma unroll
     for (int c = 0; c < kSlots; ++c)
       if (c == k - 1) col[c] = fminf(col[c], v);
@@ -49,9 +52,9 @@ __global__ void k_reduce_table(const float* __restrict__ tab, int J, int S, floa
 }
 
 cudaError_t build_table_launch(const float* T, int J, int S, int G, uint64_t gcount_packed, float* tab, float* tmin,
-                               uint8_t* args, cudaStream_t st) {
+                               uint8_t* args, unsigned long long* bad, cudaStream_t st) {
   const int n1 = J * S;
-  k_canon_table<<<(n1 + 127) / 128, 128, 0, st>>>(T, J, S, G, gcount_packed, tab);
+  k_canon_table<<<(n1 + 127) / 128, 128, 0, st>>>(T, J, S, G, gcount_packed, tab, bad);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   const int n2 = J * kSlots;

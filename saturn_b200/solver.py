@@ -566,7 +566,8 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     `objective` as for solve(): "makespan" or "completion" (sum of completion times); `weights` as for solve(),
     a sequence aligned with T's rows (the weighted sum of completion times, last_stats["weighted_completion"]);
     `due` as for solve() with objective="tardiness", a sequence aligned with T's rows; `release` as for solve(),
-    under every objective, a sequence aligned with T's rows (last_stats["total_flow_time"]).
+    under every objective, a sequence aligned with T's rows (last_stats["total_flow_time"]).  Every cell of T must be
+    >= 0 (-0.0 counts as zero), +inf or a sentinel: a negative or NaN cell raises SolverError, with or without `mask`.
 
     The table goes to the device un-reduced (sb_set_table: min over strategies with the first-minimum rule
     and its arg-min on the device, PerformanceEvaluator.py:101-115); the search runs on the reduced view
@@ -580,6 +581,9 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     T = np.ascontiguousarray(T, dtype=np.float32)
     if T.ndim != 3:
         raise SolverError("T must be [J][S][G]")
+    if np.isnan(T).any() or (T < 0).any():
+        # the device refuses them too (sb_set_table): a negative hold cannot be list-scheduled, a NaN is no runtime
+        raise SolverError("T holds a negative or NaN runtime: every cell must be >= 0, +inf or a sentinel")
     J, S, G = T.shape
     w64, w32 = _resolve_weights(weights, objective, J)
     d64, d32 = _resolve_due(due, objective, J)
