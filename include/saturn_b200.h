@@ -310,7 +310,8 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
  * saved before the launch stops moving until the launch ends, so the saved incumbent is exactly the candidate
  * its key was scored on — and a search is reproducible bit for bit whatever the interleaving of warps. */
 int sb_search_round(sb_handle* h, int rounds);
-/* device pointer to the uint64 best key ((makespan bits << 32) | global chain id) */
+/* device pointer to the uint64 best key ((makespan bits << 32) | global chain id); after every call it is the key
+ * sb_search_best returns with the saved candidate */
 int sb_search_best_key_ptr(sb_handle* h, uint64_t** key_dev);
 /* copy the best candidate found so far to host buffers: opt u8 [J], prio u8/u16 [J] */
 int sb_search_best(sb_handle* h, uint8_t* opt, void* prio, float* makespan, uint64_t* key);
@@ -326,7 +327,8 @@ int sb_search_resample(sb_handle* h);
  * population each and scores them; with SB_FLAG_SUM_COMPLETION the orders are shortest-processing-time
  * instead (ascending runtime of the chosen option), with SB_FLAG_WEIGHTED as well WSPT orders (ascending runtime / weight,
  * ties by job index), with SB_FLAG_DUE EDD orders (ascending due date, ties by runtime / weight, then job index),
- * same options and node fill.  sb_search_run = sb_search_init + seeds + `rounds` rounds in groups of
+ * same options and node fill.  Every job's option is one the search would propose: a cell below the sentinel, or
+ * for a job without one its cheapest finite cell.  sb_search_run = sb_search_init + seeds + `rounds` rounds in groups of
  * `sync_every` (tournament resampling every `resample_every` rounds inside a group is only another launch;
  * the host reads the incumbent key once per group and applies the stopping rules) + sb_search_best.
  * The multi-GPU driver (saturn_b200/search.py) runs the same steps with a key exchange per group. */
@@ -399,6 +401,13 @@ int sb_debug_tile_options(sb_handle* h, unsigned options);
 /* out[0] = the summed fetch waits, out[1] = the summed tile-loop times (ns) of every launch under option bit 1
  * since the last call; the call resets both.  Synchronous. */
 int sb_debug_tile_wait(sb_handle* h, uint64_t* out);
+/* Copy chains [first, first + count) of the search population to host buffers (any may be NULL): the current opt
+ * rows u8 [count][J], job-indexed in this header's encoding whatever layout the population is kept in, the prio rows
+ * u8/u16 [count][J] and the current scores fp32 [count] (the makespan, or the objective's score).  *layout receives
+ * how rounds run on it: 0 = propose / evaluate / accept kernels, 1 = the fused tile round, 2 = the position-major
+ * round.  For tests that check the state every chain is left in.  Synchronous. */
+int sb_debug_search_population(sb_handle* h, int64_t first, int64_t count, uint8_t* opt, void* prio, float* score,
+                               int* layout);
 /* candidates evaluated so far by this handle's searches */
 int sb_search_stats(sb_handle* h, int64_t* evaluated, int64_t* rounds_done);
 

@@ -42,7 +42,7 @@ SYMBOLS = [
     "sb_decode", "sb_xchg_create", "sb_xchg_connect", "sb_xchg_connect_local", "sb_xchg_post", "sb_xchg_reduce", "sb_xchg_check",
     "sb_search_init", "sb_search_round", "sb_search_best_key_ptr", "sb_search_best",
     "sb_search_inject", "sb_search_resample", "sb_search_seed_lpt", "sb_search_run", "sb_search_run_multi", "sb_search_wave", "sb_search_is_fused", "sb_search_stats", "sb_search_validate", "sb_search_verify_count",
-    "sb_debug_tile_options", "sb_debug_tile_wait",
+    "sb_debug_tile_options", "sb_debug_tile_wait", "sb_debug_search_population",
 ]
 
 
@@ -125,6 +125,7 @@ def load():
         "sb_search_verify_count": [vp, C.POINTER(C.c_uint64)],
         "sb_debug_tile_options": [vp, C.c_uint],
         "sb_debug_tile_wait": [vp, C.POINTER(C.c_uint64)],
+        "sb_debug_search_population": [vp, i64, i64, vp, vp, vp, C.POINTER(ci)],
     }
     for name, args in sigs.items():
         fn = getattr(lib, name)

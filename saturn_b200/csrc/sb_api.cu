@@ -1257,20 +1257,21 @@ int sb_search_seed_lpt(sb_handle* h) {
   const bool edd = spt && (s.p.flags & SB_FLAG_DUE) != 0;
   const bool rel = (s.p.flags & SB_FLAG_RELEASE) != 0;
   const double INF = HUGE_VAL;
-  // usable cells: below the sentinel threshold; a job with none falls back to any finite cell
+  // usable cells: the ones the search proposes (k_build_valid), per job: those below the sentinel threshold, and for
+  // a job with none only its cheapest finite cell (the first minimum; column 0 if it has no finite cell)
   std::vector<double> usable(static_cast<size_t>(J) * kSlots);
-  bool every_job = true;
   for (int j = 0; j < J; ++j) {
     bool any = false;
+    float best = INFINITY;
+    int best_c = 0;
     for (int c = 0; c < kSlots; ++c) {
       const float v = tmin[j * kSlots + c];
       usable[j * kSlots + c] = (v < h->sentinel) ? v : INF;
       any = any || (v < h->sentinel);
+      if (v < best) { best = v; best_c = c; }
     }
-    every_job = every_job && any;
+    if (!any) usable[j * kSlots + best_c] = best;
   }
-  if (!every_job)
-    for (size_t i = 0; i < usable.size(); ++i) usable[i] = isfinite(tmin[i]) ? tmin[i] : INF;
   const long long chains = s.d.chains;
   const long long per = std::max<long long>(1, chains / 8);
   std::vector<int> col(J), order(J);
@@ -1588,6 +1589,41 @@ int sb_debug_tile_wait(sb_handle* h, uint64_t* out) {
   }
   out[0] = v[0];
   out[1] = v[1];
+  return SB_OK;
+}
+
+int sb_debug_search_population(sb_handle* h, int64_t first, int64_t count, uint8_t* opt, void* prio, float* score,
+                               int* layout) {
+  int rc = use_device(h);
+  if (rc) return rc;
+  SearchState& s = h->search;
+  if (!s.ready) return fail(SB_ERR_STATE, "sb_search_init has not been called");
+  if (first < 0 || count < 0 || first + count > s.d.chains)
+    return fail(SB_ERR_ARG, "chains [%lld, %lld) outside the population of %lld", (long long)first,
+                (long long)(first + count), (long long)s.d.chains);
+  const size_t J = static_cast<size_t>(s.d.J), pbytes = J * s.d.pb;
+  // position-major rows need their priorities to come back job-indexed
+  std::vector<uint8_t> pr;
+  uint8_t* prio_out = static_cast<uint8_t*>(prio);
+  if (s.d.pos && opt && !prio_out) {
+    pr.resize(static_cast<size_t>(count) * pbytes);
+    prio_out = pr.data();
+  }
+  if (count > 0) {
+    if (opt)
+      CK(cudaMemcpy2DAsync(opt, J, s.d.cur_o + first * s.d.stride_o, s.d.stride_o, J, count, cudaMemcpyDeviceToHost,
+                           h->stream));
+    if (prio_out)
+      CK(cudaMemcpy2DAsync(prio_out, pbytes, s.d.cur_p + first * s.d.stride_p, s.d.stride_p, pbytes, count,
+                           cudaMemcpyDeviceToHost, h->stream));
+    if (score)
+      CK(cudaMemcpyAsync(score, s.d.cur_mk + first, static_cast<size_t>(count) * sizeof(float), cudaMemcpyDeviceToHost,
+                         h->stream));
+  }
+  CK(cudaStreamSynchronize(h->stream));
+  if (s.d.pos && opt)
+    for (int64_t c = 0; c < count; ++c) opt_from_positions(s.d.J, s.d.pb, opt + c * J, prio_out + c * pbytes);
+  if (layout) *layout = s.d.pos ? 2 : (s.fused_ok ? 1 : 0);
   return SB_OK;
 }
 

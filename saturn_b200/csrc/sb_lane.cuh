@@ -249,8 +249,15 @@ __device__ __forceinline__ void keep_best_tail(const SearchFuse& sf) {
   __threadfence();
   const int lane = threadIdx.x;
   const unsigned long long key = *reinterpret_cast<volatile unsigned long long*>(sf.keep.keys);
-  // only a strictly better MAKESPAN replaces the saved incumbent: exactly the chains that froze (frozen_by)
-  if ((key >> 32) >= (*reinterpret_cast<volatile unsigned long long*>(sf.keep.keys + 1) >> 32)) return;
+  const unsigned long long saved = *reinterpret_cast<volatile unsigned long long*>(sf.keep.keys + 1);
+  // only a strictly better MAKESPAN replaces the saved incumbent: exactly the chains that froze (frozen_by).  A
+  // lower key with the saved score (a lower chain id) names a chain that kept moving, so its rows are no longer the
+  // ones that key was scored on: the best key goes back to the saved incumbent's, or the next k_keep_best (an
+  // injection, an unfused round) would save that chain's current rows under it.
+  if ((key >> 32) >= (saved >> 32)) {
+    if (lane == 0 && key != saved) sf.keep.keys[0] = saved;
+    return;
+  }
   const long long c = static_cast<long long>(((key & 0xffffffffull) - (sf.chain_base & 0xffffffffull)) & 0xffffffffull);
   if (c >= sf.keep.chains) return;
   const uint4* so = reinterpret_cast<const uint4*>(sf.cur_o + c * sf.keep.stride_o);

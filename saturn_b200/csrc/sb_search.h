@@ -16,7 +16,9 @@ struct SearchDev {
   float *cur_mk = nullptr, *prop_mk = nullptr;
   const uint8_t* vopt = nullptr;  // [J][8]
   const int* nvalid = nullptr;    // [J]
-  unsigned long long* keys = nullptr;  // [0] best key of this population, [1] key of the saved encoding
+  // [0] best key of this population, [1] key of the saved encoding; equal after every call (k_keep_best saves
+  // the rows of [0]'s chain, so [0] must never name a chain that has moved on since it was scored)
+  unsigned long long* keys = nullptr;
   uint8_t *best_o = nullptr, *best_p = nullptr;
 };
 

@@ -484,6 +484,22 @@ class Engine:
         check(self._lib.sb_search_validate(self._h, C.byref(bad)))
         return int(bad.value)
 
+    def debug_search_population(self, first: int = 0, count: Optional[int] = None):
+        """Chains [first, first + count) of the search population (all from `first` when count is None):
+        (opt [count][J] u8 job-indexed, prio [count][J] u8/u16, score [count] fp32, layout), layout 0 for
+        propose / evaluate / accept rounds, 1 for the fused tile round, 2 for the position-major round."""
+        if count is None:
+            count = self._search_chains - first
+        J = self.J
+        opt = np.empty((count, J), dtype=np.uint8)
+        prio = np.empty((count, J), dtype=np.uint8 if J <= 256 else np.uint16)
+        score = np.empty(count, dtype=np.float32)
+        layout = C.c_int(-1)
+        check(self._lib.sb_debug_search_population(self._h, int(first), int(count), C.c_void_p(opt.ctypes.data),
+                                                   C.c_void_p(prio.ctypes.data), C.c_void_p(score.ctypes.data),
+                                                   C.byref(layout)))
+        return opt, prio, score, int(layout.value)
+
     def search_stats(self):
         ev, rd = C.c_int64(0), C.c_int64(0)
         check(self._lib.sb_search_stats(self._h, C.byref(ev), C.byref(rd)))

@@ -73,9 +73,12 @@ def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objecti
         if integer_starts:
             rel = np.ceil(rel)
     J = tmin.shape[0]
+    # the cells the search proposes: those below the sentinel, and for a job without one only its cheapest finite
+    # cell (the first minimum; column 0 when it has none)
     usable = np.where(tmin < sentinel, tmin, np.inf)
-    if not np.isfinite(usable).any(axis=1).all():
-        usable = np.where(np.isfinite(tmin), tmin, np.inf)
+    bare = ~(tmin < sentinel).any(axis=1)
+    cheapest = np.argmin(tmin, axis=1)
+    usable[bare, cheapest[bare]] = tmin[bare, cheapest[bare]]
     k = np.arange(1, 9, dtype=np.float64)[None, :]
     seeds = []
     for area_weight in (0.0, 1.0, 0.5):

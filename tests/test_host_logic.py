@@ -392,3 +392,24 @@ def test_fp32_horizon_guard():
     _check_horizon(T, found_makespan=1.5e7)
     with pytest.raises(SolverError):
         _check_horizon(T, found_makespan=float(1 << 24))
+
+
+def test_lpt_seeds_never_plant_a_sentinel_cell_of_a_job_that_has_a_usable_one():
+    """Job 0 has a usable cell (k = 8) and a 1e6 "not profiled" cell (k = 1); job 1 has no cell below the sentinel.
+    Every seed puts job 0 on k = 8 and job 1 on its cheapest cell (k = 4), the one cell the search keeps for it: a
+    job without a usable cell must not make the others fall back to their sentinel cells."""
+    from saturn_b200.search import lpt_seeds
+    tmin = np.full((2, 8), np.inf, dtype=np.float32)
+    tmin[0, 0], tmin[0, 7] = 1e6, 5e5
+    tmin[1, 0], tmin[1, 3] = 1e8, 1e6
+    for objective in ("makespan", "completion"):
+        for nodes in (1, 2):
+            seeds = lpt_seeds(tmin, nodes=nodes, objective=objective)
+            assert len(seeds) == 3
+            for ob, order in seeds:
+                assert (ob & 7).tolist() == [7, 3], (objective, nodes, ob)
+                assert sorted(order.tolist()) == [0, 1]
+    # a job with no finite cell at all keeps column 0, as the search does
+    tmin[1] = np.inf
+    for ob, _ in lpt_seeds(tmin):
+        assert ob.tolist() == [7, 0]
