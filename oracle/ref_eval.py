@@ -63,7 +63,8 @@ INF = float("inf")
 def canon_table(T: np.ndarray, gcount: Sequence[int]) -> np.ndarray:
     """T[J][S][G] + gcount[G] -> canonical tab[J][S][8] (column = k-1, +inf if absent).
 
-    If two input columns carry the same GPU count the smaller runtime is kept.
+    If two input columns carry the same GPU count the smaller runtime is kept; on equal runtimes the earlier
+    column's value, so -0.0 and +0.0 keep the sign of the first of them (as sb_set_table does).
     """
     T = np.asarray(T)
     J, S, G = T.shape
@@ -72,7 +73,7 @@ def canon_table(T: np.ndarray, gcount: Sequence[int]) -> np.ndarray:
         k = int(gcount[g])
         if not 1 <= k <= NSLOT:
             raise ValueError("gpu count %d outside 1..8" % k)
-        tab[:, :, k - 1] = np.minimum(tab[:, :, k - 1], T[:, :, g])
+        tab[:, :, k - 1] = np.where(T[:, :, g] < tab[:, :, k - 1], T[:, :, g], tab[:, :, k - 1])
     return tab
 
 
@@ -83,8 +84,9 @@ def reduce_table(tab: np.ndarray) -> Tuple[np.ndarray, np.ndarray]:
     PerformanceEvaluator.py:101-115 (`if runtime < chosen_runtime` keeps the
     first executor that attains the minimum).
     """
-    tmin = tab.min(axis=1)
     args = tab.argmin(axis=1).astype(np.uint8)  # numpy argmin returns first occurrence
+    # the value of that strategy: a min() reduction may return either zero of a -0.0 / +0.0 tie
+    tmin = np.take_along_axis(tab, args[:, None, :].astype(np.intp), axis=1)[:, 0, :]
     return tmin, args
 
 

@@ -10,9 +10,11 @@
 
 namespace sb {
 
-// one thread per (j, s): scatter the G input columns to their gpu-count column.  A negative or NaN cell sets
-// *bad: the list-scheduling step needs every hold >= 0 (-0.0 counts as zero; +inf and sentinels are legal), and
-// fminf would turn a NaN into an absent option where the oracle keeps it.
+// one thread per (j, s): scatter the G input columns to their gpu-count column.  Columns with the same GPU count
+// keep the first one (in input order) that attains their minimum, with its bits: -0.0 and +0.0 compare equal, so the
+// sign of a zero comes from the earlier column, whatever min() does with zeros of both signs.  A negative or NaN
+// cell sets *bad: the list-scheduling step needs every hold >= 0 (-0.0 counts as zero; +inf and sentinels are
+// legal), and a NaN is no runtime.
 __global__ void k_canon_table(const float* __restrict__ T, int J, int S, int G, uint64_t gcount_packed,
                               float* __restrict__ tab, unsigned long long* __restrict__ bad) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -26,7 +28,7 @@ __global__ void k_canon_table(const float* __restrict__ T, int J, int S, int G, 
     if (!(v >= 0.f)) *bad = 1ull;
 #pragma unroll
     for (int c = 0; c < kSlots; ++c)
-      if (c == k - 1) col[c] = fminf(col[c], v);
+      if (c == k - 1 && v < col[c]) col[c] = v;
   }
 #pragma unroll
   for (int c = 0; c < kSlots; ++c) tab[static_cast<size_t>(idx) * kSlots + c] = col[c];

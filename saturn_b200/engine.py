@@ -433,11 +433,12 @@ class Engine:
                            heuristic_seeds, record_history, _no_fused, int(_extra_flags) | self._release_flag(),
                            objective)
 
-    def search_wave(self, reduced: bool = False) -> int:
+    def search_wave(self, reduced: bool = False, objective: str = "makespan") -> int:
         """Chains that fill the device exactly once with the round kernel of the current table; populations
-        that are whole multiples of it leave no partially filled last wave."""
+        that are whole multiples of it leave no partially filled last wave.  The objective's per-job arrays (weights,
+        due dates) and the release dates sit beside the table and can change the round kernel's shape."""
         n = C.c_int64(0)
-        check(self._lib.sb_search_wave(self._h, _flags(False, reduced) | self._release_flag(), C.byref(n)))
+        check(self._lib.sb_search_wave(self._h, _flags(False, reduced, objective) | self._release_flag(), C.byref(n)))
         return int(n.value)
 
     def search_is_fused(self) -> bool:
@@ -619,9 +620,9 @@ class MultiEngine:
     def decode(self, *a, **kw):
         return self.engines[0].decode(*a, **kw)
 
-    def search_wave(self, reduced: bool = False) -> int:
+    def search_wave(self, reduced: bool = False, objective: str = "makespan") -> int:
         """chains PER DEVICE that fill one device exactly once."""
-        return self.engines[0].search_wave(reduced)
+        return self.engines[0].search_wave(reduced, objective)
 
     def search_run(self, chains: int, rounds: int, seed: int = 0, chain_base: int = 0, integer_starts: bool = True,
                    reduced: bool = False, t_start: float = 5e-4, t_end: float = 1e-6, warm=None,
