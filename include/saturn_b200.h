@@ -55,6 +55,13 @@
  * d = 0 gives exactly the weighted fold, due dates at or past every completion give +0, w = 2 exactly twice w = 1.
  * The score is >= +0, so the (bits << 32) | id key still orders by it.
  * The schedule, every start and every slot mask are the same under every objective.
+ * With SB_FLAG_MAX_LATENESS (per-job due dates d_j, sb_set_due) the score is the maximum lateness
+ * L_max = max_j (start_j + rt_j - d_j), emitted as the tail makespan L_max + D >= +0 with D = max_t d_t:
+ *   q_j = D - d_j (>= +0, made once in fp32 by sb_set_due), e = start + rt (as above), x = e + q (one rounding),
+ *   score = max_j x, a max fold from +0 like the makespan's.
+ * Every score the library emits then holds L_max + D, so the key still orders by it; subtract D to get L_max.  Due
+ * dates shifted by one constant give the same q, hence the same scores and plans.  d = c for a constant c gives
+ * exactly the makespan.
  * With SB_FLAG_RELEASE (per-job release dates r_j, sb_set_release; valid under every objective above) a job may not
  * start before its release:
  *       start = max(max(ready[sel]), r_j)
@@ -149,6 +156,18 @@ typedef enum sb_status {
                                      re-sorts each seed's order stably by ascending release date (ceiled with
                                      SB_FLAG_INTEGER_STARTS), so jobs released together keep the objective's order.
                                      Not available with SB_FLAG_ALT_WARPSCAN (SB_ERR_UNSUPPORTED). */
+#define SB_FLAG_MAX_LATENESS 1024u /* after sb_set_due (else SB_ERR_STATE): the objective is the maximum lateness,
+                                     scored as the tail makespan L_max + max_t d_t (see the evaluation rule above).
+                                     Not combinable with SB_FLAG_SUM_COMPLETION, SB_FLAG_WEIGHTED or SB_FLAG_DUE, and
+                                     refused when max d - min d >= 2^24 (SB_ERR_ARG both).  Below that spread the
+                                     tails of integer due dates are exact; fractional due dates get q rounded to
+                                     fp32 like any fp32 subtraction (the device and the oracle round alike).
+                                     Valid with SB_FLAG_RELEASE and several nodes; accepted wherever SB_FLAG_DUE is,
+                                     sb_search_run_multi included (every handle must hold due dates).  The search's
+                                     temperature unit is the makespan's (a fraction of the incumbent score), it has
+                                     no stop at zero (stop_reason 3 only follows target_makespan, which then targets
+                                     the tail makespan), and sb_search_seed_lpt plants the unit-weight EDD orders of
+                                     SB_FLAG_DUE.  Not available with SB_FLAG_ALT_WARPSCAN (SB_ERR_UNSUPPORTED). */
 #define SB_IPC_HANDLE_BYTES 64
 
 typedef struct sb_handle sb_handle;
@@ -186,10 +205,12 @@ int sb_set_sentinel(sb_handle* h, float threshold);
  * that differs from the table's); w = NULL clears them.  SB_ERR_STATE before sb_set_table.  sb_set_table clears
  * the weights; setting or clearing them ends the current search (sb_search_init again). */
 int sb_set_weights(sb_handle* h, const float* w, int J);
-/* Per-job due dates for SB_FLAG_DUE: d host fp32 [J] in the runtimes' units from the plan's t = 0, every value
+/* Per-job due dates for SB_FLAG_DUE and SB_FLAG_MAX_LATENESS: d host fp32 [J] in the runtimes' units from the plan's
+ * t = 0, every value
  * finite with |d| < 2^24 (negative: already overdue) (else SB_ERR_ARG, as is a J that differs from the table's);
  * d = NULL clears them.  SB_ERR_STATE before sb_set_table.  sb_set_table clears the due dates; setting or clearing
- * them ends the current search (sb_search_init again). */
+ * them ends the current search (sb_search_init again).  It also makes the delivery tails max_t d_t - d_j that
+ * SB_FLAG_MAX_LATENESS scores, once, and records whether max d - min d < 2^24 (else that flag is refused). */
 int sb_set_due(sb_handle* h, const float* d, int J);
 /* Per-job release dates for SB_FLAG_RELEASE: r host fp32 [J] in the runtimes' units from the plan's t = 0, every
  * value finite with |r| < 2^24 (r <= 0: already released) (else SB_ERR_ARG, as is a J that differs from the

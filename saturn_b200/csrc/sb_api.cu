@@ -60,7 +60,8 @@ struct SearchState {
   bool win = false, inc = false, verify = false;
   SearchDev alloc;  // the pointers as allocated (s.d's cur / prop pairs trade places when resampling)
   const float* w = nullptr;    // SB_FLAG_WEIGHTED: the handle's job weights (SB_FLAG_DUE alone: its unit weights)
-  const float* due = nullptr;  // SB_FLAG_DUE: the handle's due dates (position-major kernels)
+  const float* due = nullptr;  // SB_FLAG_DUE: the handle's due dates (SB_FLAG_MAX_LATENESS: its delivery tails)
+                               // (position-major kernels)
   const float* rel = nullptr;  // SB_FLAG_RELEASE: the handle's release dates as the flags read them (likewise)
 };
 
@@ -110,6 +111,11 @@ struct sb_handle {
   size_t d_d_cap = 0;
   std::vector<float> h_d;
   bool has_d = false;
+  // SB_FLAG_MAX_LATENESS: the delivery tails q_j = max_t d_t - d_j (fp32, padded like d_d; the kernels fold
+  // max(C + q) = L_max + max_t d_t >= +0), made by sb_set_due, and whether max d - min d < 2^24 (else even integer
+  // due dates give tails that round, and the flag is refused; fractional due dates may round below that too)
+  float* d_q = nullptr;
+  bool q_exact = false;
   // release dates (sb_set_release): device copies padded like d_w, as given (d_r) and ceiled for
   // SB_FLAG_INTEGER_STARTS (d_rc), and the host copies (seed orders); has_r is cleared by sb_set_table
   float* d_r = nullptr;
@@ -231,6 +237,7 @@ int sb_destroy(sb_handle* h) {
   cudaFree(h->d_w);
   cudaFree(h->d_d);
   cudaFree(h->d_one);
+  cudaFree(h->d_q);
   cudaFree(h->d_r);
   cudaFree(h->d_rc);
   for (int i = 0; i < 2; ++i)
@@ -390,18 +397,26 @@ int sb_set_due(sb_handle* h, const float* d, int J) {
   if (h->d_d_cap < cap) {
     cudaFree(h->d_d);
     cudaFree(h->d_one);
-    h->d_d = h->d_one = nullptr;
+    cudaFree(h->d_q);
+    h->d_d = h->d_one = h->d_q = nullptr;
     h->d_d_cap = 0;
     CK(cudaMalloc(&h->d_d, cap * sizeof(float)));
     CK(cudaMalloc(&h->d_one, cap * sizeof(float)));
+    CK(cudaMalloc(&h->d_q, cap * sizeof(float)));
     h->d_d_cap = cap;
   }
   std::vector<float> one(cap, 0.f);
   std::fill(one.begin(), one.begin() + J, 1.f);
   h->h_d.assign(d, d + J);
   h->h_d.resize(cap, 0.f);
+  const float dmax = *std::max_element(d, d + J), dmin = *std::min_element(d, d + J);
+  h->q_exact = static_cast<double>(dmax) - static_cast<double>(dmin) < 16777216.0;
+  // q >= +0: dmax - d is +0 (never -0) where d = dmax
+  std::vector<float> q(cap, 0.f);
+  for (int j = 0; j < J; ++j) q[j] = dmax - d[j];
   CK(cudaMemcpyAsync(h->d_d, h->h_d.data(), cap * sizeof(float), cudaMemcpyHostToDevice, h->stream));
   CK(cudaMemcpyAsync(h->d_one, one.data(), cap * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+  CK(cudaMemcpyAsync(h->d_q, q.data(), cap * sizeof(float), cudaMemcpyHostToDevice, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   h->has_d = true;
   return SB_OK;
@@ -447,8 +462,17 @@ int sb_set_release(sb_handle* h, const float* r, int J) {
 }
 
 // SB_FLAG_WEIGHTED and SB_FLAG_DUE are valid with SB_FLAG_SUM_COMPLETION only, and after sb_set_weights /
-// sb_set_due respectively; SB_FLAG_RELEASE under any objective, after sb_set_release
+// sb_set_due respectively; SB_FLAG_MAX_LATENESS alone among the objective flags, after sb_set_due with a due-date spread
+// below 2^24; SB_FLAG_RELEASE under any objective, after sb_set_release
 static int check_per_job(const sb_handle* h, unsigned flags) {
+  if ((flags & SB_FLAG_MAX_LATENESS) && (flags & (SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED | SB_FLAG_DUE)))
+    return fail(SB_ERR_ARG, "SB_FLAG_MAX_LATENESS is an objective of its own: it cannot be combined with "
+                "SB_FLAG_SUM_COMPLETION, SB_FLAG_WEIGHTED or SB_FLAG_DUE");
+  if ((flags & SB_FLAG_MAX_LATENESS) && !h->has_d)
+    return fail(SB_ERR_STATE, "SB_FLAG_MAX_LATENESS needs sb_set_due (sb_set_table clears the due dates)");
+  if ((flags & SB_FLAG_MAX_LATENESS) && !h->q_exact)
+    return fail(SB_ERR_ARG, "SB_FLAG_MAX_LATENESS needs max d - min d < 2^24 (beyond it the tails max d - d round even for "
+                "integer due dates)");
   if ((flags & SB_FLAG_WEIGHTED) && !(flags & SB_FLAG_SUM_COMPLETION))
     return fail(SB_ERR_ARG, "SB_FLAG_WEIGHTED weights the sum of completion times: it needs SB_FLAG_SUM_COMPLETION");
   if ((flags & SB_FLAG_DUE) && !(flags & SB_FLAG_SUM_COMPLETION))
@@ -465,6 +489,11 @@ static int check_per_job(const sb_handle* h, unsigned flags) {
 static const float* job_release(const sb_handle* h, unsigned flags) {
   if (!(flags & SB_FLAG_RELEASE)) return nullptr;
   return (flags & SB_FLAG_INTEGER_STARTS) ? h->d_rc : h->d_r;
+}
+// the due-date array the kernels read: the due dates (SB_FLAG_DUE), the delivery tails (SB_FLAG_MAX_LATENESS), or none
+static const float* job_due(const sb_handle* h, unsigned flags) {
+  if (flags & SB_FLAG_DUE) return h->d_d;
+  return (flags & SB_FLAG_MAX_LATENESS) ? h->d_q : nullptr;
 }
 // the weights the kernels read: the caller's, the unit weights of SB_FLAG_DUE alone, or none
 static const float* job_weights(const sb_handle* h, unsigned flags) {
@@ -506,7 +535,7 @@ static int make_call(sb_handle* h, const uint8_t* opt, const void* prio, int64_t
   c->stride_p = row_stride * pb;
   c->flags = flags;
   c->w = job_weights(h, flags);
-  c->d = (flags & SB_FLAG_DUE) ? h->d_d : nullptr;
+  c->d = job_due(h, flags);
   c->r = job_release(h, flags);
   return SB_OK;
 }
@@ -566,9 +595,10 @@ int sb_eval(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, int64
     }
   }
   if (flags & SB_FLAG_ALT_WARPSCAN) {
-    if (flags & (SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED | SB_FLAG_DUE | SB_FLAG_RELEASE))
+    if (flags & (SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED | SB_FLAG_DUE | SB_FLAG_RELEASE | SB_FLAG_MAX_LATENESS))
       return fail(SB_ERR_UNSUPPORTED, "SB_FLAG_ALT_WARPSCAN scores the makespan without release dates only: it "
-                  "cannot be combined with SB_FLAG_SUM_COMPLETION, SB_FLAG_WEIGHTED, SB_FLAG_DUE or SB_FLAG_RELEASE");
+                  "cannot be combined with SB_FLAG_SUM_COMPLETION, SB_FLAG_WEIGHTED, SB_FLAG_DUE, SB_FLAG_RELEASE or "
+                  "SB_FLAG_MAX_LATENESS");
     if (flags & (SB_FLAG_POST_KEY | SB_FLAG_FOLD_PREV))
       return fail(SB_ERR_UNSUPPORTED, "SB_FLAG_ALT_WARPSCAN cannot be combined with the fused key exchange");
     cudaError_t e = eval_alt_launch(h->dev, c, h->stream);
@@ -945,7 +975,7 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
   const bool due = (p->flags & SB_FLAG_DUE) != 0;
   const int arrays = job_arrays(p->flags);
   s.w = job_weights(h, p->flags);
-  s.due = due ? h->d_d : nullptr;
+  s.due = job_due(h, p->flags);
   s.rel = job_release(h, p->flags);
   d.stride_o = (J + 31) & ~31;  // 32-byte rows: TMA bulk copies for opt, 256-bit streaming loads for prio
   // make stride_p == stride_o * pb so that one element stride describes both (sb_eval contract)
@@ -1253,8 +1283,9 @@ int sb_search_seed_lpt(sb_handle* h) {
   const bool spt = (s.p.flags & SB_FLAG_SUM_COMPLETION) != 0;  // shortest first: the order that favours the sum
   // weighted sum: Smith's rule (WSPT), ascending rt / w; with unit weights exactly the SPT order
   const bool wspt = spt && (s.p.flags & SB_FLAG_WEIGHTED) != 0;
-  // tardiness: earliest due date first (EDD), ties by rt / w (rt with unit weights), then by job index
-  const bool edd = spt && (s.p.flags & SB_FLAG_DUE) != 0;
+  // tardiness: earliest due date first (EDD), ties by rt / w (rt with unit weights), then by job index; the maximum
+  // lateness the same unit-weight EDD orders (Jackson's rule, optimal for L_max on one machine)
+  const bool edd = (spt && (s.p.flags & SB_FLAG_DUE) != 0) || (s.p.flags & SB_FLAG_MAX_LATENESS) != 0;
   const bool rel = (s.p.flags & SB_FLAG_RELEASE) != 0;
   const double INF = HUGE_VAL;
   // usable cells: the ones the search proposes (k_build_valid), per job: those below the sentinel threshold, and for

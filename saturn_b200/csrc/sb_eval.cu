@@ -32,6 +32,9 @@
 //     the table is in shared memory (same TMA phase), and are read from global memory where the table is;
 //   * D (SB_FLAG_DUE, with W only): the weighted sum is of tardiness against per-job due dates instead of
 //     completions.  The due dates follow the weights, in the same memory and the same TMA phase;
+//   * D without SUM (SB_FLAG_MAX_LATENESS): the tail makespan max_j (C_j + q_j) with delivery tails q_j =
+//     max_t d_t - d_j >= 0, i.e. L_max + max_t d_t (ls_step<..., kDue> without kSum).  The tails take the due
+//     dates' place, in the same memory and the same TMA phase;
 //   * R (SB_FLAG_RELEASE, with any of the above): no job starts before its release date.  Every objective form has
 //     a release twin; the release dates follow the other per-job arrays, in the same memory and TMA phase.
 #include "sb_lane.cuh"
@@ -73,7 +76,7 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
   static_assert(!(SEARCH && (STREAM || TABG)), "the fused search round runs on shared-memory tiles only");
   static_assert(ADDR == 0 || (!TABG && !MULTI && !SEARCH), "ADDR = 1 needs the table and the opt rows in shared memory");
   static_assert(SUM || !W, "weights scale the sum of completion times only");
-  static_assert(W || !D, "due dates run on the weighted form");
+  static_assert(W || !D || !SUM, "tardiness runs on the weighted form");
   extern __shared__ __align__(128) uint8_t smem[];
   const int nw = blockDim.x >> 5;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -81,7 +84,7 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
   // W: the weights follow the table in the same TMA phase, padded to 16 bytes (TABG: both stay in global memory);
   // D: the due dates follow the weights the same way; R: the release dates follow them
   const uint32_t w_bytes = (W && !TABG) ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u;
-  const uint32_t d_bytes = D ? w_bytes : 0u;
+  const uint32_t d_bytes = D ? (W ? w_bytes : (TABG ? 0u : ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u))) : 0u;
   const uint32_t r_bytes = (R && !TABG) ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u;
   float* tab_s = reinterpret_cast<float*>(smem);
   [[maybe_unused]] float* w_s = reinterpret_cast<float*>(smem + tab_bytes);
@@ -131,7 +134,7 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
     }
   }
 
-  LaneState<INT, MULTI, ADDR, SUM, (W ? (TABG ? 2 : 1) : 0), D, (R ? (TABG ? 2 : 1) : 0)> st;
+  LaneState<INT, MULTI, ADDR, SUM, (W ? (TABG ? 2 : 1) : 0), (D ? (TABG ? 2 : 1) : 0), (R ? (TABG ? 2 : 1) : 0)> st;
   if (TABG) st.tab = a.tab;
   else st.tab = tab_s;
   if constexpr (W) {
@@ -301,7 +304,7 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
         uint32_t ob[kBatch];
         float rb[kBatch];
         [[maybe_unused]] float wb[kBatch];  // W: the batch's weights, gathered with its runtimes
-        [[maybe_unused]] float db[kBatch];  // D: the batch's due dates, likewise
+        [[maybe_unused]] float db[kBatch];  // D: the batch's due dates (or tails), likewise
         [[maybe_unused]] float xb[kBatch];  // R: the batch's release dates, likewise
         auto resolve = [&](const uint32_t* w) {  // w: the kBatch / 4 words that hold the batch's job ids
           int js[kBatch];
@@ -362,7 +365,7 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
 #pragma unroll
             for (int i = 0; i < kBatch; ++i) {
               const float x = R ? xc[i] : 0.f;
-              if constexpr (D) st.step_resolved(static_cast<int>(oc[i]), rc[i], i & 1, wc[i], dc[i], x);
+              if constexpr (D) st.step_resolved(static_cast<int>(oc[i]), rc[i], i & 1, W ? wc[i] : 0.f, dc[i], x);
               else if constexpr (W) st.step_resolved(static_cast<int>(oc[i]), rc[i], i & 1, wc[i], 0.f, x);
               else st.step_resolved(static_cast<int>(oc[i]), rc[i], i & 1, 0.f, 0.f, x);
             }
@@ -678,7 +681,7 @@ struct GenericArgs {
 template <int PB, bool INT, bool MULTI, bool SUM = false, bool W = false, bool D = false, bool R = false>
 __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
   static_assert(SUM || !W, "weights scale the sum of completion times only");
-  static_assert(W || !D, "due dates run on the weighted form");
+  static_assert(W || !D || !SUM, "tardiness runs on the weighted form");
   extern __shared__ __align__(128) uint8_t smem[];
   const float* tab = a.tab;
   const uint32_t node_bytes = MULTI ? static_cast<uint32_t>(a.nodes) * 1024u : 0u;  // per warp
@@ -691,7 +694,7 @@ __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
     tab = tab_s;
   }
   const int lane = threadIdx.x & 31;
-  LaneState<INT, MULTI, 0, SUM, (W ? 2 : 0), D, (R ? 2 : 0)> st;
+  LaneState<INT, MULTI, 0, SUM, (W ? 2 : 0), (D ? 2 : 0), (R ? 2 : 0)> st;
   st.tab = tab;
   st.wt = a.w;
   st.dd = a.d;
@@ -771,14 +774,14 @@ struct FullArgs {
   float* start;         // [B][J] by job, nullable
   uint32_t* slotmask;   // [B][J] by job, nullable
   const float* w;       // W: job weights [J]
-  const float* d;       // D: job due dates [J]
+  const float* d;       // D: job due dates [J] (without SUM: the delivery tails)
   const float* r;       // R: job release dates [J] (ceiled with INT)
 };
 
 template <int PB, bool INT, bool SUM = false, bool W = false, bool D = false, bool R = false>
 __global__ void __launch_bounds__(128) k_eval_full(const FullArgs a) {
   static_assert(SUM || !W, "weights scale the sum of completion times only");
-  static_assert(W || !D, "due dates run on the weighted form");
+  static_assert(W || !D || !SUM, "tardiness runs on the weighted form");
   const long long nthreads = static_cast<long long>(gridDim.x) * blockDim.x;
   const bool multi = a.nodes > 1;
   for (long long b = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; b < a.B; b += nthreads) {
@@ -814,7 +817,9 @@ __global__ void __launch_bounds__(128) k_eval_full(const FullArgs a) {
       const float nxt = s + hold;
       for (int g = 0; g < kSlots; ++g)
         if ((taken >> g) & 1u) rd[g] = nxt;
-      if constexpr (D)  // ls_step<..., kSum, kWeighted, kDue>
+      if constexpr (D && !SUM)  // ls_step<..., kDue>: the tail makespan
+        mk = fmaxf(mk, __fadd_rn(s + rt, __ldg(a.d + j)));
+      else if constexpr (D)  // ls_step<..., kSum, kWeighted, kDue>
         mk = __fadd_rn(mk, __fmul_rn(__ldg(a.w + j), fmaxf(__fsub_rn(s + rt, __ldg(a.d + j)), 0.f)));
       else if constexpr (W) mk = __fadd_rn(mk, __fmul_rn(__ldg(a.w + j), s + rt));  // ls_step<..., kSum, kWeighted>
       else if (SUM) mk = mk + (s + rt);  // the left fold in schedule order of ls_step<..., kSum>

@@ -32,7 +32,7 @@ static_assert(((HOOK_FORCE_GENERIC | HOOK_NO_STREAM | HOOK_NO_FUSED | HOOK_NO_IN
                 HOOK_REORDER | HOOK_NO_REORDER) &
                (SB_FLAG_INTEGER_STARTS | SB_FLAG_REDUCED | SB_FLAG_OPT_BY_POSITION | SB_FLAG_POST_KEY |
                 SB_FLAG_FOLD_PREV | SB_FLAG_ALT_WARPSCAN | SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED |
-                SB_FLAG_DUE | SB_FLAG_RELEASE)) == 0,
+                SB_FLAG_DUE | SB_FLAG_RELEASE | SB_FLAG_MAX_LATENESS)) == 0,
               "the test hooks share no bit with the SB_FLAG_* flags");
 
 // Debug options of the streamed tile kernel (sb_debug_tile_options): kept on the handle, not in the flags word, and
@@ -54,10 +54,11 @@ decltype(auto) with_pb(int pb, F&& f) {
   return pb == 1 ? f(std::integral_constant<int, 1>{}) : f(std::integral_constant<int, 2>{});
 }
 // f(PB, INT, SUM, W, D, R): the prio width, SB_FLAG_INTEGER_STARTS, SB_FLAG_SUM_COMPLETION, SB_FLAG_WEIGHTED,
-// SB_FLAG_DUE and SB_FLAG_RELEASE, the template arguments that every evaluation and search kernel takes.  W is true
-// only together with SUM, and D only together with W: no kernel that weights the makespan, or that scores tardiness
-// without weights, is ever instantiated (SB_FLAG_DUE alone runs the weighted form on unit weights, exact since
-// 1 * x = x).  R is orthogonal to the other three: each objective form has a release twin.
+// SB_FLAG_DUE or SB_FLAG_MAX_LATENESS, and SB_FLAG_RELEASE, the template arguments that every evaluation and search
+// kernel takes.  W is true only together with SUM.  With SUM, D is true only together with W: no kernel that weights
+// the makespan, or that scores tardiness without weights, is ever instantiated (SB_FLAG_DUE alone runs the weighted
+// form on unit weights, exact since 1 * x = x).  Without SUM, D (SB_FLAG_MAX_LATENESS) is the tail makespan of
+// ls_step.  R is orthogonal to the other three: each objective form has a release twin.
 template <class F>
 decltype(auto) with_eval_types(int pb, unsigned flags, F&& f) {
   return with_pb(pb, [&](auto PB) {
@@ -70,7 +71,8 @@ decltype(auto) with_eval_types(int pb, unsigned flags, F&& f) {
               else return f(PB, INT, SUM, W, std::false_type{}, R);
             });
           } else {
-            return f(PB, INT, SUM, std::false_type{}, std::false_type{}, R);
+            return with_bool(flags & SB_FLAG_MAX_LATENESS,
+                             [&](auto D) { return f(PB, INT, SUM, std::false_type{}, D, R); });
           }
         });
       });
@@ -78,10 +80,11 @@ decltype(auto) with_eval_types(int pb, unsigned flags, F&& f) {
   });
 }
 // the per-job fp32 arrays a kernel stages beside the table: the weights (SB_FLAG_WEIGHTED, or the unit weights of
-// SB_FLAG_DUE alone), then the due dates (SB_FLAG_DUE), then the release dates (SB_FLAG_RELEASE); each is padded to
-// 16 bytes
+// SB_FLAG_DUE alone), then the due dates (SB_FLAG_DUE) or the delivery tails (SB_FLAG_MAX_LATENESS), then the release
+// dates (SB_FLAG_RELEASE); each is padded to 16 bytes
 inline int job_arrays(unsigned flags) {
-  return ((flags & SB_FLAG_DUE) ? 2 : ((flags & SB_FLAG_WEIGHTED) ? 1 : 0)) + ((flags & SB_FLAG_RELEASE) ? 1 : 0);
+  return ((flags & SB_FLAG_DUE) ? 2 : ((flags & SB_FLAG_WEIGHTED) ? 1 : 0)) + ((flags & SB_FLAG_MAX_LATENESS) ? 1 : 0) +
+         ((flags & SB_FLAG_RELEASE) ? 1 : 0);
 }
 inline size_t job_array_bytes(int J) { return (static_cast<size_t>(J) * 4 + 15) & ~size_t(15); }
 
@@ -133,7 +136,8 @@ struct EvalCall {
   const float* tab = nullptr;  // canonical table actually used (full or reduced)
   const float* w = nullptr;    // SB_FLAG_WEIGHTED: the job weights [J], padded with zeros to a multiple of 4
                                // (SB_FLAG_DUE alone: J ones, padded the same way)
-  const float* d = nullptr;    // SB_FLAG_DUE: the job due dates [J], padded the same way
+  const float* d = nullptr;    // SB_FLAG_DUE: the job due dates [J], padded the same way (SB_FLAG_MAX_LATENESS: the
+                               // delivery tails max_t d_t - d_j, padded the same way)
   const float* r = nullptr;    // SB_FLAG_RELEASE: the job release dates [J] (ceiled under SB_FLAG_INTEGER_STARTS),
                                // padded the same way
   int J = 0, SG = 0;

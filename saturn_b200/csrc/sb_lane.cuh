@@ -39,11 +39,12 @@ __device__ __forceinline__ PrioChunk ld_prio32(const uint8_t* p) {
 // SUM: score = sum of completion times (SB_FLAG_SUM_COMPLETION) instead of the makespan; mk holds the running sum.
 // WGT (SB_FLAG_WEIGHTED, with SUM only): each completion is scaled by its job's weight, read from `wt` — 1: the
 // weights are in shared memory beside the table, 2: in global memory, read with ld.global.nc.
-// DUE (SB_FLAG_DUE, with WGT only): each job's tardiness against its due date, read from `dd` (in the same memory
-// as the weights) takes its completion's place.
+// DUE (SB_FLAG_DUE, with WGT only): each job's tardiness against its due date, read from `dd`, takes its
+// completion's place; without SUM (SB_FLAG_MAX_LATENESS) `dd` holds the delivery tails and the score is the tail
+// makespan (see ls_step) — 1: in shared memory beside the table, 2: in global memory, read with ld.global.nc.
 // REL (SB_FLAG_RELEASE, with any objective): no job starts before its release date, read from `rr` — 1: in shared
 // memory beside the table, 2: in global memory, read with ld.global.nc.
-template <bool INT, bool MULTI, int ADDR = 0, bool SUM = false, int WGT = 0, bool DUE = false, int REL = 0>
+template <bool INT, bool MULTI, int ADDR = 0, bool SUM = false, int WGT = 0, int DUE = 0, int REL = 0>
 struct LaneState {
   float f[8];
   float mk;
@@ -51,7 +52,7 @@ struct LaneState {
   const uint8_t* orow;  // this candidate's opt bytes (shared memory or global)
   const float* tab;     // runtime table (shared memory or global)
   const float* wt;      // WGT: the job weights [J]
-  const float* dd;      // DUE: the job due dates [J]
+  const float* dd;      // DUE: the job due dates [J] (or delivery tails)
   const float* rr;      // REL: the job release dates [J]
   int SG;
   int one;
@@ -99,11 +100,11 @@ struct LaneState {
     else if constexpr (WGT == 2) return __ldg(wt + j);
     else return 0.f;
   }
-  // the job's due date (DUE only; 0 otherwise, and then unused)
+  // the job's due date or tail (DUE only; 0 otherwise, and then unused)
   __device__ __forceinline__ float lookup_d(int j) const {
-    if constexpr (!DUE) return 0.f;
-    else if constexpr (WGT == 1) return dd[j];
-    else return __ldg(dd + j);
+    if constexpr (DUE == 1) return dd[j];
+    else if constexpr (DUE == 2) return __ldg(dd + j);
+    else return 0.f;
   }
   // the job's release date (REL only; 0 otherwise, and then unused)
   __device__ __forceinline__ float lookup_r(int j) const {
@@ -116,10 +117,10 @@ struct LaneState {
   __device__ __forceinline__ void step_resolved(int o, float rt, int ph = -1, float w = 0.f, float d = 0.f,
                                                 float r = 0.f) {
     if (!MULTI) {
-      ls_step<INT, INT, SUM, (WGT != 0), DUE, (REL != 0)>(f, mk, pend, rt, o & 7, one, ph, w, d, r);
+      ls_step<INT, INT, SUM, (WGT != 0), (DUE != 0), (REL != 0)>(f, mk, pend, rt, o & 7, one, ph, w, d, r);
     } else {
       switch_node(o >> 3);
-      ls_step<INT, true, SUM, (WGT != 0), DUE, (REL != 0)>(f, mk, pend, rt, o & 7, one, ph, w, d, r);
+      ls_step<INT, true, SUM, (WGT != 0), (DUE != 0), (REL != 0)>(f, mk, pend, rt, o & 7, one, ph, w, d, r);
     }
   }
   // ADDR = 1: the two look-ups as separate gathers, so that the streamed loop of k_eval_tiles can issue a whole
@@ -152,7 +153,7 @@ struct LaneState {
   }
   // ADDR = 1 with DUE: the due-date gather, like gather_w
   __device__ __forceinline__ float gather_d(int j) const {
-    if constexpr (!DUE) {
+    if constexpr (DUE == 0) {
       return 0.f;
     } else {
       uint32_t da;
@@ -177,24 +178,28 @@ struct LaneState {
   __device__ __forceinline__ void step(int j, int ph = -1) {
     constexpr bool W = WGT != 0;
     constexpr bool R = REL != 0;
+    constexpr bool D = DUE != 0;
     if (!MULTI && ADDR == 1) {
       const uint32_t o = gather_opt(j);
-      ls_step<INT, INT, SUM, W, DUE, R>(f, mk, pend, gather_rt(j, o), static_cast<int>(o & 7u), one, ph, gather_w(j),
+      ls_step<INT, INT, SUM, W, D, R>(f, mk, pend, gather_rt(j, o), static_cast<int>(o & 7u), one, ph, gather_w(j),
                                         gather_d(j), gather_r(j));
       return;
     }
     const int o = orow[j];
     if (!MULTI) {
       const float rt = tab[j * SG + o];
-      ls_step<INT, INT, SUM, W, DUE, R>(f, mk, pend, rt, o & 7, one, ph, lookup_w(j), lookup_d(j), lookup_r(j));
+      ls_step<INT, INT, SUM, W, D, R>(f, mk, pend, rt, o & 7, one, ph, lookup_w(j), lookup_d(j), lookup_r(j));
     } else {
       const int col = o & 7;  // reduced table only: opt = (node << 3) | (k - 1)
       const float rt = tab[j * 8 + col];
       switch_node(o >> 3);
-      ls_step<INT, true, SUM, W, DUE, R>(f, mk, pend, rt, col, one, ph, lookup_w(j), lookup_d(j), lookup_r(j));
+      ls_step<INT, true, SUM, W, D, R>(f, mk, pend, rt, col, one, ph, lookup_w(j), lookup_d(j), lookup_r(j));
     }
   }
-  __device__ __forceinline__ float result() const { return SUM ? mk : ((INT || MULTI) ? fmaxf(mk, pend) : f[7]); }
+  // the tail makespan (DUE without SUM) is tracked in mk at every shape: f[7] is a completion, not a tail sum
+  __device__ __forceinline__ float result() const {
+    return SUM ? mk : ((INT || MULTI || DUE != 0) ? fmaxf(mk, pend) : f[7]);
+  }
   // the running score a snapshot of the incremental rounds stores (SearchFuse::snap): with SUM nothing is parked,
   // so a snapshot is exact at any step, not only after an even number of steps
   __device__ __forceinline__ float running() const { return SUM ? mk : fmaxf(mk, pend); }

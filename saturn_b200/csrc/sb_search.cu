@@ -426,6 +426,7 @@ __device__ __forceinline__ PosMove make_pos_move_win(const SearchFuse& sf, int r
 // W: weight each completion by its job's weight (SB_FLAG_WEIGHTED, with SUM only); the weights follow the table in
 // shared memory with TAB = 0 and are read from global memory (ld.global.nc) with TAB = 1 / 2.
 // D: score tardiness against the jobs' due dates (SB_FLAG_DUE, with W only); the due dates follow the weights.
+// Without SUM, D is the tail makespan (SB_FLAG_MAX_LATENESS, see ls_step): the delivery tails take the due dates' place.
 // R: no job starts before its release date (SB_FLAG_RELEASE, any objective); the release dates follow the other
 // per-job arrays in shared memory with TAB = 0 and are read from global memory with TAB = 1 / 2.
 template <int PB, bool INT, bool MULTI, bool EVAL = false, int TAB = 0, bool SUM = false, bool W = false,
@@ -433,7 +434,7 @@ template <int PB, bool INT, bool MULTI, bool EVAL = false, int TAB = 0, bool SUM
 __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
   static_assert(TAB == 0 || (EVAL && !MULTI), "tables outside the CTA's shared memory: scoring only, one node");
   static_assert(SUM || !W, "weights scale the sum of completion times only");
-  static_assert(W || !D, "due dates run on the weighted form");
+  static_assert(W || !D || !SUM, "tardiness runs on the weighted form");
   extern __shared__ __align__(128) uint8_t smem[];
   const int nw = blockDim.x >> 5;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -445,7 +446,7 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
   const uint32_t tab_bytes = TAB == 1 ? 0u : (TAB == 2 ? (rank == 0 ? half * 4u : tab_all - half * 4u) : tab_all);
   const uint32_t tab_room = TAB == 1 ? 0u : (TAB == 2 ? half * 4u : tab_all);
   const uint32_t w_bytes = (W && TAB == 0) ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u;
-  const uint32_t d_bytes = D ? w_bytes : 0u;
+  const uint32_t d_bytes = D ? (W ? w_bytes : (TAB == 0 ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u)) : 0u;
   const uint32_t r_bytes = (R && TAB == 0) ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u;
   float* tab_s = reinterpret_cast<float*>(smem);
   [[maybe_unused]] float* w_s = reinterpret_cast<float*>(smem + ((tab_room + 15u) & ~15u));
@@ -481,7 +482,7 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
       }
     }
   }
-  LaneState<INT, MULTI, 0, SUM, (W ? (TAB == 0 ? 1 : 2) : 0), D, (R ? (TAB == 0 ? 1 : 2) : 0)> st;
+  LaneState<INT, MULTI, 0, SUM, (W ? (TAB == 0 ? 1 : 2) : 0), (D ? (TAB == 0 ? 1 : 2) : 0), (R ? (TAB == 0 ? 1 : 2) : 0)> st;
   st.tab = tab_s;
   if constexpr (W) st.wt = TAB == 0 ? w_s : a.w;
   if constexpr (D) st.dd = TAB == 0 ? d_s : a.d;

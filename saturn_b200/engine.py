@@ -18,19 +18,22 @@ from ._lib import FLAG_INTEGER_STARTS, FLAG_REDUCED, SaturnB200Error, SearchPara
 NSLOT = 8
 
 
-OBJECTIVES = ("makespan", "completion", "weighted_completion", "tardiness", "weighted_tardiness")
+OBJECTIVES = ("makespan", "completion", "weighted_completion", "tardiness", "weighted_tardiness", "max_lateness")
 
 
 def objective_flag(objective: str) -> int:
     """SB_FLAG_SUM_COMPLETION for objective="completion" (score = sum of completion times), SB_FLAG_SUM_COMPLETION |
     SB_FLAG_WEIGHTED for "weighted_completion" (the sum weighted by the engine's set_weights), SB_FLAG_SUM_COMPLETION |
     SB_FLAG_DUE for "tardiness" (total tardiness against the engine's set_due) and SB_FLAG_SUM_COMPLETION |
-    SB_FLAG_DUE | SB_FLAG_WEIGHTED for "weighted_tardiness", 0 for "makespan"."""
+    SB_FLAG_DUE | SB_FLAG_WEIGHTED for "weighted_tardiness", SB_FLAG_MAX_LATENESS for "max_lateness" (the maximum
+    lateness against the engine's set_due, scored as L_max + Engine.due_shift) and 0 for "makespan"."""
     if objective not in OBJECTIVES:
         from .solver import SolverError
         raise SolverError("objective must be one of %s, not %r" % (", ".join(map(repr, OBJECTIVES)), objective))
     if objective == "makespan":
         return 0
+    if objective == "max_lateness":
+        return _lib.FLAG_MAX_LATENESS
     return _lib.FLAG_SUM_COMPLETION | (_lib.FLAG_WEIGHTED if objective.startswith("weighted_") else 0) | (
         _lib.FLAG_DUE if objective.endswith("tardiness") else 0)
 
@@ -95,9 +98,9 @@ def _flags(integer_starts: bool, reduced: bool, objective: str = "makespan") -> 
 
 
 def _require_due(due, objective: str):
-    """The tardiness objectives score against the due dates of set_due: refuse them, before any device call, on an
-    engine that has none (set_table clears them)."""
-    if objective.endswith("tardiness") and due is None:
+    """The tardiness objectives and the maximum lateness score against the due dates of set_due: refuse them, before
+    any device call, on an engine that has none (set_table clears them)."""
+    if (objective.endswith("tardiness") or objective == "max_lateness") and due is None:
         from .solver import SolverError
         raise SolverError("objective=%r needs due dates: call set_due after set_table" % (objective,))
 
@@ -126,7 +129,8 @@ class Engine:
         self.gcount = None
         self.nodes = 1
         self.weights = None  # fp32 job weights of objective="weighted_completion" (set_weights)
-        self.due = None  # fp32 job due dates of objective="tardiness" / "weighted_tardiness" (set_due)
+        self.due = None  # fp32 job due dates of objective="tardiness" / "weighted_tardiness" / "max_lateness" (set_due)
+        self.due_shift = None  # max of self.due: objective="max_lateness" scores L_max + due_shift (>= 0)
         self.release = None  # fp32 job release dates, under every objective (set_release)
 
     # ------------------------------------------------------------------ lifecycle
@@ -173,6 +177,7 @@ class Engine:
         self.nodes = int(nodes)
         self.weights = None  # sb_set_table clears them
         self.due = None
+        self.due_shift = None
         self.release = None
         return self
 
@@ -191,14 +196,18 @@ class Engine:
     def set_due(self, d) -> "Engine":
         """Per-job due dates (J values, finite with |d| < 2^24, converted to fp32) for objective="tardiness", which
         scores sum_j max(0, start_j + rt_j - d_j), and "weighted_tardiness" (each term times the set_weights
-        weight).  None clears them; set_table clears them too."""
+        weight), and "max_lateness", which scores max_j (start_j + rt_j + q_j) with the tails q_j = D - d_j (fp32),
+        D = due_shift = max_j d_j: that is L_max + D >= 0, and subtracting D gives L_max.  None clears them; set_table
+        clears them too."""
         if d is None:
             check(self._lib.sb_set_due(self._h, None, 0))
             self.due = None
+            self.due_shift = None
             return self
         d32 = np.ascontiguousarray(due_f32(d, self.J))
         check(self._lib.sb_set_due(self._h, C.c_void_p(d32.ctypes.data), int(self.J)))
         self.due = d32
+        self.due_shift = float(d32.max())
         return self
 
     def set_release(self, r) -> "Engine":
@@ -608,6 +617,7 @@ class MultiEngine:
         return self
 
     due = property(lambda self: self.engines[0].due)
+    due_shift = property(lambda self: self.engines[0].due_shift)
 
     def set_release(self, r):
         """Engine.set_release on every device."""

@@ -56,7 +56,8 @@ def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objecti
     `weights`: WSPT order (Smith's rule), ascending runtime / weight in float64, ties by job index — for unit
     weights exactly the shortest-processing-time order.  objective="tardiness" / "weighted_tardiness" with the fp32
     `due` dates: EDD order (earliest due date first), ties by runtime (by runtime / weight when weighted), then by
-    job index.  With the fp32 `release` dates (any objective) each order is then re-sorted stably by ascending
+    job index; objective="max_lateness" the unit-weight EDD order of "tardiness" (Jackson's rule, optimal for the
+    maximum lateness on one machine).  With the fp32 `release` dates (any objective) each order is then re-sorted stably by ascending
     release date (ceiled when `integer_starts`, as the device schedules them), so jobs released together keep the
     objective's order."""
     objective_flag(objective)
@@ -64,7 +65,8 @@ def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objecti
         if weights is None:
             raise ValueError("objective=%r needs the job weights" % objective)
         w64 = np.asarray(weights, dtype=np.float32).astype(np.float64)
-    if objective.endswith("tardiness"):
+    edd = objective.endswith("tardiness") or objective == "max_lateness"
+    if edd:
         if due is None:
             raise ValueError("objective=%r needs the job due dates" % objective)
         d32 = np.asarray(due, dtype=np.float32)
@@ -85,7 +87,7 @@ def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objecti
         cost = usable.astype(np.float64) * (k ** area_weight)
         col = np.argmin(cost, axis=1)
         rt = usable[np.arange(J), col]
-        if objective.endswith("tardiness"):
+        if edd:
             tie = rt.astype(np.float64) / w64 if objective == "weighted_tardiness" else rt.astype(np.float64)
             order = np.lexsort((np.arange(J), tie, d32))
         elif objective == "weighted_completion":
@@ -121,6 +123,8 @@ def run_search(engine: Engine, chains: int = 1 << 16, rounds: int = 200, seed: i
     `target_makespan` then hold / target that sum.  objective="weighted_completion" minimises the sum weighted by
     the engine's set_weights.  objective="tardiness" / "weighted_tardiness" minimises the total (weighted) tardiness
     against the engine's set_due, and stops as soon as the incumbent's tardiness is 0, which no plan can beat.
+    objective="max_lateness" minimises the maximum lateness against the engine's set_due; every score holds
+    L_max + engine.due_shift, and there is no stop at zero (L_max has no floor).
 
     `rounds` device rounds are issued in groups of `exchange_every` (tournament resampling every
     `resample_every` rounds inside a group is only another launch); after each group the ranks exchange

@@ -193,11 +193,13 @@ def _engine(devices=None):
     return _MULTI[devices]
 
 
-def _check_horizon(T, found_makespan=None, release=None):
+def _check_horizon(T, found_makespan=None, release=None, tails=None):
     """The kernels keep schedule times in fp32: `start + ceil(rt)` is exact only below 2^24 s (194 days).
     Before the search: a table whose lower bound of the makespan — the area bound sum_j min_k k * rt_jk / 8, and
     with `release` (per-task release dates) also max_j (r_j + min_k rt_jk) — already reaches that bound cannot
-    have an exactly representable plan and is refused.  After the search (`found_makespan`, the
+    have an exactly representable plan and is refused.  With `tails` (objective="max_lateness": the delivery tails
+    q_t = max d - d_t) the device's score is the tail makespan max_t (C_t + q_t), bounded below by
+    max_t (min_k rt_tk + q_t), plus r_t with `release`.  After the search (`found_makespan`, the
     device's value): every time inside the winning schedule is <= its makespan, and fp32 addition rounds
     monotonically, so a makespan below 2^24 proves that all of its starts were computed exactly; anything
     else is refused instead of returned with silently rounded starts (rescale to coarser time units)."""
@@ -212,14 +214,19 @@ def _check_horizon(T, found_makespan=None, release=None):
     if release is not None:
         shortest = np.where(np.isfinite(T), T.astype(np.float64), np.inf).reshape(T.shape[0], -1).min(axis=1)
         lower = max(lower, float(np.max(np.asarray(release, dtype=np.float64) + shortest)))
+    if tails is not None:
+        shortest = np.where(np.isfinite(T), T.astype(np.float64), np.inf).reshape(T.shape[0], -1).min(axis=1)
+        rel = np.asarray(release, dtype=np.float64) if release is not None else 0.0
+        lower = max(lower, float(np.max(rel + shortest + np.asarray(tails, dtype=np.float64))))
     if lower >= FP32_EXACT_HORIZON:
         raise SolverError("area lower bound of the makespan is %.3g s >= 2^24 s: schedule times are not exact in "
                           "fp32 at that horizon; express runtimes in coarser units (e.g. minutes) or drop sentinel "
                           "options" % lower)
 
 def _check_objective(objective, hysteresis=False, release=None):
-    if objective not in ("makespan", "completion", "tardiness"):
-        raise SolverError("objective must be 'makespan', 'completion' or 'tardiness', not %r" % (objective,))
+    if objective not in ("makespan", "completion", "tardiness", "max_lateness"):
+        raise SolverError("objective must be 'makespan', 'completion', 'tardiness' or 'max_lateness', not %r"
+                          % (objective,))
     if objective != "makespan" and hysteresis:
         raise SolverError("hysteresis=True compares plans by makespan (milp.py:363-442); it is not defined for "
                           "objective=%r" % (objective,))
@@ -259,16 +266,20 @@ def _resolve_weights(weights, objective, J, task_list=None):
 
 def _resolve_due(due, objective, J, task_list=None):
     """The caller's per-task due dates as (float64 values in task order, fp32 array for the device), or (None, None)
-    without objective="tardiness", which requires them.  Raises SolverError before any device call."""
-    if objective != "tardiness":
+    without objective="tardiness" or "max_lateness", which require them.  Raises SolverError before any device
+    call."""
+    if objective not in ("tardiness", "max_lateness"):
         if due is not None:
-            raise SolverError("due dates apply to objective='tardiness' only, not to %r" % (objective,))
+            raise SolverError("due dates apply to objective='tardiness' or 'max_lateness' only, not to %r" % (objective,))
         return None, None
     if due is None:
-        raise SolverError("objective='tardiness' needs due dates (due=...)")
+        raise SolverError("objective=%r needs due dates (due=...)" % (objective,))
     due = _per_task(due, "due", task_list)
     from .engine import due_f32
     d32 = due_f32(due, J)
+    if objective == "max_lateness" and J > 0 and not float(d32.max()) - float(d32.min()) < FP32_EXACT_HORIZON:
+        # the device scores the tails max d - d_t in fp32: beyond 2^24 they round even for integer due dates
+        raise SolverError("objective='max_lateness' needs max(due) - min(due) < 2^24")
     return [float(x) for x in due], d32
 
 
@@ -291,6 +302,8 @@ def _set_objective(eng, objective, w32, d32, r32=None):
         eng.set_weights(w32)
     if d32 is not None:
         eng.set_due(d32)
+        if objective == "max_lateness":
+            return objective
         return "weighted_tardiness" if w32 is not None else "tardiness"
     return "weighted_completion" if w32 is not None else objective
 
@@ -301,6 +314,17 @@ def _tardiness_stats(start, rts, w64, d64):
     w = w64 if w64 is not None else [1.0] * len(late)
     return {"weighted_tardiness": sum(wi * max(0.0, x) for wi, x in zip(w, late)),
             "late_tasks": sum(1 for x in late if x > 0)}
+
+
+def _lateness_stats(start, rts, d64):
+    """max_lateness, max_t (C_t - d_t), and late_tasks of a plan, in float64."""
+    late = [float(s) + float(r) - d for s, r, d in zip(start, rts, d64)]
+    return {"max_lateness": max(late), "late_tasks": sum(1 for x in late if x > 0)}
+
+
+def _tails(d32):
+    """The delivery tails max d - d_t of objective="max_lateness", as the device forms them (fp32)."""
+    return d32.max() - d32 if d32 is not None else None
 
 
 def _flow_stats(start, rts, r64):
@@ -361,6 +385,17 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     C_t > d_t) are computed in float64 from the emitted plan, the tasks' own runtimes and the caller's d and w;
     last_stats["device_makespan"] holds the device's fp32 tardiness.
 
+    Maximum lateness.  objective="max_lateness" with `due` (as above) minimises L_max = max_t (C_t - d_t), which can be
+    negative: it maximises the smallest margin any task keeps against its due date, where "tardiness" stops at the
+    first plan that is not late.  L_max <= 0 means every due date is met; L_max > 0 is the smallest uniform delay of
+    the due dates that makes them all feasible.  With `release` and due = release (+ a target), it is the longest
+    any task waits from its release to its result.  `weights`, hysteresis=True and due dates spread over 2^24 or more
+    raise SolverError before any device call, as do the `due` errors above.  The device scores L_max + max_t d_t
+    (>= 0); last_stats["max_lateness"] and last_stats["late_tasks"] are recomputed in float64 from the emitted plan,
+    the tasks' own runtimes and the caller's due dates, and last_stats["device_makespan"] holds the device's fp32
+    score minus max_t d_t.  Shifting every due date by one constant gives the same plan.  The 6th element stays the
+    plan's makespan.
+
     Release dates.  `release` (a sequence aligned with task_list, or a mapping keyed by Task, in the runtimes' units
     from the plan's t = 0) keeps every task from starting before its release date, under every objective: a
     dataset or a parent checkpoint that is only ready later, a job that arrives tomorrow.  r <= 0 means already
@@ -412,7 +447,7 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     for j in range(J):
         if usable[j].any():
             Tdev[j, 0, ~usable[j]] = np.inf
-    _check_horizon(Tdev, release=r64)
+    _check_horizon(Tdev, release=r64, tails=_tails(d32) if objective == "max_lateness" else None)
     if nodes is None:
         nodes = _default_nodes()
     nodes = int(nodes)
@@ -435,7 +470,7 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     res = run_search(eng, chains=chains, rounds=rounds, seed=seed, integer_starts=integer_starts, reduced=True,
                      time_budget_s=budget, patience=max(40, rounds // 4), warm=warm,
                      **({"objective": search_objective} if search_objective != "makespan" else {}))
-    if objective == "makespan":
+    if objective in ("makespan", "max_lateness"):
         _check_horizon(Tdev, res.makespan)
     dec = eng.decode(res.opt, res.prio, integer_starts=integer_starts, reduced=True)
     gpus = dec["gpus"].astype(np.int64)
@@ -462,7 +497,10 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
                   "total_completion": sum(float(dec["start"][i]) + float(rts[i]) for i in range(J))}
     if w64 is not None:
         last_stats["weighted_completion"] = sum(w64[i] * (float(dec["start"][i]) + float(rts[i])) for i in range(J))
-    if d64 is not None:
+    if objective == "max_lateness":
+        last_stats.update(_lateness_stats(dec["start"], rts, d64))
+        last_stats["device_makespan"] = res.makespan - eng.due_shift
+    elif d64 is not None:
         last_stats.update(_tardiness_stats(dec["start"], rts, w64, d64))
     if r64 is not None:
         last_stats.update(_flow_stats(dec["start"], rts, r64))
@@ -565,7 +603,7 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     """solve() on the dense profiler tensor T[J][S][G] (+ mask of usable cells, + gcount[G] GPU counts).
     `objective` as for solve(): "makespan" or "completion" (sum of completion times); `weights` as for solve(),
     a sequence aligned with T's rows (the weighted sum of completion times, last_stats["weighted_completion"]);
-    `due` as for solve() with objective="tardiness", a sequence aligned with T's rows; `release` as for solve(),
+    `due` as for solve() with objective="tardiness" or "max_lateness", a sequence aligned with T's rows; `release` as for solve(),
     under every objective, a sequence aligned with T's rows (last_stats["total_flow_time"]).  Every cell of T must be
     >= 0 (-0.0 counts as zero), +inf or a sentinel: a negative or NaN cell raises SolverError, with or without `mask`.
 
@@ -601,7 +639,7 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
         Tdev[j] = np.where(np.isfinite(T[j]), T[j], np.inf)      # nothing usable: the sentinels are all it has
     if not np.isfinite(Tdev.reshape(J, -1)).any(axis=1).all():
         raise SolverError("a task has no finite cell in T")
-    _check_horizon(Tdev, release=r64)
+    _check_horizon(Tdev, release=r64, tails=_tails(d32) if objective == "max_lateness" else None)
     eng = engine if engine is not None else _engine(devices)
     nodes = int(_default_nodes() if nodes is None else nodes)
     eng.set_table(Tdev, gcount, sentinel=float("inf"), nodes=nodes)
@@ -623,7 +661,7 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     res = run_search(eng, chains=chains, rounds=rounds, seed=seed, integer_starts=integer_starts, reduced=True,
                      time_budget_s=budget, patience=max(40, rounds // 4), warm=warm,
                      **({"objective": search_objective} if search_objective != "makespan" else {}))
-    if objective == "makespan":
+    if objective in ("makespan", "max_lateness"):
         _check_horizon(Tdev, res.makespan)
     dec = eng.decode(res.opt, res.prio, integer_starts=integer_starts, reduced=True)
     gpus = dec["gpus"].astype(np.int64)
@@ -643,7 +681,10 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
                   "objective": objective, "total_completion": sum(float(dec["start"][j]) + rts[j] for j in range(J))}
     if w64 is not None:
         last_stats["weighted_completion"] = sum(w64[j] * (float(dec["start"][j]) + rts[j]) for j in range(J))
-    if d64 is not None:
+    if objective == "max_lateness":
+        last_stats.update(_lateness_stats(dec["start"], rts, d64))
+        last_stats["device_makespan"] = res.makespan - eng.due_shift
+    elif d64 is not None:
         last_stats.update(_tardiness_stats(dec["start"], rts, w64, d64))
     if r64 is not None:
         last_stats.update(_flow_stats(dec["start"], rts, r64))

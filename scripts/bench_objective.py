@@ -1,5 +1,5 @@
-"""Cost and effect of the sum-of-completion-times objectives (plain and weighted), of the weighted tardiness and of
-release dates on one GPU; prints one JSON line.
+"""Cost and effect of the sum-of-completion-times objectives (plain and weighted), of the weighted tardiness, of the
+maximum lateness and of release dates on one GPU; prints one JSON line.
 
     python scripts/bench_objective.py [--steps 200] [--warmup 20] [--solve-chains 0] [--solve-rounds 400]
 
@@ -7,13 +7,15 @@ kernel: sb_eval on bench.py's C4 batch (J = 256, S = 8, 946,176 candidates, the 
         starts), scored for the makespan, the sum of completion times, the weighted sum (seeded weights) and the
         weighted tardiness (the same weights, seeded due dates), and the release twins of the makespan and the
         weighted tardiness (seeded integer release dates in [0, 20000) s, SB_FLAG_RELEASE, a second handle on the
-        same device), the six launches alternated in one process (the order rotates every step) and timed with CUDA
+        same device), and the maximum lateness (the tail makespan over the same due dates), the seven launches
+        alternated in one process (the order rotates every step) and timed with CUDA
         events; median of --steps launches each.
 solve:  solve() wall time on a 256-task set (synthetic table, seed 3, 4 strategies) for the makespan, the sum of
         completion times and the weighted sum (seeded weights: 32 tasks of weight 8, the rest 1), each plan scored
         on all three measures (float64, the tasks' own runtimes); and the total tardiness (unit weights, seeded
         integer due dates in [0, 200000) s): its tardiness and late tasks against those of the makespan and
-        completion plans.
+        completion plans; and the maximum lateness (the same due dates): its L_max and late tasks against those of
+        the tardiness and makespan plans.
 release: the same 256-task set with seeded release dates in [0, 0.5 x the makespan plan's makespan): per objective
         (makespan, completion, tardiness) the release-aware plan (solve(release=...)) against the release-blind plan
         (solve() without them, its options and list order rescored under the release rule), on makespan, total flow
@@ -73,7 +75,7 @@ def main():
     out = torch.empty(B, dtype=torch.float32, device=eng.device)
     key = torch.full((1,), 2 ** 63 - 1, dtype=torch.int64, device=eng.device)
     objs = ("makespan", "completion", "weighted_completion", "weighted_tardiness", "release_makespan",
-            "release_weighted_tardiness")
+            "release_weighted_tardiness", "max_lateness")
     times = {o: [] for o in objs}
     for i in range(args.warmup + args.steps):
         for obj in objs[i % len(objs):] + objs[:i % len(objs)]:
@@ -96,6 +98,7 @@ def main():
     kernel["release_over_makespan"] = kernel["release_makespan"]["median_ms"] / kernel["makespan"]["median_ms"]
     kernel["release_over_tardiness"] = (kernel["release_weighted_tardiness"]["median_ms"] /
                                         kernel["weighted_tardiness"]["median_ms"])
+    kernel["max_lateness_over_makespan"] = kernel["max_lateness"]["median_ms"] / kernel["makespan"]["median_ms"]
     kernel.update(B=B, J=J, S=Sx, path=path, steps=args.steps)
     del opt, prio, out
     eng_r.close()
@@ -122,11 +125,14 @@ def main():
     S.solve(tasks, None, rounds=4, engine=eng, objective="completion", weights=w)
     due = [float(x) for x in np.random.default_rng(4).integers(0, 200000, size=len(tasks))]
     S.solve(tasks, None, rounds=4, engine=eng, objective="tardiness", due=due)
+    S.solve(tasks, None, rounds=4, engine=eng, objective="max_lateness", due=due)
     solve = {}
     for name, obj, weights in (("makespan", "makespan", None), ("completion", "completion", None),
-                               ("weighted_completion", "completion", w), ("tardiness", "tardiness", None)):
+                               ("weighted_completion", "completion", w), ("tardiness", "tardiness", None),
+                               ("max_lateness", "max_lateness", None)):
         t0 = time.perf_counter()
-        res = S.solve(tasks, None, objective=obj, weights=weights, **({"due": due} if obj == "tardiness" else {}), **kw)
+        res = S.solve(tasks, None, objective=obj, weights=weights,
+                      **({"due": due} if obj in ("tardiness", "max_lateness") else {}), **kw)
         wall = time.perf_counter() - t0
         st = S.last_stats
         # the plan scored on all three measures, in float64 from its starts and the tasks' own runtimes
@@ -138,6 +144,7 @@ def main():
                        "heavy_mean_completion": float(np.mean([c for wi, c in zip(w, comp) if wi > 1])),
                        "tardiness": sum(max(0.0, c - d) for c, d in zip(comp, due)),
                        "late_tasks": sum(1 for c, d in zip(comp, due) if c > d),
+                       "max_lateness": max(c - d for c, d in zip(comp, due)),
                        "rounds": st["rounds"], "candidates": st["candidates"]}
     print(json.dumps({"card": card(0), "kernel": kernel, "solve": solve,
                       "release": release_effect(S, R, tasks, due, solve["makespan"]["makespan"], kw)}))
