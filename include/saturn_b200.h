@@ -54,6 +54,14 @@
  *   l = e - d, t = max(l, +0), acc = acc + (w * t), every step rounded on its own (no fused or reassociated step).
  * d = 0 gives exactly the weighted fold, due dates at or past every completion give +0, w = 2 exactly twice w = 1.
  * The score is >= +0, so the (bits << 32) | id key still orders by it.
+ * With SB_FLAG_LATE_COUNT as well it is the (weighted) number of late jobs instead:
+ *   total = sum_j w_j [start_j + rt_j > d_j], from +0 in schedule order per job: e = start + rt (as above),
+ *   acc = acc + (e > d ? w : +0), one rounding per job.  A job that completes exactly at its due date is on time.
+ * Unit weights give the exact count; integer weights with sum_j w_j < 2^24 give an exact sum in any order.  Due dates
+ * at or past every completion give +0, due dates below every completion give sum_j w_j, w = 2 exactly twice w = 1.
+ * The comparison is made in fp32 on the fp32 due date, so a completion within rounding of a fractional due date is
+ * decided as the tardiness fold decides it.  A candidate that gives a job an option it does not have (rt = +inf)
+ * scores +inf, as under every other objective, though the fold alone would add only that job's weight.
  * The schedule, every start and every slot mask are the same under every objective.
  * With SB_FLAG_MAX_LATENESS (per-job due dates d_j, sb_set_due) the score is the maximum lateness
  * L_max = max_j (start_j + rt_j - d_j), emitted as the tail makespan L_max + D >= +0 with D = max_t d_t:
@@ -168,6 +176,20 @@ typedef enum sb_status {
                                      no stop at zero (stop_reason 3 only follows target_makespan, which then targets
                                      the tail makespan), and sb_search_seed_lpt plants the unit-weight EDD orders of
                                      SB_FLAG_DUE.  Not available with SB_FLAG_ALT_WARPSCAN (SB_ERR_UNSUPPORTED). */
+#define SB_FLAG_LATE_COUNT 2048u   /* with SB_FLAG_SUM_COMPLETION | SB_FLAG_DUE only (SB_FLAG_WEIGHTED optional; else
+                                     SB_ERR_ARG, as with SB_FLAG_MAX_LATENESS): the objective is the (weighted)
+                                     number of late jobs, sum_j w_j [C_j > d_j], instead of their tardiness (see the
+                                     evaluation rule above).  It reads the weights and due dates of SB_FLAG_DUE and
+                                     needs nothing else.  Accepted by sb_eval, sb_eval_host, sb_eval_full, sb_decode
+                                     and the search, sb_search_run_multi included; every score the library emits
+                                     then holds the count, and target_makespan targets it.  The search's temperature
+                                     unit becomes sum_j w_j (the count of all jobs with unit weights), it stops as
+                                     soon as the incumbent is +0 (stop_reason 3), and sb_search_seed_lpt plants the
+                                     EDD orders of SB_FLAG_DUE repaired by Moore-Hodgson's rule: while the list
+                                     schedule of the on-time sequence has a late job, the job with the largest
+                                     k * rt / w up to and including the first late one (the later on ties) moves to
+                                     the back, where the moved jobs keep their EDD order.  Not available with
+                                     SB_FLAG_ALT_WARPSCAN (SB_ERR_UNSUPPORTED). */
 #define SB_IPC_HANDLE_BYTES 64
 
 typedef struct sb_handle sb_handle;

@@ -463,8 +463,13 @@ int sb_set_release(sb_handle* h, const float* r, int J) {
 
 // SB_FLAG_WEIGHTED and SB_FLAG_DUE are valid with SB_FLAG_SUM_COMPLETION only, and after sb_set_weights /
 // sb_set_due respectively; SB_FLAG_MAX_LATENESS alone among the objective flags, after sb_set_due with a due-date spread
-// below 2^24; SB_FLAG_RELEASE under any objective, after sb_set_release
+// below 2^24; SB_FLAG_LATE_COUNT with SB_FLAG_SUM_COMPLETION | SB_FLAG_DUE only (it changes what the tardiness form
+// adds per job); SB_FLAG_RELEASE under any objective, after sb_set_release
 static int check_per_job(const sb_handle* h, unsigned flags) {
+  constexpr unsigned kTardiness = SB_FLAG_SUM_COMPLETION | SB_FLAG_DUE;
+  if ((flags & SB_FLAG_LATE_COUNT) && (flags & kTardiness) != kTardiness)
+    return fail(SB_ERR_ARG, "SB_FLAG_LATE_COUNT counts late jobs on the tardiness form: it needs SB_FLAG_SUM_COMPLETION "
+                "and SB_FLAG_DUE");
   if ((flags & SB_FLAG_MAX_LATENESS) && (flags & (SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED | SB_FLAG_DUE)))
     return fail(SB_ERR_ARG, "SB_FLAG_MAX_LATENESS is an objective of its own: it cannot be combined with "
                 "SB_FLAG_SUM_COMPLETION, SB_FLAG_WEIGHTED or SB_FLAG_DUE");
@@ -595,10 +600,11 @@ int sb_eval(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, int64
     }
   }
   if (flags & SB_FLAG_ALT_WARPSCAN) {
-    if (flags & (SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED | SB_FLAG_DUE | SB_FLAG_RELEASE | SB_FLAG_MAX_LATENESS))
+    if (flags & (SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED | SB_FLAG_DUE | SB_FLAG_RELEASE | SB_FLAG_MAX_LATENESS |
+                 SB_FLAG_LATE_COUNT))
       return fail(SB_ERR_UNSUPPORTED, "SB_FLAG_ALT_WARPSCAN scores the makespan without release dates only: it "
-                  "cannot be combined with SB_FLAG_SUM_COMPLETION, SB_FLAG_WEIGHTED, SB_FLAG_DUE, SB_FLAG_RELEASE or "
-                  "SB_FLAG_MAX_LATENESS");
+                  "cannot be combined with SB_FLAG_SUM_COMPLETION, SB_FLAG_WEIGHTED, SB_FLAG_DUE, SB_FLAG_RELEASE, "
+                  "SB_FLAG_MAX_LATENESS or SB_FLAG_LATE_COUNT");
     if (flags & (SB_FLAG_POST_KEY | SB_FLAG_FOLD_PREV))
       return fail(SB_ERR_UNSUPPORTED, "SB_FLAG_ALT_WARPSCAN cannot be combined with the fused key exchange");
     cudaError_t e = eval_alt_launch(h->dev, c, h->stream);
@@ -1063,6 +1069,9 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
     }
     s.scale = std::max(s.scale, static_cast<float>(move / (weighted ? h->w_sum : static_cast<double>(J))));
   }
+  // the late count moves in steps of one job's weight and is 0 at many incumbents: its unit is the count of every job,
+  // sum_j w_j (J with unit weights), so that an uphill move of one mean weight is accepted with e^(-1 / (J t))
+  if (p->flags & SB_FLAG_LATE_COUNT) s.scale = static_cast<float>(weighted ? h->w_sum : static_cast<double>(J));
   s.evaluated = d.chains;
   s.rounds_done = 0;
   s.launches = 0;
@@ -1272,6 +1281,55 @@ int sb_search_inject(sb_handle* h, const uint8_t* opt, const void* prio, int64_t
   return SB_OK;
 }
 
+// Moore-Hodgson's repair of a seed order for the late count.  The on-time sequence (at first `order`) is list-scheduled
+// on the host in float64 by the device's rule: job j takes the k = col[j] + 1 slots of node[j] that are free first,
+// starts when the k-th is free (and not before its release r[j]), holds them for rt[j] (ceil(rt[j]) with integer
+// starts) and completes at start + rt[j].  At the first job that completes after its due date d[j], the job with the
+// largest k * rt / w among it and the jobs before it (the later one on ties) leaves the sequence for a late list, and
+// the schedule is resumed from that job's position; until no job of the sequence is late.  The order becomes the
+// on-time sequence followed by the late list in `order`'s order.  One gang size, one node and unit weights make it
+// Moore-Hodgson's algorithm, which minimises the number of late jobs; otherwise it is a heuristic.  An order without a
+// late job is unchanged.  search.lpt_seeds restates it.
+static void moore_hodgson(std::vector<int>& order, const std::vector<int>& col, const std::vector<double>& rt,
+                          const std::vector<int>& node, int nodes, const std::vector<float>* w,
+                          const std::vector<float>& d, const std::vector<float>* r, bool integer_starts) {
+  const int J = static_cast<int>(order.size());
+  const size_t state = static_cast<size_t>(nodes) * kSlots;  // the slots' free times, ascending per node
+  std::vector<double> snap((static_cast<size_t>(J) + 1) * state, 0.0);  // snap[q]: before sequence position q
+  std::vector<int> seq(order), late_list;
+  std::vector<int> pos(J);
+  for (int q = 0; q < J; ++q) pos[order[q]] = q;
+  auto ratio = [&](int j) { return (col[j] + 1) * rt[j] / (w ? static_cast<double>((*w)[j]) : 1.0); };
+  size_t q = 0;
+  while (q < seq.size()) {
+    const int j = seq[q];
+    double* cur = snap.data() + (q + 1) * state;
+    std::copy(snap.data() + q * state, snap.data() + (q + 1) * state, cur);
+    double* f = cur + static_cast<size_t>(node[j]) * kSlots;
+    const int k = col[j] + 1;
+    double st = f[k - 1];
+    if (r) st = std::max(st, static_cast<double>((*r)[j]));
+    const double v = st + (integer_starts ? ceil(rt[j]) : rt[j]);
+    for (int g = 0; g < k; ++g) f[g] = v;
+    std::sort(f, f + kSlots);
+    if (st + rt[j] > static_cast<double>(d[j])) {
+      size_t out = 0;
+      double best = -HUGE_VAL;
+      for (size_t p = 0; p <= q; ++p)
+        if (ratio(seq[p]) >= best) { best = ratio(seq[p]); out = p; }
+      late_list.push_back(seq[out]);
+      seq.erase(seq.begin() + static_cast<long>(out));
+      q = out;
+      continue;
+    }
+    ++q;
+  }
+  if (late_list.empty()) return;
+  std::sort(late_list.begin(), late_list.end(), [&](int a, int b) { return pos[a] < pos[b]; });
+  seq.insert(seq.end(), late_list.begin(), late_list.end());
+  order = seq;
+}
+
 int sb_search_seed_lpt(sb_handle* h) {
   int rc = use_device(h);
   if (rc) return rc;
@@ -1287,6 +1345,8 @@ int sb_search_seed_lpt(sb_handle* h) {
   // lateness the same unit-weight EDD orders (Jackson's rule, optimal for L_max on one machine)
   const bool edd = (spt && (s.p.flags & SB_FLAG_DUE) != 0) || (s.p.flags & SB_FLAG_MAX_LATENESS) != 0;
   const bool rel = (s.p.flags & SB_FLAG_RELEASE) != 0;
+  // the late count: each EDD order repaired by Moore-Hodgson's rule (see moore_hodgson)
+  const bool late = (s.p.flags & SB_FLAG_LATE_COUNT) != 0;
   const double INF = HUGE_VAL;
   // usable cells: the ones the search proposes (k_build_valid), per job: those below the sentinel threshold, and for
   // a job with none only its cheapest finite cell (the first minimum; column 0 if it has no finite cell)
@@ -1352,6 +1412,14 @@ int sb_search_seed_lpt(sb_handle* h) {
       }
     } else if (!reduced) {
       for (int j = 0; j < J; ++j) opt[j] = static_cast<uint8_t>((h->h_args[j * kSlots + col[j]] << 3) | col[j]);
+    }
+    if (late) {
+      std::vector<int> node(J, 0);
+      if (nodes > 1)
+        for (int j = 0; j < J; ++j) node[j] = opt[j] >> 3;
+      const std::vector<float>* r = rel ? ((s.p.flags & SB_FLAG_INTEGER_STARTS) ? &h->h_rc : &h->h_r) : nullptr;
+      moore_hodgson(order, col, rt, node, nodes, (s.p.flags & SB_FLAG_WEIGHTED) ? &h->h_w : nullptr, h->h_d, r,
+                    (s.p.flags & SB_FLAG_INTEGER_STARTS) != 0);
     }
     for (int q = 0; q < J; ++q) { prio8[q] = static_cast<uint8_t>(order[q]); prio16[q] = static_cast<uint16_t>(order[q]); }
     const long long first = std::min<long long>(i * per, std::max<long long>(0, chains - per));

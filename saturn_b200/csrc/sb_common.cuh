@@ -163,19 +163,23 @@ __device__ __forceinline__ float fmax3_mk(float mk, float b, float c) {
 // reproduce); w = 1 then gives the unweighted fold bit for bit.
 // kDue (SB_FLAG_DUE, with kWeighted only): the job's tardiness max(e - d, +0) against its due date `d` takes the
 // completion's place, acc = acc + (w * max(e - d, +0)), each step rounded on its own; d = 0 gives the weighted fold.
+// kDue = 2 (SB_FLAG_LATE_COUNT, with kSum and kWeighted only): the job's weight if it is late, acc = acc + (e > d ? w
+// : +0), one rounding per step; a job that completes exactly at its due date is on time (as its tardiness is +0).
 // kDue without kSum (SB_FLAG_MAX_LATENESS): the tail makespan max(e + d), where `d` is the job's delivery tail
 // q = max_t d_t - d_t >= +0 (not its due date), so that the score is L_max + max_t d_t >= +0.  x = e + d is one
 // rounding, and x is folded like the makespan's completion (`ph`, `pend`), whatever kTrackMk says: f[7] is not x.
 // kRelease (SB_FLAG_RELEASE, with any of the above): the job starts no earlier than its release date `r`,
 // s = max(f[km1], r) (ceil(r) under integer starts, made once by sb_set_release, so s stays an integer).  The slot
 // update below stays valid because it only needs v >= f[km1]; r <= 0 gives s = f[km1] exactly.
+// kDue is 0 (no due dates), 1 (tardiness with kSum, the tail makespan without) or 2 (the late count).
 template <bool kIntegerStarts, bool kTrackMk = kIntegerStarts, bool kSum = false, bool kWeighted = false,
-          bool kDue = false, bool kRelease = false>
+          int kDue = 0, bool kRelease = false>
 __device__ __forceinline__ void ls_step(float (&f)[8], float& mk, float& pend, float rt, int km1, int one, int ph,
                                         float w = 0.f, float d = 0.f, float r = 0.f) {
   static_assert(kSum || !kWeighted, "weights scale the sum of completion times only");
   static_assert(kWeighted || !kDue || !kSum, "tardiness runs on the weighted form (unit weights for plain tardiness)");
   static_assert(!(kDue && !kSum && kWeighted), "the tail makespan is not weighted");
+  static_assert(kDue != 2 || kSum, "the late count is a sum");
   const float INF = inf_f();
   const int b2 = km1 & 4, b1 = km1 & 2, b0 = km1 & 1;
   // stage "shift by 4"
@@ -198,7 +202,11 @@ __device__ __forceinline__ void ls_step(float (&f)[8], float& mk, float& pend, f
   }
   if (kSum) {
     const float e = kIntegerStarts ? s + rt : v;
-    if (kDue) mk = __fadd_rn(mk, __fmul_rn(w, fmaxf(__fsub_rn(e, d), 0.f)));
+    // the late count: w * 1 = w and w * 0 = +0 exactly (w > 0 finite), so this adds (e > d ? w : +0); the product
+    // keeps the tardiness form's data flow, which ptxas allocates without the spills a bare select causes in some
+    // position-major search kernels at the 128-register cap
+    if (kDue == 2) mk = __fadd_rn(mk, __fmul_rn(w, e > d ? 1.f : 0.f));
+    else if (kDue) mk = __fadd_rn(mk, __fmul_rn(w, fmaxf(__fsub_rn(e, d), 0.f)));
     else if (kWeighted) mk = __fadd_rn(mk, __fmul_rn(w, e));
     else mk = mk + e;
   } else if (kDue) {

@@ -32,6 +32,8 @@
 //     the table is in shared memory (same TMA phase), and are read from global memory where the table is;
 //   * D (SB_FLAG_DUE, with W only): the weighted sum is of tardiness against per-job due dates instead of
 //     completions.  The due dates follow the weights, in the same memory and the same TMA phase;
+//   * D = 2 (SB_FLAG_LATE_COUNT, with W only): the weighted sum is of the late jobs' weights, w_j [C_j > d_j],
+//     instead of their tardiness (ls_step<..., kDue = 2>), on the same due dates in the same memory;
 //   * D without SUM (SB_FLAG_MAX_LATENESS): the tail makespan max_j (C_j + q_j) with delivery tails q_j =
 //     max_t d_t - d_j >= 0, i.e. L_max + max_t d_t (ls_step<..., kDue> without kSum).  The tails take the due
 //     dates' place, in the same memory and the same TMA phase;
@@ -71,7 +73,7 @@ struct TileArgs {
 // TABG: the runtime table stays in global memory (read through L1/L2) — for tables larger than the
 // shared memory left beside the opt tiles (e.g. J = 1024 with 8 strategies: 256 KB).
 template <int PB, bool INT, bool STREAM, bool MULTI, bool SEARCH = false, bool TABG = false, int ADDR = 0,
-          bool SUM = false, bool W = false, bool D = false, bool R = false>
+          bool SUM = false, bool W = false, int D = 0, bool R = false>
 __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const TileArgs a) {
   static_assert(!(SEARCH && (STREAM || TABG)), "the fused search round runs on shared-memory tiles only");
   static_assert(ADDR == 0 || (!TABG && !MULTI && !SEARCH), "ADDR = 1 needs the table and the opt rows in shared memory");
@@ -121,7 +123,7 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
         for (uint32_t off = 0; off < w_bytes; off += 32768u)
           tma_bulk_g2s(smem + tab_bytes + off, wsrc + off, min(32768u, w_bytes - off), bar_tab);
       }
-      if constexpr (D) {
+      if constexpr (D != 0) {
         const uint8_t* dsrc = reinterpret_cast<const uint8_t*>(a.d);
         for (uint32_t off = 0; off < d_bytes; off += 32768u)
           tma_bulk_g2s(smem + tab_bytes + w_bytes + off, dsrc + off, min(32768u, d_bytes - off), bar_tab);
@@ -134,14 +136,15 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
     }
   }
 
-  LaneState<INT, MULTI, ADDR, SUM, (W ? (TABG ? 2 : 1) : 0), (D ? (TABG ? 2 : 1) : 0), (R ? (TABG ? 2 : 1) : 0)> st;
+  LaneState<INT, MULTI, ADDR, SUM, (W ? (TABG ? 2 : 1) : 0), (D ? (TABG ? 2 : 1) : 0), (R ? (TABG ? 2 : 1) : 0),
+            (D == 2)> st;
   if (TABG) st.tab = a.tab;
   else st.tab = tab_s;
   if constexpr (W) {
     st.wt = TABG ? a.w : w_s;
     st.wt_s = smem_u32(w_s);
   }
-  if constexpr (D) {
+  if constexpr (D != 0) {
     st.dd = TABG ? a.d : d_s;
     st.dd_s = smem_u32(d_s);
   }
@@ -318,7 +321,7 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
 #pragma unroll
             for (int i = 0; i < kBatch; ++i) wb[i] = st.gather_w(js[i]);
           }
-          if constexpr (D) {
+          if constexpr (D != 0) {
 #pragma unroll
             for (int i = 0; i < kBatch; ++i) db[i] = st.gather_d(js[i]);
           }
@@ -353,7 +356,7 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
 #pragma unroll
               for (int i = 0; i < kBatch; ++i) wc[i] = wb[i];
             }
-            if constexpr (D) {
+            if constexpr (D != 0) {
 #pragma unroll
               for (int i = 0; i < kBatch; ++i) dc[i] = db[i];
             }
@@ -365,7 +368,8 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
 #pragma unroll
             for (int i = 0; i < kBatch; ++i) {
               const float x = R ? xc[i] : 0.f;
-              if constexpr (D) st.step_resolved(static_cast<int>(oc[i]), rc[i], i & 1, W ? wc[i] : 0.f, dc[i], x);
+              if constexpr (D != 0)
+                st.step_resolved(static_cast<int>(oc[i]), rc[i], i & 1, W ? wc[i] : 0.f, dc[i], x);
               else if constexpr (W) st.step_resolved(static_cast<int>(oc[i]), rc[i], i & 1, wc[i], 0.f, x);
               else st.step_resolved(static_cast<int>(oc[i]), rc[i], i & 1, 0.f, 0.f, x);
             }
@@ -423,7 +427,7 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
           }
         }
       }
-      return st.result();
+      return st.result(a.nodes);
     };
     // SEARCH rounds: score the lane's rows from window `w0` on (warp-uniform).  w0 > 0 resumes from the
     // snapshot taken in front of that window (buffer bit w0-1 of `par`); `save` stores the state in front of
@@ -470,7 +474,7 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
           for (int t = 0; t < rem; ++t) st.step(PB == 1 ? prio_row_s[c * STEPS + t] : reinterpret_cast<const uint16_t*>(prio_row_s)[c * STEPS + t], -1);
         }
       }
-      return st.result();
+      return st.result(a.nodes);
     };
     if (!SEARCH) {
       float mk = 0.f;
@@ -678,7 +682,7 @@ struct GenericArgs {
   const float* r;  // R: job release dates [J], likewise
 };
 
-template <int PB, bool INT, bool MULTI, bool SUM = false, bool W = false, bool D = false, bool R = false>
+template <int PB, bool INT, bool MULTI, bool SUM = false, bool W = false, int D = 0, bool R = false>
 __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
   static_assert(SUM || !W, "weights scale the sum of completion times only");
   static_assert(W || !D || !SUM, "tardiness runs on the weighted form");
@@ -694,7 +698,7 @@ __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
     tab = tab_s;
   }
   const int lane = threadIdx.x & 31;
-  LaneState<INT, MULTI, 0, SUM, (W ? 2 : 0), (D ? 2 : 0), (R ? 2 : 0)> st;
+  LaneState<INT, MULTI, 0, SUM, (W ? 2 : 0), (D ? 2 : 0), (R ? 2 : 0), (D == 2)> st;
   st.tab = tab;
   st.wt = a.w;
   st.dd = a.d;
@@ -729,7 +733,7 @@ __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
 #pragma unroll
           for (int t = 0; t < BATCH; ++t) xs[t] = st.lookup_r(js[t]);
         }
-        if constexpr (D) {
+        if constexpr (D != 0) {
           float ws[BATCH], ds[BATCH];
 #pragma unroll
           for (int t = 0; t < BATCH; ++t) ws[t] = st.lookup_w(js[t]);
@@ -749,7 +753,7 @@ __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
         }
       }
       for (; i < a.J; ++i) st.step(PB == 1 ? prow[i] : reinterpret_cast<const uint16_t*>(prow)[i]);
-      mk = st.result();
+      mk = st.result(a.nodes);
       a.out[b] = mk;
     }
     if (a.best_key != nullptr) fold_best(a.best_key, active, mk, a.id_base + static_cast<uint32_t>(b), lane);
@@ -778,7 +782,7 @@ struct FullArgs {
   const float* r;       // R: job release dates [J] (ceiled with INT)
 };
 
-template <int PB, bool INT, bool SUM = false, bool W = false, bool D = false, bool R = false>
+template <int PB, bool INT, bool SUM = false, bool W = false, int D = 0, bool R = false>
 __global__ void __launch_bounds__(128) k_eval_full(const FullArgs a) {
   static_assert(SUM || !W, "weights scale the sum of completion times only");
   static_assert(W || !D || !SUM, "tardiness runs on the weighted form");
@@ -817,9 +821,12 @@ __global__ void __launch_bounds__(128) k_eval_full(const FullArgs a) {
       const float nxt = s + hold;
       for (int g = 0; g < kSlots; ++g)
         if ((taken >> g) & 1u) rd[g] = nxt;
-      if constexpr (D && !SUM)  // ls_step<..., kDue>: the tail makespan
+      if constexpr (D != 0 && !SUM)  // ls_step<..., kDue>: the tail makespan
         mk = fmaxf(mk, __fadd_rn(s + rt, __ldg(a.d + j)));
-      else if constexpr (D)  // ls_step<..., kSum, kWeighted, kDue>
+      else if constexpr (D == 2)  // ls_step<..., kSum, kWeighted, kDue = 2>: the late count, +inf once a job has
+        // no runtime (LaneState::result)
+        mk = isinf(s + rt) ? INFINITY : __fadd_rn(mk, __fmul_rn(__ldg(a.w + j), s + rt > __ldg(a.d + j) ? 1.f : 0.f));
+      else if constexpr (D != 0)  // ls_step<..., kSum, kWeighted, kDue>
         mk = __fadd_rn(mk, __fmul_rn(__ldg(a.w + j), fmaxf(__fsub_rn(s + rt, __ldg(a.d + j)), 0.f)));
       else if constexpr (W) mk = __fadd_rn(mk, __fmul_rn(__ldg(a.w + j), s + rt));  // ls_step<..., kSum, kWeighted>
       else if (SUM) mk = mk + (s + rt);  // the left fold in schedule order of ls_step<..., kSum>

@@ -32,7 +32,7 @@ static_assert(((HOOK_FORCE_GENERIC | HOOK_NO_STREAM | HOOK_NO_FUSED | HOOK_NO_IN
                 HOOK_REORDER | HOOK_NO_REORDER) &
                (SB_FLAG_INTEGER_STARTS | SB_FLAG_REDUCED | SB_FLAG_OPT_BY_POSITION | SB_FLAG_POST_KEY |
                 SB_FLAG_FOLD_PREV | SB_FLAG_ALT_WARPSCAN | SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED |
-                SB_FLAG_DUE | SB_FLAG_RELEASE | SB_FLAG_MAX_LATENESS)) == 0,
+                SB_FLAG_DUE | SB_FLAG_RELEASE | SB_FLAG_MAX_LATENESS | SB_FLAG_LATE_COUNT)) == 0,
               "the test hooks share no bit with the SB_FLAG_* flags");
 
 // Debug options of the streamed tile kernel (sb_debug_tile_options): kept on the handle, not in the flags word, and
@@ -53,12 +53,16 @@ template <class F>
 decltype(auto) with_pb(int pb, F&& f) {
   return pb == 1 ? f(std::integral_constant<int, 1>{}) : f(std::integral_constant<int, 2>{});
 }
+template <int N>
+using int_c = std::integral_constant<int, N>;
 // f(PB, INT, SUM, W, D, R): the prio width, SB_FLAG_INTEGER_STARTS, SB_FLAG_SUM_COMPLETION, SB_FLAG_WEIGHTED,
-// SB_FLAG_DUE or SB_FLAG_MAX_LATENESS, and SB_FLAG_RELEASE, the template arguments that every evaluation and search
-// kernel takes.  W is true only together with SUM.  With SUM, D is true only together with W: no kernel that weights
-// the makespan, or that scores tardiness without weights, is ever instantiated (SB_FLAG_DUE alone runs the weighted
-// form on unit weights, exact since 1 * x = x).  Without SUM, D (SB_FLAG_MAX_LATENESS) is the tail makespan of
-// ls_step.  R is orthogonal to the other three: each objective form has a release twin.
+// the due-date form, and SB_FLAG_RELEASE, the template arguments that every evaluation and search kernel takes.  W is
+// true only together with SUM.  D is an int: 0 without due dates, 1 for SB_FLAG_DUE (tardiness) with SUM and for
+// SB_FLAG_MAX_LATENESS (the tail makespan of ls_step) without it, 2 for SB_FLAG_DUE | SB_FLAG_LATE_COUNT (the late
+// count).  With SUM, D is nonzero only together with W: no kernel that weights the makespan, or that scores tardiness
+// or the late count without weights, is ever instantiated (SB_FLAG_DUE alone runs the weighted form on unit weights,
+// exact since 1 * x = x and 1 is the count of one late job).  R is orthogonal to the other three: each objective form
+// has a release twin.
 template <class F>
 decltype(auto) with_eval_types(int pb, unsigned flags, F&& f) {
   return with_pb(pb, [&](auto PB) {
@@ -67,12 +71,22 @@ decltype(auto) with_eval_types(int pb, unsigned flags, F&& f) {
         return with_bool(flags & SB_FLAG_SUM_COMPLETION, [&](auto SUM) {
           if constexpr (SUM) {
             return with_bool(flags & (SB_FLAG_WEIGHTED | SB_FLAG_DUE), [&](auto W) {
-              if constexpr (W) return with_bool(flags & SB_FLAG_DUE, [&](auto D) { return f(PB, INT, SUM, W, D, R); });
-              else return f(PB, INT, SUM, W, std::false_type{}, R);
+              if constexpr (W) {
+                return with_bool(flags & SB_FLAG_DUE, [&](auto DUE) {
+                  if constexpr (DUE)
+                    return with_bool(flags & SB_FLAG_LATE_COUNT, [&](auto LATE) {
+                      return f(PB, INT, SUM, W, int_c<decltype(LATE)::value ? 2 : 1>{}, R);
+                    });
+                  else return f(PB, INT, SUM, W, int_c<0>{}, R);
+                });
+              } else {
+                return f(PB, INT, SUM, W, int_c<0>{}, R);
+              }
             });
           } else {
-            return with_bool(flags & SB_FLAG_MAX_LATENESS,
-                             [&](auto D) { return f(PB, INT, SUM, std::false_type{}, D, R); });
+            return with_bool(flags & SB_FLAG_MAX_LATENESS, [&](auto D) {
+              return f(PB, INT, SUM, std::false_type{}, int_c<decltype(D)::value ? 1 : 0>{}, R);
+            });
           }
         });
       });

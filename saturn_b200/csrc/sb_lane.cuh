@@ -42,10 +42,15 @@ __device__ __forceinline__ PrioChunk ld_prio32(const uint8_t* p) {
 // DUE (SB_FLAG_DUE, with WGT only): each job's tardiness against its due date, read from `dd`, takes its
 // completion's place; without SUM (SB_FLAG_MAX_LATENESS) `dd` holds the delivery tails and the score is the tail
 // makespan (see ls_step) — 1: in shared memory beside the table, 2: in global memory, read with ld.global.nc.
+// LATE (SB_FLAG_LATE_COUNT, with SUM, WGT and DUE only): the job's weight counts if it is late, instead of its
+// weighted tardiness (ls_step<..., kDue = 2>).
 // REL (SB_FLAG_RELEASE, with any objective): no job starts before its release date, read from `rr` — 1: in shared
 // memory beside the table, 2: in global memory, read with ld.global.nc.
-template <bool INT, bool MULTI, int ADDR = 0, bool SUM = false, int WGT = 0, int DUE = 0, int REL = 0>
+template <bool INT, bool MULTI, int ADDR = 0, bool SUM = false, int WGT = 0, int DUE = 0, int REL = 0,
+          bool LATE = false>
 struct LaneState {
+  static_assert(!LATE || (SUM && WGT != 0 && DUE != 0), "the late count runs on the weighted tardiness form");
+  static constexpr int kDue = DUE == 0 ? 0 : (LATE ? 2 : 1);  // ls_step's form
   float f[8];
   float mk;
   float pend;  // a completion time parked by an even step (see ls_step; never used with SUM)
@@ -117,10 +122,10 @@ struct LaneState {
   __device__ __forceinline__ void step_resolved(int o, float rt, int ph = -1, float w = 0.f, float d = 0.f,
                                                 float r = 0.f) {
     if (!MULTI) {
-      ls_step<INT, INT, SUM, (WGT != 0), (DUE != 0), (REL != 0)>(f, mk, pend, rt, o & 7, one, ph, w, d, r);
+      ls_step<INT, INT, SUM, (WGT != 0), kDue, (REL != 0)>(f, mk, pend, rt, o & 7, one, ph, w, d, r);
     } else {
       switch_node(o >> 3);
-      ls_step<INT, true, SUM, (WGT != 0), (DUE != 0), (REL != 0)>(f, mk, pend, rt, o & 7, one, ph, w, d, r);
+      ls_step<INT, true, SUM, (WGT != 0), kDue, (REL != 0)>(f, mk, pend, rt, o & 7, one, ph, w, d, r);
     }
   }
   // ADDR = 1: the two look-ups as separate gathers, so that the streamed loop of k_eval_tiles can issue a whole
@@ -178,26 +183,35 @@ struct LaneState {
   __device__ __forceinline__ void step(int j, int ph = -1) {
     constexpr bool W = WGT != 0;
     constexpr bool R = REL != 0;
-    constexpr bool D = DUE != 0;
     if (!MULTI && ADDR == 1) {
       const uint32_t o = gather_opt(j);
-      ls_step<INT, INT, SUM, W, D, R>(f, mk, pend, gather_rt(j, o), static_cast<int>(o & 7u), one, ph, gather_w(j),
-                                        gather_d(j), gather_r(j));
+      ls_step<INT, INT, SUM, W, kDue, R>(f, mk, pend, gather_rt(j, o), static_cast<int>(o & 7u), one, ph,
+                                         gather_w(j), gather_d(j), gather_r(j));
       return;
     }
     const int o = orow[j];
     if (!MULTI) {
       const float rt = tab[j * SG + o];
-      ls_step<INT, INT, SUM, W, D, R>(f, mk, pend, rt, o & 7, one, ph, lookup_w(j), lookup_d(j), lookup_r(j));
+      ls_step<INT, INT, SUM, W, kDue, R>(f, mk, pend, rt, o & 7, one, ph, lookup_w(j), lookup_d(j), lookup_r(j));
     } else {
       const int col = o & 7;  // reduced table only: opt = (node << 3) | (k - 1)
       const float rt = tab[j * 8 + col];
       switch_node(o >> 3);
-      ls_step<INT, true, SUM, W, D, R>(f, mk, pend, rt, col, one, ph, lookup_w(j), lookup_d(j), lookup_r(j));
+      ls_step<INT, true, SUM, W, kDue, R>(f, mk, pend, rt, col, one, ph, lookup_w(j), lookup_d(j), lookup_r(j));
     }
   }
-  // the tail makespan (DUE without SUM) is tracked in mk at every shape: f[7] is a completion, not a tail sum
-  __device__ __forceinline__ float result() const {
+  // the tail makespan (DUE without SUM) is tracked in mk at every shape: f[7] is a completion, not a tail sum.
+  // LATE: a job with no runtime (+inf cell) adds only its weight to the count, but the candidate is infeasible and
+  // scores +inf, as under every other objective.  Such a job leaves +inf in the slots it held, and slot times never
+  // decrease, so one look at each node's latest slot time at the end finds it (`nodes`: MULTI only; the node in
+  // f[] is checked there, the others in their shared-memory columns, where a stale copy of it is never +inf wrongly).
+  __device__ __forceinline__ float result(int nodes = 1) const {
+    if constexpr (LATE) {
+      float last = f[7];
+      if constexpr (MULTI)
+        for (int n = 0; n < nodes; ++n) last = fmaxf(last, ns[(2 * n + 1) * 32].w);
+      return last == inf_f() ? inf_f() : mk;
+    }
     return SUM ? mk : ((INT || MULTI || DUE != 0) ? fmaxf(mk, pend) : f[7]);
   }
   // the running score a snapshot of the incremental rounds stores (SearchFuse::snap): with SUM nothing is parked,

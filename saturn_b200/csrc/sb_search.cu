@@ -426,11 +426,12 @@ __device__ __forceinline__ PosMove make_pos_move_win(const SearchFuse& sf, int r
 // W: weight each completion by its job's weight (SB_FLAG_WEIGHTED, with SUM only); the weights follow the table in
 // shared memory with TAB = 0 and are read from global memory (ld.global.nc) with TAB = 1 / 2.
 // D: score tardiness against the jobs' due dates (SB_FLAG_DUE, with W only); the due dates follow the weights.
+// D = 2 scores the late count instead (SB_FLAG_LATE_COUNT, with W only), on the same due dates.
 // Without SUM, D is the tail makespan (SB_FLAG_MAX_LATENESS, see ls_step): the delivery tails take the due dates' place.
 // R: no job starts before its release date (SB_FLAG_RELEASE, any objective); the release dates follow the other
 // per-job arrays in shared memory with TAB = 0 and are read from global memory with TAB = 1 / 2.
 template <int PB, bool INT, bool MULTI, bool EVAL = false, int TAB = 0, bool SUM = false, bool W = false,
-          bool D = false, bool R = false>
+          int D = 0, bool R = false>
 __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
   static_assert(TAB == 0 || (EVAL && !MULTI), "tables outside the CTA's shared memory: scoring only, one node");
   static_assert(SUM || !W, "weights scale the sum of completion times only");
@@ -470,7 +471,7 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
         for (uint32_t off = 0; off < w_bytes; off += 32768u)
           tma_bulk_g2s(reinterpret_cast<uint8_t*>(w_s) + off, wsrc + off, min(32768u, w_bytes - off), bar_tab);
       }
-      if constexpr (D && TAB == 0) {
+      if constexpr (D != 0 && TAB == 0) {
         const uint8_t* dsrc = reinterpret_cast<const uint8_t*>(a.d);
         for (uint32_t off = 0; off < d_bytes; off += 32768u)
           tma_bulk_g2s(reinterpret_cast<uint8_t*>(d_s) + off, dsrc + off, min(32768u, d_bytes - off), bar_tab);
@@ -482,10 +483,11 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
       }
     }
   }
-  LaneState<INT, MULTI, 0, SUM, (W ? (TAB == 0 ? 1 : 2) : 0), (D ? (TAB == 0 ? 1 : 2) : 0), (R ? (TAB == 0 ? 1 : 2) : 0)> st;
+  LaneState<INT, MULTI, 0, SUM, (W ? (TAB == 0 ? 1 : 2) : 0), (D ? (TAB == 0 ? 1 : 2) : 0), (R ? (TAB == 0 ? 1 : 2) : 0),
+            (D == 2)> st;
   st.tab = tab_s;
   if constexpr (W) st.wt = TAB == 0 ? w_s : a.w;
-  if constexpr (D) st.dd = TAB == 0 ? d_s : a.d;
+  if constexpr (D != 0) st.dd = TAB == 0 ? d_s : a.d;
   if constexpr (R) st.rr = TAB == 0 ? r_s : a.r;
   st.SG = a.SG;
   st.one = a.one;
@@ -580,7 +582,7 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
           for (int t = 0; t < 32; ++t) {
             const int j = prio_at<PB>(qp[(t * PB) / 32].w, t % (32 / PB));
             const int o = prio_at<1>(qo.w, t);
-            if constexpr (D) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j), st.lookup_d(j), st.lookup_r(j));
+            if constexpr (D != 0) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j), st.lookup_d(j), st.lookup_r(j));
             else if constexpr (W) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j), 0.f, st.lookup_r(j));
             else st.step_resolved(o, lookup(j, o), t & 1, 0.f, 0.f, st.lookup_r(j));
           }
@@ -590,7 +592,7 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
             if (base + t < J) {
               const int j = prio_at<PB>(qp[(t * PB) / 32].w, t % (32 / PB));
               const int o = prio_at<1>(qo.w, t);
-              if constexpr (D) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j), st.lookup_d(j), st.lookup_r(j));
+              if constexpr (D != 0) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j), st.lookup_d(j), st.lookup_r(j));
               else if constexpr (W) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j), 0.f, st.lookup_r(j));
               else st.step_resolved(o, lookup(j, o), t & 1, 0.f, 0.f, st.lookup_r(j));
             }
@@ -600,7 +602,7 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
 #pragma unroll
         for (int h = 0; h < PCH; ++h) qp[h] = np[h];
       }
-      return st.result();
+      return st.result(a.nodes);
     };
     PosMove none;
     none.kind = 0; none.a = none.b = none.va = none.vb = none.oa = none.ob = 0;

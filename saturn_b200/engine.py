@@ -18,7 +18,8 @@ from ._lib import FLAG_INTEGER_STARTS, FLAG_REDUCED, SaturnB200Error, SearchPara
 NSLOT = 8
 
 
-OBJECTIVES = ("makespan", "completion", "weighted_completion", "tardiness", "weighted_tardiness", "max_lateness")
+OBJECTIVES = ("makespan", "completion", "weighted_completion", "tardiness", "weighted_tardiness", "max_lateness",
+              "late_tasks", "weighted_late_tasks")
 
 
 def objective_flag(objective: str) -> int:
@@ -26,7 +27,9 @@ def objective_flag(objective: str) -> int:
     SB_FLAG_WEIGHTED for "weighted_completion" (the sum weighted by the engine's set_weights), SB_FLAG_SUM_COMPLETION |
     SB_FLAG_DUE for "tardiness" (total tardiness against the engine's set_due) and SB_FLAG_SUM_COMPLETION |
     SB_FLAG_DUE | SB_FLAG_WEIGHTED for "weighted_tardiness", SB_FLAG_MAX_LATENESS for "max_lateness" (the maximum
-    lateness against the engine's set_due, scored as L_max + Engine.due_shift) and 0 for "makespan"."""
+    lateness against the engine's set_due, scored as L_max + Engine.due_shift), SB_FLAG_SUM_COMPLETION | SB_FLAG_DUE |
+    SB_FLAG_LATE_COUNT for "late_tasks" (the number of tasks that complete after their set_due date), the same |
+    SB_FLAG_WEIGHTED for "weighted_late_tasks" (the sum of their set_weights weights) and 0 for "makespan"."""
     if objective not in OBJECTIVES:
         from .solver import SolverError
         raise SolverError("objective must be one of %s, not %r" % (", ".join(map(repr, OBJECTIVES)), objective))
@@ -34,8 +37,9 @@ def objective_flag(objective: str) -> int:
         return 0
     if objective == "max_lateness":
         return _lib.FLAG_MAX_LATENESS
+    late = objective.endswith("late_tasks")
     return _lib.FLAG_SUM_COMPLETION | (_lib.FLAG_WEIGHTED if objective.startswith("weighted_") else 0) | (
-        _lib.FLAG_DUE if objective.endswith("tardiness") else 0)
+        _lib.FLAG_DUE if objective.endswith("tardiness") or late else 0) | (_lib.FLAG_LATE_COUNT if late else 0)
 
 
 def weights_f32(w, J: int) -> np.ndarray:
@@ -98,9 +102,10 @@ def _flags(integer_starts: bool, reduced: bool, objective: str = "makespan") -> 
 
 
 def _require_due(due, objective: str):
-    """The tardiness objectives and the maximum lateness score against the due dates of set_due: refuse them, before
-    any device call, on an engine that has none (set_table clears them)."""
-    if (objective.endswith("tardiness") or objective == "max_lateness") and due is None:
+    """The tardiness objectives, the late counts and the maximum lateness score against the due dates of set_due:
+    refuse them, before any device call, on an engine that has none (set_table clears them)."""
+    if (objective.endswith("tardiness") or objective.endswith("late_tasks") or objective == "max_lateness") and \
+            due is None:
         from .solver import SolverError
         raise SolverError("objective=%r needs due dates: call set_due after set_table" % (objective,))
 
@@ -129,7 +134,7 @@ class Engine:
         self.gcount = None
         self.nodes = 1
         self.weights = None  # fp32 job weights of objective="weighted_completion" (set_weights)
-        self.due = None  # fp32 job due dates of objective="tardiness" / "weighted_tardiness" / "max_lateness" (set_due)
+        self.due = None  # fp32 job due dates of the tardiness, late-count and max-lateness objectives (set_due)
         self.due_shift = None  # max of self.due: objective="max_lateness" scores L_max + due_shift (>= 0)
         self.release = None  # fp32 job release dates, under every objective (set_release)
 
@@ -197,7 +202,8 @@ class Engine:
         """Per-job due dates (J values, finite with |d| < 2^24, converted to fp32) for objective="tardiness", which
         scores sum_j max(0, start_j + rt_j - d_j), and "weighted_tardiness" (each term times the set_weights
         weight), and "max_lateness", which scores max_j (start_j + rt_j + q_j) with the tails q_j = D - d_j (fp32),
-        D = due_shift = max_j d_j: that is L_max + D >= 0, and subtracting D gives L_max.  None clears them; set_table
+        D = due_shift = max_j d_j: that is L_max + D >= 0, and subtracting D gives L_max, and "late_tasks" /
+        "weighted_late_tasks", which count (or weigh) the jobs with start_j + rt_j > d_j.  None clears them; set_table
         clears them too."""
         if d is None:
             check(self._lib.sb_set_due(self._h, None, 0))

@@ -54,11 +54,12 @@ def orchestrate(task_list, log=False, interval=1000, gurobi=True, *,
     batches_to_run, interval, node_per_task, task_dependency_dict)` stands in for
     saturn.executor.execute; returns the list of per-interval records (plan makespan, tasks run).
 
-    A `due` mapping Task -> due date in `solver_kwargs` (objective="tardiness" or "max_lateness") is measured from
-    the first plan's t = 0: the solve for interval n plans from n * interval on, so it receives {t: d - n * interval},
-    and the lateness each solve reports is against the original due dates (both sides shift alike).  A sequence
-    `due` raises SolverError, since the task list shrinks from interval to interval.  A `release` mapping
-    Task -> release date is shifted the same way, {t: r - n * interval}; a sequence `release` raises SolverError.
+    A `due` mapping Task -> due date in `solver_kwargs` (objective="tardiness", "max_lateness" or "late_tasks") is
+    measured from the first plan's t = 0: the solve for interval n plans from n * interval on, so it receives
+    {t: d - n * interval}, and the lateness each solve reports is against the original due dates (both sides shift
+    alike).  A sequence `due` raises SolverError, since the task list shrinks from interval to interval.  A `release`
+    mapping Task -> release date is shifted the same way, {t: r - n * interval}; a sequence `release` raises
+    SolverError.
     """
     logging.basicConfig(level=logging.INFO if log else logging.WARNING,
                         format="%(asctime)s %(levelname)-8s %(message)s", datefmt="%Y-%m-%d %H:%M:%S")

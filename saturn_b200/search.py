@@ -10,6 +10,7 @@ There is no reference counterpart: the reference solver is a single-process CPU 
 """
 from __future__ import annotations
 
+import math
 import time
 from dataclasses import dataclass, field
 from typing import List, Optional, Tuple
@@ -59,13 +60,15 @@ def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objecti
     job index; objective="max_lateness" the unit-weight EDD order of "tardiness" (Jackson's rule, optimal for the
     maximum lateness on one machine).  With the fp32 `release` dates (any objective) each order is then re-sorted stably by ascending
     release date (ceiled when `integer_starts`, as the device schedules them), so jobs released together keep the
-    objective's order."""
+    objective's order.  objective="late_tasks" / "weighted_late_tasks": the EDD orders of "tardiness" /
+    "weighted_tardiness", each repaired by Moore-Hodgson's rule after the node fill (moore_hodgson)."""
     objective_flag(objective)
     if objective.startswith("weighted_"):
         if weights is None:
             raise ValueError("objective=%r needs the job weights" % objective)
         w64 = np.asarray(weights, dtype=np.float32).astype(np.float64)
-    edd = objective.endswith("tardiness") or objective == "max_lateness"
+    late = objective.endswith("late_tasks")
+    edd = objective.endswith("tardiness") or objective == "max_lateness" or late
     if edd:
         if due is None:
             raise ValueError("objective=%r needs the job due dates" % objective)
@@ -88,7 +91,8 @@ def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objecti
         col = np.argmin(cost, axis=1)
         rt = usable[np.arange(J), col]
         if edd:
-            tie = rt.astype(np.float64) / w64 if objective == "weighted_tardiness" else rt.astype(np.float64)
+            weighted = objective in ("weighted_tardiness", "weighted_late_tasks")
+            tie = rt.astype(np.float64) / w64 if weighted else rt.astype(np.float64)
             order = np.lexsort((np.arange(J), tie, d32))
         elif objective == "weighted_completion":
             order = np.argsort(rt.astype(np.float64) / w64, kind="stable")
@@ -106,8 +110,61 @@ def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objecti
                 n = int(np.argmin(load))
                 load[n] += float(rt[j]) * (int(col[j]) + 1)
                 ob[j] |= n << 3
+        if late:
+            order = moore_hodgson(order, col, rt, ob >> 3 if nodes > 1 else np.zeros(J, dtype=np.int64), nodes,
+                                  w64 if objective == "weighted_late_tasks" else None, d32,
+                                  rel if release is not None else None, integer_starts)
         seeds.append((ob, order))
     return seeds
+
+
+def moore_hodgson(order, col, rt, node, nodes, weights, due, release, integer_starts):
+    """Moore-Hodgson's repair of a seed order for the late count (sb_search_seed_lpt's rule, decision for decision).
+    The on-time sequence, at first `order`, is list-scheduled in float64 on the fp32 inputs by the device's rule: job j
+    takes the k = col[j] + 1 slots of node[j] that are free first, starts when the k-th is free (and not before its
+    release), holds them for rt[j] (ceil(rt[j]) with `integer_starts`) and completes at start + rt[j].  At the first
+    job that completes after its due date, the job with the largest k * rt / w among it and the jobs before it (the
+    later one on ties) moves to a late list, and the schedule resumes from that job's position, until no job of the
+    sequence is late.  Returns the on-time sequence followed by the late list in `order`'s order.  With one gang size,
+    one node and unit weights this is Moore-Hodgson's algorithm (a minimum number of late jobs)."""
+    k = [int(c) + 1 for c in col]
+    rt64 = [float(x) for x in rt]
+    hold = [math.ceil(x) if integer_starts and math.isfinite(x) else x for x in rt64]
+    d64 = [float(x) for x in due]
+    r64 = [float(x) for x in release] if release is not None else None
+    w = [float(x) for x in weights] if weights is not None else [1.0] * len(rt64)
+    ratio = [k[j] * rt64[j] / w[j] for j in range(len(rt64))]
+    nd = [int(x) for x in node]
+    seq = [int(j) for j in order]
+    pos = {j: q for q, j in enumerate(seq)}
+    snap = [[[0.0] * 8 for _ in range(nodes)]]  # snap[q]: the slots' free times (ascending per node) before position q
+    late = []
+    q = 0
+    while q < len(seq):
+        j = seq[q]
+        state = [list(f) for f in snap[q]]
+        f = state[nd[j]]
+        st = f[k[j] - 1]
+        if r64 is not None:
+            st = max(st, r64[j])
+        v = st + hold[j]
+        f[:k[j]] = [v] * k[j]
+        f.sort()
+        del snap[q + 1:]
+        snap.append(state)
+        if st + rt64[j] > d64[j]:
+            out, best = 0, -math.inf
+            for p in range(q + 1):
+                if ratio[seq[p]] >= best:
+                    out, best = p, ratio[seq[p]]
+            late.append(seq.pop(out))
+            q = out
+            continue
+        q += 1
+    if not late:
+        return np.asarray(order)
+    late.sort(key=pos.__getitem__)
+    return np.asarray(seq + late, dtype=np.asarray(order).dtype)
 
 
 def run_search(engine: Engine, chains: int = 1 << 16, rounds: int = 200, seed: int = 0,
@@ -124,7 +181,9 @@ def run_search(engine: Engine, chains: int = 1 << 16, rounds: int = 200, seed: i
     the engine's set_weights.  objective="tardiness" / "weighted_tardiness" minimises the total (weighted) tardiness
     against the engine's set_due, and stops as soon as the incumbent's tardiness is 0, which no plan can beat.
     objective="max_lateness" minimises the maximum lateness against the engine's set_due; every score holds
-    L_max + engine.due_shift, and there is no stop at zero (L_max has no floor).
+    L_max + engine.due_shift, and there is no stop at zero (L_max has no floor).  objective="late_tasks" /
+    "weighted_late_tasks" minimises the (weighted) number of tasks that complete after their due date, and stops at
+    0 like the tardiness.
 
     `rounds` device rounds are issued in groups of `exchange_every` (tournament resampling every
     `resample_every` rounds inside a group is only another launch); after each group the ranks exchange
@@ -207,7 +266,8 @@ def run_search(engine: Engine, chains: int = 1 << 16, rounds: int = 200, seed: i
     if record_history:
         history.append((time.perf_counter() - t0, chains * world, key_makespan(key)))
     exchange_every = max(1, int(exchange_every))
-    at_zero = objective.endswith("tardiness")  # a tardiness of +0 (key bits 0) cannot be beaten
+    # a tardiness or late count of +0 (key bits 0) cannot be beaten
+    at_zero = objective.endswith("tardiness") or objective.endswith("late_tasks")
     reason = 3 if at_zero and (best_seen >> 32) == 0 else 0
     while reason == 0 and done_rounds < rounds:
         # one group of rounds, no host synchronisation; the library resamples on its own cadence

@@ -224,9 +224,9 @@ def _check_horizon(T, found_makespan=None, release=None, tails=None):
                           "options" % lower)
 
 def _check_objective(objective, hysteresis=False, release=None):
-    if objective not in ("makespan", "completion", "tardiness", "max_lateness"):
-        raise SolverError("objective must be 'makespan', 'completion', 'tardiness' or 'max_lateness', not %r"
-                          % (objective,))
+    if objective not in ("makespan", "completion", "tardiness", "max_lateness", "late_tasks"):
+        raise SolverError("objective must be 'makespan', 'completion', 'tardiness', 'max_lateness' or 'late_tasks', "
+                          "not %r" % (objective,))
     if objective != "makespan" and hysteresis:
         raise SolverError("hysteresis=True compares plans by makespan (milp.py:363-442); it is not defined for "
                           "objective=%r" % (objective,))
@@ -256,8 +256,9 @@ def _resolve_weights(weights, objective, J, task_list=None):
     Raises SolverError before any device call."""
     if weights is None:
         return None, None
-    if objective not in ("completion", "tardiness"):
-        raise SolverError("weights apply to objective='completion' or 'tardiness' only, not to %r" % (objective,))
+    if objective not in ("completion", "tardiness", "late_tasks"):
+        raise SolverError("weights apply to objective='completion', 'tardiness' or 'late_tasks' only, not to %r"
+                          % (objective,))
     weights = _per_task(weights, "weights", task_list)
     from .engine import weights_f32
     w32 = weights_f32(weights, J)
@@ -266,11 +267,12 @@ def _resolve_weights(weights, objective, J, task_list=None):
 
 def _resolve_due(due, objective, J, task_list=None):
     """The caller's per-task due dates as (float64 values in task order, fp32 array for the device), or (None, None)
-    without objective="tardiness" or "max_lateness", which require them.  Raises SolverError before any device
-    call."""
-    if objective not in ("tardiness", "max_lateness"):
+    without objective="tardiness", "max_lateness" or "late_tasks", which require them.  Raises SolverError before
+    any device call."""
+    if objective not in ("tardiness", "max_lateness", "late_tasks"):
         if due is not None:
-            raise SolverError("due dates apply to objective='tardiness' or 'max_lateness' only, not to %r" % (objective,))
+            raise SolverError("due dates apply to objective='tardiness', 'max_lateness' or 'late_tasks' only, not to %r"
+                              % (objective,))
         return None, None
     if due is None:
         raise SolverError("objective=%r needs due dates (due=...)" % (objective,))
@@ -304,6 +306,8 @@ def _set_objective(eng, objective, w32, d32, r32=None):
         eng.set_due(d32)
         if objective == "max_lateness":
             return objective
+        if objective == "late_tasks":
+            return "weighted_late_tasks" if w32 is not None else "late_tasks"
         return "weighted_tardiness" if w32 is not None else "tardiness"
     return "weighted_completion" if w32 is not None else objective
 
@@ -314,6 +318,14 @@ def _tardiness_stats(start, rts, w64, d64):
     w = w64 if w64 is not None else [1.0] * len(late)
     return {"weighted_tardiness": sum(wi * max(0.0, x) for wi, x in zip(w, late)),
             "late_tasks": sum(1 for x in late if x > 0)}
+
+
+def _late_count_stats(start, rts, w64, d64):
+    """_tardiness_stats, and with w64 weighted_late_tasks, the weight of the tasks with C_t > d_t, in float64."""
+    stats = _tardiness_stats(start, rts, w64, d64)
+    if w64 is not None:
+        stats["weighted_late_tasks"] = sum(w for s, r, d, w in zip(start, rts, d64, w64) if float(s) + float(r) - d > 0)
+    return stats
 
 
 def _lateness_stats(start, rts, d64):
@@ -395,6 +407,17 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     the tasks' own runtimes and the caller's due dates, and last_stats["device_makespan"] holds the device's fp32
     score minus max_t d_t.  Shifting every due date by one constant gives the same plan.  The 6th element stays the
     plan's makespan.
+
+    Late tasks.  objective="late_tasks" with `due` (as above) minimises the number of tasks that finish after their
+    due date, C_t > d_t: the question of how many jobs miss a deadline, which any delay misses alike.  A task that
+    finishes exactly at its due date is on time.  With `weights` as well it minimises sum_t w_t [C_t > d_t].  The
+    `due` and `weights` rules and errors are those above, as is the refusal of hysteresis=True; `release` is valid.
+    The search stops as soon as it finds a plan with no late task.  The device decides C_t > d_t in fp32 on the fp32
+    due date, like the tardiness: with fractional data a completion within rounding of its due date may count either
+    way.  last_stats["late_tasks"] and last_stats["weighted_tardiness"] are recomputed in float64 from the emitted
+    plan, the tasks' own runtimes and the caller's d (and w), with `weights` also last_stats["weighted_late_tasks"],
+    the weight of the late tasks; last_stats["device_makespan"] holds the device's fp32 score.  The 6th element
+    stays the plan's makespan.
 
     Release dates.  `release` (a sequence aligned with task_list, or a mapping keyed by Task, in the runtimes' units
     from the plan's t = 0) keeps every task from starting before its release date, under every objective: a
@@ -500,6 +523,8 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     if objective == "max_lateness":
         last_stats.update(_lateness_stats(dec["start"], rts, d64))
         last_stats["device_makespan"] = res.makespan - eng.due_shift
+    elif objective == "late_tasks":
+        last_stats.update(_late_count_stats(dec["start"], rts, w64, d64))
     elif d64 is not None:
         last_stats.update(_tardiness_stats(dec["start"], rts, w64, d64))
     if r64 is not None:
@@ -603,8 +628,9 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     """solve() on the dense profiler tensor T[J][S][G] (+ mask of usable cells, + gcount[G] GPU counts).
     `objective` as for solve(): "makespan" or "completion" (sum of completion times); `weights` as for solve(),
     a sequence aligned with T's rows (the weighted sum of completion times, last_stats["weighted_completion"]);
-    `due` as for solve() with objective="tardiness" or "max_lateness", a sequence aligned with T's rows; `release` as for solve(),
-    under every objective, a sequence aligned with T's rows (last_stats["total_flow_time"]).  Every cell of T must be
+    `due` as for solve() with objective="tardiness", "max_lateness" or "late_tasks" (last_stats as there), a sequence
+    aligned with T's rows; `release` as for solve(), under every objective, a sequence aligned with T's rows
+    (last_stats["total_flow_time"]).  Every cell of T must be
     >= 0 (-0.0 counts as zero), +inf or a sentinel: a negative or NaN cell raises SolverError, with or without `mask`.
 
     The table goes to the device un-reduced (sb_set_table: min over strategies with the first-minimum rule
@@ -684,6 +710,8 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     if objective == "max_lateness":
         last_stats.update(_lateness_stats(dec["start"], rts, d64))
         last_stats["device_makespan"] = res.makespan - eng.due_shift
+    elif objective == "late_tasks":
+        last_stats.update(_late_count_stats(dec["start"], rts, w64, d64))
     elif d64 is not None:
         last_stats.update(_tardiness_stats(dec["start"], rts, w64, d64))
     if r64 is not None:

@@ -1,5 +1,5 @@
 """Cost and effect of the sum-of-completion-times objectives (plain and weighted), of the weighted tardiness, of the
-maximum lateness and of release dates on one GPU; prints one JSON line.
+maximum lateness, of the (weighted) number of late tasks and of release dates on one GPU; prints one JSON line.
 
     python scripts/bench_objective.py [--steps 200] [--warmup 20] [--solve-chains 0] [--solve-rounds 400]
 
@@ -7,15 +7,18 @@ kernel: sb_eval on bench.py's C4 batch (J = 256, S = 8, 946,176 candidates, the 
         starts), scored for the makespan, the sum of completion times, the weighted sum (seeded weights) and the
         weighted tardiness (the same weights, seeded due dates), and the release twins of the makespan and the
         weighted tardiness (seeded integer release dates in [0, 20000) s, SB_FLAG_RELEASE, a second handle on the
-        same device), and the maximum lateness (the tail makespan over the same due dates), the seven launches
-        alternated in one process (the order rotates every step) and timed with CUDA
-        events; median of --steps launches each.
+        same device), the maximum lateness (the tail makespan over the same due dates) and the weighted late count
+        (the same weights and due dates), the eight launches alternated in one process (the order rotates every
+        step) and timed with CUDA events; median of --steps launches each.
 solve:  solve() wall time on a 256-task set (synthetic table, seed 3, 4 strategies) for the makespan, the sum of
         completion times and the weighted sum (seeded weights: 32 tasks of weight 8, the rest 1), each plan scored
         on all three measures (float64, the tasks' own runtimes); and the total tardiness (unit weights, seeded
         integer due dates in [0, 200000) s): its tardiness and late tasks against those of the makespan and
-        completion plans; and the maximum lateness (the same due dates): its L_max and late tasks against those of
-        the tardiness and makespan plans.
+        completion plans; the maximum lateness (the same due dates): its L_max and late tasks against those of
+        the tardiness and makespan plans; and the number of late tasks, unweighted and weighted (the same due dates
+        and weights), every plan scored on late tasks, weighted late tasks, tardiness and L_max.  late_unit compares
+        the late-count search's temperature unit, sum w (shipped), with the mean weight sum w / J (the same solve with
+        t_start and t_end divided by J).
 release: the same 256-task set with seeded release dates in [0, 0.5 x the makespan plan's makespan): per objective
         (makespan, completion, tardiness) the release-aware plan (solve(release=...)) against the release-blind plan
         (solve() without them, its options and list order rescored under the release rule), on makespan, total flow
@@ -75,7 +78,7 @@ def main():
     out = torch.empty(B, dtype=torch.float32, device=eng.device)
     key = torch.full((1,), 2 ** 63 - 1, dtype=torch.int64, device=eng.device)
     objs = ("makespan", "completion", "weighted_completion", "weighted_tardiness", "release_makespan",
-            "release_weighted_tardiness", "max_lateness")
+            "release_weighted_tardiness", "max_lateness", "weighted_late_tasks")
     times = {o: [] for o in objs}
     for i in range(args.warmup + args.steps):
         for obj in objs[i % len(objs):] + objs[:i % len(objs)]:
@@ -99,6 +102,8 @@ def main():
     kernel["release_over_tardiness"] = (kernel["release_weighted_tardiness"]["median_ms"] /
                                         kernel["weighted_tardiness"]["median_ms"])
     kernel["max_lateness_over_makespan"] = kernel["max_lateness"]["median_ms"] / kernel["makespan"]["median_ms"]
+    kernel["late_tasks_over_weighted_tardiness"] = (kernel["weighted_late_tasks"]["median_ms"] /
+                                                    kernel["weighted_tardiness"]["median_ms"])
     kernel.update(B=B, J=J, S=Sx, path=path, steps=args.steps)
     del opt, prio, out
     eng_r.close()
@@ -126,13 +131,16 @@ def main():
     due = [float(x) for x in np.random.default_rng(4).integers(0, 200000, size=len(tasks))]
     S.solve(tasks, None, rounds=4, engine=eng, objective="tardiness", due=due)
     S.solve(tasks, None, rounds=4, engine=eng, objective="max_lateness", due=due)
+    S.solve(tasks, None, rounds=4, engine=eng, objective="late_tasks", due=due)
+    S.solve(tasks, None, rounds=4, engine=eng, objective="late_tasks", due=due, weights=w)
     solve = {}
     for name, obj, weights in (("makespan", "makespan", None), ("completion", "completion", None),
                                ("weighted_completion", "completion", w), ("tardiness", "tardiness", None),
-                               ("max_lateness", "max_lateness", None)):
+                               ("max_lateness", "max_lateness", None), ("late_tasks", "late_tasks", None),
+                               ("weighted_late_tasks", "late_tasks", w)):
         t0 = time.perf_counter()
         res = S.solve(tasks, None, objective=obj, weights=weights,
-                      **({"due": due} if obj in ("tardiness", "max_lateness") else {}), **kw)
+                      **({"due": due} if obj in ("tardiness", "max_lateness", "late_tasks") else {}), **kw)
         wall = time.perf_counter() - t0
         st = S.last_stats
         # the plan scored on all three measures, in float64 from its starts and the tasks' own runtimes
@@ -145,10 +153,40 @@ def main():
                        "tardiness": sum(max(0.0, c - d) for c, d in zip(comp, due)),
                        "late_tasks": sum(1 for c, d in zip(comp, due) if c > d),
                        "max_lateness": max(c - d for c, d in zip(comp, due)),
+                       "weighted_late_tasks": sum(wi for wi, c, d in zip(w, comp, due) if c > d),
                        "rounds": st["rounds"], "candidates": st["candidates"]}
-    print(json.dumps({"card": card(0), "kernel": kernel, "solve": solve,
+    late_unit = late_unit_effect(S, R, tasks, due, w, kw)
+    print(json.dumps({"card": card(0), "kernel": kernel, "solve": solve, "late_unit": late_unit,
                       "release": release_effect(S, R, tasks, due, solve["makespan"]["makespan"], kw)}))
     eng.close()
+
+
+def late_unit_effect(S, R, tasks, due, w, kw):
+    """The late-count plans (unweighted and weighted) under the shipped temperature unit, sum w, and under the mean
+    weight, sum w / J: the same solve with t_start and t_end divided by J (run_search's defaults)."""
+    import inspect
+    from saturn_b200 import search as SE
+    J = len(tasks)
+    tuples = [[(g, s.runtime) for g, s in t.strategies.items()] for t in tasks]
+    dflt = inspect.signature(SE.run_search).parameters
+    t_start, t_end = dflt["t_start"].default, dflt["t_end"].default
+    base = SE.run_search
+    out = {}
+    for unit, scale in (("sum_w", 1.0), ("mean_w", 1.0 / J)):
+        def run(*a, **k):
+            return base(*a, t_start=t_start * scale, t_end=t_end * scale, **k)
+        SE.run_search = run
+        try:
+            for name, weights in (("late_tasks", None), ("weighted_late_tasks", w)):
+                res = S.solve(tasks, None, objective="late_tasks", due=due, weights=weights, **kw)
+                comp = [p[0] + p[2] for p in R.plan_from_arrays(tuples, res[0], res[1], res[2], res[3])]
+                out["%s_%s" % (name, unit)] = {
+                    "late_tasks": sum(1 for c, d in zip(comp, due) if c > d),
+                    "weighted_late_tasks": sum(wi for wi, c, d in zip(w, comp, due) if c > d),
+                    "rounds": S.last_stats["rounds"]}
+        finally:
+            SE.run_search = base
+    return out
 
 
 def release_effect(S, R, tasks, due, makespan, kw):

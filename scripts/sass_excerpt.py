@@ -73,15 +73,16 @@ def main():
           "R2P %d; tensor-core opcodes (HMMA / IMMA / UTCHMMA / UTCQMMA / QGMMA): %d.\n" % (
               len(fns), len(allins), hist["UBLKCP"], hist["SYNCS"], "LDG.*.128", full["LDG.*.128"], hist["R2P"],
               sum(hist[k] for k in hist if k in ("HMMA", "IMMA", "UTCHMMA", "UTCQMMA", "QGMMA", "UTCIMMA", "BMMA"))))
-    want = [("_ZN2sb12k_eval_tilesILi1ELb1ELb1ELb0ELb0ELb0ELi1ELb0ELb0ELb0ELb0EEEvNS_8TileArgsE", "the measured kernel (bench `value`): C4, integer starts, prio streamed, look-up addresses on the FMA pipe", 32),
-            ("_ZN2sb12k_eval_tilesILi1ELb1ELb1ELb0ELb0ELb0ELi1ELb1ELb0ELb0ELb0EEEvNS_8TileArgsE", "the same kernel scoring the sum of completion times (SB_FLAG_SUM_COMPLETION): one FADD per step instead of half a VIMNMX3", 32),
-            ("_ZN2sb12k_eval_tilesILi1ELb1ELb1ELb0ELb0ELb0ELi1ELb1ELb1ELb0ELb0EEEvNS_8TileArgsE", "the same kernel scoring the weighted sum of completion times (SB_FLAG_WEIGHTED): one more gather (IMAD + LDS) and one FMUL per step", 32),
-            ("_ZN2sb12k_eval_tilesILi1ELb1ELb1ELb0ELb0ELb0ELi1ELb1ELb1ELb1ELb0EEEvNS_8TileArgsE", "the same kernel scoring the weighted tardiness (SB_FLAG_DUE): one more gather (IMAD + LDS), one FADD and one FMNMX per step", 32),
-            ("_ZN2sb12k_eval_tilesILi1ELb1ELb1ELb0ELb0ELb0ELi1ELb0ELb0ELb0ELb1EEEvNS_8TileArgsE", "the measured kernel with release dates (SB_FLAG_RELEASE): one more gather (IMAD + LDS) and one FMNMX per step", 32),
-            ("_ZN2sb12k_eval_tilesILi1ELb1ELb1ELb0ELb0ELb0ELi1ELb1ELb1ELb1ELb1EEEvNS_8TileArgsE", "the weighted-tardiness kernel with release dates (SB_FLAG_DUE | SB_FLAG_RELEASE)", 32),
-            ("_ZN2sb12k_eval_tilesILi1ELb1ELb1ELb0ELb0ELb0ELi0ELb0ELb0ELb0ELb0EEEvNS_8TileArgsE", "the same kernel with plain C++ addressing (test hook HOOK_PLAIN_ADDR; the round-1 form)", 32),
-            ("_ZN2sb12k_eval_tilesILi1ELb1ELb0ELb0ELb1ELb0ELi0ELb0ELb0ELb0ELb0EEEvNS_8TileArgsE", "fused search round (solve()): rows in shared memory, incremental scoring", 16),
-            ("_ZN2sb12k_search_posILi2ELb1ELb0ELb0ELi0ELb0ELb0ELb0ELb0EEEvNS_7PosArgsE", "position-major search round (J > ~450, u16 priorities)", 32),
+    want = [("_ZN2sb12k_eval_tilesILi1ELb1ELb1ELb0ELb0ELb0ELi1ELb0ELb0ELi0ELb0EEEvNS_8TileArgsE", "the measured kernel (bench `value`): C4, integer starts, prio streamed, look-up addresses on the FMA pipe", 32),
+            ("_ZN2sb12k_eval_tilesILi1ELb1ELb1ELb0ELb0ELb0ELi1ELb1ELb0ELi0ELb0EEEvNS_8TileArgsE", "the same kernel scoring the sum of completion times (SB_FLAG_SUM_COMPLETION): one FADD per step instead of half a VIMNMX3", 32),
+            ("_ZN2sb12k_eval_tilesILi1ELb1ELb1ELb0ELb0ELb0ELi1ELb1ELb1ELi0ELb0EEEvNS_8TileArgsE", "the same kernel scoring the weighted sum of completion times (SB_FLAG_WEIGHTED): one more gather (IMAD + LDS) and one FMUL per step", 32),
+            ("_ZN2sb12k_eval_tilesILi1ELb1ELb1ELb0ELb0ELb0ELi1ELb1ELb1ELi1ELb0EEEvNS_8TileArgsE", "the same kernel scoring the weighted tardiness (SB_FLAG_DUE): one more gather (IMAD + LDS), one FADD and one FMNMX per step", 32),
+            ("_ZN2sb12k_eval_tilesILi1ELb1ELb1ELb0ELb0ELb0ELi1ELb1ELb1ELi2ELb0EEEvNS_8TileArgsE", "the same kernel scoring the weighted number of late tasks (SB_FLAG_DUE | SB_FLAG_LATE_COUNT): w * [e > d] as FSET + FMUL, then the FADD, in place of the tardiness' FADD + FMNMX + FMUL + FADD", 32),
+            ("_ZN2sb12k_eval_tilesILi1ELb1ELb1ELb0ELb0ELb0ELi1ELb0ELb0ELi0ELb1EEEvNS_8TileArgsE", "the measured kernel with release dates (SB_FLAG_RELEASE): one more gather (IMAD + LDS) and one FMNMX per step", 32),
+            ("_ZN2sb12k_eval_tilesILi1ELb1ELb1ELb0ELb0ELb0ELi1ELb1ELb1ELi1ELb1EEEvNS_8TileArgsE", "the weighted-tardiness kernel with release dates (SB_FLAG_DUE | SB_FLAG_RELEASE)", 32),
+            ("_ZN2sb12k_eval_tilesILi1ELb1ELb1ELb0ELb0ELb0ELi0ELb0ELb0ELi0ELb0EEEvNS_8TileArgsE", "the same kernel with plain C++ addressing (test hook HOOK_PLAIN_ADDR; the round-1 form)", 32),
+            ("_ZN2sb12k_eval_tilesILi1ELb1ELb0ELb0ELb1ELb0ELi0ELb0ELb0ELi0ELb0EEEvNS_8TileArgsE", "fused search round (solve()): rows in shared memory, incremental scoring", 16),
+            ("_ZN2sb12k_search_posILi2ELb1ELb0ELb0ELi0ELb0ELb0ELi0ELb0EEEvNS_7PosArgsE", "position-major search round (J > ~450, u16 priorities)", 32),
             ("_ZN2sb13k_eval_groupsILi1ELb1EEEvNS_7AltArgsE", "the alternate shape (SB_FLAG_ALT_WARPSCAN): 8 lanes per candidate, shuffles; the block is the 8 steps of one look-up batch for 4 candidates", 8)]
     for name, what, steps in want:
         if name not in fns:
