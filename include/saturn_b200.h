@@ -62,6 +62,13 @@
  * The comparison is made in fp32 on the fp32 due date, so a completion within rounding of a fractional due date is
  * decided as the tardiness fold decides it.  A candidate that gives a job an option it does not have (rt = +inf)
  * scores +inf, as under every other objective, though the fold alone would add only that job's weight.
+ * With SB_FLAG_MAX_TARDINESS instead it is the maximum weighted tardiness:
+ *   score = max_j w_j max(0, start_j + rt_j - d_j), from +0 in schedule order per job: e = start + rt, l = e - d,
+ *   t = max(l, +0), x = w * t (each rounded on its own, the tardiness fold's term bit for bit), acc = max(acc, x).
+ * d = 0 with unit weights gives exactly the makespan, due dates at or past every completion give +0, w = 2 exactly
+ * twice w = 1 (barring overflow).  The score is >= +0.  A job with no runtime (rt = +inf) gives a +inf term, so the
+ * candidate scores +inf without a special case.  w_j = 1 / p*_j and d_j = max(r_j, 0), with p*_j a lower bound on
+ * job j's runtime, make it the maximum stretch (slowdown) of the jobs, max_j (C_j - max(r_j, 0)) / p*_j.
  * The schedule, every start and every slot mask are the same under every objective.
  * With SB_FLAG_MAX_LATENESS (per-job due dates d_j, sb_set_due) the score is the maximum lateness
  * L_max = max_j (start_j + rt_j - d_j), emitted as the tail makespan L_max + D >= +0 with D = max_t d_t:
@@ -189,6 +196,18 @@ typedef enum sb_status {
                                      schedule of the on-time sequence has a late job, the job with the largest
                                      k * rt / w up to and including the first late one (the later on ties) moves to
                                      the back, where the moved jobs keep their EDD order.  Not available with
+                                     SB_FLAG_ALT_WARPSCAN (SB_ERR_UNSUPPORTED). */
+#define SB_FLAG_MAX_TARDINESS 4096u /* with SB_FLAG_SUM_COMPLETION | SB_FLAG_DUE only (SB_FLAG_WEIGHTED optional; else
+                                     SB_ERR_ARG), and not with SB_FLAG_LATE_COUNT or SB_FLAG_MAX_LATENESS (SB_ERR_ARG):
+                                     the tardiness terms are folded with max instead of +, and the objective is the
+                                     maximum (weighted) tardiness max_j w_j max(0, C_j - d_j) (see the evaluation
+                                     rule above).  It reads the weights and due dates of SB_FLAG_DUE and needs
+                                     nothing else.  Accepted by sb_eval, sb_eval_host, sb_eval_full, sb_decode and
+                                     the search, sb_search_run_multi included; every score the library emits then
+                                     holds the maximum, and target_makespan targets it.  The search's temperature
+                                     unit becomes max(incumbent, max_j w_j min_k rt_jk) (a max, not divided by
+                                     sum_j w_j), it stops as soon as the incumbent is +0 (stop_reason 3), and
+                                     sb_search_seed_lpt plants the EDD orders of SB_FLAG_DUE.  Not available with
                                      SB_FLAG_ALT_WARPSCAN (SB_ERR_UNSUPPORTED). */
 #define SB_IPC_HANDLE_BYTES 64
 

@@ -464,12 +464,18 @@ int sb_set_release(sb_handle* h, const float* r, int J) {
 // SB_FLAG_WEIGHTED and SB_FLAG_DUE are valid with SB_FLAG_SUM_COMPLETION only, and after sb_set_weights /
 // sb_set_due respectively; SB_FLAG_MAX_LATENESS alone among the objective flags, after sb_set_due with a due-date spread
 // below 2^24; SB_FLAG_LATE_COUNT with SB_FLAG_SUM_COMPLETION | SB_FLAG_DUE only (it changes what the tardiness form
-// adds per job); SB_FLAG_RELEASE under any objective, after sb_set_release
+// adds per job); SB_FLAG_MAX_TARDINESS likewise (it changes how the tardiness form folds its terms), and not with
+// SB_FLAG_LATE_COUNT or SB_FLAG_MAX_LATENESS; SB_FLAG_RELEASE under any objective, after sb_set_release
 static int check_per_job(const sb_handle* h, unsigned flags) {
   constexpr unsigned kTardiness = SB_FLAG_SUM_COMPLETION | SB_FLAG_DUE;
   if ((flags & SB_FLAG_LATE_COUNT) && (flags & kTardiness) != kTardiness)
     return fail(SB_ERR_ARG, "SB_FLAG_LATE_COUNT counts late jobs on the tardiness form: it needs SB_FLAG_SUM_COMPLETION "
                 "and SB_FLAG_DUE");
+  if ((flags & SB_FLAG_MAX_TARDINESS) && (flags & kTardiness) != kTardiness)
+    return fail(SB_ERR_ARG, "SB_FLAG_MAX_TARDINESS folds the tardiness form with max: it needs SB_FLAG_SUM_COMPLETION "
+                "and SB_FLAG_DUE");
+  if ((flags & SB_FLAG_MAX_TARDINESS) && (flags & (SB_FLAG_LATE_COUNT | SB_FLAG_MAX_LATENESS)))
+    return fail(SB_ERR_ARG, "SB_FLAG_MAX_TARDINESS cannot be combined with SB_FLAG_LATE_COUNT or SB_FLAG_MAX_LATENESS");
   if ((flags & SB_FLAG_MAX_LATENESS) && (flags & (SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED | SB_FLAG_DUE)))
     return fail(SB_ERR_ARG, "SB_FLAG_MAX_LATENESS is an objective of its own: it cannot be combined with "
                 "SB_FLAG_SUM_COMPLETION, SB_FLAG_WEIGHTED or SB_FLAG_DUE");
@@ -601,10 +607,10 @@ int sb_eval(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, int64
   }
   if (flags & SB_FLAG_ALT_WARPSCAN) {
     if (flags & (SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED | SB_FLAG_DUE | SB_FLAG_RELEASE | SB_FLAG_MAX_LATENESS |
-                 SB_FLAG_LATE_COUNT))
+                 SB_FLAG_LATE_COUNT | SB_FLAG_MAX_TARDINESS))
       return fail(SB_ERR_UNSUPPORTED, "SB_FLAG_ALT_WARPSCAN scores the makespan without release dates only: it "
                   "cannot be combined with SB_FLAG_SUM_COMPLETION, SB_FLAG_WEIGHTED, SB_FLAG_DUE, SB_FLAG_RELEASE, "
-                  "SB_FLAG_MAX_LATENESS or SB_FLAG_LATE_COUNT");
+                  "SB_FLAG_MAX_LATENESS, SB_FLAG_LATE_COUNT or SB_FLAG_MAX_TARDINESS");
     if (flags & (SB_FLAG_POST_KEY | SB_FLAG_FOLD_PREV))
       return fail(SB_ERR_UNSUPPORTED, "SB_FLAG_ALT_WARPSCAN cannot be combined with the fused key exchange");
     cudaError_t e = eval_alt_launch(h->dev, c, h->stream);
@@ -1056,7 +1062,7 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
     // tardiness can be 0 or tiny at the incumbent: the unit is at least the weighted mean of each job's smallest
     // proposable runtime, the size of the score change one move makes
     const float* tmin = h->h_tmin.data();
-    double move = 0.0;
+    double move = 0.0, move_max = 0.0;
     for (int j = 0; j < J; ++j) {
       double lo = HUGE_VAL, lo_any = HUGE_VAL;
       for (int k = 0; k < kSlots; ++k) {
@@ -1065,9 +1071,17 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
         if (isfinite(v)) lo_any = std::min(lo_any, static_cast<double>(v));
       }
       if (!isfinite(lo)) lo = lo_any;
-      if (isfinite(lo)) move += (weighted ? static_cast<double>(h->h_w[j]) : 1.0) * lo;
+      if (isfinite(lo)) {
+        const double x = (weighted ? static_cast<double>(h->h_w[j]) : 1.0) * lo;
+        move += x;
+        move_max = std::max(move_max, x);
+      }
     }
-    s.scale = std::max(s.scale, static_cast<float>(move / (weighted ? h->w_sum : static_cast<double>(J))));
+    // the maximum tardiness is a max, not a sum: its unit is the incumbent itself (the mean-completion division of
+    // SB_FLAG_SUM_COMPLETION does not apply), and at least the largest weighted smallest runtime, the same floor taken
+    // as a max.  A starting point, not a measured choice (DESIGN §3)
+    if (p->flags & SB_FLAG_MAX_TARDINESS) s.scale = std::max(mk, static_cast<float>(move_max));
+    else s.scale = std::max(s.scale, static_cast<float>(move / (weighted ? h->w_sum : static_cast<double>(J))));
   }
   // the late count moves in steps of one job's weight and is 0 at many incumbents: its unit is the count of every job,
   // sum_j w_j (J with unit weights), so that an uphill move of one mean weight is accepted with e^(-1 / (J t))

@@ -165,13 +165,17 @@ __device__ __forceinline__ float fmax3_mk(float mk, float b, float c) {
 // completion's place, acc = acc + (w * max(e - d, +0)), each step rounded on its own; d = 0 gives the weighted fold.
 // kDue = 2 (SB_FLAG_LATE_COUNT, with kSum and kWeighted only): the job's weight if it is late, acc = acc + (e > d ? w
 // : +0), one rounding per step; a job that completes exactly at its due date is on time (as its tardiness is +0).
+// kDue = 3 (SB_FLAG_MAX_TARDINESS, with kSum and kWeighted only): the maximum weighted tardiness, mk = max(mk, w *
+// max(e - d, +0)), the tardiness form's term bit for bit folded with max instead of +.  Every term is >= +0, so mk is
+// exact at every step like a sum (no parked `pend`); a job with no runtime (rt = +inf, w > 0) gives a +inf term.
 // kDue without kSum (SB_FLAG_MAX_LATENESS): the tail makespan max(e + d), where `d` is the job's delivery tail
 // q = max_t d_t - d_t >= +0 (not its due date), so that the score is L_max + max_t d_t >= +0.  x = e + d is one
 // rounding, and x is folded like the makespan's completion (`ph`, `pend`), whatever kTrackMk says: f[7] is not x.
 // kRelease (SB_FLAG_RELEASE, with any of the above): the job starts no earlier than its release date `r`,
 // s = max(f[km1], r) (ceil(r) under integer starts, made once by sb_set_release, so s stays an integer).  The slot
 // update below stays valid because it only needs v >= f[km1]; r <= 0 gives s = f[km1] exactly.
-// kDue is 0 (no due dates), 1 (tardiness with kSum, the tail makespan without) or 2 (the late count).
+// kDue is 0 (no due dates), 1 (tardiness with kSum, the tail makespan without), 2 (the late count) or 3 (the
+// maximum weighted tardiness).
 template <bool kIntegerStarts, bool kTrackMk = kIntegerStarts, bool kSum = false, bool kWeighted = false,
           int kDue = 0, bool kRelease = false>
 __device__ __forceinline__ void ls_step(float (&f)[8], float& mk, float& pend, float rt, int km1, int one, int ph,
@@ -180,6 +184,7 @@ __device__ __forceinline__ void ls_step(float (&f)[8], float& mk, float& pend, f
   static_assert(kWeighted || !kDue || !kSum, "tardiness runs on the weighted form (unit weights for plain tardiness)");
   static_assert(!(kDue && !kSum && kWeighted), "the tail makespan is not weighted");
   static_assert(kDue != 2 || kSum, "the late count is a sum");
+  static_assert(kDue != 3 || kSum, "the maximum tardiness runs on the weighted tardiness form");
   const float INF = inf_f();
   const int b2 = km1 & 4, b1 = km1 & 2, b0 = km1 & 1;
   // stage "shift by 4"
@@ -206,6 +211,12 @@ __device__ __forceinline__ void ls_step(float (&f)[8], float& mk, float& pend, f
     // keeps the tardiness form's data flow, which ptxas allocates without the spills a bare select causes in some
     // position-major search kernels at the 128-register cap
     if (kDue == 2) mk = __fadd_rn(mk, __fmul_rn(w, e > d ? 1.f : 0.f));
+    // the maximum tardiness, max(mk, w * max(e - d, +0)), as one integer max over the product's bits: mk >= +0, and
+    // w * (e - d) with w > 0 is either that term (e - d > 0), or +0, a negative value or -0 (e - d <= 0), which all
+    // lose to mk as signed integers exactly as the +0 term does as a float.  Same value, one FMNMX fewer; the
+    // float form gave two position-major search kernels more spills than their tardiness siblings
+    else if (kDue == 3)
+      mk = __int_as_float(max(__float_as_int(mk), __float_as_int(__fmul_rn(w, __fsub_rn(e, d)))));
     else if (kDue) mk = __fadd_rn(mk, __fmul_rn(w, fmaxf(__fsub_rn(e, d), 0.f)));
     else if (kWeighted) mk = __fadd_rn(mk, __fmul_rn(w, e));
     else mk = mk + e;

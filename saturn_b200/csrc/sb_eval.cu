@@ -34,6 +34,8 @@
 //     completions.  The due dates follow the weights, in the same memory and the same TMA phase;
 //   * D = 2 (SB_FLAG_LATE_COUNT, with W only): the weighted sum is of the late jobs' weights, w_j [C_j > d_j],
 //     instead of their tardiness (ls_step<..., kDue = 2>), on the same due dates in the same memory;
+//   * D = 3 (SB_FLAG_MAX_TARDINESS, with W only): the weighted tardiness terms are folded with max instead of +,
+//     max_j w_j max(C_j - d_j, +0) (ls_step<..., kDue = 3>), on the same weights and due dates in the same memory;
 //   * D without SUM (SB_FLAG_MAX_LATENESS): the tail makespan max_j (C_j + q_j) with delivery tails q_j =
 //     max_t d_t - d_j >= 0, i.e. L_max + max_t d_t (ls_step<..., kDue> without kSum).  The tails take the due
 //     dates' place, in the same memory and the same TMA phase;
@@ -137,7 +139,7 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
   }
 
   LaneState<INT, MULTI, ADDR, SUM, (W ? (TABG ? 2 : 1) : 0), (D ? (TABG ? 2 : 1) : 0), (R ? (TABG ? 2 : 1) : 0),
-            (D == 2)> st;
+            (D == 0 ? 1 : D)> st;
   if (TABG) st.tab = a.tab;
   else st.tab = tab_s;
   if constexpr (W) {
@@ -698,7 +700,7 @@ __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
     tab = tab_s;
   }
   const int lane = threadIdx.x & 31;
-  LaneState<INT, MULTI, 0, SUM, (W ? 2 : 0), (D ? 2 : 0), (R ? 2 : 0), (D == 2)> st;
+  LaneState<INT, MULTI, 0, SUM, (W ? 2 : 0), (D ? 2 : 0), (R ? 2 : 0), (D == 0 ? 1 : D)> st;
   st.tab = tab;
   st.wt = a.w;
   st.dd = a.d;
@@ -826,6 +828,8 @@ __global__ void __launch_bounds__(128) k_eval_full(const FullArgs a) {
       else if constexpr (D == 2)  // ls_step<..., kSum, kWeighted, kDue = 2>: the late count, +inf once a job has
         // no runtime (LaneState::result)
         mk = isinf(s + rt) ? INFINITY : __fadd_rn(mk, __fmul_rn(__ldg(a.w + j), s + rt > __ldg(a.d + j) ? 1.f : 0.f));
+      else if constexpr (D == 3)  // ls_step<..., kSum, kWeighted, kDue = 3>: the maximum weighted tardiness
+        mk = fmaxf(mk, __fmul_rn(__ldg(a.w + j), fmaxf(__fsub_rn(s + rt, __ldg(a.d + j)), 0.f)));
       else if constexpr (D != 0)  // ls_step<..., kSum, kWeighted, kDue>
         mk = __fadd_rn(mk, __fmul_rn(__ldg(a.w + j), fmaxf(__fsub_rn(s + rt, __ldg(a.d + j)), 0.f)));
       else if constexpr (W) mk = __fadd_rn(mk, __fmul_rn(__ldg(a.w + j), s + rt));  // ls_step<..., kSum, kWeighted>

@@ -32,7 +32,8 @@ static_assert(((HOOK_FORCE_GENERIC | HOOK_NO_STREAM | HOOK_NO_FUSED | HOOK_NO_IN
                 HOOK_REORDER | HOOK_NO_REORDER) &
                (SB_FLAG_INTEGER_STARTS | SB_FLAG_REDUCED | SB_FLAG_OPT_BY_POSITION | SB_FLAG_POST_KEY |
                 SB_FLAG_FOLD_PREV | SB_FLAG_ALT_WARPSCAN | SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED |
-                SB_FLAG_DUE | SB_FLAG_RELEASE | SB_FLAG_MAX_LATENESS | SB_FLAG_LATE_COUNT)) == 0,
+                SB_FLAG_DUE | SB_FLAG_RELEASE | SB_FLAG_MAX_LATENESS | SB_FLAG_LATE_COUNT |
+                SB_FLAG_MAX_TARDINESS)) == 0,
               "the test hooks share no bit with the SB_FLAG_* flags");
 
 // Debug options of the streamed tile kernel (sb_debug_tile_options): kept on the handle, not in the flags word, and
@@ -59,10 +60,11 @@ using int_c = std::integral_constant<int, N>;
 // the due-date form, and SB_FLAG_RELEASE, the template arguments that every evaluation and search kernel takes.  W is
 // true only together with SUM.  D is an int: 0 without due dates, 1 for SB_FLAG_DUE (tardiness) with SUM and for
 // SB_FLAG_MAX_LATENESS (the tail makespan of ls_step) without it, 2 for SB_FLAG_DUE | SB_FLAG_LATE_COUNT (the late
-// count).  With SUM, D is nonzero only together with W: no kernel that weights the makespan, or that scores tardiness
-// or the late count without weights, is ever instantiated (SB_FLAG_DUE alone runs the weighted form on unit weights,
-// exact since 1 * x = x and 1 is the count of one late job).  R is orthogonal to the other three: each objective form
-// has a release twin.
+// count), 3 for SB_FLAG_DUE | SB_FLAG_MAX_TARDINESS (the maximum weighted tardiness).  With SUM, D is nonzero only
+// together with W: no kernel that weights the makespan, or that scores tardiness, the late count or the maximum
+// tardiness without weights, is ever instantiated (SB_FLAG_DUE alone runs the weighted form on unit weights, exact
+// since 1 * x = x and 1 is the count of one late job).  R is orthogonal to the other three: each objective form has a
+// release twin.
 template <class F>
 decltype(auto) with_eval_types(int pb, unsigned flags, F&& f) {
   return with_pb(pb, [&](auto PB) {
@@ -75,7 +77,10 @@ decltype(auto) with_eval_types(int pb, unsigned flags, F&& f) {
                 return with_bool(flags & SB_FLAG_DUE, [&](auto DUE) {
                   if constexpr (DUE)
                     return with_bool(flags & SB_FLAG_LATE_COUNT, [&](auto LATE) {
-                      return f(PB, INT, SUM, W, int_c<decltype(LATE)::value ? 2 : 1>{}, R);
+                      if constexpr (LATE) return f(PB, INT, SUM, W, int_c<2>{}, R);
+                      else return with_bool(flags & SB_FLAG_MAX_TARDINESS, [&](auto MAXT) {
+                        return f(PB, INT, SUM, W, int_c<decltype(MAXT)::value ? 3 : 1>{}, R);
+                      });
                     });
                   else return f(PB, INT, SUM, W, int_c<0>{}, R);
                 });

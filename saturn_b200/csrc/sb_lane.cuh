@@ -42,15 +42,18 @@ __device__ __forceinline__ PrioChunk ld_prio32(const uint8_t* p) {
 // DUE (SB_FLAG_DUE, with WGT only): each job's tardiness against its due date, read from `dd`, takes its
 // completion's place; without SUM (SB_FLAG_MAX_LATENESS) `dd` holds the delivery tails and the score is the tail
 // makespan (see ls_step) — 1: in shared memory beside the table, 2: in global memory, read with ld.global.nc.
-// LATE (SB_FLAG_LATE_COUNT, with SUM, WGT and DUE only): the job's weight counts if it is late, instead of its
-// weighted tardiness (ls_step<..., kDue = 2>).
+// FORM (with SUM, WGT and DUE only): what the tardiness form folds per job, ls_step's kDue — 1: the weighted
+// tardiness, summed; 2 (SB_FLAG_LATE_COUNT): the job's weight if it is late, summed; 3 (SB_FLAG_MAX_TARDINESS): the
+// weighted tardiness, folded with max.  Without SUM a nonzero DUE is always the tail makespan (kDue = 1).
 // REL (SB_FLAG_RELEASE, with any objective): no job starts before its release date, read from `rr` — 1: in shared
 // memory beside the table, 2: in global memory, read with ld.global.nc.
 template <bool INT, bool MULTI, int ADDR = 0, bool SUM = false, int WGT = 0, int DUE = 0, int REL = 0,
-          bool LATE = false>
+          int FORM = 1>
 struct LaneState {
-  static_assert(!LATE || (SUM && WGT != 0 && DUE != 0), "the late count runs on the weighted tardiness form");
-  static constexpr int kDue = DUE == 0 ? 0 : (LATE ? 2 : 1);  // ls_step's form
+  static_assert(FORM == 1 || (SUM && WGT != 0 && DUE != 0), "the late count and the maximum tardiness run on the "
+                "weighted tardiness form");
+  static constexpr bool LATE = FORM == 2;
+  static constexpr int kDue = DUE == 0 ? 0 : FORM;  // ls_step's form
   float f[8];
   float mk;
   float pend;  // a completion time parked by an even step (see ls_step; never used with SUM)
@@ -215,7 +218,8 @@ struct LaneState {
     return SUM ? mk : ((INT || MULTI || DUE != 0) ? fmaxf(mk, pend) : f[7]);
   }
   // the running score a snapshot of the incremental rounds stores (SearchFuse::snap): with SUM nothing is parked,
-  // so a snapshot is exact at any step, not only after an even number of steps
+  // so a snapshot is exact at any step, not only after an even number of steps; the maximum tardiness (FORM = 3)
+  // runs under SUM and parks nothing either
   __device__ __forceinline__ float running() const { return SUM ? mk : fmaxf(mk, pend); }
 };
 

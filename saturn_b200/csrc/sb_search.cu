@@ -427,6 +427,7 @@ __device__ __forceinline__ PosMove make_pos_move_win(const SearchFuse& sf, int r
 // shared memory with TAB = 0 and are read from global memory (ld.global.nc) with TAB = 1 / 2.
 // D: score tardiness against the jobs' due dates (SB_FLAG_DUE, with W only); the due dates follow the weights.
 // D = 2 scores the late count instead (SB_FLAG_LATE_COUNT, with W only), on the same due dates.
+// D = 3 folds the weighted tardiness terms with max instead of + (SB_FLAG_MAX_TARDINESS, with W only).
 // Without SUM, D is the tail makespan (SB_FLAG_MAX_LATENESS, see ls_step): the delivery tails take the due dates' place.
 // R: no job starts before its release date (SB_FLAG_RELEASE, any objective); the release dates follow the other
 // per-job arrays in shared memory with TAB = 0 and are read from global memory with TAB = 1 / 2.
@@ -484,7 +485,7 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
     }
   }
   LaneState<INT, MULTI, 0, SUM, (W ? (TAB == 0 ? 1 : 2) : 0), (D ? (TAB == 0 ? 1 : 2) : 0), (R ? (TAB == 0 ? 1 : 2) : 0),
-            (D == 2)> st;
+            (D == 0 ? 1 : D)> st;
   st.tab = tab_s;
   if constexpr (W) st.wt = TAB == 0 ? w_s : a.w;
   if constexpr (D != 0) st.dd = TAB == 0 ? d_s : a.d;

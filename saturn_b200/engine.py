@@ -19,7 +19,7 @@ NSLOT = 8
 
 
 OBJECTIVES = ("makespan", "completion", "weighted_completion", "tardiness", "weighted_tardiness", "max_lateness",
-              "late_tasks", "weighted_late_tasks")
+              "late_tasks", "weighted_late_tasks", "max_tardiness", "weighted_max_tardiness")
 
 
 def objective_flag(objective: str) -> int:
@@ -29,7 +29,10 @@ def objective_flag(objective: str) -> int:
     SB_FLAG_DUE | SB_FLAG_WEIGHTED for "weighted_tardiness", SB_FLAG_MAX_LATENESS for "max_lateness" (the maximum
     lateness against the engine's set_due, scored as L_max + Engine.due_shift), SB_FLAG_SUM_COMPLETION | SB_FLAG_DUE |
     SB_FLAG_LATE_COUNT for "late_tasks" (the number of tasks that complete after their set_due date), the same |
-    SB_FLAG_WEIGHTED for "weighted_late_tasks" (the sum of their set_weights weights) and 0 for "makespan"."""
+    SB_FLAG_WEIGHTED for "weighted_late_tasks" (the sum of their set_weights weights), SB_FLAG_SUM_COMPLETION |
+    SB_FLAG_DUE | SB_FLAG_MAX_TARDINESS for "max_tardiness" (the largest tardiness against set_due), the same |
+    SB_FLAG_WEIGHTED for "weighted_max_tardiness" (the largest set_weights-weighted tardiness; with weights 1 / p* and
+    due dates at the release dates, the maximum stretch) and 0 for "makespan"."""
     if objective not in OBJECTIVES:
         from .solver import SolverError
         raise SolverError("objective must be one of %s, not %r" % (", ".join(map(repr, OBJECTIVES)), objective))
@@ -38,8 +41,10 @@ def objective_flag(objective: str) -> int:
     if objective == "max_lateness":
         return _lib.FLAG_MAX_LATENESS
     late = objective.endswith("late_tasks")
+    max_t = objective.endswith("max_tardiness")
     return _lib.FLAG_SUM_COMPLETION | (_lib.FLAG_WEIGHTED if objective.startswith("weighted_") else 0) | (
-        _lib.FLAG_DUE if objective.endswith("tardiness") or late else 0) | (_lib.FLAG_LATE_COUNT if late else 0)
+        _lib.FLAG_DUE if objective.endswith("tardiness") or late else 0) | (_lib.FLAG_LATE_COUNT if late else 0) | (
+        _lib.FLAG_MAX_TARDINESS if max_t else 0)
 
 
 def weights_f32(w, J: int) -> np.ndarray:
@@ -102,8 +107,9 @@ def _flags(integer_starts: bool, reduced: bool, objective: str = "makespan") -> 
 
 
 def _require_due(due, objective: str):
-    """The tardiness objectives, the late counts and the maximum lateness score against the due dates of set_due:
-    refuse them, before any device call, on an engine that has none (set_table clears them)."""
+    """The tardiness objectives (the maximum tardiness among them), the late counts and the maximum lateness score
+    against the due dates of set_due: refuse them, before any device call, on an engine that has none (set_table
+    clears them)."""
     if (objective.endswith("tardiness") or objective.endswith("late_tasks") or objective == "max_lateness") and \
             due is None:
         from .solver import SolverError
@@ -203,7 +209,8 @@ class Engine:
         scores sum_j max(0, start_j + rt_j - d_j), and "weighted_tardiness" (each term times the set_weights
         weight), and "max_lateness", which scores max_j (start_j + rt_j + q_j) with the tails q_j = D - d_j (fp32),
         D = due_shift = max_j d_j: that is L_max + D >= 0, and subtracting D gives L_max, and "late_tasks" /
-        "weighted_late_tasks", which count (or weigh) the jobs with start_j + rt_j > d_j.  None clears them; set_table
+        "weighted_late_tasks", which count (or weigh) the jobs with start_j + rt_j > d_j, and "max_tardiness" /
+        "weighted_max_tardiness", which score max_j w_j max(0, start_j + rt_j - d_j).  None clears them; set_table
         clears them too."""
         if d is None:
             check(self._lib.sb_set_due(self._h, None, 0))

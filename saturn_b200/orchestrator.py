@@ -59,7 +59,9 @@ def orchestrate(task_list, log=False, interval=1000, gurobi=True, *,
     {t: d - n * interval}, and the lateness each solve reports is against the original due dates (both sides shift
     alike).  A sequence `due` raises SolverError, since the task list shrinks from interval to interval.  A `release`
     mapping Task -> release date is shifted the same way, {t: r - n * interval}; a sequence `release` raises
-    SolverError.
+    SolverError.  Under objective="max_stretch" the shifted release dates are what each solve measures stretch
+    from, and each interval's fastest runtime p*_t comes from the runtimes `forecast` has shrunk: each solve
+    minimises the stretch of the work that remains, not of the whole task.
     """
     logging.basicConfig(level=logging.INFO if log else logging.WARNING,
                         format="%(asctime)s %(levelname)-8s %(message)s", datefmt="%Y-%m-%d %H:%M:%S")

@@ -61,7 +61,9 @@ def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objecti
     maximum lateness on one machine).  With the fp32 `release` dates (any objective) each order is then re-sorted stably by ascending
     release date (ceiled when `integer_starts`, as the device schedules them), so jobs released together keep the
     objective's order.  objective="late_tasks" / "weighted_late_tasks": the EDD orders of "tardiness" /
-    "weighted_tardiness", each repaired by Moore-Hodgson's rule after the node fill (moore_hodgson)."""
+    "weighted_tardiness", each repaired by Moore-Hodgson's rule after the node fill (moore_hodgson).
+    objective="max_tardiness" / "weighted_max_tardiness": the EDD orders of "tardiness" / "weighted_tardiness"
+    unchanged."""
     objective_flag(objective)
     if objective.startswith("weighted_"):
         if weights is None:
@@ -91,7 +93,7 @@ def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objecti
         col = np.argmin(cost, axis=1)
         rt = usable[np.arange(J), col]
         if edd:
-            weighted = objective in ("weighted_tardiness", "weighted_late_tasks")
+            weighted = objective in ("weighted_tardiness", "weighted_late_tasks", "weighted_max_tardiness")
             tie = rt.astype(np.float64) / w64 if weighted else rt.astype(np.float64)
             order = np.lexsort((np.arange(J), tie, d32))
         elif objective == "weighted_completion":
@@ -183,7 +185,8 @@ def run_search(engine: Engine, chains: int = 1 << 16, rounds: int = 200, seed: i
     objective="max_lateness" minimises the maximum lateness against the engine's set_due; every score holds
     L_max + engine.due_shift, and there is no stop at zero (L_max has no floor).  objective="late_tasks" /
     "weighted_late_tasks" minimises the (weighted) number of tasks that complete after their due date, and stops at
-    0 like the tardiness.
+    0 like the tardiness.  objective="max_tardiness" / "weighted_max_tardiness" minimises the largest (weighted)
+    tardiness, and stops at 0 like the tardiness.
 
     `rounds` device rounds are issued in groups of `exchange_every` (tournament resampling every
     `resample_every` rounds inside a group is only another launch); after each group the ranks exchange

@@ -224,9 +224,9 @@ def _check_horizon(T, found_makespan=None, release=None, tails=None):
                           "options" % lower)
 
 def _check_objective(objective, hysteresis=False, release=None):
-    if objective not in ("makespan", "completion", "tardiness", "max_lateness", "late_tasks"):
-        raise SolverError("objective must be 'makespan', 'completion', 'tardiness', 'max_lateness' or 'late_tasks', "
-                          "not %r" % (objective,))
+    if objective not in ("makespan", "completion", "tardiness", "max_lateness", "late_tasks", "max_stretch"):
+        raise SolverError("objective must be 'makespan', 'completion', 'tardiness', 'max_lateness', 'late_tasks' or "
+                          "'max_stretch', not %r" % (objective,))
     if objective != "makespan" and hysteresis:
         raise SolverError("hysteresis=True compares plans by makespan (milp.py:363-442); it is not defined for "
                           "objective=%r" % (objective,))
@@ -256,6 +256,9 @@ def _resolve_weights(weights, objective, J, task_list=None):
     Raises SolverError before any device call."""
     if weights is None:
         return None, None
+    if objective == "max_stretch":
+        raise SolverError("objective='max_stretch' weighs every task by 1 / its fastest runtime: it takes no weights "
+                          "(for a weighted mean stretch use objective='completion' with weights)")
     if objective not in ("completion", "tardiness", "late_tasks"):
         raise SolverError("weights apply to objective='completion', 'tardiness' or 'late_tasks' only, not to %r"
                           % (objective,))
@@ -269,6 +272,9 @@ def _resolve_due(due, objective, J, task_list=None):
     """The caller's per-task due dates as (float64 values in task order, fp32 array for the device), or (None, None)
     without objective="tardiness", "max_lateness" or "late_tasks", which require them.  Raises SolverError before
     any device call."""
+    if objective == "max_stretch" and due is not None:
+        raise SolverError("objective='max_stretch' measures every task from its release date: it takes no due dates "
+                          "(pass release=...)")
     if objective not in ("tardiness", "max_lateness", "late_tasks"):
         if due is not None:
             raise SolverError("due dates apply to objective='tardiness', 'max_lateness' or 'late_tasks' only, not to %r"
@@ -308,6 +314,8 @@ def _set_objective(eng, objective, w32, d32, r32=None):
             return objective
         if objective == "late_tasks":
             return "weighted_late_tasks" if w32 is not None else "late_tasks"
+        if objective == "max_stretch":
+            return "weighted_max_tardiness"
         return "weighted_tardiness" if w32 is not None else "tardiness"
     return "weighted_completion" if w32 is not None else objective
 
@@ -332,6 +340,36 @@ def _lateness_stats(start, rts, d64):
     """max_lateness, max_t (C_t - d_t), and late_tasks of a plan, in float64."""
     late = [float(s) + float(r) - d for s, r, d in zip(start, rts, d64)]
     return {"max_lateness": max(late), "late_tasks": sum(1 for x in late if x > 0)}
+
+
+def _stretch_form(Tdev, r32):
+    """objective="max_stretch" as the weighted maximum tardiness: per task its fastest runtime p*_t, the smallest
+    finite cell of the device table Tdev (the cells the search may propose; a task whose only cells are sentinels
+    keeps the sentinel's value, the cell the search uses for it), the fp32 weights fp32(1 / p*_t) (the reciprocal
+    in float64) and the fp32 due dates max(r32_t, +0) (+0 without release dates).  Raises SolverError, before any
+    device call, when a p*_t is 0 (its stretch is undefined) or fp32(1 / p*_t) * 2^24 overflows fp32."""
+    J = Tdev.shape[0]
+    pstar = np.where(np.isfinite(Tdev), Tdev, np.inf).reshape(J, -1).min(axis=1).astype(np.float64)
+    if not np.isfinite(pstar).all():
+        raise SolverError("objective='max_stretch' needs a finite runtime for every task")
+    if (pstar == 0).any():
+        raise SolverError("objective='max_stretch' is undefined for a task whose fastest runtime is 0 (task %d)"
+                          % int(np.argmax(pstar == 0)))
+    with np.errstate(over="ignore"):
+        w32 = (1.0 / pstar).astype(np.float32)
+        scaled = w32 * np.float32(FP32_EXACT_HORIZON)
+    if not np.isfinite(scaled).all():
+        raise SolverError("objective='max_stretch': 1 / the fastest runtime of task %d overflows fp32 over a 2^24 "
+                          "horizon; express runtimes in finer units" % int(np.argmax(~np.isfinite(scaled))))
+    d32 = np.zeros(J, dtype=np.float32) if r32 is None else np.where(r32 > 0, r32, np.float32(0)).astype(np.float32)
+    return pstar, w32, d32
+
+
+def _stretch_stats(start, rts, pstar, r64):
+    """max_stretch and mean_stretch of a plan, (C_t - max(r_t, 0)) / p*_t in float64 (r_t = 0 without r64)."""
+    r = r64 if r64 is not None else [0.0] * len(rts)
+    st = [(float(s) + float(rt) - max(x, 0.0)) / float(p) for s, rt, x, p in zip(start, rts, r, pstar)]
+    return {"max_stretch": max(st), "mean_stretch": sum(st) / len(st)}
 
 
 def _tails(d32):
@@ -419,6 +457,19 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     the weight of the late tasks; last_stats["device_makespan"] holds the device's fp32 score.  The 6th element
     stays the plan's makespan.
 
+    Maximum stretch.  objective="max_stretch" minimises max_t S_t, the stretch (slowdown) of each task: its time from
+    release to result divided by the time it would take with the cluster to itself, S_t = (C_t - max(r_t, 0)) /
+    p*_t, where p*_t is the task's fastest runtime over the options the search may propose (its sentinel options
+    only when it has nothing else, and then the sentinel's value).  It keeps every task's wait in proportion to its
+    size, where "completion" favours short tasks and "makespan" lets a short task wait behind a long one.  It runs
+    as the weighted maximum tardiness with w_t = fp32(1 / p*_t) (the reciprocal taken in float64) and due dates
+    max(r_t, 0) in fp32 (0 without `release`); `release` is valid, `weights`, `due` and hysteresis=True raise
+    SolverError, as does a task whose p*_t is 0 or whose fp32(1 / p*_t) * 2^24 overflows fp32, all before any device
+    call.  last_stats["max_stretch"] and last_stats["mean_stretch"] are recomputed in float64 from the emitted plan, the
+    tasks' own runtimes (p*_t over the same options) and the caller's r; last_stats["device_makespan"] holds the
+    device's fp32 max stretch.  The 6th element stays the plan's makespan.  The mean stretch needs no objective of
+    its own: objective="completion" with weights={t: 1 / p*_t} minimises sum_t (C_t - r_t) / p*_t up to a constant.
+
     Release dates.  `release` (a sequence aligned with task_list, or a mapping keyed by Task, in the runtimes' units
     from the plan's t = 0) keeps every task from starting before its release date, under every objective: a
     dataset or a parent checkpoint that is only ready later, a job that arrives tomorrow.  r <= 0 means already
@@ -471,6 +522,11 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
         if usable[j].any():
             Tdev[j, 0, ~usable[j]] = np.inf
     _check_horizon(Tdev, release=r64, tails=_tails(d32) if objective == "max_lateness" else None)
+    if objective == "max_stretch":
+        _, w32, d32 = _stretch_form(Tdev, r32)
+        # p*_t in the tasks' own runtimes: the fastest option among the cells the device table keeps
+        pstar = [min(float(list(t.strategies.values())[int(optindex[j, g])].runtime)
+                     for g in range(NSLOT) if np.isfinite(Tdev[j, 0, g])) for j, t in enumerate(task_list)]
     if nodes is None:
         nodes = _default_nodes()
     nodes = int(nodes)
@@ -525,6 +581,8 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
         last_stats["device_makespan"] = res.makespan - eng.due_shift
     elif objective == "late_tasks":
         last_stats.update(_late_count_stats(dec["start"], rts, w64, d64))
+    elif objective == "max_stretch":
+        last_stats.update(_stretch_stats(dec["start"], rts, pstar, r64))
     elif d64 is not None:
         last_stats.update(_tardiness_stats(dec["start"], rts, w64, d64))
     if r64 is not None:
@@ -630,7 +688,9 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     a sequence aligned with T's rows (the weighted sum of completion times, last_stats["weighted_completion"]);
     `due` as for solve() with objective="tardiness", "max_lateness" or "late_tasks" (last_stats as there), a sequence
     aligned with T's rows; `release` as for solve(), under every objective, a sequence aligned with T's rows
-    (last_stats["total_flow_time"]).  Every cell of T must be
+    (last_stats["total_flow_time"]).  objective="max_stretch" as for solve(), with p*_t the smallest cell of row t
+    the search may propose, over every strategy (last_stats["max_stretch"] and ["mean_stretch"] from T's values).
+    Every cell of T must be
     >= 0 (-0.0 counts as zero), +inf or a sentinel: a negative or NaN cell raises SolverError, with or without `mask`.
 
     The table goes to the device un-reduced (sb_set_table: min over strategies with the first-minimum rule
@@ -666,6 +726,8 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     if not np.isfinite(Tdev.reshape(J, -1)).any(axis=1).all():
         raise SolverError("a task has no finite cell in T")
     _check_horizon(Tdev, release=r64, tails=_tails(d32) if objective == "max_lateness" else None)
+    if objective == "max_stretch":
+        pstar, w32, d32 = _stretch_form(Tdev, r32)
     eng = engine if engine is not None else _engine(devices)
     nodes = int(_default_nodes() if nodes is None else nodes)
     eng.set_table(Tdev, gcount, sentinel=float("inf"), nodes=nodes)
@@ -712,6 +774,8 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
         last_stats["device_makespan"] = res.makespan - eng.due_shift
     elif objective == "late_tasks":
         last_stats.update(_late_count_stats(dec["start"], rts, w64, d64))
+    elif objective == "max_stretch":
+        last_stats.update(_stretch_stats(dec["start"], rts, pstar, r64))
     elif d64 is not None:
         last_stats.update(_tardiness_stats(dec["start"], rts, w64, d64))
     if r64 is not None:

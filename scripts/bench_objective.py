@@ -1,15 +1,18 @@
 """Cost and effect of the sum-of-completion-times objectives (plain and weighted), of the weighted tardiness, of the
-maximum lateness, of the (weighted) number of late tasks and of release dates on one GPU; prints one JSON line.
+maximum lateness, of the (weighted) number of late tasks, of the maximum stretch and of release dates on one GPU;
+prints one JSON line.
 
     python scripts/bench_objective.py [--steps 200] [--warmup 20] [--solve-chains 0] [--solve-rounds 400]
+                                      [--only max_stretch]
 
 kernel: sb_eval on bench.py's C4 batch (J = 256, S = 8, 946,176 candidates, the same seeded inputs, integer
         starts), scored for the makespan, the sum of completion times, the weighted sum (seeded weights) and the
         weighted tardiness (the same weights, seeded due dates), and the release twins of the makespan and the
         weighted tardiness (seeded integer release dates in [0, 20000) s, SB_FLAG_RELEASE, a second handle on the
         same device), the maximum lateness (the tail makespan over the same due dates) and the weighted late count
-        (the same weights and due dates), the eight launches alternated in one process (the order rotates every
-        step) and timed with CUDA events; median of --steps launches each.
+        (the same weights and due dates) and the weighted maximum tardiness (the same weights and due dates), the
+        nine launches alternated in one process (the order rotates every step) and timed with CUDA events; median
+        of --steps launches each.
 solve:  solve() wall time on a 256-task set (synthetic table, seed 3, 4 strategies) for the makespan, the sum of
         completion times and the weighted sum (seeded weights: 32 tasks of weight 8, the rest 1), each plan scored
         on all three measures (float64, the tasks' own runtimes); and the total tardiness (unit weights, seeded
@@ -23,6 +26,11 @@ release: the same 256-task set with seeded release dates in [0, 0.5 x the makesp
         (makespan, completion, tardiness) the release-aware plan (solve(release=...)) against the release-blind plan
         (solve() without them, its options and list order rescored under the release rule), on makespan, total flow
         time sum_t (C_t - max(r_t, 0)) and, for the tardiness objective, the tardiness; all in float64.
+stretch: the same 256-task set and release dates: solve(objective="max_stretch") against the completion, makespan
+        and completion-with-w = 1 / p* plans (all release-aware), each rescored in float64 on max stretch, mean
+        stretch and makespan (stretch (C_t - max(r_t, 0)) / p*_t, p*_t the task's fastest proposable runtime).
+--only max_stretch times only the weighted tardiness and the weighted maximum tardiness and runs only the stretch
+comparison.
 The card's name and power limit are read in the same run (nvidia-smi, read-only queries).
 """
 import argparse
@@ -54,6 +62,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--solve-chains", type=int, default=0, help="0 = solve()'s default population")
     ap.add_argument("--solve-rounds", type=int, default=400)
+    ap.add_argument("--only", choices=("all", "max_stretch"), default="all")
     args = ap.parse_args()
     import numpy as np
     import torch
@@ -78,7 +87,9 @@ def main():
     out = torch.empty(B, dtype=torch.float32, device=eng.device)
     key = torch.full((1,), 2 ** 63 - 1, dtype=torch.int64, device=eng.device)
     objs = ("makespan", "completion", "weighted_completion", "weighted_tardiness", "release_makespan",
-            "release_weighted_tardiness", "max_lateness", "weighted_late_tasks")
+            "release_weighted_tardiness", "max_lateness", "weighted_late_tasks", "weighted_max_tardiness")
+    if args.only == "max_stretch":
+        objs = ("weighted_tardiness", "weighted_max_tardiness")
     times = {o: [] for o in objs}
     for i in range(args.warmup + args.steps):
         for obj in objs[i % len(objs):] + objs[:i % len(objs)]:
@@ -91,10 +102,24 @@ def main():
             if i >= args.warmup:
                 times[obj].append(a.elapsed_time(b))
     path = eng.last_eval_path()
-    assert eng_r.last_eval_path() == path
+    assert args.only != "all" or eng_r.last_eval_path() == path
     kernel = {o: {"median_ms": float(np.median(t)), "p10_ms": float(np.percentile(t, 10)),
                   "p90_ms": float(np.percentile(t, 90)), "candidates_per_s": B / (float(np.median(t)) * 1e-3)}
               for o, t in times.items()}
+    kernel["max_tardiness_over_weighted_tardiness"] = (kernel["weighted_max_tardiness"]["median_ms"] /
+                                                       kernel["weighted_tardiness"]["median_ms"])
+    if args.only == "max_stretch":
+        kernel.update(B=B, J=J, S=Sx, path=path, steps=args.steps)
+        del opt, prio, out
+        eng_r.close()
+        torch.cuda.empty_cache()
+        tasks = _tasks256()
+        kw = dict(rounds=args.solve_rounds, seed=1, engine=eng, **({"chains": args.solve_chains}
+                                                                   if args.solve_chains else {}))
+        makespan = S.solve(tasks, None, **kw)[5]
+        print(json.dumps({"card": card(0), "kernel": kernel, "stretch": stretch_effect(S, R, tasks, makespan, kw)}))
+        eng.close()
+        return
     kernel["completion_over_makespan"] = kernel["completion"]["median_ms"] / kernel["makespan"]["median_ms"]
     kernel["weighted_over_completion"] = kernel["weighted_completion"]["median_ms"] / kernel["completion"]["median_ms"]
     kernel["tardiness_over_weighted"] = kernel["weighted_tardiness"]["median_ms"] / kernel["weighted_completion"]["median_ms"]
@@ -109,18 +134,7 @@ def main():
     eng_r.close()
     torch.cuda.empty_cache()
 
-    from saturn_b200.solver import strategies_from_table
-
-    class _Task:
-        def __init__(self, name, strategies):
-            self.name, self.strategies, self.selected_strategy = name, strategies, None
-
-        def select_strategy(self, s):
-            self.selected_strategy = s
-
-    T2, valid2 = synth_table(256, 4, 8, seed=3)
-    strategies = strategies_from_table(T2, valid2)
-    tasks = [_Task("t%d" % j, strategies[j]) for j in range(256)]
+    tasks = _tasks256()
     kw = dict(rounds=args.solve_rounds, seed=1, engine=eng)
     if args.solve_chains:
         kw["chains"] = args.solve_chains
@@ -157,8 +171,53 @@ def main():
                        "rounds": st["rounds"], "candidates": st["candidates"]}
     late_unit = late_unit_effect(S, R, tasks, due, w, kw)
     print(json.dumps({"card": card(0), "kernel": kernel, "solve": solve, "late_unit": late_unit,
-                      "release": release_effect(S, R, tasks, due, solve["makespan"]["makespan"], kw)}))
+                      "release": release_effect(S, R, tasks, due, solve["makespan"]["makespan"], kw),
+                      "stretch": stretch_effect(S, R, tasks, solve["makespan"]["makespan"], kw)}))
     eng.close()
+
+
+class _Task:
+    def __init__(self, name, strategies):
+        self.name, self.strategies, self.selected_strategy = name, strategies, None
+
+    def select_strategy(self, s):
+        self.selected_strategy = s
+
+
+def _tasks256():
+    """The 256-task set of the solve measurements: synthetic table, seed 3, 4 strategies."""
+    from saturn_b200.solver import strategies_from_table
+    from saturn_b200.synth import synth_table
+    T2, valid2 = synth_table(256, 4, 8, seed=3)
+    strategies = strategies_from_table(T2, valid2)
+    return [_Task("t%d" % j, strategies[j]) for j in range(256)]
+
+
+def stretch_effect(S, R, tasks, makespan, kw):
+    """The max-stretch plan against the completion, makespan and completion-with-w = 1 / p* plans on the 256-task set
+    with the release dates of release_effect, every plan rescored in float64 (see the module doc)."""
+    import numpy as np
+    J = len(tasks)
+    tuples = [[(g, s.runtime) for g, s in t.strategies.items()] for t in tasks]
+    r = [float(x) for x in np.random.default_rng(6).integers(0, int(0.5 * makespan), size=J)]
+    # p*_t: the fastest of the task's own runtimes over the options solve() lets the search propose
+    T, usable, optindex = S.build_table(tasks)
+    pstar = []
+    for j, t in enumerate(tasks):
+        cells = [g for g in range(8) if np.isfinite(T[j, 0, g]) and (usable[j, g] or not usable[j].any())]
+        pstar.append(min(float(list(t.strategies.values())[int(optindex[j, g])].runtime) for g in cells))
+    out = {}
+    for name, obj, weights in (("max_stretch", "max_stretch", None), ("completion", "completion", None),
+                               ("makespan", "makespan", None),
+                               ("completion_w_inv_pstar", "completion", [1.0 / p for p in pstar])):
+        t0 = time.perf_counter()
+        res = S.solve(tasks, None, objective=obj, weights=weights, release=r, **kw)
+        wall = time.perf_counter() - t0
+        comp = [p[0] + p[2] for p in R.plan_from_arrays(tuples, res[0], res[1], res[2], res[3])]
+        st = [(c - max(x, 0.0)) / p for c, x, p in zip(comp, r, pstar)]
+        out[name] = {"max_stretch": max(st), "mean_stretch": sum(st) / J, "makespan": max(comp), "wall_s": wall,
+                     "rounds": S.last_stats["rounds"]}
+    return out
 
 
 def late_unit_effect(S, R, tasks, due, w, kw):

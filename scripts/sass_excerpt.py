@@ -78,6 +78,7 @@ def main():
             ("_ZN2sb12k_eval_tilesILi1ELb1ELb1ELb0ELb0ELb0ELi1ELb1ELb1ELi0ELb0EEEvNS_8TileArgsE", "the same kernel scoring the weighted sum of completion times (SB_FLAG_WEIGHTED): one more gather (IMAD + LDS) and one FMUL per step", 32),
             ("_ZN2sb12k_eval_tilesILi1ELb1ELb1ELb0ELb0ELb0ELi1ELb1ELb1ELi1ELb0EEEvNS_8TileArgsE", "the same kernel scoring the weighted tardiness (SB_FLAG_DUE): one more gather (IMAD + LDS), one FADD and one FMNMX per step", 32),
             ("_ZN2sb12k_eval_tilesILi1ELb1ELb1ELb0ELb0ELb0ELi1ELb1ELb1ELi2ELb0EEEvNS_8TileArgsE", "the same kernel scoring the weighted number of late tasks (SB_FLAG_DUE | SB_FLAG_LATE_COUNT): w * [e > d] as FSET + FMUL, then the FADD, in place of the tardiness' FADD + FMNMX + FMUL + FADD", 32),
+            ("_ZN2sb12k_eval_tilesILi1ELb1ELb1ELb0ELb0ELb0ELi1ELb1ELb1ELi3ELb0EEEvNS_8TileArgsE", "the same kernel scoring the weighted maximum tardiness (SB_FLAG_DUE | SB_FLAG_MAX_TARDINESS): the product w * (e - d) folded by one VIMNMX, in place of the tardiness' FMNMX + FADD", 32),
             ("_ZN2sb12k_eval_tilesILi1ELb1ELb1ELb0ELb0ELb0ELi1ELb0ELb0ELi0ELb1EEEvNS_8TileArgsE", "the measured kernel with release dates (SB_FLAG_RELEASE): one more gather (IMAD + LDS) and one FMNMX per step", 32),
             ("_ZN2sb12k_eval_tilesILi1ELb1ELb1ELb0ELb0ELb0ELi1ELb1ELb1ELi1ELb1EEEvNS_8TileArgsE", "the weighted-tardiness kernel with release dates (SB_FLAG_DUE | SB_FLAG_RELEASE)", 32),
             ("_ZN2sb12k_eval_tilesILi1ELb1ELb1ELb0ELb0ELb0ELi0ELb0ELb0ELi0ELb0EEEvNS_8TileArgsE", "the same kernel with plain C++ addressing (test hook HOOK_PLAIN_ADDR; the round-1 form)", 32),
