@@ -7,16 +7,20 @@ with `fractions.Fraction` instead of floating point:
     start = max(max(ready[sel]), r_j)            (r_j -> ceil(r_j) with integer starts)
     ready[sel] = start + (integer_starts ? ceil(rt) : rt)
     e = start + rt
-    makespan             mk  = max(mk, e)
-    completion           acc = acc + e
-    weighted_completion  acc = acc + w e
-    (weighted) tardiness acc = acc + w max(e - d, 0)
+    makespan                  mk  = max(mk, e)
+    completion                acc = acc + e
+    weighted_completion       acc = acc + w e
+    (weighted) tardiness      acc = acc + w max(e - d, 0)
+    max_lateness              q = D - d (D = max_t d_t),  acc = max(acc, e + q)   (the device's tail score L_max + D)
+    (weighted) late_tasks     acc = acc + (e > d ? w : 0)
+    (weighted) max_tardiness  acc = max(acc, w max(e - d, 0))
 
 On an input where fp32 rounds nothing, every floating-point restatement (the fp32 and float64 oracles, the
 kernels) must reproduce this value for value.  `schedule(..., exact32=True)` asserts that: every input and every
-intermediate it forms (starts, slot times, completions, e - d, products, partial sums) must be exactly representable
-in fp32, so an input that breaks exactness fails loudly instead of weakening a comparison.  +inf (an absent or
-selected sentinel cell) is carried as float('inf'); it is exact.
+intermediate it forms (starts, slot times, completions, e - d, tails q and e + q, products, partial sums) must be
+exactly representable in fp32, so an input that breaks exactness fails loudly instead of weakening a comparison.
++inf (an absent or selected sentinel cell) is carried as float('inf'); it is exact.  The objectives and their flag
+bits are those of saturn_b200.engine, restated here so that the oracle loads no library.
 """
 from __future__ import annotations
 
@@ -26,8 +30,34 @@ from fractions import Fraction
 import numpy as np
 
 NSLOT = 8
-OBJECTIVES = ("makespan", "completion", "weighted_completion", "tardiness", "weighted_tardiness")
+# saturn_b200.engine.OBJECTIVES, in its order
+OBJECTIVES = ("makespan", "completion", "weighted_completion", "tardiness", "weighted_tardiness", "max_lateness",
+              "late_tasks", "weighted_late_tasks", "max_tardiness", "weighted_max_tardiness")
 INF = float("inf")
+# saturn_b200._lib's flag bits, restated so that the oracle loads no library
+FLAG_SUM_COMPLETION, FLAG_WEIGHTED, FLAG_DUE, FLAG_MAX_LATENESS, FLAG_LATE_COUNT, FLAG_MAX_TARDINESS = (
+    64, 128, 256, 1024, 2048, 4096)
+
+
+def objective_flag(objective):
+    """The SB_FLAG_* objective bits of saturn_b200.engine.objective_flag, restated."""
+    if objective not in OBJECTIVES:
+        raise ValueError("objective must be one of %s, not %r" % (OBJECTIVES, objective))
+    if objective == "makespan":
+        return 0
+    if objective == "max_lateness":
+        return FLAG_MAX_LATENESS
+    late = objective.endswith("late_tasks")
+    return FLAG_SUM_COMPLETION | (FLAG_WEIGHTED if objective.startswith("weighted_") else 0) | (
+        FLAG_DUE if objective.endswith("tardiness") or late else 0) | (FLAG_LATE_COUNT if late else 0) | (
+        FLAG_MAX_TARDINESS if objective.endswith("max_tardiness") else 0)
+
+
+def needs(objective):
+    """(weights, due dates): whether the objective reads per-job weights (SB_FLAG_WEIGHTED) and due dates
+    (SB_FLAG_DUE, or SB_FLAG_MAX_LATENESS for the tails)."""
+    f = objective_flag(objective)
+    return bool(f & FLAG_WEIGHTED), bool(f & (FLAG_DUE | FLAG_MAX_LATENESS))
 
 
 class NotExact(AssertionError):
@@ -59,22 +89,24 @@ def schedule(tab, opt, prio, release=None, integer_starts=True, nodes=1, objecti
     """One candidate.  tab[J][S][8] (S = 1 when nodes > 1), opt[J] bytes, prio[J] the schedule order; release,
     weights and due are J values or None (no release dates; unit weights; no due dates).  Returns (score, start[J],
     mask[J]) with Fractions (or +inf), mask[j] = (node << 16) | slot bits when nodes > 1."""
-    if objective not in OBJECTIVES:
-        raise ValueError("objective must be one of %s" % (OBJECTIVES,))
+    _, use_due = needs(objective)
+    f = objective_flag(objective)
     J = len(prio)
     chk = _check if exact32 else (lambda x, what: x)
     r = [Fraction(0)] * J if release is None else [_q(x) for x in release]
     if integer_starts:
         r = [_ceil(x) for x in r]
     w = [Fraction(1)] * J if weights is None else [_q(x) for x in weights]
-    tardy = objective.endswith("tardiness")
-    if tardy and due is None:
+    if use_due and due is None:
         raise ValueError("objective=%r needs due dates" % objective)
-    d = [_q(x) for x in due] if tardy else [Fraction(0)] * J
+    d = [_q(x) for x in due] if use_due else [Fraction(0)] * J
     for j in range(J):
         chk(r[j], "release[%d]" % j)
         chk(w[j], "weight[%d]" % j)
         chk(d[j], "due[%d]" % j)
+    if f & FLAG_MAX_LATENESS:                         # the delivery tails take the due dates' place
+        D = max(d)
+        d = [chk(D - x, "tail q[%d]" % j) for j, x in enumerate(d)]
     ready = [[Fraction(0)] * NSLOT for _ in range(nodes)]
     start = [Fraction(0)] * J
     mask = [0] * J
@@ -100,13 +132,16 @@ def schedule(tab, opt, prio, release=None, integer_starts=True, nodes=1, objecti
         e = chk(s + rt, "completion[%d]" % j)
         if objective == "makespan":
             acc = max(acc, e)
-        elif objective == "completion":
-            acc = chk(acc + e, "partial sum at job %d" % j)
-        elif objective == "weighted_completion":
-            acc = chk(acc + chk(w[j] * e, "w e of job %d" % j), "partial sum at job %d" % j)
+        elif f & FLAG_MAX_LATENESS:
+            acc = max(acc, chk(e + d[j], "e + q of job %d" % j))
+        elif f & FLAG_LATE_COUNT:
+            acc = INF if e == INF else chk(acc + w[j], "partial sum at job %d" % j) if e > d[j] else acc
+        elif not f & FLAG_DUE:
+            acc = chk(acc + (chk(w[j] * e, "w e of job %d" % j) if f & FLAG_WEIGHTED else e),
+                      "partial sum at job %d" % j)
         else:
-            late = max(chk(e - d[j], "e - d of job %d" % j), Fraction(0))
-            acc = chk(acc + chk(w[j] * late, "w t of job %d" % j), "partial sum at job %d" % j)
+            x = chk(w[j] * max(chk(e - d[j], "e - d of job %d" % j), Fraction(0)), "w t of job %d" % j)
+            acc = max(acc, x) if f & FLAG_MAX_TARDINESS else chk(acc + x, "partial sum at job %d" % j)
     return acc, start, mask
 
 

@@ -37,7 +37,6 @@ import math
 import os
 import subprocess
 import time
-from fractions import Fraction
 from typing import Sequence
 
 import numpy as np
@@ -107,22 +106,11 @@ def evaluate(tab, opt, prio, due, release=None, integer_starts=True, dtype=np.fl
 
 
 def exact(tab, opt, prio, due, release=None, integer_starts=True, nodes=1, weights=None):
-    """sum_j w_j [C_j > d_j] of one candidate in exact arithmetic, the starts from ref_exact.schedule (which asserts
-    that every input and intermediate of the schedule is exact in fp32).  Returns a Fraction (or +inf)."""
-    mk, start, _ = X.schedule(tab, opt, prio, release, integer_starts, nodes)
-    if mk == X.INF:
-        return X.INF
-    J = len(prio)
-    w = [Fraction(1)] * J if weights is None else [Fraction(float(np.float32(x))) for x in weights]
-    total = Fraction(0)
-    for j in range(J):
-        o = int(opt[j])
-        rt = tab[j][0 if nodes > 1 else o >> 3][o & 7]
-        if not np.isfinite(rt):
-            return X.INF
-        if start[j] + Fraction(float(rt)) > Fraction(float(np.float32(due[j]))):
-            total += w[j]
-    return total
+    """sum_j w_j [C_j > d_j] of one candidate in exact arithmetic: ref_exact.schedule's late_tasks fold
+    (weighted_late_tasks with weights), which asserts that every input and intermediate is exact in fp32.  Returns a
+    Fraction (or +inf)."""
+    obj = "late_tasks" if weights is None else "weighted_late_tasks"
+    return X.schedule(tab, opt, prio, release, integer_starts, nodes, obj, weights, due)[0]
 
 
 def brute_force(tab, valid_opts: Sequence[Sequence[int]], due, release=None, integer_starts=True,

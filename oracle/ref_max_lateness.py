@@ -29,7 +29,6 @@ import itertools
 import os
 import subprocess
 import time
-from fractions import Fraction
 from typing import Sequence
 
 import numpy as np
@@ -90,21 +89,10 @@ def evaluate(tab, opt, prio, due, release=None, integer_starts=True, dtype=np.fl
 
 
 def exact(tab, opt, prio, due, release=None, integer_starts=True, nodes=1):
-    """max_j (C_j + (D - d_j)) of one candidate in exact arithmetic, the starts from ref_exact.schedule (which asserts
-    that every input and intermediate of the schedule is exact in fp32).  Returns a Fraction (or +inf)."""
-    mk, start, _ = X.schedule(tab, opt, prio, release, integer_starts, nodes)
-    if mk == X.INF:
-        return X.INF
-    d = [Fraction(float(x)) for x in due]
-    D = max(d)
-    best = Fraction(0)
-    for j in range(len(prio)):
-        o = int(opt[j])
-        rt = tab[j][0 if nodes > 1 else o >> 3][o & 7]
-        if not np.isfinite(rt):
-            return X.INF
-        best = max(best, start[j] + Fraction(float(rt)) + (D - d[j]))
-    return best
+    """max_j (C_j + (D - d_j)) of one candidate in exact arithmetic: ref_exact.schedule's max_lateness fold, which
+    asserts that every input and intermediate (the schedule, the tails and every C + q) is exact in fp32.  Returns a
+    Fraction (or +inf)."""
+    return X.schedule(tab, opt, prio, release, integer_starts, nodes, "max_lateness", due=due)[0]
 
 
 def brute_force(tab, valid_opts: Sequence[Sequence[int]], due, release=None, integer_starts=True,

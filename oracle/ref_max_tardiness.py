@@ -34,7 +34,6 @@ import itertools
 import os
 import subprocess
 import time
-from fractions import Fraction
 from typing import Sequence
 
 import numpy as np
@@ -105,22 +104,11 @@ def evaluate(tab, opt, prio, due, release=None, integer_starts=True, dtype=np.fl
 
 
 def exact(tab, opt, prio, due, release=None, integer_starts=True, nodes=1, weights=None):
-    """max_j w_j max(0, C_j - d_j) of one candidate in exact arithmetic, the starts from ref_exact.schedule (which
-    asserts that every input and intermediate of the schedule is exact in fp32), w and d as their fp32 values.
-    Returns a Fraction (or +inf)."""
-    mk, start, _ = X.schedule(tab, opt, prio, release, integer_starts, nodes)
-    if mk == X.INF:
-        return X.INF
-    J = len(prio)
-    w = [Fraction(1)] * J if weights is None else [Fraction(float(np.float32(x))) for x in weights]
-    best = Fraction(0)
-    for j in range(J):
-        o = int(opt[j])
-        rt = tab[j][0 if nodes > 1 else o >> 3][o & 7]
-        if not np.isfinite(rt):
-            return X.INF
-        best = max(best, w[j] * max(Fraction(0), start[j] + Fraction(float(rt)) - Fraction(float(np.float32(due[j])))))
-    return best
+    """max_j w_j max(0, C_j - d_j) of one candidate in exact arithmetic: ref_exact.schedule's max_tardiness fold
+    (weighted_max_tardiness with weights), which asserts that every input and intermediate is exact in fp32.  Returns
+    a Fraction (or +inf)."""
+    obj = "max_tardiness" if weights is None else "weighted_max_tardiness"
+    return X.schedule(tab, opt, prio, release, integer_starts, nodes, obj, weights, due)[0]
 
 
 def brute_force(tab, valid_opts: Sequence[Sequence[int]], due, release=None, integer_starts=True,

@@ -20,7 +20,9 @@ Every score fold of the other oracles runs on this schedule, step for step as th
 in schedule order from +0, each step rounded on its own.
 
 Also here:
-  * `c_evaluate` — the same schedule and folds in plain C (`oracle/ref_release.c`, a library of its own);
+  * `c_evaluate` — the same schedule and folds in plain C (`oracle/ref_release.c`, a library of its own), and the
+    other five objectives of the library (`C_OBJECTIVES`) through the C ports of ref_max_lateness, ref_late_tasks and
+    ref_max_tardiness;
   * `brute_force` — the exhaustive list-schedule optimum (every option vector and permutation, scored by the C port);
   * `milp_solve` — the MILPs of ref_milp / ref_completion / ref_weighted / ref_tardiness plus
     sta[g][t] - r_t * tga[t][g] >= 0 for every g, with the big-M horizon raised to
@@ -30,6 +32,7 @@ Also here:
 from __future__ import annotations
 
 import ctypes
+import importlib
 import itertools
 import math
 import os
@@ -43,6 +46,10 @@ from . import ref_eval as R
 
 OBJECTIVES = ("makespan", "completion", "weighted_completion", "tardiness", "weighted_tardiness")
 _CODE = {o: i for i, o in enumerate(OBJECTIVES)}
+# the objectives c_evaluate scores through another oracle's C port (ref_release.c folds OBJECTIVES only)
+_PORTS = {"max_lateness": "ref_max_lateness", "late_tasks": "ref_late_tasks", "weighted_late_tasks": "ref_late_tasks",
+          "max_tardiness": "ref_max_tardiness", "weighted_max_tardiness": "ref_max_tardiness"}
+C_OBJECTIVES = OBJECTIVES + tuple(_PORTS)          # every objective c_evaluate accepts, in the library's order
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _SO = os.path.join(_HERE, "libref_release.so")
 _lib = None
@@ -217,7 +224,12 @@ def _load():
 def c_evaluate(tab, opt, prio, release, integer_starts=True, dtype=np.float32, nslot=8, want_plan=False, threads=0,
                nodes=1, objective="makespan", weights=None, due=None):
     """Scores of B candidates in C: tab[J][S][8], opt[B][J] u8, prio[B][J] u8/u16, release[J] -> score[B]
-    (+ start, mask)."""
+    (+ start, mask).  `objective` is any of C_OBJECTIVES."""
+    if objective in _PORTS:
+        port = importlib.import_module("." + _PORTS[objective], __package__)
+        kw = {} if objective == "max_lateness" else {"weights": weights}
+        return port.c_evaluate(tab, opt, prio, due, release, integer_starts, dtype, nslot, want_plan, threads, nodes,
+                               **kw)
     tab = np.ascontiguousarray(tab, dtype=dtype)
     J, S, W = tab.shape
     assert W == 8

@@ -4,19 +4,23 @@ The per-feature suites draw log-uniform non-integer runtimes and uniform random 
 ready times, a release date equal to a slot's ready time, a completion equal to its due date) almost never occur, and
 their references are fp32 restatements of the same arithmetic.  Here:
 
-* `oracle/ref_exact.py` is the list schedule in exact rational arithmetic, under every fold, with and without release
-  dates, on 1..8 nodes.  On the EXACT FAMILIES below fp32 rounds nothing, and the reference asserts that for every
-  value it forms; the CPU tests pin it against the float64 oracle and the fp32 C port, value for value, starts and
-  slot masks included.
+* `oracle/ref_exact.py` is the list schedule in exact rational arithmetic, under every fold of the library (the ten
+  objectives of saturn_b200.engine.OBJECTIVES), with and without release dates, on 1..8 nodes.  On the EXACT
+  FAMILIES below fp32 rounds nothing, and the reference asserts that for every value it forms; the CPU tests pin it
+  against the float64 oracle and the fp32 C port, value for value, starts and slot masks included.
 * Seeded generators make the ties: equal runtimes, runtimes in {1, 2, 3}, dyadic fractions, zeros and -0.0; gang
   patterns of explicit opt rows (every job on 8, on 1, 1 and 8 alternating, k cycling 1..8, every job on 7: all three
   shifter stages); identity, reversed and random orders; release dates equal to exact slot ready times, <= 0 and
-  -0.0; due dates equal to exact completions, negative and beyond every completion; weights in {1/4 .. 4}.
+  -0.0; due dates equal to exact completions, one exact step before them (late by the smallest margin of the
+  family), -0.0 (with zero runtimes: on time), negative and beyond every completion; weights in {1/4 .. 4}, and the
+  same scaled by 2^-140 into the fp32 subnormal range.
 * GPU: a shape sweep (J from 1 to 65535, B around one wave of the tile kernel, 1..8 nodes) runs every route a shape
   admits and checks every score against the fp32 C oracle bit for bit, the arg-min key, and on the exact families the
   exact reference's scores, starts and masks.  The kernel path of every run is recorded, and the last test asserts
-  that every path occurred.  Inputs that are not exact families (runtimes in [2^22, 2^23], r = 2^24 - 1, selected
-  1e8 and +inf cells) are checked against the fp32 oracle only.
+  that every path occurred, under every fold.  Inputs that are not exact families (runtimes in [2^22, 2^23],
+  r = 2^24 - 1, selected 1e8 and +inf cells, a due-date spread of 2^24 - 1 under the maximum lateness, late-count due
+  dates at the fp32 neighbours of rounded completions, the maximum stretch's weights fp32(1 / p*)) are checked against
+  the fp32 oracle only.
 * GPU: short searches on tie-heavy exact tables with the incremental-score verifier.
 * The table refusal: negative and NaN cells are refused by sb_set_table (host or device T) and by solve_table.
 """
@@ -26,9 +30,14 @@ import numpy as np
 import pytest
 
 from oracle import ref_exact as X
+from oracle import ref_late_tasks as LT
+from oracle import ref_max_lateness as ML
+from oracle import ref_max_tardiness as MT
 from oracle import ref_release as RR
+from saturn_b200.engine import OBJECTIVES
 
-FOLDS = X.OBJECTIVES
+FOLDS = OBJECTIVES
+NEW_FOLDS = FOLDS[5:]                # the folds of other oracles than ref_release's list schedule
 GANGS = ("k8", "k1", "alt18", "cycle", "k7")
 ORDERS = ("identity", "reversed", "random")
 WEIGHTS = np.array([0.25, 0.5, 1.0, 2.0, 4.0])
@@ -40,8 +49,8 @@ ID_BASE = 7
 def rt_table(family, J, S, seed):
     """T[J][S][8] fp32 with one column per GPU count (gcount = 1..8, so it is already the canonical table).
     Exact families: "equal" (every cell 2.5), "small" ({1, 2, 3}), "dyadic" (multiples of 1/8 in (0, 2]), "zeros" (0,
-    -0.0, 1 and 2).  fp32-only families: "large" (values in [2^22, 2^23]), "sentinel" ({1, 2, 3} with 1e8 and +inf
-    cells)."""
+    -0.0, 1 and 2).  fp32-only families: "large" (values in [2^22, 2^23]), "mid" (values in [2^16, 2^17]: sums of up
+    to 128 stay below 2^24 and round), "sentinel" ({1, 2, 3} with 1e8 and +inf cells)."""
     rng = np.random.default_rng(seed)
     shape = (J, S, 8)
     if family == "equal":
@@ -54,6 +63,8 @@ def rt_table(family, J, S, seed):
         a = np.array([0.0, -0.0, 1.0, 2.0])[rng.integers(0, 4, shape)]
     elif family == "large":
         a = rng.uniform(2.0 ** 22, 2.0 ** 23, shape)
+    elif family == "mid":
+        a = rng.uniform(2.0 ** 16, 2.0 ** 17, shape)
     elif family == "sentinel":
         a = rng.integers(1, 4, shape).astype(np.float64)
         pick = rng.uniform(size=shape)
@@ -112,26 +123,30 @@ def release_dates(family, tab, opt, prio, ints, nodes, seed):
 
 
 def due_dates(tab, opt, prio, ints, nodes, release, seed):
-    """Per job one of: the exact completion of candidate 0 (e - d = 0 there), a negative multiple of 1/8 (a negative
-    integer above J = 300, where sums of tardiness need the whole fp32 mantissa), or 2^19 (beyond every completion of
-    these tables)."""
+    """Per job one of: the exact completion e of candidate 0 (e - d = 0 there: on time), e minus one step of the
+    family (1/8, or 1 above J = 300: late by the smallest exact margin), -0.0 (a zero-runtime job at +0 is on time), a
+    negative multiple of 1/8 (a negative integer above J = 300, where sums of tardiness need the whole fp32 mantissa),
+    or 2^19 (beyond every completion of these tables)."""
     J = len(prio[0])
     rng = np.random.default_rng(seed)
     _, st, _ = X.schedule(tab, opt[0], prio[0], release, ints, nodes)
     e = np.array([float(st[j]) + float(tab[j][0 if nodes > 1 else opt[0][j] >> 3][opt[0][j] & 7]) for j in range(J)])
-    pick = rng.integers(0, 3, J)
+    pick = rng.integers(0, 5, J)
+    step = 0.125 if J <= 300 else 1.0
     neg = -rng.integers(1, 64, J) / 8.0 if J <= 300 else -rng.integers(1, 8, J).astype(np.float64)
-    d = np.where(pick == 0, e, np.where(pick == 1, neg, 2.0 ** 19))
+    d = np.select([pick == 0, pick == 1, pick == 2, pick == 3], [e, e - step, np.full(J, -0.0), neg], 2.0 ** 19)
     return d.astype(np.float32)
 
 
-def per_job(fold, tab, opt, prio, ints, nodes, release, seed):
+def per_job(fold, tab, opt, prio, ints, nodes, release, seed, tiny=False):
     """Weights in {1/4, 1/2, 1, 2, 4} ({1, 2, 4} above J = 300, where sums of weighted completions need the whole
-    fp32 mantissa) and due_dates(), as the fold needs them."""
+    fp32 mantissa), scaled by 2^-140 (fp32 subnormals) with `tiny`, and due_dates(), as the fold's flag bits need
+    them."""
     J = len(prio[0])
-    w = WEIGHTS[np.random.default_rng(seed).integers(0 if J <= 300 else 2, 5, J)].astype(np.float32) \
-        if fold.startswith("weighted") else None
-    d = due_dates(tab, opt, prio, ints, nodes, release, seed + 1) if fold.endswith("tardiness") else None
+    use_w, use_d = X.needs(fold)
+    w = (WEIGHTS[np.random.default_rng(seed).integers(0 if J <= 300 else 2, 5, J)] * (2.0 ** -140 if tiny else 1.0)
+         ).astype(np.float32) if use_w else None
+    d = due_dates(tab, opt, prio, ints, nodes, release, seed + 1) if use_d else None
     return w, d
 
 
@@ -140,6 +155,21 @@ def c_ref(tab, opt, prio, release, ints, nodes, fold, w, d, want_plan=False):
     r = np.zeros(J, np.float32) if release is None else release
     return RR.c_evaluate(tab, opt, prio, r, ints, np.float32, threads=8, nodes=nodes, objective=fold, weights=w,
                          due=d, want_plan=want_plan)
+
+
+def f64_ref(tab, opt, prio, release, ints, nodes, fold, w, d):
+    """(score[B], start[B][J], mask[B][J]) of the float64 restatement: ref_release's Python list schedule, or the
+    fold's own oracle (use_c=False) for the folds ref_release does not know."""
+    if fold in NEW_FOLDS:
+        mod = {"max_lateness": ML, "late_tasks": LT, "weighted_late_tasks": LT, "max_tardiness": MT,
+               "weighted_max_tardiness": MT}[fold]
+        kw = {} if mod is ML else {"weights": w}
+        return mod.evaluate(tab, opt, prio, d, release, ints, np.float64, nodes, use_c=False, want_plan=True, **kw)
+    r64 = np.zeros(opt.shape[1]) if release is None else release
+    out = [RR.list_schedule(tab, opt[b], prio[b], r64, ints, np.float64, nodes=nodes, objective=fold, weights=w, due=d)
+           for b in range(len(opt))]
+    return (np.array([o[0] for o in out]), np.array([o[1] for o in out], np.float64),
+            np.array([o[2] for o in out], np.uint32))
 
 
 # --------------------------------------------------------------------------- CPU: pin the exact reference
@@ -153,23 +183,41 @@ PIN_CASES = [(1, 1, "equal", True), (2, 8, "zeros", False), (7, 3, "small", True
 @pytest.mark.parametrize("fold", FOLDS)
 def test_exact_reference_agrees_with_both_oracles(case, rel, fold):
     """On exact-family inputs the exact reference, the float64 oracle and the fp32 C port agree value for value on the
-    score, every start and every slot mask (15 candidates: every gang pattern under every order)."""
+    score, every start and every slot mask (15 candidates: every gang pattern under every order); weights are
+    subnormal with the non-positive release dates."""
     J, nodes, fam, ints = case
     S = 1 if nodes > 1 else 3
     seed = J * 101 + nodes
     tab = rt_table(fam, J, S, seed)
     opt, prio = candidates(J, 15, nodes if nodes > 1 else S, seed + 1)
     r = release_dates(rel, tab, opt, prio, ints, nodes, seed + 2)
-    w, d = per_job(fold, tab, opt, prio, ints, nodes, r, seed + 3)
+    w, d = per_job(fold, tab, opt, prio, ints, nodes, r, seed + 3, tiny=rel == "nonpos")
     exact, xst, xm = X.batch(tab, opt, prio, r, ints, nodes, fold, w, d)
     c32, cst, cm = c_ref(tab, opt, prio, r, ints, nodes, fold, w, d, want_plan=True)
-    r64 = np.zeros(J) if r is None else r
+    s64, st64, m64 = f64_ref(tab, opt, prio, r, ints, nodes, fold, w, d)
     for b in range(len(opt)):
-        s64, st64, m64, _ = RR.list_schedule(tab, opt[b], prio[b], r64, ints, np.float64, nodes=nodes, objective=fold,
-                                             weights=w, due=d)
-        assert exact[b] == s64 == float(c32[b]), (b, exact[b], s64, c32[b])
-        assert np.array_equal(xst[b], np.asarray(st64, np.float64)) and np.array_equal(xst[b], cst[b].astype(np.float64))
-        assert np.array_equal(xm[b], np.asarray(m64, np.uint32)) and np.array_equal(xm[b], cm[b])
+        assert exact[b] == s64[b] == float(c32[b]), (b, exact[b], s64[b], c32[b])
+        assert np.array_equal(xst[b], st64[b]) and np.array_equal(xst[b], cst[b].astype(np.float64))
+        assert np.array_equal(xm[b], m64[b]) and np.array_equal(xm[b], cm[b])
+
+
+def test_every_objective_has_both_references_and_every_sweep():
+    """The objectives of the library, ref_exact's folds, the objectives ref_release.c_evaluate scores and the folds of
+    the three sweeps (this file, test_gpu_search_state's cases, test_gpu_strategy_axis's tile sweep) are the same
+    list: an objective cannot be added without joining them.  Both references agree on a small input under each, with
+    the library's flag bits."""
+    import test_gpu_search_state as SS
+    import test_gpu_strategy_axis as SA
+    from saturn_b200.engine import objective_flag
+    assert X.OBJECTIVES == RR.C_OBJECTIVES == FOLDS == SA.FOLDS == OBJECTIVES
+    assert {c["objective"] for c in SS.CASES} == set(OBJECTIVES)
+    tab = np.array([[[1.0, 0.5] + [2.0] * 6], [[3.0] * 8]], np.float32)
+    opt, prio = np.array([[1, 0]], np.uint8), np.array([[1, 0]], np.uint8)
+    w, d = np.array([2.0, 0.5], np.float32), np.array([3.0, 2.0], np.float32)
+    for o in OBJECTIVES:
+        assert X.objective_flag(o) == objective_flag(o), o
+        c32 = RR.c_evaluate(tab, opt, prio, np.zeros(2), objective=o, weights=w, due=d)
+        assert float(c32[0]) == float(X.schedule(tab, opt[0], prio[0], objective=o, weights=w, due=d)[0]), o
 
 
 def test_exact_reference_refuses_inputs_that_fp32_would_round():
@@ -337,14 +385,14 @@ def _subsample(B, J, seed):
     return sorted(set([0, B - 1] + rng.choice(B, size=n - 2, replace=False).tolist()))
 
 
-def _sweep_one(engine, J, nodes, S, fam, fold, rel, B, ints, seed):
+def _sweep_one(engine, J, nodes, S, fam, fold, rel, B, ints, seed, tiny=False):
     """One shape: set the table and per-job data, build tie-heavy candidates, run every route against the fp32 oracle
     and the exact reference, plus eval_full and decode."""
     T = rt_table(fam, J, S, seed)
     engine.set_table(T, nodes=nodes)
     opt, prio = candidates(J, B, nodes if nodes > 1 else S, seed + 1)
     r = release_dates(rel, T, opt, prio, ints, nodes, seed + 2)
-    w, d = per_job(fold, T, opt, prio, ints, nodes, r, seed + 3)
+    w, d = per_job(fold, T, opt, prio, ints, nodes, r, seed + 3, tiny)
     _set_per_job(engine, r, w, d)
     ref = c_ref(T, opt, prio, r, ints, nodes, fold, w, d)
     label = (J, nodes, fold, r is not None)
@@ -390,12 +438,14 @@ OBJ_J = [33, 256, 257, 1024]
 @pytest.mark.parametrize("fold", FOLDS)
 def test_every_objective_with_and_without_release(engine, fold, J, nodes):
     """Every fold, release off and on, at J in {33, 256, 257, 1024} on 1, 6 and 8 nodes.  One node uses the full
-    table with S = 8 at J = 1024 (too large to sit beside the tiles: path 4 without the re-order) and S = 4 below."""
+    table with S = 8 at J = 1024 (too large to sit beside the tiles: path 4 without the re-order) and S = 4 below.
+    Weights are subnormal in one of the two runs."""
     S = 1 if nodes > 1 else (8 if J == 1024 else 4)
     for k, rel in enumerate([None, "ready"]):
         seed = 7919 * OBJ_J.index(J) + 31 * nodes + 3 * FOLDS.index(fold) + k
         fam = ["small", "zeros", "equal", "dyadic"][(seed // 3) % (4 if J <= 300 else 2)]
-        _sweep_one(engine, J, nodes, S, fam, fold, rel, 33 if k == 0 else 97, (seed % 2) == 0, seed)
+        _sweep_one(engine, J, nodes, S, fam, fold, rel, 33 if k == 0 else 97, (seed % 2) == 0, seed,
+                   tiny=(k + nodes) % 2 == 1)
     SWEEP_DONE.add((fold, J, nodes))
 
 
@@ -423,27 +473,66 @@ def test_eval_host_over_several_chunks(engine):
     assert np.array_equal(xs, got[rows].astype(np.float64))
 
 
+# case: (table family, folds)
+FP32_EDGES = {"large": ("large", ("makespan", "weighted_tardiness")),
+              "huge_release": ("small", ("makespan", "weighted_tardiness")),
+              "sentinel": ("sentinel", ("makespan", "weighted_tardiness")),
+              "lateness_spread": ("dyadic", ("max_lateness",)),
+              "late_neighbours": ("mid", ("late_tasks", "weighted_late_tasks")),
+              "stretch_weights": ("dyadic", ("weighted_max_tardiness",))}
+
+
+def _fp32_edge_per_job(case, fold, T, opt, prio, ints, seed):
+    """(release, weights, due) of one fp32-only case."""
+    J = T.shape[0]
+    rng = np.random.default_rng(seed)
+    r = w = d = None
+    if case == "huge_release":
+        r = release_dates("huge", T, opt, prio, ints, 1, 0)
+    if fold == "weighted_tardiness":
+        w = WEIGHTS[np.random.default_rng(seed).integers(0, 5, J)].astype(np.float32)
+        d = (np.random.default_rng(seed).uniform(0, 2.0 ** 23, J) * (J / 8)).astype(np.float32)
+        d = np.minimum(d, np.float32(2.0 ** 24 - 1))
+    elif case == "lateness_spread":
+        # the widest spread sb_set_due takes for the maximum lateness: the tails q = D - d are exact integers up to
+        # 2^24 - 1, and e + q rounds (e is a multiple of 1/8)
+        d = rng.integers(0, 2 ** 24, J).astype(np.float32)
+        d[0], d[-1] = 0.0, 2.0 ** 24 - 1
+    elif case == "late_neighbours":
+        # per job candidate 0's fp32 completion e (on time), or its fp32 neighbour below (late) or above (on time)
+        _, st, _ = c_ref(T, opt[:1], prio[:1], None, ints, 1, "makespan", None, None, want_plan=True)
+        rt = T[np.arange(J), opt[0] >> 3, opt[0] & 7]
+        e = (st[0] + rt).astype(np.float32)
+        assert (e.astype(np.float64) != st[0].astype(np.float64) + rt).any()        # some completions rounded
+        d = np.stack([e, np.nextafter(e, np.float32(-np.inf)), np.nextafter(e, np.float32(np.inf))])
+        d = d[rng.integers(0, 3, J), np.arange(J)]
+        if fold.startswith("weighted"):
+            w = WEIGHTS[rng.integers(0, 5, J)].astype(np.float32)
+    elif case == "stretch_weights":
+        # solve(objective="max_stretch")'s weighted maximum tardiness: w = fp32(1 / p*), d = max(r, +0)
+        from saturn_b200.solver import _stretch_form
+        r = release_dates("ready", T, opt, prio, ints, 1, seed)
+        _, w, d = _stretch_form(T, r)
+    return r, w, d
+
+
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", ["large", "huge_release", "sentinel"])
+@pytest.mark.parametrize("case", list(FP32_EDGES))
 @pytest.mark.parametrize("J", [33, 97])
 def test_fp32_only_edges(engine, case, J):
-    """Inputs where fp32 rounds, against the fp32 oracle only: runtimes in [2^22, 2^23] (times cross 2^23, where the
-    ulp is 1), release dates of 2^24 - 1, and selected 1e8 / +inf cells (+inf scores; the key is still the arg-min),
-    under the makespan and the weighted tardiness, every route."""
+    """Inputs where fp32 rounds, against the fp32 oracle only, every route, integer and real starts: runtimes in
+    [2^22, 2^23] (times cross 2^23, where the ulp is 1), release dates of 2^24 - 1, and selected 1e8 / +inf cells
+    (+inf scores; the key is still the arg-min) under the makespan and the weighted tardiness; a due-date spread of
+    2^24 - 1 under the maximum lateness; late-count due dates at the fp32 neighbours of rounded completions; the
+    maximum stretch's weights fp32(1 / p*) with its due dates max(r, 0)."""
     seed = J + len(case)
-    fam = {"large": "large", "huge_release": "small", "sentinel": "sentinel"}[case]
+    fam, folds = FP32_EDGES[case]
     T = rt_table(fam, J, 2, seed)
-    for fold in ("makespan", "weighted_tardiness"):
+    for fold in folds:
         for ints in (True, False):
             engine.set_table(T)
             opt, prio = candidates(J, 200, 2, seed + 1)
-            r = release_dates("huge", T, opt, prio, ints, 1, 0) if case == "huge_release" else None
-            w = WEIGHTS[np.random.default_rng(seed).integers(0, 5, J)].astype(np.float32) \
-                if fold == "weighted_tardiness" else None
-            d = (np.random.default_rng(seed).uniform(0, 2.0 ** 23, J) * (J / 8)).astype(np.float32) \
-                if fold == "weighted_tardiness" else None
-            if d is not None:
-                d = np.minimum(d, np.float32(2.0 ** 24 - 1))
+            r, w, d = _fp32_edge_per_job(case, fold, T, opt, prio, ints, seed)
             _set_per_job(engine, r, w, d)
             ref, cst, cm = c_ref(T, opt, prio, r, ints, 1, fold, w, d, want_plan=True)
             if case == "sentinel":
@@ -502,7 +591,7 @@ SEARCHES = [("fused_tile", 256, 1), ("position_major", 1024, 1), ("six_nodes", 9
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name,J,nodes", SEARCHES)
-@pytest.mark.parametrize("fold", ["makespan", "weighted_tardiness"])
+@pytest.mark.parametrize("fold", ["makespan", "weighted_tardiness", "late_tasks", "weighted_max_tardiness"])
 def test_search_on_tie_heavy_tables(engine, fold, name, J, nodes):
     """Short searches with release dates under the incremental-score verifier: no mismatch, a valid population, and a
     best plan whose exact score equals the reported one.  J = 4096 may be refused as unsupported, nothing else."""
@@ -534,8 +623,9 @@ def test_search_on_tie_heavy_tables(engine, fold, name, J, nodes):
 # --------------------------------------------------------------------------- GPU: coverage accounting
 @pytest.mark.gpu
 def test_zz_every_kernel_path_was_exercised():
-    """Runs after the sweep: paths 0-5 and 7-9 each scored something, and path 6 under the makespan.  Skipped when
-    only part of the sweep ran (a -k selection or an earlier failure)."""
+    """Runs after the sweep: paths 0-5 and 7-9 each scored something, and path 6 under the makespan; under each fold
+    of the other oracles, paths 0, 3, 4 or 9, 5, 7 and 8.  Skipped when only part of the sweep ran (a -k selection
+    or an earlier failure)."""
     want = {("sweep", J) for J in SWEEP_J} | {(f, J, n) for f in FOLDS for J in OBJ_J for n in (1, 6, 8)}
     if want - SWEEP_DONE:
         pytest.skip("the sweep did not run completely")
@@ -543,6 +633,10 @@ def test_zz_every_kernel_path_was_exercised():
     for p in (0, 1, 2, 3, 4, 5, 7, 8, 9):
         assert p in seen, ("path never ran", p, sorted(seen))
     assert 6 in {rec[4] for rec in COVERAGE if rec[2] == "makespan"}
+    for fold in NEW_FOLDS:
+        paths = {rec[4] for rec in COVERAGE if rec[2] == fold and rec[4] is not None}
+        print("paths under %s:" % fold, sorted(paths))
+        assert {0, 3, 5, 7, 8} <= paths and paths & {4, 9}, (fold, sorted(paths))
     by = {}
     for J, nodes, fold, rel, path in COVERAGE:
         if J in (6145, 16384, 65535) or nodes == 8:

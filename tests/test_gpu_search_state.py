@@ -23,20 +23,18 @@ bits and bytes):
   I9 count   search_stats() evaluated = chains * (1 + rounds) + the injected copies.
 
 The cases cover the three layouts (fused tile rounds, incremental or not; the propose / evaluate / accept kernels;
-the position-major kernel), 1 to 8 nodes, the full table, every objective with release dates off and on, populations
-of 1 to one wave + 17 chains, random tables with masks and sentinel cells and tie-heavy tables (all runtimes equal,
-or in {1, 2, 3}), where `<=` acceptance and `<` tournaments differ.
+the position-major kernel), 1 to 8 nodes, the full table, all ten objectives with release dates off and on,
+populations of 1 to one wave + 17 chains, random tables with masks and sentinel cells and tie-heavy tables (all
+runtimes equal, or in {1, 2, 3}), where `<=` acceptance and `<` tournaments differ.
 """
 import numpy as np
 import pytest
 
-from oracle import c_oracle
-from oracle import ref_completion as RC
 from oracle import ref_eval as R
+from oracle import ref_exact as X
 from oracle import ref_release as RR
-from oracle import ref_tardiness as RT
-from oracle import ref_weighted as RW
 from saturn_b200 import _lib
+from saturn_b200.engine import OBJECTIVES
 from saturn_b200.search import lpt_seeds
 
 SENTINEL = 1.0e6
@@ -94,7 +92,8 @@ def proposable(tmin, args, reduced, sentinel=SENTINEL):
 
 
 def per_job(T, objective, release, ints, seed):
-    """fp32 weights / due dates / release dates at the scale of the table's plans."""
+    """fp32 weights / due dates / release dates at the scale of the table's plans, as the objective's flag bits need
+    them."""
     rng = np.random.default_rng(seed)
     J = T.shape[0]
     usable = np.where(T < SENTINEL, T, np.inf).min(axis=(1, 2))
@@ -102,9 +101,10 @@ def per_job(T, objective, release, ints, seed):
     horizon = float(usable.sum()) / 4 + 1.0
     integral = bool((T[np.isfinite(T)] == np.round(T[np.isfinite(T)])).all())
     w = d = r = None
-    if objective.startswith("weighted_"):
+    use_w, use_d = X.needs(objective)
+    if use_w:
         w = rng.choice([0.5, 1.0, 2.0, 3.0], J).astype(np.float32)
-    if objective.endswith("tardiness"):
+    if use_d:
         d = rng.uniform(-0.05, 1.0, J) * horizon
         d = (np.round(d) if integral else d).astype(np.float32)
     if release:
@@ -126,19 +126,9 @@ class Ctx:
 
     def score(self, opt, prio):
         """fp32 scores of rows opt[B][J], prio[B][J] (the C ports, bit-exact with the kernels)."""
-        tab, ints, nodes, obj = self.tab, self.ints, self.nodes, self.objective
-        opt = np.ascontiguousarray(opt)
-        prio = np.ascontiguousarray(prio)
-        if self.r is not None:
-            return RR.c_evaluate(tab, opt, prio, self.r, ints, np.float32, nodes=nodes, objective=obj, weights=self.w,
-                                 due=self.d)
-        if obj == "makespan":
-            return c_oracle.evaluate(tab, opt, prio, ints, np.float32, nodes=nodes)
-        if obj == "completion":
-            return RC.c_evaluate(tab, opt, prio, ints, np.float32, nodes=nodes)
-        if obj == "weighted_completion":
-            return RW.c_evaluate(tab, opt, prio, ints, np.float32, nodes=nodes, weights=self.w)
-        return RT.c_evaluate(tab, opt, prio, self.d, ints, np.float32, nodes=nodes, weights=self.w)
+        r = np.zeros(self.J, np.float32) if self.r is None else self.r
+        return RR.c_evaluate(self.tab, np.ascontiguousarray(opt), np.ascontiguousarray(prio), r, self.ints, np.float32,
+                             nodes=self.nodes, objective=self.objective, weights=self.w, due=self.d)
 
     def candidate(self, rng):
         """A random candidate built from proposable cells only (job-indexed opt row, prio row)."""
@@ -375,17 +365,23 @@ for _c in [
     ("seedtrap_reduced", 64, 33, None, dict(family="seedtrap")),
     ("seedtrap_full", 64, 1000, None, dict(family="seedtrap", S=2, reduced=False)),
     ("seedtrap_nodes2", 64, 31, None, dict(family="seedtrap", nodes=2, resample=-1)),
+    # forms whose scores tie in bulk: a late count on equal runtimes at temperature 0, a max fold on the full table and
+    # on 8 nodes
+    ("late_tasks_equal_t0", 256, 1000, 1, dict(objective="late_tasks", family="equal", resample=-1, t0=True)),
+    ("wmax_tardiness_full_S3", 64, 1000, None, dict(S=3, reduced=False, objective="weighted_max_tardiness",
+                                                     release=True, warm=True)),
+    ("max_lateness_nodes8", 200, 4097, None, dict(nodes=8, objective="max_lateness", resample=-1)),
 ]:
     CASES.append(case(_c[0], _c[1], _c[2], _c[3], **_c[4]))
 
 # every objective, release dates off and on, at J in {256, 700} on 1 and 2 nodes
 _SHAPES = [(256, 1), (700, 1), (256, 2), (700, 2)]
-for _i, _obj in enumerate(RR.OBJECTIVES):
+for _i, _obj in enumerate(OBJECTIVES):
     for _k, _rel in enumerate((False, True)):
         _J, _n = _SHAPES[(2 * _i + _k) % 4]
         CASES.append(case("%s_%s_J%d_n%d" % (_obj, "rel" if _rel else "norel", _J, _n), _J, 1000 if _J == 256 else 300,
                           None, nodes=_n, objective=_obj, release=_rel, family="small" if _k else "rnd",
-                          resample=-1 if _i % 2 else 0, t0=_i == 4, warm=_k == 1, twice=_i == 3 and _k == 1))
+                          resample=-1 if _i % 2 else 0, t0=_i % 5 == 4, warm=_k == 1, twice=_i % 5 == 3 and _k == 1))
 
 
 # --------------------------------------------------------------------------- CPU

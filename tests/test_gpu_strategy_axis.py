@@ -14,8 +14,9 @@ position-major or unfused.  With S <= 8 and J <= 256 the table is at most 64 KB,
 * GPU: the reduced table in bits; the headline tile kernel at 16, 15, 11, 4, 3 and 2 warps per CTA under every
   objective (release dates lower the warp count) with its debug options; path 4 by default, path 9, the generic
   kernel with the table in shared and in global memory, by-position paths 5 / 7 / 8, eval_host, eval_full, decode
-  and validate; the population invariants of test_gpu_search_state on full-table searches of every layout;
-  search_run against the Python driver; solve_table against solve() at 32 executors.
+  and validate, also under the objectives whose per-job arrays move a shape to another route; the population
+  invariants of test_gpu_search_state on full-table searches of every layout, those objectives included; search_run
+  against the Python driver; solve_table against solve() at 32 executors.
 """
 import numpy as np
 import pytest
@@ -28,11 +29,12 @@ from oracle import ref_release as RR
 from oracle import ref_tardiness as RT
 from oracle import ref_weighted as RW
 from saturn_b200 import _lib
+from saturn_b200.engine import OBJECTIVES, objective_flag
 from test_exact_edges import c_ref, candidates, release_dates, rt_table
 from test_exact_edges import per_job as exact_per_job
 from test_gpu_search_state import case, make_table, proposable, run_script
 
-FOLDS = RR.OBJECTIVES
+FOLDS = OBJECTIVES
 KEY_MAX = 2 ** 63 - 1
 ID_BASE = 0x7ffff000          # keys of b >= 4096 carry into bit 31 of the id
 PATHS_SEEN = {}               # path -> set of (J, S) that took it, at S > 8
@@ -54,9 +56,12 @@ def _round_row(b):
 
 
 def job_arrays(objective, release):
-    """The per-job fp32 arrays staged beside the table: weights (and the unit weights of "tardiness"), due dates,
-    release dates."""
-    return (2 if objective.endswith("tardiness") else 1 if objective.startswith("weighted") else 0) + bool(release)
+    """job_arrays(flags) of sb_internal.h: the per-job fp32 arrays staged beside the table, from the objective's flag
+    bits: weights and due dates with SB_FLAG_DUE (unit weights without SB_FLAG_WEIGHTED), weights alone with
+    SB_FLAG_WEIGHTED, the delivery tails with SB_FLAG_MAX_LATENESS, release dates with SB_FLAG_RELEASE."""
+    f = objective_flag(objective)
+    return (2 if f & _lib.FLAG_DUE else 1 if f & _lib.FLAG_WEIGHTED else 0) + bool(f & _lib.FLAG_MAX_LATENESS) + bool(
+        release)
 
 
 def plan_tiles(J, SG, stream, arrays=0, tab_global=False, nodes=1):
@@ -112,18 +117,28 @@ def generic_table_in_smem(J, S):
 # (J, S, arrays): (sb_eval path, warps), (search layout, warps)
 ROUTE_MAP = {
     (256, 9, 0): ((3, 16), (1, 9)),
+    (256, 9, 1): ((3, 16), (1, 9)),
+    (256, 9, 2): ((3, 16), (1, 8)),
     (256, 10, 0): ((3, 16), (1, 8)),
     (256, 11, 0): ((3, 16), (1, 8)),
+    (256, 11, 1): ((3, 16), (1, 8)),
+    (256, 11, 2): ((3, 16), (1, 8)),
     (256, 11, 3): ((3, 15), (2, 16)),
     (256, 12, 0): ((3, 15), (2, 16)),
     (256, 16, 0): ((3, 11), (2, 16)),
     (256, 24, 0): ((3, 4), (2, 16)),
+    (256, 24, 1): ((3, 3), (2, 16)),
+    (256, 24, 2): ((3, 3), (2, 16)),
     (256, 25, 0): ((3, 3), (2, 16)),
+    (256, 25, 1): ((3, 3), (2, 16)),
+    (256, 25, 2): ((3, 2), (2, 16)),
     (208, 32, 0): ((3, 2), (2, 16)),
     (216, 31, 3): ((3, 2), (2, 16)),
     (200, 24, 0): ((3, 11), (2, 16)),
     (224, 32, 0): ((4, 16), (2, 16)),
     (256, 28, 0): ((4, 16), (2, 16)),
+    (256, 28, 1): ((4, 16), (2, 16)),
+    (256, 28, 2): ((4, 16), (2, 16)),
     (256, 28, 3): ((9, 16), (0, 4)),
     (256, 32, 0): ((9, 16), (0, 4)),
     (300, 16, 0): ((3, 8), (2, 16)),
@@ -138,6 +153,10 @@ def test_route_rules_pin_the_shapes_this_file_uses():
         assert route_eval(J, S, arrays) == ev, (J, S, arrays, route_eval(J, S, arrays))
         assert route_search(J, S, arrays) == se, (J, S, arrays, route_search(J, S, arrays))
     assert generic_table_in_smem(128, 28) and not generic_table_in_smem(128, 29)
+    # one array per form of job_arrays(flags): the tails of max_lateness, weights and due dates of the late count and
+    # the maximum tardiness, weighted or not
+    assert [job_arrays(o, False) for o in OBJECTIVES] == [0, 0, 1, 2, 2, 1, 2, 2, 2, 2]
+    assert job_arrays("late_tasks", True) == 3 and job_arrays("max_lateness", True) == 2
     # the tables of S <= 8 and J <= 256 never leave the headline shape: 16 warps, fused search
     for S in range(1, 9):
         assert route_eval(256, S) == (3, 16) and route_search(256, S)[0] == 1
@@ -149,8 +168,8 @@ def _bits(x):
 
 @pytest.mark.parametrize("S", [9, 17, 32])
 def test_c_ports_equal_the_python_list_schedule(S):
-    """Every fold's C port equals the Python list schedule (fp32) bit for bit, scores, starts and masks, with
-    opt bytes spanning 0x00..(S - 1) << 3 | 7 (0xFF at S = 32), both start modes, release dates off and on."""
+    """Every C port of a ref_release fold equals its Python list schedule (fp32) bit for bit, scores, starts and masks,
+    with opt bytes spanning 0x00..(S - 1) << 3 | 7 (0xFF at S = 32), both start modes, release dates off and on."""
     J, B = 24, 12
     rng = np.random.default_rng(S)
     tab = (rng.uniform(0.5, 40.0, (J, S, 8)) * rng.choice([1.0, 1.0, 3.0], (J, S, 8))).astype(np.float32)
@@ -166,7 +185,7 @@ def test_c_ports_equal_the_python_list_schedule(S):
     for ints in (True, False):
         for rel in (False, True):
             r = rng.uniform(-10, 60, J).astype(np.float32) if rel else np.zeros(J, np.float32)
-            for fold in FOLDS:
+            for fold in RR.OBJECTIVES:
                 wf = w if fold.startswith("weighted") else None
                 df = d if fold.endswith("tardiness") else None
                 got, gst, gm = RR.c_evaluate(tab, opt, prio, r, ints, np.float32, want_plan=True, objective=fold,
@@ -381,14 +400,15 @@ def test_reduced_table_equals_the_oracle_in_bits(engine, S, G):
 
 
 # --------------------------------------------------------------------------- GPU: the evaluation sweep
-# the path-3 shapes on u8 rows: (J, S) with 16, 15, 11, 4, 3 and 2 warps per CTA without per-job arrays
+# the path-3 shapes on u8 rows: (J, S) with 16, 15, 11, 4, 3 and 2 warps per CTA without per-job arrays (one or
+# two arrays take (256, 24) to 3 warps and two take (256, 25) to 2)
 TILE_SHAPES = [(256, 9), (256, 12), (256, 16), (256, 24), (256, 25), (208, 32)]
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("J,S", TILE_SHAPES, ids=["J%d-S%d" % s for s in TILE_SHAPES])
 def test_headline_kernel_at_every_warp_count(engine, J, S):
-    """Every fold with release dates off and on, integer and real starts alternating, at batch sizes of one CTA's
+    """Every objective with release dates off and on, integer and real starts alternating, at batch sizes of one CTA's
     worth (no warp has two tiles: no stagger), one and a half waves and one tile past a wave (grid * nw tiles);
     each on the default route, with one bulk copy per row, and without the stagger, against the fp32 oracle and on
     sampled rows the exact reference."""
@@ -445,7 +465,9 @@ def _every_route(engine, J, S, fold, rel, B, ints, seed, fam="small"):
 ROUTE_CASES = [(224, 32, "makespan", False), (256, 28, "weighted_completion", False),
                (256, 28, "tardiness", True), (256, 32, "makespan", False), (256, 32, "weighted_tardiness", True),
                (1024, 8, "completion", False), (300, 16, "makespan", True), (128, 28, "makespan", False),
-               (128, 29, "weighted_tardiness", False), (216, 31, "tardiness", True), (256, 11, "makespan", False)]
+               (128, 29, "weighted_tardiness", False), (216, 31, "tardiness", True), (256, 11, "makespan", False),
+               (256, 24, "max_lateness", False), (256, 25, "weighted_late_tasks", False),
+               (256, 11, "late_tasks", True), (256, 28, "late_tasks", True), (256, 28, "max_tardiness", False)]
 
 
 @pytest.mark.gpu
@@ -552,13 +574,18 @@ for _c in [
     # the J = 256, S = 11 boundary: the per-job arrays move the population from the tile to position-major
     ("bound_S11_makespan", 256, 1000, dict(S=11, warm=True)),
     ("bound_S11_wtard_rel", 256, 1000, dict(S=11, objective="weighted_tardiness", release=True, resample=-1)),
+    ("bound_S11_late_rel", 256, 1000, dict(S=11, objective="late_tasks", release=True, family="small", t0=True)),
+    ("bound_S11_max_lateness", 256, 1000, dict(S=11, objective="max_lateness", release=True, resample=-1)),
     # unfused rounds the library falls back to by itself
     ("unfused_S32_J256", 256, 1000, dict(S=32, warm=True)),
     ("unfused_S32_J256_tie_t0", 256, 33, dict(S=32, family="small", resample=-1, t0=True)),
     ("unfused_C5_J1024_S8", 1024, 300, dict(S=8, resample=-1)),
+    ("unfused_S28_late_rel", 256, 1000, dict(S=28, objective="late_tasks", release=True, warm=True)),
     # fused tile rounds at 8 and 9 warps
     ("tile_S10_J256", 256, 1000, dict(S=10, resample=-1, warm=True)),
     ("tile_S9_J256_tie_t0", 256, "wave+17", dict(S=9, family="small", resample=-1, t0=True)),
+    ("tile_S9_wmax_tardiness", 256, 1000, dict(S=9, objective="weighted_max_tardiness", resample=-1, twice=True)),
+    ("tile_S9_max_lateness", 256, 1000, dict(S=9, objective="max_lateness", warm=True)),
 ]:
     _k = dict(_c[3])
     _c_ = case(_c[0], _c[1], _c[2], reduced=False, **_k)
