@@ -435,7 +435,8 @@ int sb_search_run_multi(sb_handle** handles, int n, const sb_search_params* p, c
                         void* prio_out /*host [J]*/, sb_search_result* result);
 /* Population size that fills the device exactly once with the round kernel this table gets (resident warps
  * per SM x 32 lanes x SMs).  A population that is a whole multiple of it leaves no partially filled last
- * wave: 131,072 chains on 132 SMs x 12 warps are 2.6 waves and cost 3. */
+ * wave: 131,072 chains on 132 SMs x 12 warps are 2.6 waves and cost 3.  A combination of objective flags that sb_eval
+ * refuses is SB_ERR_ARG here too. */
 int sb_search_wave(sb_handle* h, unsigned flags, int64_t* chains);
 /* 1 if rounds run as ONE fused kernel (move + evaluate + accept), 0 if they run as propose / evaluate /
  * accept kernels.  Fused rounds keep both rows of a tile's 32 candidates in shared memory when they fit

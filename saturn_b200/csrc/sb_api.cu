@@ -36,12 +36,18 @@ static int fail(int code, const char* fmt, ...) {
       return fail(SB_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e__), __FILE__, __LINE__); \
   } while (0)
 
+// The objective a flags word selects (sb_common.cuh: Obj), and whose weights it reads
+struct Objective {
+  Obj obj = Obj::Makespan;
+  bool weighted = false;  // SB_FLAG_WEIGHTED: the caller's weights (sb_set_weights); unit weights otherwise
+};
+
 struct SearchState {
   bool ready = false;
   SearchDev d;
   sb_search_params p;
-  float scale = 0.f;  // temperature unit: incumbent makespan after initialisation (SB_FLAG_SUM_COMPLETION: sum / J;
-                      // with SB_FLAG_WEIGHTED: weighted sum / sum of the weights; SB_FLAG_DUE: see sb_search_init)
+  float scale = 0.f;  // temperature unit: incumbent makespan after initialisation (the sums: sum / J, or weighted
+                      // sum / sum of the weights; the due-date objectives: see sb_search_init)
   long long evaluated = 0;
   int rounds_done = 0;
   bool fused_ok = true;  // run rounds with the fused kernel while its tiles fit
@@ -59,8 +65,9 @@ struct SearchState {
   unsigned long long* verify_bad = nullptr;
   bool win = false, inc = false, verify = false;
   SearchDev alloc;  // the pointers as allocated (s.d's cur / prop pairs trade places when resampling)
-  const float* w = nullptr;    // SB_FLAG_WEIGHTED: the handle's job weights (SB_FLAG_DUE alone: its unit weights)
-  const float* due = nullptr;  // SB_FLAG_DUE: the handle's due dates (SB_FLAG_MAX_LATENESS: its delivery tails)
+  Objective obj;                // the objective of p.flags
+  const float* w = nullptr;    // obj_weights: the handle's job weights (or its unit weights)
+  const float* due = nullptr;  // obj_due: the handle's due dates (TailMakespan: its delivery tails)
                                // (position-major kernels)
   const float* rel = nullptr;  // SB_FLAG_RELEASE: the handle's release dates as the flags read them (likewise)
 };
@@ -461,36 +468,54 @@ int sb_set_release(sb_handle* h, const float* r, int J) {
   return SB_OK;
 }
 
-// SB_FLAG_WEIGHTED and SB_FLAG_DUE are valid with SB_FLAG_SUM_COMPLETION only, and after sb_set_weights /
-// sb_set_due respectively; SB_FLAG_MAX_LATENESS alone among the objective flags, after sb_set_due with a due-date spread
-// below 2^24; SB_FLAG_LATE_COUNT with SB_FLAG_SUM_COMPLETION | SB_FLAG_DUE only (it changes what the tardiness form
-// adds per job); SB_FLAG_MAX_TARDINESS likewise (it changes how the tardiness form folds its terms), and not with
-// SB_FLAG_LATE_COUNT or SB_FLAG_MAX_LATENESS; SB_FLAG_RELEASE under any objective, after sb_set_release
-static int check_per_job(const sb_handle* h, unsigned flags) {
-  constexpr unsigned kTardiness = SB_FLAG_SUM_COMPLETION | SB_FLAG_DUE;
-  if ((flags & SB_FLAG_LATE_COUNT) && (flags & kTardiness) != kTardiness)
+// The one reader of the objective flags.  SB_FLAG_WEIGHTED and SB_FLAG_DUE are valid with SB_FLAG_SUM_COMPLETION only;
+// SB_FLAG_MAX_LATENESS alone among the objective flags; SB_FLAG_LATE_COUNT and SB_FLAG_MAX_TARDINESS with
+// SB_FLAG_SUM_COMPLETION | SB_FLAG_DUE only (they change what the tardiness form adds per job, and how it folds its
+// terms), and not together or with SB_FLAG_MAX_LATENESS.  Every other combination is SB_ERR_ARG.
+static int decode_objective(unsigned flags, Objective* o) {
+  const bool sum = flags & SB_FLAG_SUM_COMPLETION, weighted = flags & SB_FLAG_WEIGHTED, due = flags & SB_FLAG_DUE;
+  const bool lateness = flags & SB_FLAG_MAX_LATENESS, late = flags & SB_FLAG_LATE_COUNT;
+  const bool max_tardiness = flags & SB_FLAG_MAX_TARDINESS;
+  if (late && !(sum && due))
     return fail(SB_ERR_ARG, "SB_FLAG_LATE_COUNT counts late jobs on the tardiness form: it needs SB_FLAG_SUM_COMPLETION "
                 "and SB_FLAG_DUE");
-  if ((flags & SB_FLAG_MAX_TARDINESS) && (flags & kTardiness) != kTardiness)
+  if (max_tardiness && !(sum && due))
     return fail(SB_ERR_ARG, "SB_FLAG_MAX_TARDINESS folds the tardiness form with max: it needs SB_FLAG_SUM_COMPLETION "
                 "and SB_FLAG_DUE");
-  if ((flags & SB_FLAG_MAX_TARDINESS) && (flags & (SB_FLAG_LATE_COUNT | SB_FLAG_MAX_LATENESS)))
+  if (max_tardiness && (late || lateness))
     return fail(SB_ERR_ARG, "SB_FLAG_MAX_TARDINESS cannot be combined with SB_FLAG_LATE_COUNT or SB_FLAG_MAX_LATENESS");
-  if ((flags & SB_FLAG_MAX_LATENESS) && (flags & (SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED | SB_FLAG_DUE)))
+  if (lateness && (sum || weighted || due))
     return fail(SB_ERR_ARG, "SB_FLAG_MAX_LATENESS is an objective of its own: it cannot be combined with "
                 "SB_FLAG_SUM_COMPLETION, SB_FLAG_WEIGHTED or SB_FLAG_DUE");
-  if ((flags & SB_FLAG_MAX_LATENESS) && !h->has_d)
-    return fail(SB_ERR_STATE, "SB_FLAG_MAX_LATENESS needs sb_set_due (sb_set_table clears the due dates)");
-  if ((flags & SB_FLAG_MAX_LATENESS) && !h->q_exact)
-    return fail(SB_ERR_ARG, "SB_FLAG_MAX_LATENESS needs max d - min d < 2^24 (beyond it the tails max d - d round even for "
-                "integer due dates)");
-  if ((flags & SB_FLAG_WEIGHTED) && !(flags & SB_FLAG_SUM_COMPLETION))
+  if (weighted && !sum)
     return fail(SB_ERR_ARG, "SB_FLAG_WEIGHTED weights the sum of completion times: it needs SB_FLAG_SUM_COMPLETION");
-  if ((flags & SB_FLAG_DUE) && !(flags & SB_FLAG_SUM_COMPLETION))
+  if (due && !sum)
     return fail(SB_ERR_ARG, "SB_FLAG_DUE scores the tardiness of the completion times: it needs SB_FLAG_SUM_COMPLETION");
-  if ((flags & SB_FLAG_WEIGHTED) && !h->has_w)
+  o->weighted = weighted;
+  if (lateness) o->obj = Obj::TailMakespan;
+  else if (!sum) o->obj = Obj::Makespan;
+  else if (late) o->obj = Obj::LateCount;
+  else if (max_tardiness) o->obj = Obj::MaxTardiness;
+  else if (due) o->obj = Obj::Tardiness;
+  else o->obj = weighted ? Obj::WeightedSum : Obj::Sum;
+  return SB_OK;
+}
+
+// the objectives folded from the tardiness form (SB_FLAG_DUE): their scores reach +0, which no plan can beat
+static bool tardiness_form(Obj o) { return o == Obj::Tardiness || o == Obj::LateCount || o == Obj::MaxTardiness; }
+
+// decode_objective, then the per-job arrays the objective reads (and SB_FLAG_RELEASE's) must be set on the handle
+static int check_per_job(const sb_handle* h, unsigned flags, Objective* o) {
+  if (int rc = decode_objective(flags, o)) return rc;
+  if (o->obj == Obj::TailMakespan) {
+    if (!h->has_d) return fail(SB_ERR_STATE, "SB_FLAG_MAX_LATENESS needs sb_set_due (sb_set_table clears the due dates)");
+    if (!h->q_exact)
+      return fail(SB_ERR_ARG, "SB_FLAG_MAX_LATENESS needs max d - min d < 2^24 (beyond it the tails max d - d round even "
+                  "for integer due dates)");
+  }
+  if (o->weighted && !h->has_w)
     return fail(SB_ERR_STATE, "SB_FLAG_WEIGHTED needs sb_set_weights (sb_set_table clears the weights)");
-  if ((flags & SB_FLAG_DUE) && !h->has_d)
+  if (obj_due(o->obj) && !h->has_d)
     return fail(SB_ERR_STATE, "SB_FLAG_DUE needs sb_set_due (sb_set_table clears the due dates)");
   if ((flags & SB_FLAG_RELEASE) && !h->has_r)
     return fail(SB_ERR_STATE, "SB_FLAG_RELEASE needs sb_set_release (sb_set_table clears the release dates)");
@@ -501,15 +526,15 @@ static const float* job_release(const sb_handle* h, unsigned flags) {
   if (!(flags & SB_FLAG_RELEASE)) return nullptr;
   return (flags & SB_FLAG_INTEGER_STARTS) ? h->d_rc : h->d_r;
 }
-// the due-date array the kernels read: the due dates (SB_FLAG_DUE), the delivery tails (SB_FLAG_MAX_LATENESS), or none
-static const float* job_due(const sb_handle* h, unsigned flags) {
-  if (flags & SB_FLAG_DUE) return h->d_d;
-  return (flags & SB_FLAG_MAX_LATENESS) ? h->d_q : nullptr;
+// the due-date array the kernels read: the due dates, TailMakespan's delivery tails, or none
+static const float* job_due(const sb_handle* h, Obj obj) {
+  if (!obj_due(obj)) return nullptr;
+  return obj == Obj::TailMakespan ? h->d_q : h->d_d;
 }
-// the weights the kernels read: the caller's, the unit weights of SB_FLAG_DUE alone, or none
-static const float* job_weights(const sb_handle* h, unsigned flags) {
-  if (flags & SB_FLAG_WEIGHTED) return h->d_w;
-  return (flags & SB_FLAG_DUE) ? h->d_one : nullptr;
+// the weights the kernels read: the caller's, unit weights, or none
+static const float* job_weights(const sb_handle* h, const Objective& o) {
+  if (!obj_weights(o.obj)) return nullptr;
+  return o.weighted ? h->d_w : h->d_one;
 }
 
 int sb_get_reduced(sb_handle* h, float* tmin, uint8_t* args) {
@@ -528,7 +553,8 @@ static int make_call(sb_handle* h, const uint8_t* opt, const void* prio, int64_t
   if (B < 0) return fail(SB_ERR_ARG, "B=%lld is negative", static_cast<long long>(B));
   if (B > 0 && (!opt || !prio)) return fail(SB_ERR_ARG, "opt / prio is null");
   if (row_stride < h->J) return fail(SB_ERR_ARG, "row_stride=%lld < J=%d", static_cast<long long>(row_stride), h->J);
-  if (int rc = check_per_job(h, flags)) return rc;
+  Objective o;
+  if (int rc = check_per_job(h, flags, &o)) return rc;
   if (B > 0xffffffffll) return fail(SB_ERR_ARG, "B=%lld exceeds 2^32-1 candidates per call", static_cast<long long>(B));
   const int pb = h->J <= 256 ? 1 : 2;
   const bool reduced = (flags & SB_FLAG_REDUCED) != 0;
@@ -545,8 +571,9 @@ static int make_call(sb_handle* h, const uint8_t* opt, const void* prio, int64_t
   c->stride_o = row_stride;
   c->stride_p = row_stride * pb;
   c->flags = flags;
-  c->w = job_weights(h, flags);
-  c->d = job_due(h, flags);
+  c->obj = o.obj;
+  c->w = job_weights(h, o);
+  c->d = job_due(h, o.obj);
   c->r = job_release(h, flags);
   return SB_OK;
 }
@@ -586,7 +613,7 @@ int sb_eval(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, int64
                                  SB_FLAG_FOLD_PREV | SB_FLAG_ALT_WARPSCAN)) != 0;
     const bool aligned = row_stride % 32 == 0 && reinterpret_cast<uintptr_t>(opt) % 32 == 0 &&
                          reinterpret_cast<uintptr_t>(prio) % 32 == 0;
-    const int home = eval_pos_home(h->dev, c.J, c.SG, c.nodes, flags);
+    const int home = eval_pos_home(h->dev, c.J, c.SG, c.nodes, flags, c.obj);
     if (!hooks && aligned && B > 0 && c.J <= 6144 && home >= 0 && (home != 0 || c.J >= 1024 || (flags & HOOK_REORDER))) {
       const size_t need = static_cast<size_t>(B) * static_cast<size_t>(row_stride);
       if (need > h->by_pos_bytes) {
@@ -606,8 +633,7 @@ int sb_eval(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, int64
     }
   }
   if (flags & SB_FLAG_ALT_WARPSCAN) {
-    if (flags & (SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED | SB_FLAG_DUE | SB_FLAG_RELEASE | SB_FLAG_MAX_LATENESS |
-                 SB_FLAG_LATE_COUNT | SB_FLAG_MAX_TARDINESS))
+    if (c.obj != Obj::Makespan || (flags & SB_FLAG_RELEASE))
       return fail(SB_ERR_UNSUPPORTED, "SB_FLAG_ALT_WARPSCAN scores the makespan without release dates only: it "
                   "cannot be combined with SB_FLAG_SUM_COMPLETION, SB_FLAG_WEIGHTED, SB_FLAG_DUE, SB_FLAG_RELEASE, "
                   "SB_FLAG_MAX_LATENESS, SB_FLAG_LATE_COUNT or SB_FLAG_MAX_TARDINESS");
@@ -946,8 +972,8 @@ static int search_eval(sb_handle* h, bool cur_rows, long long first, long long c
     SearchFuse sf = {};
     sf.cur_mk = s.d.cur_mk;
     const bool reduced = (s.p.flags & SB_FLAG_REDUCED) != 0;
-    CK(search_pos_launch(h->dev, s.d, reduced ? h->tmin : h->tab, s.w, s.due, s.rel, (reduced ? 1 : h->S) * kSlots, s.p.flags, first,
-                         count, true, sf, h->stream));
+    CK(search_pos_launch(h->dev, s.d, reduced ? h->tmin : h->tab, s.w, s.due, s.rel, (reduced ? 1 : h->S) * kSlots, s.p.flags,
+                         s.obj.obj, first, count, true, sf, h->stream));
     return SB_OK;
   }
   EvalCall c;
@@ -968,11 +994,13 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
   if (h->J == 0) return fail(SB_ERR_STATE, "sb_set_table has not been called");
   if (!p) return fail(SB_ERR_ARG, "params is null");
   if (p->chains < 1 || p->chains > (1ll << 31)) return fail(SB_ERR_ARG, "chains=%lld out of range", (long long)p->chains);
-  if ((rc = check_per_job(h, p->flags))) return rc;
+  Objective o;
+  if ((rc = check_per_job(h, p->flags, &o))) return rc;
   CK(cudaStreamSynchronize(h->stream));
   SearchState& s = h->search;
   s.ready = false;
   s.p = *p;
+  s.obj = o;
   if (s.p.total_rounds < 1) s.p.total_rounds = 1;
   const int J = h->J;
   const int pb = J <= 256 ? 1 : 2;
@@ -983,11 +1011,9 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
   d.chains = p->chains;
   d.chain_base = p->chain_base;
   d.seed = p->seed;
-  const bool weighted = (p->flags & SB_FLAG_WEIGHTED) != 0;
-  const bool due = (p->flags & SB_FLAG_DUE) != 0;
-  const int arrays = job_arrays(p->flags);
-  s.w = job_weights(h, p->flags);
-  s.due = job_due(h, p->flags);
+  const int arrays = job_arrays(o.obj, p->flags);
+  s.w = job_weights(h, o);
+  s.due = job_due(h, o.obj);
   s.rel = job_release(h, p->flags);
   d.stride_o = (J + 31) & ~31;  // 32-byte rows: TMA bulk copies for opt, 256-bit streaming loads for prio
   // make stride_p == stride_o * pb so that one element stride describes both (sb_eval contract)
@@ -1056,9 +1082,10 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
   // the temperature unit: the incumbent's makespan, or its mean completion time (the sum / J; weighted: the weighted
   // sum / the sum of the weights, the same fp32 value for unit weights), so that t_start / t_end mean the same
   // fraction of a typical score difference under every objective
+  const bool weighted = o.weighted;
   const float per = weighted ? static_cast<float>(h->w_sum) : static_cast<float>(J);
-  s.scale = isfinite(mk) ? ((p->flags & SB_FLAG_SUM_COMPLETION) ? mk / per : mk) : 1.0f;
-  if (due && isfinite(mk)) {
+  s.scale = isfinite(mk) ? (obj_sum(o.obj) ? mk / per : mk) : 1.0f;
+  if (tardiness_form(o.obj) && isfinite(mk)) {
     // tardiness can be 0 or tiny at the incumbent: the unit is at least the weighted mean of each job's smallest
     // proposable runtime, the size of the score change one move makes
     const float* tmin = h->h_tmin.data();
@@ -1080,12 +1107,12 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
     // the maximum tardiness is a max, not a sum: its unit is the incumbent itself (the mean-completion division of
     // SB_FLAG_SUM_COMPLETION does not apply), and at least the largest weighted smallest runtime, the same floor taken
     // as a max.  A starting point, not a measured choice (DESIGN §3)
-    if (p->flags & SB_FLAG_MAX_TARDINESS) s.scale = std::max(mk, static_cast<float>(move_max));
+    if (o.obj == Obj::MaxTardiness) s.scale = std::max(mk, static_cast<float>(move_max));
     else s.scale = std::max(s.scale, static_cast<float>(move / (weighted ? h->w_sum : static_cast<double>(J))));
   }
   // the late count moves in steps of one job's weight and is 0 at many incumbents: its unit is the count of every job,
   // sum_j w_j (J with unit weights), so that an uphill move of one mean weight is accepted with e^(-1 / (J t))
-  if (p->flags & SB_FLAG_LATE_COUNT) s.scale = static_cast<float>(weighted ? h->w_sum : static_cast<double>(J));
+  if (o.obj == Obj::LateCount) s.scale = static_cast<float>(weighted ? h->w_sum : static_cast<double>(J));
   s.evaluated = d.chains;
   s.rounds_done = 0;
   s.launches = 0;
@@ -1187,8 +1214,8 @@ int sb_search_round(sb_handle* h, int rounds) {
       SearchFuse sf = make_fuse(s, round, n);
       sf.resample_every = 0;
       const bool reduced = (s.p.flags & SB_FLAG_REDUCED) != 0;
-      CK(search_pos_launch(h->dev, s.d, reduced ? h->tmin : h->tab, s.w, s.due, s.rel, (reduced ? 1 : h->S) * kSlots, s.p.flags, 0,
-                           s.d.chains, false, sf, h->stream));  // keeps the incumbent in its tail
+      CK(search_pos_launch(h->dev, s.d, reduced ? h->tmin : h->tab, s.w, s.due, s.rel, (reduced ? 1 : h->S) * kSlots, s.p.flags,
+                           s.obj.obj, 0, s.d.chains, false, sf, h->stream));  // keeps the incumbent in its tail
       fused = true;
     } else if (s.fused_ok) {
       EvalCall c;
@@ -1352,15 +1379,17 @@ int sb_search_seed_lpt(sb_handle* h) {
   const int J = h->J, nodes = h->nodes;
   const bool reduced = (s.p.flags & SB_FLAG_REDUCED) != 0;
   const float* tmin = h->h_tmin.data();
-  const bool spt = (s.p.flags & SB_FLAG_SUM_COMPLETION) != 0;  // shortest first: the order that favours the sum
+  const Obj obj = s.obj.obj;
+  // shortest first: the order that favours the sum (and, below, the tie-break of the due-date orders)
+  const bool spt = obj != Obj::Makespan && obj != Obj::TailMakespan;
   // weighted sum: Smith's rule (WSPT), ascending rt / w; with unit weights exactly the SPT order
-  const bool wspt = spt && (s.p.flags & SB_FLAG_WEIGHTED) != 0;
-  // tardiness: earliest due date first (EDD), ties by rt / w (rt with unit weights), then by job index; the maximum
-  // lateness the same unit-weight EDD orders (Jackson's rule, optimal for L_max on one machine)
-  const bool edd = (spt && (s.p.flags & SB_FLAG_DUE) != 0) || (s.p.flags & SB_FLAG_MAX_LATENESS) != 0;
+  const bool wspt = spt && s.obj.weighted;
+  // the due-date objectives: earliest due date first (EDD), ties by rt / w (rt with unit weights), then by job index;
+  // the maximum lateness the same unit-weight EDD orders (Jackson's rule, optimal for L_max on one machine)
+  const bool edd = obj_due(obj);
   const bool rel = (s.p.flags & SB_FLAG_RELEASE) != 0;
   // the late count: each EDD order repaired by Moore-Hodgson's rule (see moore_hodgson)
-  const bool late = (s.p.flags & SB_FLAG_LATE_COUNT) != 0;
+  const bool late = obj == Obj::LateCount;
   const double INF = HUGE_VAL;
   // usable cells: the ones the search proposes (k_build_valid), per job: those below the sentinel threshold, and for
   // a job with none only its cheapest finite cell (the first minimum; column 0 if it has no finite cell)
@@ -1432,7 +1461,7 @@ int sb_search_seed_lpt(sb_handle* h) {
       if (nodes > 1)
         for (int j = 0; j < J; ++j) node[j] = opt[j] >> 3;
       const std::vector<float>* r = rel ? ((s.p.flags & SB_FLAG_INTEGER_STARTS) ? &h->h_rc : &h->h_r) : nullptr;
-      moore_hodgson(order, col, rt, node, nodes, (s.p.flags & SB_FLAG_WEIGHTED) ? &h->h_w : nullptr, h->h_d, r,
+      moore_hodgson(order, col, rt, node, nodes, s.obj.weighted ? &h->h_w : nullptr, h->h_d, r,
                     (s.p.flags & SB_FLAG_INTEGER_STARTS) != 0);
     }
     for (int q = 0; q < J; ++q) { prio8[q] = static_cast<uint8_t>(order[q]); prio16[q] = static_cast<uint16_t>(order[q]); }
@@ -1561,8 +1590,8 @@ static int search_run_impl(sb_handle** hs, int n, const sb_search_params* p, con
   unsigned long long best = 0, key = 0;
   if ((rc = exchange(&best))) return rc;
   record(best);
-  // SB_FLAG_DUE: a tardiness of +0 (key bits 0) cannot be beaten
-  const bool stop_at_zero = (p->flags & SB_FLAG_DUE) != 0;
+  // a score of +0 (key bits 0) cannot be beaten
+  const bool stop_at_zero = tardiness_form(hs[0]->search.obj.obj);
   int done = 0, stale = 0, reason = (stop_at_zero && (best >> 32) == 0) ? 3 : 0;
   bool first_group = true;
   while (reason == 0 && done < c->rounds) {
@@ -1633,7 +1662,9 @@ int sb_search_wave(sb_handle* h, unsigned flags, int64_t* chains) {
   const bool reduced = (flags & SB_FLAG_REDUCED) != 0;
   const int SG = (reduced ? 1 : h->S) * kSlots;
   const int pb = h->J <= 256 ? 1 : 2;
-  const int arrays = job_arrays(flags);
+  Objective o;
+  if (int rc = decode_objective(flags, &o)) return rc;
+  const int arrays = job_arrays(o.obj, flags);
   int warps = 0;
   TilePlan tp;
   if (search_round_mode(h->dev, h->J, SG, h->nodes, arrays) == 2) {

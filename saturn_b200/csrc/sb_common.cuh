@@ -18,6 +18,32 @@ constexpr float kSentinel = 1.0e6f;  // reference's "unprofiled" runtime, Perfor
 
 __device__ __forceinline__ float inf_f() { return __int_as_float(0x7f800000); }
 
+// ---------------------------------------------------------------- the objective
+// The seven scores the kernels compute, and the SB_FLAG_* bits that select each (sb_api.cu: decode_objective; every
+// form also runs with SB_FLAG_RELEASE).  C is a job's completion, w its weight, d its due date.
+//   Obj           flags                                              score
+//   Makespan      none                                               max C
+//   TailMakespan  MAX_LATENESS                                       max (C + q), tails q = max d - d (L_max + max d)
+//   Sum           SUM_COMPLETION                                     sum C
+//   WeightedSum   SUM_COMPLETION | WEIGHTED                          sum w C
+//   Tardiness     SUM_COMPLETION | DUE [| WEIGHTED]                  sum w max(C - d, 0), unit weights without WEIGHTED
+//   LateCount     SUM_COMPLETION | DUE | LATE_COUNT [| WEIGHTED]     sum (C > d ? w : 0)
+//   MaxTardiness  SUM_COMPLETION | DUE | MAX_TARDINESS [| WEIGHTED]  max w max(C - d, 0)
+// Every other combination of those flags is refused.  The history of each form is in DESIGN.md.
+enum class Obj { Makespan, TailMakespan, Sum, WeightedSum, Tardiness, LateCount, MaxTardiness };
+// the score is a sum over the jobs, folded in schedule order
+__host__ __device__ constexpr bool obj_sum(Obj o) {
+  return o == Obj::Sum || o == Obj::WeightedSum || o == Obj::Tardiness || o == Obj::LateCount;
+}
+// the score reads the job weights (the caller's, or unit weights without SB_FLAG_WEIGHTED)
+__host__ __device__ constexpr bool obj_weights(Obj o) {
+  return o == Obj::WeightedSum || o == Obj::Tardiness || o == Obj::LateCount || o == Obj::MaxTardiness;
+}
+// the score reads the due-date array: the due dates, or TailMakespan's tails
+__host__ __device__ constexpr bool obj_due(Obj o) {
+  return o == Obj::TailMakespan || o == Obj::Tardiness || o == Obj::LateCount || o == Obj::MaxTardiness;
+}
+
 // ---------------------------------------------------------------- mbarrier + TMA bulk copy (1-D)
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
@@ -149,42 +175,30 @@ __device__ __forceinline__ float fmax3_mk(float mk, float b, float c) {
   return __int_as_float(__vimax3_s32(__float_as_int(mk), __float_as_int(b), __float_as_int(c)));
 }
 
-// kTrackMk: fold this job's completion (s + rt) into mk.  Needed with integer starts (the slot
-// state holds s + ceil(rt), not the completion) and with several nodes (no single f[7] at the end).
-// `ph` pairs the completions of two consecutive steps into one 3-input max: 0 parks this step's
-// completion in `pend`, 1 folds max(mk, pend, completion); callers with unrolled loops pass t & 1 (a
-// compile-time constant after unrolling), others pass -1 for the plain 2-input max.  A parked value
-// that is never folded is picked up by the final max(mk, pend) (LaneState::result).
-// kSum (SB_FLAG_SUM_COMPLETION): mk is the running SUM of completions instead, one add per step in schedule
-// order (acc = acc + (s + rt), the oracle's left fold bit for bit); `ph` and `pend` are unused, and the
-// completion is tracked whatever kTrackMk says.  The slot update is the same: only the score differs.
-// kWeighted (SB_FLAG_WEIGHTED, with kSum only): the job's weight `w` scales its completion, acc = acc + (w * e) with
-// TWO roundings (__fmul_rn, __fadd_rn: nvcc would otherwise contract them into one FFMA, which the oracle cannot
-// reproduce); w = 1 then gives the unweighted fold bit for bit.
-// kDue (SB_FLAG_DUE, with kWeighted only): the job's tardiness max(e - d, +0) against its due date `d` takes the
-// completion's place, acc = acc + (w * max(e - d, +0)), each step rounded on its own; d = 0 gives the weighted fold.
-// kDue = 2 (SB_FLAG_LATE_COUNT, with kSum and kWeighted only): the job's weight if it is late, acc = acc + (e > d ? w
-// : +0), one rounding per step; a job that completes exactly at its due date is on time (as its tardiness is +0).
-// kDue = 3 (SB_FLAG_MAX_TARDINESS, with kSum and kWeighted only): the maximum weighted tardiness, mk = max(mk, w *
-// max(e - d, +0)), the tardiness form's term bit for bit folded with max instead of +.  Every term is >= +0, so mk is
-// exact at every step like a sum (no parked `pend`); a job with no runtime (rt = +inf, w > 0) gives a +inf term.
-// kDue without kSum (SB_FLAG_MAX_LATENESS): the tail makespan max(e + d), where `d` is the job's delivery tail
-// q = max_t d_t - d_t >= +0 (not its due date), so that the score is L_max + max_t d_t >= +0.  x = e + d is one
-// rounding, and x is folded like the makespan's completion (`ph`, `pend`), whatever kTrackMk says: f[7] is not x.
-// kRelease (SB_FLAG_RELEASE, with any of the above): the job starts no earlier than its release date `r`,
-// s = max(f[km1], r) (ceil(r) under integer starts, made once by sb_set_release, so s stays an integer).  The slot
-// update below stays valid because it only needs v >= f[km1]; r <= 0 gives s = f[km1] exactly.
-// kDue is 0 (no due dates), 1 (tardiness with kSum, the tail makespan without), 2 (the late count) or 3 (the
-// maximum weighted tardiness).
-template <bool kIntegerStarts, bool kTrackMk = kIntegerStarts, bool kSum = false, bool kWeighted = false,
-          int kDue = 0, bool kRelease = false>
+// The job's completion e = s + rt is folded into mk by the objective kObj; `w` is the job's weight, `d` its due date
+// (TailMakespan: its tail q), each read only by the forms that use it.  Every product and sum is rounded on its own
+// (__fmul_rn, __fadd_rn: nvcc would otherwise contract them into one FFMA, which the oracle cannot reproduce).
+//   Makespan     : only with kTrackMk (integer starts: the slot state holds s + ceil(rt), not the completion; several
+//                  nodes: no single f[7] at the end), mk = max(mk, e).  `ph` pairs the completions of two consecutive
+//                  steps into one 3-input max: 0 parks this step's completion in `pend`, 1 folds max(mk, pend, e);
+//                  callers with unrolled loops pass t & 1 (a compile-time constant after unrolling), others pass -1
+//                  for the plain 2-input max.  A parked value that is never folded is picked up by the final
+//                  max(mk, pend) (LaneState::result).
+//   TailMakespan : x = e + q, one rounding, folded like the makespan's completion (`ph`, `pend`) whatever kTrackMk
+//                  says: f[7] is not x.  q = max_t d_t - d_j >= +0, so the score is L_max + max_t d_t >= +0.
+//   the others   : mk is exact after every step (nothing parked, `ph` unused), one fold per step in schedule order,
+//                  the oracle's left fold bit for bit.  Sum: mk + e.  WeightedSum: mk + w * e (w = 1 gives Sum bit for
+//                  bit).  Tardiness: mk + w * max(e - d, +0) (d = 0 gives WeightedSum).  LateCount: mk + (e > d ? w :
+//                  +0); a job that completes exactly at its due date is on time.  MaxTardiness: max(mk, w * max(e - d,
+//                  +0)), Tardiness's term bit for bit folded with max; a job with no runtime (rt = +inf, w > 0) gives
+//                  a +inf term.
+// The slot update is the same under every objective: only the score differs.
+// kRelease (SB_FLAG_RELEASE): the job starts no earlier than its release date `r`, s = max(f[km1], r) (ceil(r) under
+// integer starts, made once by sb_set_release, so s stays an integer).  The slot update below stays valid because it
+// only needs v >= f[km1]; r <= 0 gives s = f[km1] exactly.
+template <bool kIntegerStarts, bool kTrackMk = kIntegerStarts, Obj kObj = Obj::Makespan, bool kRelease = false>
 __device__ __forceinline__ void ls_step(float (&f)[8], float& mk, float& pend, float rt, int km1, int one, int ph,
                                         float w = 0.f, float d = 0.f, float r = 0.f) {
-  static_assert(kSum || !kWeighted, "weights scale the sum of completion times only");
-  static_assert(kWeighted || !kDue || !kSum, "tardiness runs on the weighted form (unit weights for plain tardiness)");
-  static_assert(!(kDue && !kSum && kWeighted), "the tail makespan is not weighted");
-  static_assert(kDue != 2 || kSum, "the late count is a sum");
-  static_assert(kDue != 3 || kSum, "the maximum tardiness runs on the weighted tardiness form");
   const float INF = inf_f();
   const int b2 = km1 & 4, b1 = km1 & 2, b0 = km1 & 1;
   // stage "shift by 4"
@@ -205,26 +219,26 @@ __device__ __forceinline__ void ls_step(float (&f)[8], float& mk, float& pend, f
   } else {
     v = s + rt;
   }
-  if (kSum) {
-    const float e = kIntegerStarts ? s + rt : v;
-    // the late count: w * 1 = w and w * 0 = +0 exactly (w > 0 finite), so this adds (e > d ? w : +0); the product
-    // keeps the tardiness form's data flow, which ptxas allocates without the spills a bare select causes in some
-    // position-major search kernels at the 128-register cap
-    if (kDue == 2) mk = __fadd_rn(mk, __fmul_rn(w, e > d ? 1.f : 0.f));
-    // the maximum tardiness, max(mk, w * max(e - d, +0)), as one integer max over the product's bits: mk >= +0, and
-    // w * (e - d) with w > 0 is either that term (e - d > 0), or +0, a negative value or -0 (e - d <= 0), which all
-    // lose to mk as signed integers exactly as the +0 term does as a float.  Same value, one FMNMX fewer; the
-    // float form gave two position-major search kernels more spills than their tardiness siblings
-    else if (kDue == 3)
-      mk = __int_as_float(max(__float_as_int(mk), __float_as_int(__fmul_rn(w, __fsub_rn(e, d)))));
-    else if (kDue) mk = __fadd_rn(mk, __fmul_rn(w, fmaxf(__fsub_rn(e, d), 0.f)));
-    else if (kWeighted) mk = __fadd_rn(mk, __fmul_rn(w, e));
-    else mk = mk + e;
-  } else if (kDue) {
+  if constexpr (kObj == Obj::TailMakespan) {
     const float x = __fadd_rn(kIntegerStarts ? s + rt : v, d);
     if (ph < 0) mk = fmaxf(mk, x);
     else if (ph == 0) pend = x;
     else mk = fmax3_mk(mk, pend, x);
+  } else if constexpr (kObj != Obj::Makespan) {
+    const float e = kIntegerStarts ? s + rt : v;
+    // the late count: w * 1 = w and w * 0 = +0 exactly (w > 0 finite), so this adds (e > d ? w : +0); the product
+    // keeps the tardiness form's data flow, which ptxas allocates without the spills a bare select causes in some
+    // position-major search kernels at the 128-register cap
+    if constexpr (kObj == Obj::LateCount) mk = __fadd_rn(mk, __fmul_rn(w, e > d ? 1.f : 0.f));
+    // the maximum tardiness, max(mk, w * max(e - d, +0)), as one integer max over the product's bits: mk >= +0, and
+    // w * (e - d) with w > 0 is either that term (e - d > 0), or +0, a negative value or -0 (e - d <= 0), which all
+    // lose to mk as signed integers exactly as the +0 term does as a float.  Same value, one FMNMX fewer; the
+    // float form gave two position-major search kernels more spills than their tardiness siblings
+    else if constexpr (kObj == Obj::MaxTardiness)
+      mk = __int_as_float(max(__float_as_int(mk), __float_as_int(__fmul_rn(w, __fsub_rn(e, d)))));
+    else if constexpr (kObj == Obj::Tardiness) mk = __fadd_rn(mk, __fmul_rn(w, fmaxf(__fsub_rn(e, d), 0.f)));
+    else if constexpr (kObj == Obj::WeightedSum) mk = __fadd_rn(mk, __fmul_rn(w, e));
+    else mk = mk + e;
   } else if (kTrackMk) {
     const float e = kIntegerStarts ? s + rt : v;
     if (ph < 0) mk = fmaxf(mk, e);

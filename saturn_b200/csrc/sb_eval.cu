@@ -26,20 +26,11 @@
 //     conflict-free); a step loads the state of the job's node, updates it, stores it back;
 //   * makespans are written coalesced (128 B per warp); an optional 64-bit arg-min key is
 //     folded with one redux + one atomicMin per warp;
-//   * SUM (SB_FLAG_SUM_COMPLETION): every kernel here also comes in a form that scores the sum of completion
-//     times instead of the makespan (ls_step<..., kSum>); the schedule, and every start, is the same;
-//   * W (SB_FLAG_WEIGHTED, with SUM only): the sum is weighted per job.  The weights sit beside the table wherever
-//     the table is in shared memory (same TMA phase), and are read from global memory where the table is;
-//   * D (SB_FLAG_DUE, with W only): the weighted sum is of tardiness against per-job due dates instead of
-//     completions.  The due dates follow the weights, in the same memory and the same TMA phase;
-//   * D = 2 (SB_FLAG_LATE_COUNT, with W only): the weighted sum is of the late jobs' weights, w_j [C_j > d_j],
-//     instead of their tardiness (ls_step<..., kDue = 2>), on the same due dates in the same memory;
-//   * D = 3 (SB_FLAG_MAX_TARDINESS, with W only): the weighted tardiness terms are folded with max instead of +,
-//     max_j w_j max(C_j - d_j, +0) (ls_step<..., kDue = 3>), on the same weights and due dates in the same memory;
-//   * D without SUM (SB_FLAG_MAX_LATENESS): the tail makespan max_j (C_j + q_j) with delivery tails q_j =
-//     max_t d_t - d_j >= 0, i.e. L_max + max_t d_t (ls_step<..., kDue> without kSum).  The tails take the due
-//     dates' place, in the same memory and the same TMA phase;
-//   * R (SB_FLAG_RELEASE, with any of the above): no job starts before its release date.  Every objective form has
+//   * OBJ: every kernel here comes in a form per objective (sb_common.cuh: Obj), folded by ls_step; the schedule,
+//     and every start, is the same under all of them.  The per-job arrays an objective reads (weights,
+//     due dates or tails) sit beside the table wherever the table is in shared memory (same TMA phase), and are
+//     read from global memory where the table is;
+//   * R (SB_FLAG_RELEASE, with any objective): no job starts before its release date.  Every objective form has
 //     a release twin; the release dates follow the other per-job arrays, in the same memory and TMA phase.
 #include "sb_lane.cuh"
 
@@ -63,8 +54,8 @@ struct TileArgs {
   int one;  // run-time 1 (see pmov_fma)
   SearchFuse sf;  // SEARCH variant only
   XchgPost xp;    // xp.counter != nullptr: the last CTA to finish posts *best_key to every peer's mailbox
-  const float* w;  // W: job weights [J], zero-padded to a multiple of 4 (16 bytes)
-  const float* d;  // D: job due dates [J], padded the same way
+  const float* w;  // obj_weights(OBJ): job weights [J], zero-padded to a multiple of 4 (16 bytes)
+  const float* d;  // obj_due(OBJ): job due dates (or tails) [J], padded the same way
   const float* r;  // R: job release dates [J], padded the same way
   // the streamed tile kernel (STREAM, one node, table in shared memory) only; see "Tile boundaries" below
   int packed;    // consecutive candidates' rows lie back to back (stride_o == copy_o == row_o, stride_p == copy_p)
@@ -75,20 +66,19 @@ struct TileArgs {
 // TABG: the runtime table stays in global memory (read through L1/L2) — for tables larger than the
 // shared memory left beside the opt tiles (e.g. J = 1024 with 8 strategies: 256 KB).
 template <int PB, bool INT, bool STREAM, bool MULTI, bool SEARCH = false, bool TABG = false, int ADDR = 0,
-          bool SUM = false, bool W = false, int D = 0, bool R = false>
+          Obj OBJ = Obj::Makespan, bool R = false>
 __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const TileArgs a) {
   static_assert(!(SEARCH && (STREAM || TABG)), "the fused search round runs on shared-memory tiles only");
   static_assert(ADDR == 0 || (!TABG && !MULTI && !SEARCH), "ADDR = 1 needs the table and the opt rows in shared memory");
-  static_assert(SUM || !W, "weights scale the sum of completion times only");
-  static_assert(W || !D || !SUM, "tardiness runs on the weighted form");
   extern __shared__ __align__(128) uint8_t smem[];
   const int nw = blockDim.x >> 5;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t tab_bytes = TABG ? 0u : static_cast<uint32_t>(a.J) * a.SG * 4u;  // a multiple of 32 (SG = S * 8)
-  // W: the weights follow the table in the same TMA phase, padded to 16 bytes (TABG: both stay in global memory);
-  // D: the due dates follow the weights the same way; R: the release dates follow them
-  const uint32_t w_bytes = (W && !TABG) ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u;
-  const uint32_t d_bytes = D ? (W ? w_bytes : (TABG ? 0u : ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u))) : 0u;
+  // the per-job arrays the objective reads follow the table in the same TMA phase, each padded to 16 bytes: the
+  // weights, the due dates (or tails), the release dates (TABG: they all stay in global memory)
+  constexpr bool kW = obj_weights(OBJ), kD = obj_due(OBJ);
+  const uint32_t w_bytes = (kW && !TABG) ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u;
+  const uint32_t d_bytes = kD ? (kW ? w_bytes : (TABG ? 0u : ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u))) : 0u;
   const uint32_t r_bytes = (R && !TABG) ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u;
   float* tab_s = reinterpret_cast<float*>(smem);
   [[maybe_unused]] float* w_s = reinterpret_cast<float*>(smem + tab_bytes);
@@ -120,33 +110,20 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
         uint32_t n = min(32768u, tab_bytes - off);
         tma_bulk_g2s(smem + off, src + off, n, bar_tab);
       }
-      if constexpr (W) {
-        const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(a.w);
-        for (uint32_t off = 0; off < w_bytes; off += 32768u)
-          tma_bulk_g2s(smem + tab_bytes + off, wsrc + off, min(32768u, w_bytes - off), bar_tab);
-      }
-      if constexpr (D != 0) {
-        const uint8_t* dsrc = reinterpret_cast<const uint8_t*>(a.d);
-        for (uint32_t off = 0; off < d_bytes; off += 32768u)
-          tma_bulk_g2s(smem + tab_bytes + w_bytes + off, dsrc + off, min(32768u, d_bytes - off), bar_tab);
-      }
-      if constexpr (R) {
-        const uint8_t* rsrc = reinterpret_cast<const uint8_t*>(a.r);
-        for (uint32_t off = 0; off < r_bytes; off += 32768u)
-          tma_bulk_g2s(smem + tab_bytes + w_bytes + d_bytes + off, rsrc + off, min(32768u, r_bytes - off), bar_tab);
-      }
+      if constexpr (kW) stage_job_array(smem + tab_bytes, a.w, w_bytes, bar_tab);
+      if constexpr (kD) stage_job_array(smem + tab_bytes + w_bytes, a.d, d_bytes, bar_tab);
+      if constexpr (R) stage_job_array(smem + tab_bytes + w_bytes + d_bytes, a.r, r_bytes, bar_tab);
     }
   }
 
-  LaneState<INT, MULTI, ADDR, SUM, (W ? (TABG ? 2 : 1) : 0), (D ? (TABG ? 2 : 1) : 0), (R ? (TABG ? 2 : 1) : 0),
-            (D == 0 ? 1 : D)> st;
+  LaneState<INT, MULTI, ADDR, OBJ, TABG ? 2 : 1, R> st;
   if (TABG) st.tab = a.tab;
   else st.tab = tab_s;
-  if constexpr (W) {
+  if constexpr (kW) {
     st.wt = TABG ? a.w : w_s;
     st.wt_s = smem_u32(w_s);
   }
-  if constexpr (D != 0) {
+  if constexpr (kD) {
     st.dd = TABG ? a.d : d_s;
     st.dd_s = smem_u32(d_s);
   }
@@ -308,8 +285,8 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
         const int nch = (J + STEPS - 1) / STEPS, nfull = J / STEPS;
         uint32_t ob[kBatch];
         float rb[kBatch];
-        [[maybe_unused]] float wb[kBatch];  // W: the batch's weights, gathered with its runtimes
-        [[maybe_unused]] float db[kBatch];  // D: the batch's due dates (or tails), likewise
+        [[maybe_unused]] float wb[kBatch];  // kW: the batch's weights, gathered with its runtimes
+        [[maybe_unused]] float db[kBatch];  // kD: the batch's due dates (or tails), likewise
         [[maybe_unused]] float xb[kBatch];  // R: the batch's release dates, likewise
         auto resolve = [&](const uint32_t* w) {  // w: the kBatch / 4 words that hold the batch's job ids
           int js[kBatch];
@@ -319,11 +296,11 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
           for (int i = 0; i < kBatch; ++i) ob[i] = st.gather_opt(js[i]);
 #pragma unroll
           for (int i = 0; i < kBatch; ++i) rb[i] = st.gather_rt(js[i], ob[i]);
-          if constexpr (W) {
+          if constexpr (kW) {
 #pragma unroll
             for (int i = 0; i < kBatch; ++i) wb[i] = st.gather_w(js[i]);
           }
-          if constexpr (D != 0) {
+          if constexpr (kD) {
 #pragma unroll
             for (int i = 0; i < kBatch; ++i) db[i] = st.gather_d(js[i]);
           }
@@ -354,11 +331,11 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
             [[maybe_unused]] float xc[kBatch];
 #pragma unroll
             for (int i = 0; i < kBatch; ++i) { oc[i] = ob[i]; rc[i] = rb[i]; }
-            if constexpr (W) {
+            if constexpr (kW) {
 #pragma unroll
               for (int i = 0; i < kBatch; ++i) wc[i] = wb[i];
             }
-            if constexpr (D != 0) {
+            if constexpr (kD) {
 #pragma unroll
               for (int i = 0; i < kBatch; ++i) dc[i] = db[i];
             }
@@ -368,13 +345,9 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
             }
             resolve(b + 1 < STEPS / kBatch ? q.w + (b + 1) * (kBatch / 4) : head);
 #pragma unroll
-            for (int i = 0; i < kBatch; ++i) {
-              const float x = R ? xc[i] : 0.f;
-              if constexpr (D != 0)
-                st.step_resolved(static_cast<int>(oc[i]), rc[i], i & 1, W ? wc[i] : 0.f, dc[i], x);
-              else if constexpr (W) st.step_resolved(static_cast<int>(oc[i]), rc[i], i & 1, wc[i], 0.f, x);
-              else st.step_resolved(static_cast<int>(oc[i]), rc[i], i & 1, 0.f, 0.f, x);
-            }
+            for (int i = 0; i < kBatch; ++i)
+              st.step_resolved(static_cast<int>(oc[i]), rc[i], i & 1, kW ? wc[i] : 0.f, kD ? dc[i] : 0.f,
+                               R ? xc[i] : 0.f);
           }
           q = nxt;
         }
@@ -434,9 +407,8 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
     // SEARCH rounds: score the lane's rows from window `w0` on (warp-uniform).  w0 > 0 resumes from the
     // snapshot taken in front of that window (buffer bit w0-1 of `par`); `save` stores the state in front of
     // every later window into the OTHER buffer (the proposal's boundary states; the caller flips the bits of
-    // `par` if it accepts the move).  Snapshot = the 8 sorted slot times + the running score (makespan, or the
-    // running sum with SUM); a completion parked in `pend` is always folded at a window boundary (even number of
-    // steps per window) — the sum parks nothing, so its snapshot is exact at any step.
+    // `par` if it accepts the move).  Snapshot = the 8 sorted slot times + the running score (LaneState::running);
+    // a completion parked in `pend` is always folded at a window boundary (even number of steps per window).
     [[maybe_unused]] auto eval_from = [&](const uint8_t* prio_row_s, int w0, uint32_t par, bool save,
                                           float* snap_t) -> float {
       const int J = a.J;
@@ -679,15 +651,13 @@ struct GenericArgs {
   int tab_in_smem;
   int nodes;
   int one;
-  const float* w;  // W: job weights [J], read with ld.global.nc
-  const float* d;  // D: job due dates [J], likewise
+  const float* w;  // obj_weights(OBJ): job weights [J], read with ld.global.nc
+  const float* d;  // obj_due(OBJ): job due dates (or tails) [J], likewise
   const float* r;  // R: job release dates [J], likewise
 };
 
-template <int PB, bool INT, bool MULTI, bool SUM = false, bool W = false, int D = 0, bool R = false>
+template <int PB, bool INT, bool MULTI, Obj OBJ = Obj::Makespan, bool R = false>
 __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
-  static_assert(SUM || !W, "weights scale the sum of completion times only");
-  static_assert(W || !D || !SUM, "tardiness runs on the weighted form");
   extern __shared__ __align__(128) uint8_t smem[];
   const float* tab = a.tab;
   const uint32_t node_bytes = MULTI ? static_cast<uint32_t>(a.nodes) * 1024u : 0u;  // per warp
@@ -700,7 +670,7 @@ __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
     tab = tab_s;
   }
   const int lane = threadIdx.x & 31;
-  LaneState<INT, MULTI, 0, SUM, (W ? 2 : 0), (D ? 2 : 0), (R ? 2 : 0), (D == 0 ? 1 : D)> st;
+  LaneState<INT, MULTI, 0, OBJ, 2, R> st;
   st.tab = tab;
   st.wt = a.w;
   st.dd = a.d;
@@ -730,29 +700,24 @@ __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
         for (int t = 0; t < BATCH; ++t) os[t] = st.lookup_opt(js[t]);
 #pragma unroll
         for (int t = 0; t < BATCH; ++t) rts[t] = st.lookup_rt(js[t], os[t]);
-        [[maybe_unused]] float xs[BATCH];  // R: the batch's release dates, gathered with its runtimes
+        // the batch's release dates, weights and due dates (or tails), gathered with its runtimes
+        [[maybe_unused]] float xs[BATCH], ws[BATCH], ds[BATCH];
         if constexpr (R) {
 #pragma unroll
           for (int t = 0; t < BATCH; ++t) xs[t] = st.lookup_r(js[t]);
         }
-        if constexpr (D != 0) {
-          float ws[BATCH], ds[BATCH];
+        if constexpr (obj_weights(OBJ)) {
 #pragma unroll
           for (int t = 0; t < BATCH; ++t) ws[t] = st.lookup_w(js[t]);
+        }
+        if constexpr (obj_due(OBJ)) {
 #pragma unroll
           for (int t = 0; t < BATCH; ++t) ds[t] = st.lookup_d(js[t]);
-#pragma unroll
-          for (int t = 0; t < BATCH; ++t) st.step_resolved(os[t], rts[t], t & 1, ws[t], ds[t], R ? xs[t] : 0.f);
-        } else if constexpr (W) {
-          float ws[BATCH];
-#pragma unroll
-          for (int t = 0; t < BATCH; ++t) ws[t] = st.lookup_w(js[t]);
-#pragma unroll
-          for (int t = 0; t < BATCH; ++t) st.step_resolved(os[t], rts[t], t & 1, ws[t], 0.f, R ? xs[t] : 0.f);
-        } else {
-#pragma unroll
-          for (int t = 0; t < BATCH; ++t) st.step_resolved(os[t], rts[t], t & 1, 0.f, 0.f, R ? xs[t] : 0.f);
         }
+#pragma unroll
+        for (int t = 0; t < BATCH; ++t)
+          st.step_resolved(os[t], rts[t], t & 1, obj_weights(OBJ) ? ws[t] : 0.f, obj_due(OBJ) ? ds[t] : 0.f,
+                           R ? xs[t] : 0.f);
       }
       for (; i < a.J; ++i) st.step(PB == 1 ? prow[i] : reinterpret_cast<const uint16_t*>(prow)[i]);
       mk = st.result(a.nodes);
@@ -779,15 +744,15 @@ struct FullArgs {
   float* out;
   float* start;         // [B][J] by job, nullable
   uint32_t* slotmask;   // [B][J] by job, nullable
-  const float* w;       // W: job weights [J]
-  const float* d;       // D: job due dates [J] (without SUM: the delivery tails)
+  const float* w;       // obj_weights(OBJ): job weights [J]
+  const float* d;       // obj_due(OBJ): job due dates [J] (TailMakespan: the delivery tails)
   const float* r;       // R: job release dates [J] (ceiled with INT)
 };
 
-template <int PB, bool INT, bool SUM = false, bool W = false, int D = 0, bool R = false>
+// The score is folded here on its own, not through ls_step: this kernel is the library's slot-exact cross-check of
+// the fast kernels, so it restates every objective's fold (in the same fp32 operations).
+template <int PB, bool INT, Obj OBJ = Obj::Makespan, bool R = false>
 __global__ void __launch_bounds__(128) k_eval_full(const FullArgs a) {
-  static_assert(SUM || !W, "weights scale the sum of completion times only");
-  static_assert(W || !D || !SUM, "tardiness runs on the weighted form");
   const long long nthreads = static_cast<long long>(gridDim.x) * blockDim.x;
   const bool multi = a.nodes > 1;
   for (long long b = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; b < a.B; b += nthreads) {
@@ -823,17 +788,16 @@ __global__ void __launch_bounds__(128) k_eval_full(const FullArgs a) {
       const float nxt = s + hold;
       for (int g = 0; g < kSlots; ++g)
         if ((taken >> g) & 1u) rd[g] = nxt;
-      if constexpr (D != 0 && !SUM)  // ls_step<..., kDue>: the tail makespan
+      if constexpr (OBJ == Obj::TailMakespan)
         mk = fmaxf(mk, __fadd_rn(s + rt, __ldg(a.d + j)));
-      else if constexpr (D == 2)  // ls_step<..., kSum, kWeighted, kDue = 2>: the late count, +inf once a job has
-        // no runtime (LaneState::result)
+      else if constexpr (OBJ == Obj::LateCount)  // +inf once a job has no runtime (LaneState::result)
         mk = isinf(s + rt) ? INFINITY : __fadd_rn(mk, __fmul_rn(__ldg(a.w + j), s + rt > __ldg(a.d + j) ? 1.f : 0.f));
-      else if constexpr (D == 3)  // ls_step<..., kSum, kWeighted, kDue = 3>: the maximum weighted tardiness
+      else if constexpr (OBJ == Obj::MaxTardiness)
         mk = fmaxf(mk, __fmul_rn(__ldg(a.w + j), fmaxf(__fsub_rn(s + rt, __ldg(a.d + j)), 0.f)));
-      else if constexpr (D != 0)  // ls_step<..., kSum, kWeighted, kDue>
+      else if constexpr (OBJ == Obj::Tardiness)
         mk = __fadd_rn(mk, __fmul_rn(__ldg(a.w + j), fmaxf(__fsub_rn(s + rt, __ldg(a.d + j)), 0.f)));
-      else if constexpr (W) mk = __fadd_rn(mk, __fmul_rn(__ldg(a.w + j), s + rt));  // ls_step<..., kSum, kWeighted>
-      else if (SUM) mk = mk + (s + rt);  // the left fold in schedule order of ls_step<..., kSum>
+      else if constexpr (OBJ == Obj::WeightedSum) mk = __fadd_rn(mk, __fmul_rn(__ldg(a.w + j), s + rt));
+      else if constexpr (OBJ == Obj::Sum) mk = mk + (s + rt);  // the left fold in schedule order
       else mk = fmaxf(mk, s + rt);
       if (a.start) a.start[b * a.J + j] = s;
       if (a.slotmask) a.slotmask[b * a.J + j] = (static_cast<uint32_t>(node) << 16) | taken;
@@ -946,7 +910,7 @@ cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, i
   const bool bulk_ok = bulk_aligned(c);
   const bool stream_ok = bulk_ok && (c.stride_p % 32 == 0) && (reinterpret_cast<uintptr_t>(c.prio) % 32 == 0) &&
                          !(c.flags & HOOK_NO_STREAM);
-  const int arrays = job_arrays(c.flags);
+  const int arrays = job_arrays(c.obj, c.flags);
   TilePlan tp;
   int nw = 0;
   bool stream = false, tabg = false;
@@ -976,14 +940,14 @@ cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, i
       a.stagger = !(c.tile_debug & TILE_DEBUG_NO_STAGGER);
       a.tile_wait = c.tile_wait;
     }
-    const TileKernel kern = with_eval_types(pb, c.flags, [&](auto PB, auto INT, auto SUM, auto W, auto D, auto R) -> TileKernel {
-      if (tabg) return k_eval_tiles<PB, INT, true, false, false, true, 0, SUM, W, D, R>;
+    const TileKernel kern = with_eval_types(pb, c.flags, c.obj, [&](auto PB, auto INT, auto OBJ, auto R) -> TileKernel {
+      if (tabg) return k_eval_tiles<PB, INT, true, false, false, true, 0, OBJ, R>;
       if constexpr (PB == 1) {
-        if (fma_addr) return k_eval_tiles<1, INT, true, false, false, false, 1, SUM, W, D, R>;
+        if (fma_addr) return k_eval_tiles<1, INT, true, false, false, false, 1, OBJ, R>;
       }
       return with_bool(stream, [&](auto STREAM) {
         return with_bool(multi, [&](auto MULTI) -> TileKernel {
-          return k_eval_tiles<PB, INT, STREAM, MULTI, false, false, 0, SUM, W, D, R>;
+          return k_eval_tiles<PB, INT, STREAM, MULTI, false, false, 0, OBJ, R>;
         });
       });
     });
@@ -1004,8 +968,8 @@ cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, i
   long long cap = static_cast<long long>(dev.sm_count) * 8;
   int grid = static_cast<int>(blocks < cap ? blocks : cap);
   if (grid < 1) grid = 1;
-  const auto kern = with_eval_types(pb, c.flags, [&](auto PB, auto INT, auto SUM, auto W, auto D, auto R) {
-    return with_bool(multi, [&](auto MULTI) { return k_eval_generic<PB, INT, MULTI, SUM, W, D, R>; });
+  const auto kern = with_eval_types(pb, c.flags, c.obj, [&](auto PB, auto INT, auto OBJ, auto R) {
+    return with_bool(multi, [&](auto MULTI) { return k_eval_generic<PB, INT, MULTI, OBJ, R>; });
   });
   return launch(kern, grid, 128, smem, st, g);
 }
@@ -1026,16 +990,16 @@ cudaError_t search_round_launch(const Device& dev, const EvalCall& c, const Sear
   if (c.B <= 0) return cudaSuccess;
   const int pb = c.J <= 256 ? 1 : 2;
   TilePlan tp;
-  const int arrays = job_arrays(c.flags);
+  const int arrays = job_arrays(c.obj, c.flags);
   if (search_round_mode(dev, c.J, c.SG, c.nodes, arrays) == 0 || !bulk_aligned(c)) return cudaErrorNotSupported;
   plan_tiles(dev, c.J, c.SG, pb, false, c.nodes, &tp, false, arrays);
   if (c.stride_o < tp.copy_o || c.stride_p < tp.copy_p) return cudaErrorNotSupported;
   TileArgs a = tile_args(c, tp);
   a.use_bulk = 1;
   a.sf = sf;
-  const TileKernel kern = with_eval_types(pb, c.flags, [&](auto PB, auto INT, auto SUM, auto W, auto D, auto R) {
+  const TileKernel kern = with_eval_types(pb, c.flags, c.obj, [&](auto PB, auto INT, auto OBJ, auto R) {
     return with_bool(c.nodes > 1, [&](auto MULTI) -> TileKernel {
-      return k_eval_tiles<PB, INT, false, MULTI, true, false, 0, SUM, W, D, R>;
+      return k_eval_tiles<PB, INT, false, MULTI, true, false, 0, OBJ, R>;
     });
   });
   return launch_tiles(dev, kern, a, tp, st);
@@ -1051,8 +1015,8 @@ cudaError_t eval_full_launch(const Device& dev, const EvalCall& c, float* start,
   long long blocks = (c.B + 127) / 128;
   long long cap = static_cast<long long>(dev.sm_count) * 16;
   int grid = static_cast<int>(blocks < cap ? blocks : cap);
-  const auto kern = with_eval_types(pb, c.flags, [](auto PB, auto INT, auto SUM, auto W, auto D, auto R) {
-    return k_eval_full<PB, INT, SUM, W, D, R>;
+  const auto kern = with_eval_types(pb, c.flags, c.obj, [](auto PB, auto INT, auto OBJ, auto R) {
+    return k_eval_full<PB, INT, OBJ, R>;
   });
   return launch(kern, grid, 128, 0, st, a);
 }

@@ -54,56 +54,37 @@ template <class F>
 decltype(auto) with_pb(int pb, F&& f) {
   return pb == 1 ? f(std::integral_constant<int, 1>{}) : f(std::integral_constant<int, 2>{});
 }
-template <int N>
-using int_c = std::integral_constant<int, N>;
-// f(PB, INT, SUM, W, D, R): the prio width, SB_FLAG_INTEGER_STARTS, SB_FLAG_SUM_COMPLETION, SB_FLAG_WEIGHTED,
-// the due-date form, and SB_FLAG_RELEASE, the template arguments that every evaluation and search kernel takes.  W is
-// true only together with SUM.  D is an int: 0 without due dates, 1 for SB_FLAG_DUE (tardiness) with SUM and for
-// SB_FLAG_MAX_LATENESS (the tail makespan of ls_step) without it, 2 for SB_FLAG_DUE | SB_FLAG_LATE_COUNT (the late
-// count), 3 for SB_FLAG_DUE | SB_FLAG_MAX_TARDINESS (the maximum weighted tardiness).  With SUM, D is nonzero only
-// together with W: no kernel that weights the makespan, or that scores tardiness, the late count or the maximum
-// tardiness without weights, is ever instantiated (SB_FLAG_DUE alone runs the weighted form on unit weights, exact
-// since 1 * x = x and 1 is the count of one late job).  R is orthogonal to the other three: each objective form has a
-// release twin.
+template <Obj O>
+using obj_c = std::integral_constant<Obj, O>;
 template <class F>
-decltype(auto) with_eval_types(int pb, unsigned flags, F&& f) {
+decltype(auto) with_obj(Obj obj, F&& f) {
+  switch (obj) {
+    case Obj::TailMakespan: return f(obj_c<Obj::TailMakespan>{});
+    case Obj::Sum: return f(obj_c<Obj::Sum>{});
+    case Obj::WeightedSum: return f(obj_c<Obj::WeightedSum>{});
+    case Obj::Tardiness: return f(obj_c<Obj::Tardiness>{});
+    case Obj::LateCount: return f(obj_c<Obj::LateCount>{});
+    case Obj::MaxTardiness: return f(obj_c<Obj::MaxTardiness>{});
+    default: return f(obj_c<Obj::Makespan>{});
+  }
+}
+// f(PB, INT, OBJ, R): the prio width, SB_FLAG_INTEGER_STARTS, the objective and SB_FLAG_RELEASE, the template
+// arguments that every evaluation and search kernel takes.  R is orthogonal to OBJ: each objective has a release twin.
+template <class F>
+decltype(auto) with_eval_types(int pb, unsigned flags, Obj obj, F&& f) {
   return with_pb(pb, [&](auto PB) {
     return with_bool(flags & SB_FLAG_INTEGER_STARTS, [&](auto INT) {
       return with_bool(flags & SB_FLAG_RELEASE, [&](auto R) {
-        return with_bool(flags & SB_FLAG_SUM_COMPLETION, [&](auto SUM) {
-          if constexpr (SUM) {
-            return with_bool(flags & (SB_FLAG_WEIGHTED | SB_FLAG_DUE), [&](auto W) {
-              if constexpr (W) {
-                return with_bool(flags & SB_FLAG_DUE, [&](auto DUE) {
-                  if constexpr (DUE)
-                    return with_bool(flags & SB_FLAG_LATE_COUNT, [&](auto LATE) {
-                      if constexpr (LATE) return f(PB, INT, SUM, W, int_c<2>{}, R);
-                      else return with_bool(flags & SB_FLAG_MAX_TARDINESS, [&](auto MAXT) {
-                        return f(PB, INT, SUM, W, int_c<decltype(MAXT)::value ? 3 : 1>{}, R);
-                      });
-                    });
-                  else return f(PB, INT, SUM, W, int_c<0>{}, R);
-                });
-              } else {
-                return f(PB, INT, SUM, W, int_c<0>{}, R);
-              }
-            });
-          } else {
-            return with_bool(flags & SB_FLAG_MAX_LATENESS, [&](auto D) {
-              return f(PB, INT, SUM, std::false_type{}, int_c<decltype(D)::value ? 1 : 0>{}, R);
-            });
-          }
-        });
+        return with_obj(obj, [&](auto OBJ) { return f(PB, INT, OBJ, R); });
       });
     });
   });
 }
-// the per-job fp32 arrays a kernel stages beside the table: the weights (SB_FLAG_WEIGHTED, or the unit weights of
-// SB_FLAG_DUE alone), then the due dates (SB_FLAG_DUE) or the delivery tails (SB_FLAG_MAX_LATENESS), then the release
-// dates (SB_FLAG_RELEASE); each is padded to 16 bytes
-inline int job_arrays(unsigned flags) {
-  return ((flags & SB_FLAG_DUE) ? 2 : ((flags & SB_FLAG_WEIGHTED) ? 1 : 0)) + ((flags & SB_FLAG_MAX_LATENESS) ? 1 : 0) +
-         ((flags & SB_FLAG_RELEASE) ? 1 : 0);
+// the per-job fp32 arrays a kernel stages beside the table: the weights, then the due dates (or tails), then the
+// release dates (SB_FLAG_RELEASE), each where the objective reads it (stage_job_array, sb_lane.cuh); each is padded to 16
+// bytes
+inline int job_arrays(Obj obj, unsigned flags) {
+  return (obj_weights(obj) ? 1 : 0) + (obj_due(obj) ? 1 : 0) + ((flags & SB_FLAG_RELEASE) ? 1 : 0);
 }
 inline size_t job_array_bytes(int J) { return (static_cast<size_t>(J) * 4 + 15) & ~size_t(15); }
 
@@ -153,10 +134,10 @@ struct TilePlan {
 
 struct EvalCall {
   const float* tab = nullptr;  // canonical table actually used (full or reduced)
-  const float* w = nullptr;    // SB_FLAG_WEIGHTED: the job weights [J], padded with zeros to a multiple of 4
-                               // (SB_FLAG_DUE alone: J ones, padded the same way)
-  const float* d = nullptr;    // SB_FLAG_DUE: the job due dates [J], padded the same way (SB_FLAG_MAX_LATENESS: the
-                               // delivery tails max_t d_t - d_j, padded the same way)
+  const float* w = nullptr;    // obj_weights(obj): the job weights [J], padded with zeros to a multiple of 4 (unit
+                               // weights without SB_FLAG_WEIGHTED)
+  const float* d = nullptr;    // obj_due(obj): the job due dates [J] (TailMakespan: the delivery tails max_t d_t - d_j),
+                               // padded the same way
   const float* r = nullptr;    // SB_FLAG_RELEASE: the job release dates [J] (ceiled under SB_FLAG_INTEGER_STARTS),
                                // padded the same way
   int J = 0, SG = 0;
@@ -165,6 +146,7 @@ struct EvalCall {
   long long B = 0;
   long long stride_o = 0, stride_p = 0;  // bytes
   unsigned flags = 0;
+  Obj obj = Obj::Makespan;  // the objective the flags select (decode_objective)
   int nodes = 1;  // > 1: multi-node (reduced table, opt = (node << 3) | (k - 1))
   float* out = nullptr;
   unsigned long long* best_key = nullptr;
@@ -216,7 +198,7 @@ struct SearchFuse {
   } keep;
 };
 
-// arrays: job_arrays(flags), the per-job arrays staged beside the table (unless tab_global: then they all stay in
+// arrays: job_arrays(obj, flags), the per-job arrays staged beside the table (unless tab_global: then they all stay in
 // global memory)
 int plan_tiles(const Device& dev, int J, int SG, int pb, bool stream, int nodes, TilePlan* tp, bool tab_global = false,
                int arrays = 0);

@@ -31,43 +31,38 @@ __device__ __forceinline__ PrioChunk ld_prio32(const uint8_t* p) {
   return c;
 }
 
+// The per-job fp32 arrays a kernel stages beside its table, in this order: the weights (obj_weights), the due dates or
+// tails (obj_due), the release dates (SB_FLAG_RELEASE).  Each is padded to 16 bytes (each kernel spells the padding
+// out per array: computing it once changes the generated code) and is fetched by stage_job_array with TMA bulk
+// copies in the table's mbarrier phase.
+__device__ __forceinline__ void stage_job_array(uint8_t* dst, const float* src, uint32_t bytes, uint64_t* bar) {
+  const uint8_t* s = reinterpret_cast<const uint8_t*>(src);
+  for (uint32_t off = 0; off < bytes; off += 32768u) tma_bulk_g2s(dst + off, s + off, min(32768u, bytes - off), bar);
+}
+
 // Per-lane evaluation state + the per-job step.
 // ADDR = 1 (shared-memory table and opt rows only): the two look-up addresses of a step are formed with
 // `mad.lo` on run-time multipliers, which ptxas must issue as IMAD on the FMA pipe instead of IADD3 / LEA on
 // the ALU pipe — the step is bound by the ALU pipe (half rate) and by issue together, so the same instruction
 // count with two fewer ALU instructions is the cheaper mix.
-// SUM: score = sum of completion times (SB_FLAG_SUM_COMPLETION) instead of the makespan; mk holds the running sum.
-// WGT (SB_FLAG_WEIGHTED, with SUM only): each completion is scaled by its job's weight, read from `wt` — 1: the
-// weights are in shared memory beside the table, 2: in global memory, read with ld.global.nc.
-// DUE (SB_FLAG_DUE, with WGT only): each job's tardiness against its due date, read from `dd`, takes its
-// completion's place; without SUM (SB_FLAG_MAX_LATENESS) `dd` holds the delivery tails and the score is the tail
-// makespan (see ls_step) — 1: in shared memory beside the table, 2: in global memory, read with ld.global.nc.
-// FORM (with SUM, WGT and DUE only): what the tardiness form folds per job, ls_step's kDue — 1: the weighted
-// tardiness, summed; 2 (SB_FLAG_LATE_COUNT): the job's weight if it is late, summed; 3 (SB_FLAG_MAX_TARDINESS): the
-// weighted tardiness, folded with max.  Without SUM a nonzero DUE is always the tail makespan (kDue = 1).
-// REL (SB_FLAG_RELEASE, with any objective): no job starts before its release date, read from `rr` — 1: in shared
-// memory beside the table, 2: in global memory, read with ld.global.nc.
-template <bool INT, bool MULTI, int ADDR = 0, bool SUM = false, int WGT = 0, int DUE = 0, int REL = 0,
-          int FORM = 1>
+// OBJ: the objective that ls_step folds (sb_common.cuh).  REL (SB_FLAG_RELEASE, with any objective): no job starts
+// before its release date.  HOME: where the per-job arrays these read live (stage_job_array) — 1: in shared memory
+// beside the table, 2: in global memory, read with ld.global.nc.
+template <bool INT, bool MULTI, int ADDR = 0, Obj OBJ = Obj::Makespan, int HOME = 0, bool REL = false>
 struct LaneState {
-  static_assert(FORM == 1 || (SUM && WGT != 0 && DUE != 0), "the late count and the maximum tardiness run on the "
-                "weighted tardiness form");
-  static constexpr bool LATE = FORM == 2;
-  static constexpr int kDue = DUE == 0 ? 0 : FORM;  // ls_step's form
+  static constexpr bool kW = obj_weights(OBJ), kD = obj_due(OBJ);
   float f[8];
   float mk;
-  float pend;  // a completion time parked by an even step (see ls_step; never used with SUM)
+  float pend;  // a completion time parked by an even step (see ls_step; the makespan forms only)
   const uint8_t* orow;  // this candidate's opt bytes (shared memory or global)
   const float* tab;     // runtime table (shared memory or global)
-  const float* wt;      // WGT: the job weights [J]
-  const float* dd;      // DUE: the job due dates [J] (or delivery tails)
+  const float* wt;      // kW: the job weights [J]
+  const float* dd;      // kD: the job due dates [J] (or delivery tails)
   const float* rr;      // REL: the job release dates [J]
   int SG;
   int one;
   uint32_t orow_s, tab_s, four;  // ADDR = 1: shared-window addresses of orow / tab, and a run-time 4
-  uint32_t wt_s;                 // ADDR = 1 with WGT: shared-window address of wt
-  uint32_t dd_s;                 // ADDR = 1 with DUE: shared-window address of dd
-  uint32_t rr_s;                 // ADDR = 1 with REL: shared-window address of rr
+  uint32_t wt_s, dd_s, rr_s;     // ADDR = 1: shared-window addresses of wt / dd / rr
   float4* ns;  // MULTI: lane-private node-state column; node n lives at ns[(2n)*32], ns[(2n+1)*32]
   int cur;     // MULTI: the node whose state is currently in f[] (its shared-memory copy is stale)
 
@@ -102,33 +97,21 @@ struct LaneState {
   __device__ __forceinline__ float lookup_rt(int j, int o) const {
     return MULTI ? tab[j * 8 + (o & 7)] : tab[j * SG + o];
   }
-  // the job's weight (WGT only; 0 otherwise, and then unused)
-  __device__ __forceinline__ float lookup_w(int j) const {
-    if constexpr (WGT == 1) return wt[j];
-    else if constexpr (WGT == 2) return __ldg(wt + j);
-    else return 0.f;
-  }
-  // the job's due date or tail (DUE only; 0 otherwise, and then unused)
-  __device__ __forceinline__ float lookup_d(int j) const {
-    if constexpr (DUE == 1) return dd[j];
-    else if constexpr (DUE == 2) return __ldg(dd + j);
-    else return 0.f;
-  }
-  // the job's release date (REL only; 0 otherwise, and then unused)
-  __device__ __forceinline__ float lookup_r(int j) const {
-    if constexpr (REL == 1) return rr[j];
-    else if constexpr (REL == 2) return __ldg(rr + j);
-    else return 0.f;
-  }
-  // ph: t & 1 inside fully unrolled loops, -1 elsewhere (see ls_step); w, d, r: the job's weight (WGT only), due
-  // date (DUE only) and release date (REL only)
+  // the job's entry of a per-job array: shared memory (HOME = 1) or global memory (HOME = 2)
+  __device__ __forceinline__ float job_at(const float* a, int j) const { return HOME == 1 ? a[j] : __ldg(a + j); }
+  // the job's weight, due date (or tail) and release date; 0 where the kernel reads none
+  __device__ __forceinline__ float lookup_w(int j) const { if constexpr (kW) return job_at(wt, j); else return 0.f; }
+  __device__ __forceinline__ float lookup_d(int j) const { if constexpr (kD) return job_at(dd, j); else return 0.f; }
+  __device__ __forceinline__ float lookup_r(int j) const { if constexpr (REL) return job_at(rr, j); else return 0.f; }
+  // ph: t & 1 inside fully unrolled loops, -1 elsewhere (see ls_step); w, d, r: the job's weight, due date (or tail)
+  // and release date, each read only where the objective (or REL) uses it
   __device__ __forceinline__ void step_resolved(int o, float rt, int ph = -1, float w = 0.f, float d = 0.f,
                                                 float r = 0.f) {
     if (!MULTI) {
-      ls_step<INT, INT, SUM, (WGT != 0), kDue, (REL != 0)>(f, mk, pend, rt, o & 7, one, ph, w, d, r);
+      ls_step<INT, INT, OBJ, REL>(f, mk, pend, rt, o & 7, one, ph, w, d, r);
     } else {
       switch_node(o >> 3);
-      ls_step<INT, true, SUM, (WGT != 0), kDue, (REL != 0)>(f, mk, pend, rt, o & 7, one, ph, w, d, r);
+      ls_step<INT, true, OBJ, REL>(f, mk, pend, rt, o & 7, one, ph, w, d, r);
     }
   }
   // ADDR = 1: the two look-ups as separate gathers, so that the streamed loop of k_eval_tiles can issue a whole
@@ -147,80 +130,57 @@ struct LaneState {
     asm("ld.shared.f32 %0, [%1];" : "=f"(rt) : "r"(ta));
     return rt;
   }
-  // ADDR = 1 with WGT = 1: the weight gather, its address formed on the FMA pipe like the two above
-  __device__ __forceinline__ float gather_w(int j) const {
-    if constexpr (WGT == 0) {
-      return 0.f;
-    } else {
-      uint32_t wa;
-      float w;
-      asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(wa) : "r"(j), "r"(four), "r"(wt_s));
-      asm("ld.shared.f32 %0, [%1];" : "=f"(w) : "r"(wa));
-      return w;
-    }
+  // ADDR = 1: the job's entry of a per-job array at shared-window address `base`, its address formed on the FMA pipe
+  // like the two above
+  __device__ __forceinline__ float gather_at(uint32_t base, int j) const {
+    uint32_t a;
+    float v;
+    asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(a) : "r"(j), "r"(four), "r"(base));
+    asm("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(a));
+    return v;
   }
-  // ADDR = 1 with DUE: the due-date gather, like gather_w
-  __device__ __forceinline__ float gather_d(int j) const {
-    if constexpr (DUE == 0) {
-      return 0.f;
-    } else {
-      uint32_t da;
-      float d;
-      asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(da) : "r"(j), "r"(four), "r"(dd_s));
-      asm("ld.shared.f32 %0, [%1];" : "=f"(d) : "r"(da));
-      return d;
-    }
-  }
-  // ADDR = 1 with REL = 1: the release-date gather, like gather_w
-  __device__ __forceinline__ float gather_r(int j) const {
-    if constexpr (REL == 0) {
-      return 0.f;
-    } else {
-      uint32_t ra;
-      float r;
-      asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(ra) : "r"(j), "r"(four), "r"(rr_s));
-      asm("ld.shared.f32 %0, [%1];" : "=f"(r) : "r"(ra));
-      return r;
-    }
-  }
+  __device__ __forceinline__ float gather_w(int j) const { if constexpr (kW) return gather_at(wt_s, j); else return 0.f; }
+  __device__ __forceinline__ float gather_d(int j) const { if constexpr (kD) return gather_at(dd_s, j); else return 0.f; }
+  __device__ __forceinline__ float gather_r(int j) const { if constexpr (REL) return gather_at(rr_s, j); else return 0.f; }
   __device__ __forceinline__ void step(int j, int ph = -1) {
-    constexpr bool W = WGT != 0;
-    constexpr bool R = REL != 0;
     if (!MULTI && ADDR == 1) {
       const uint32_t o = gather_opt(j);
-      ls_step<INT, INT, SUM, W, kDue, R>(f, mk, pend, gather_rt(j, o), static_cast<int>(o & 7u), one, ph,
-                                         gather_w(j), gather_d(j), gather_r(j));
+      ls_step<INT, INT, OBJ, REL>(f, mk, pend, gather_rt(j, o), static_cast<int>(o & 7u), one, ph, gather_w(j),
+                                  gather_d(j), gather_r(j));
       return;
     }
     const int o = orow[j];
     if (!MULTI) {
       const float rt = tab[j * SG + o];
-      ls_step<INT, INT, SUM, W, kDue, R>(f, mk, pend, rt, o & 7, one, ph, lookup_w(j), lookup_d(j), lookup_r(j));
+      ls_step<INT, INT, OBJ, REL>(f, mk, pend, rt, o & 7, one, ph, lookup_w(j), lookup_d(j), lookup_r(j));
     } else {
       const int col = o & 7;  // reduced table only: opt = (node << 3) | (k - 1)
       const float rt = tab[j * 8 + col];
       switch_node(o >> 3);
-      ls_step<INT, true, SUM, W, kDue, R>(f, mk, pend, rt, col, one, ph, lookup_w(j), lookup_d(j), lookup_r(j));
+      ls_step<INT, true, OBJ, REL>(f, mk, pend, rt, col, one, ph, lookup_w(j), lookup_d(j), lookup_r(j));
     }
   }
-  // the tail makespan (DUE without SUM) is tracked in mk at every shape: f[7] is a completion, not a tail sum.
-  // LATE: a job with no runtime (+inf cell) adds only its weight to the count, but the candidate is infeasible and
-  // scores +inf, as under every other objective.  Such a job leaves +inf in the slots it held, and slot times never
+  // the tail makespan is tracked in mk at every shape: f[7] is a completion, not a tail sum.
+  // LateCount: a job with no runtime (+inf cell) adds only its weight to the count, but the candidate is infeasible
+  // and scores +inf, as under every other objective.  Such a job leaves +inf in the slots it held, and slot times never
   // decrease, so one look at each node's latest slot time at the end finds it (`nodes`: MULTI only; the node in
   // f[] is checked there, the others in their shared-memory columns, where a stale copy of it is never +inf wrongly).
   __device__ __forceinline__ float result(int nodes = 1) const {
-    if constexpr (LATE) {
+    if constexpr (OBJ == Obj::LateCount) {
       float last = f[7];
       if constexpr (MULTI)
         for (int n = 0; n < nodes; ++n) last = fmaxf(last, ns[(2 * n + 1) * 32].w);
       return last == inf_f() ? inf_f() : mk;
     }
-    return SUM ? mk : ((INT || MULTI || DUE != 0) ? fmaxf(mk, pend) : f[7]);
+    if constexpr (OBJ == Obj::Makespan) return (INT || MULTI) ? fmaxf(mk, pend) : f[7];
+    else if constexpr (OBJ == Obj::TailMakespan) return fmaxf(mk, pend);
+    else return mk;
   }
-  // the running score a snapshot of the incremental rounds stores (SearchFuse::snap): with SUM nothing is parked,
-  // so a snapshot is exact at any step, not only after an even number of steps; the maximum tardiness (FORM = 3)
-  // runs under SUM and parks nothing either
-  __device__ __forceinline__ float running() const { return SUM ? mk : fmaxf(mk, pend); }
+  // the running score a snapshot of the incremental rounds stores (SearchFuse::snap): only the makespan forms park a
+  // completion, so the other objectives' snapshots are exact at any step, not only after an even number of steps
+  __device__ __forceinline__ float running() const {
+    return (OBJ == Obj::Makespan || OBJ == Obj::TailMakespan) ? fmaxf(mk, pend) : mk;
+  }
 };
 
 template <int PB>

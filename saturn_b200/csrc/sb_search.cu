@@ -328,8 +328,8 @@ struct PosArgs {
   int eval_only;  // 1: score the rows as they are and store cur_mk (initialisation, injected rows)
   int one;
   SearchFuse sf;
-  const float* w;  // W: job weights [J], zero-padded to a multiple of 4 (16 bytes)
-  const float* d;  // D: job due dates [J], padded the same way
+  const float* w;  // obj_weights(OBJ): job weights [J], zero-padded to a multiple of 4 (16 bytes)
+  const float* d;  // obj_due(OBJ): job due dates (or tails) [J], padded the same way
   const float* r;  // R: job release dates [J], padded the same way
 };
 
@@ -422,21 +422,12 @@ __device__ __forceinline__ PosMove make_pos_move_win(const SearchFuse& sf, int r
 // 2 = split over the shared memory of a CTA PAIR (cluster of 2): each CTA loads one half with TMA and every
 // look-up is a `ld.shared::cluster` to whichever CTA owns the entry (distributed shared memory) — the
 // alternative to 1, kept behind a test hook.
-// SUM: score the sum of completion times instead of the makespan (SB_FLAG_SUM_COMPLETION, see ls_step).
-// W: weight each completion by its job's weight (SB_FLAG_WEIGHTED, with SUM only); the weights follow the table in
-// shared memory with TAB = 0 and are read from global memory (ld.global.nc) with TAB = 1 / 2.
-// D: score tardiness against the jobs' due dates (SB_FLAG_DUE, with W only); the due dates follow the weights.
-// D = 2 scores the late count instead (SB_FLAG_LATE_COUNT, with W only), on the same due dates.
-// D = 3 folds the weighted tardiness terms with max instead of + (SB_FLAG_MAX_TARDINESS, with W only).
-// Without SUM, D is the tail makespan (SB_FLAG_MAX_LATENESS, see ls_step): the delivery tails take the due dates' place.
-// R: no job starts before its release date (SB_FLAG_RELEASE, any objective); the release dates follow the other
-// per-job arrays in shared memory with TAB = 0 and are read from global memory with TAB = 1 / 2.
-template <int PB, bool INT, bool MULTI, bool EVAL = false, int TAB = 0, bool SUM = false, bool W = false,
-          int D = 0, bool R = false>
+// OBJ: the objective (sb_common.cuh), folded by ls_step.  R: no job starts before its release date (SB_FLAG_RELEASE,
+// any objective).  The per-job arrays they read (stage_job_array, sb_lane.cuh) follow the table in shared memory with TAB = 0 and are
+// read from global memory (ld.global.nc) with TAB = 1 / 2.
+template <int PB, bool INT, bool MULTI, bool EVAL = false, int TAB = 0, Obj OBJ = Obj::Makespan, bool R = false>
 __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
   static_assert(TAB == 0 || (EVAL && !MULTI), "tables outside the CTA's shared memory: scoring only, one node");
-  static_assert(SUM || !W, "weights scale the sum of completion times only");
-  static_assert(W || !D || !SUM, "tardiness runs on the weighted form");
   extern __shared__ __align__(128) uint8_t smem[];
   const int nw = blockDim.x >> 5;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -447,8 +438,9 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
   const uint32_t tab_off = TAB == 2 ? rank * half * 4u : 0u;
   const uint32_t tab_bytes = TAB == 1 ? 0u : (TAB == 2 ? (rank == 0 ? half * 4u : tab_all - half * 4u) : tab_all);
   const uint32_t tab_room = TAB == 1 ? 0u : (TAB == 2 ? half * 4u : tab_all);
-  const uint32_t w_bytes = (W && TAB == 0) ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u;
-  const uint32_t d_bytes = D ? (W ? w_bytes : (TAB == 0 ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u)) : 0u;
+  constexpr bool kW = obj_weights(OBJ), kD = obj_due(OBJ);
+  const uint32_t w_bytes = (kW && TAB == 0) ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u;
+  const uint32_t d_bytes = kD ? (kW ? w_bytes : (TAB == 0 ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u)) : 0u;
   const uint32_t r_bytes = (R && TAB == 0) ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u;
   float* tab_s = reinterpret_cast<float*>(smem);
   [[maybe_unused]] float* w_s = reinterpret_cast<float*>(smem + ((tab_room + 15u) & ~15u));
@@ -467,28 +459,15 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
       mbar_arrive_expect_tx(bar_tab, tab_bytes + w_bytes + d_bytes + r_bytes);
       const uint8_t* src = reinterpret_cast<const uint8_t*>(a.tab) + tab_off;
       for (uint32_t off = 0; off < tab_bytes; off += 32768u) tma_bulk_g2s(smem + off, src + off, min(32768u, tab_bytes - off), bar_tab);
-      if constexpr (W && TAB == 0) {
-        const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(a.w);
-        for (uint32_t off = 0; off < w_bytes; off += 32768u)
-          tma_bulk_g2s(reinterpret_cast<uint8_t*>(w_s) + off, wsrc + off, min(32768u, w_bytes - off), bar_tab);
-      }
-      if constexpr (D != 0 && TAB == 0) {
-        const uint8_t* dsrc = reinterpret_cast<const uint8_t*>(a.d);
-        for (uint32_t off = 0; off < d_bytes; off += 32768u)
-          tma_bulk_g2s(reinterpret_cast<uint8_t*>(d_s) + off, dsrc + off, min(32768u, d_bytes - off), bar_tab);
-      }
-      if constexpr (R && TAB == 0) {
-        const uint8_t* rsrc = reinterpret_cast<const uint8_t*>(a.r);
-        for (uint32_t off = 0; off < r_bytes; off += 32768u)
-          tma_bulk_g2s(reinterpret_cast<uint8_t*>(r_s) + off, rsrc + off, min(32768u, r_bytes - off), bar_tab);
-      }
+      if constexpr (kW && TAB == 0) stage_job_array(reinterpret_cast<uint8_t*>(w_s), a.w, w_bytes, bar_tab);
+      if constexpr (kD && TAB == 0) stage_job_array(reinterpret_cast<uint8_t*>(d_s), a.d, d_bytes, bar_tab);
+      if constexpr (R && TAB == 0) stage_job_array(reinterpret_cast<uint8_t*>(r_s), a.r, r_bytes, bar_tab);
     }
   }
-  LaneState<INT, MULTI, 0, SUM, (W ? (TAB == 0 ? 1 : 2) : 0), (D ? (TAB == 0 ? 1 : 2) : 0), (R ? (TAB == 0 ? 1 : 2) : 0),
-            (D == 0 ? 1 : D)> st;
+  LaneState<INT, MULTI, 0, OBJ, TAB == 0 ? 1 : 2, R> st;
   st.tab = tab_s;
-  if constexpr (W) st.wt = TAB == 0 ? w_s : a.w;
-  if constexpr (D != 0) st.dd = TAB == 0 ? d_s : a.d;
+  if constexpr (kW) st.wt = TAB == 0 ? w_s : a.w;
+  if constexpr (kD) st.dd = TAB == 0 ? d_s : a.d;
   if constexpr (R) st.rr = TAB == 0 ? r_s : a.r;
   st.SG = a.SG;
   st.one = a.one;
@@ -583,9 +562,7 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
           for (int t = 0; t < 32; ++t) {
             const int j = prio_at<PB>(qp[(t * PB) / 32].w, t % (32 / PB));
             const int o = prio_at<1>(qo.w, t);
-            if constexpr (D != 0) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j), st.lookup_d(j), st.lookup_r(j));
-            else if constexpr (W) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j), 0.f, st.lookup_r(j));
-            else st.step_resolved(o, lookup(j, o), t & 1, 0.f, 0.f, st.lookup_r(j));
+            st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j), st.lookup_d(j), st.lookup_r(j));
           }
         } else {
 #pragma unroll
@@ -593,9 +570,7 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
             if (base + t < J) {
               const int j = prio_at<PB>(qp[(t * PB) / 32].w, t % (32 / PB));
               const int o = prio_at<1>(qo.w, t);
-              if constexpr (D != 0) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j), st.lookup_d(j), st.lookup_r(j));
-              else if constexpr (W) st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j), 0.f, st.lookup_r(j));
-              else st.step_resolved(o, lookup(j, o), t & 1, 0.f, 0.f, st.lookup_r(j));
+              st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j), st.lookup_d(j), st.lookup_r(j));
             }
           }
         }
@@ -787,15 +762,15 @@ using PosKernel = void (*)(PosArgs);
 
 // Scoring-only launches with the table outside the CTA's own shared memory (TAB = tab_home = 1 / 2 of k_search_pos).
 static cudaError_t eval_pos_far_launch(const Device& dev, const PosArgs& a, int tab_home, int pb, unsigned flags,
-                                       cudaStream_t st) {
+                                       Obj obj, cudaStream_t st) {
   const int warps = 16;
   const size_t smem = tab_home == 2 ? static_cast<size_t>(pos_tab_half(a.J, a.SG)) * 4 + 16 : 16;
   if (smem > dev.smem_optin) return cudaErrorNotSupported;
   const long long ntiles = (a.chains + 31) / 32;
   const long long ctas = (ntiles + warps - 1) / warps;
-  const PosKernel kern = with_eval_types(pb, flags, [&](auto PB, auto INT, auto SUM, auto W, auto D, auto R) {
-    return tab_home == 2 ? k_search_pos<PB, INT, false, true, 2, SUM, W, D, R>
-                         : k_search_pos<PB, INT, false, true, 1, SUM, W, D, R>;
+  const PosKernel kern = with_eval_types(pb, flags, obj, [&](auto PB, auto INT, auto OBJ, auto R) {
+    return tab_home == 2 ? k_search_pos<PB, INT, false, true, 2, OBJ, R>
+                         : k_search_pos<PB, INT, false, true, 1, OBJ, R>;
   });
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
   if (e != cudaSuccess) return e;
@@ -828,8 +803,8 @@ static cudaError_t eval_pos_far_launch(const Device& dev, const PosArgs& a, int 
 // tab_home: 0 = the table in every CTA's shared memory (cudaErrorNotSupported when it does not fit);
 // scoring only, one node: 2 = split over CTA pairs, 1 = global memory
 cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float* tab, const float* w, const float* d,
-                              const float* r, int SG, unsigned flags, long long first, long long count, bool eval_only, const SearchFuse& sf,
-                              cudaStream_t st, int tab_home) {
+                              const float* r, int SG, unsigned flags, Obj obj, long long first, long long count, bool eval_only,
+                              const SearchFuse& sf, cudaStream_t st, int tab_home) {
   if (count <= 0) return cudaSuccess;
   PosArgs a;
   a.tab = tab; a.J = s.J; a.SG = SG; a.nodes = s.nodes;
@@ -847,18 +822,18 @@ cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float
   const bool multi = s.nodes > 1;
   if (tab_home != 0) {
     if (!eval_only || multi) return cudaErrorNotSupported;
-    return eval_pos_far_launch(dev, a, tab_home, s.pb, flags, st);
+    return eval_pos_far_launch(dev, a, tab_home, s.pb, flags, obj, st);
   }
   const int warps = 16;
-  const size_t smem = search_pos_smem(s.J, SG, s.nodes, warps, job_arrays(flags));
+  const size_t smem = search_pos_smem(s.J, SG, s.nodes, warps, job_arrays(obj, flags));
   if (smem > dev.smem_optin) return cudaErrorNotSupported;
   const long long ntiles = (count + 31) / 32;
   const long long ctas = (ntiles + warps - 1) / warps;
   const int grid = static_cast<int>(ctas < dev.sm_count ? ctas : dev.sm_count);
-  const PosKernel kern = with_eval_types(s.pb, flags, [&](auto PB, auto INT, auto SUM, auto W, auto D, auto R) {
+  const PosKernel kern = with_eval_types(s.pb, flags, obj, [&](auto PB, auto INT, auto OBJ, auto R) {
     return with_bool(multi, [&](auto MULTI) {
       return with_bool(eval_only, [&](auto EVAL) -> PosKernel {
-        return k_search_pos<PB, INT, MULTI, EVAL, 0, SUM, W, D, R>;
+        return k_search_pos<PB, INT, MULTI, EVAL, 0, OBJ, R>;
       });
     });
   });
@@ -869,11 +844,11 @@ cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float
 // a one-node table that does not fit there: 1 = global memory, read through L1 / L2 (with no tile in shared
 // memory the SM's whole array is L1); -1 = nowhere (multi-node table beyond shared memory).
 // HOOK_TABLE_PAIR forces 2 (split over CTA pairs: scattered 4-byte ld.shared::cluster), HOOK_TABLE_GLOBAL forces 1.
-int eval_pos_home(const Device& dev, int J, int SG, int nodes, unsigned flags) {
+int eval_pos_home(const Device& dev, int J, int SG, int nodes, unsigned flags, Obj obj) {
   const bool pair_ok = nodes == 1 && static_cast<size_t>(pos_tab_half(J, SG)) * 4 + 16 <= dev.smem_optin;
   if (flags & HOOK_TABLE_PAIR) return pair_ok ? 2 : -1;
   if (flags & HOOK_TABLE_GLOBAL) return nodes == 1 ? 1 : -1;
-  if (search_pos_smem(J, SG, nodes, 16, job_arrays(flags)) <= dev.smem_optin) return 0;
+  if (search_pos_smem(J, SG, nodes, 16, job_arrays(obj, flags)) <= dev.smem_optin) return 0;
   return nodes == 1 ? 1 : -1;
 }
 
@@ -882,7 +857,7 @@ int eval_pos_home(const Device& dev, int J, int SG, int nodes, unsigned flags) {
 cudaError_t eval_pos_launch(const Device& dev, const EvalCall& c, cudaStream_t st, int* path) {
   if (c.stride_o % 32 != 0 || reinterpret_cast<uintptr_t>(c.opt) % 32 != 0 || reinterpret_cast<uintptr_t>(c.prio) % 32 != 0)
     return cudaErrorNotSupported;
-  const int home = eval_pos_home(dev, c.J, c.SG, c.nodes, c.flags);
+  const int home = eval_pos_home(dev, c.J, c.SG, c.nodes, c.flags, c.obj);
   if (home < 0) return cudaErrorNotSupported;
   if (path) *path = home == 0 ? 5 : (home == 2 ? 7 : 8);
   if (c.B <= 0) return cudaSuccess;
@@ -895,7 +870,7 @@ cudaError_t eval_pos_launch(const Device& dev, const EvalCall& c, cudaStream_t s
   s.keys = c.best_key;
   SearchFuse sf = {};
   sf.cur_mk = c.out;
-  return search_pos_launch(dev, s, c.tab, c.w, c.d, c.r, c.SG, c.flags, 0, c.B, true, sf, st, home);
+  return search_pos_launch(dev, s, c.tab, c.w, c.d, c.r, c.SG, c.flags, c.obj, 0, c.B, true, sf, st, home);
 }
 
 // Job-indexed opt rows -> schedule order (out[i] = opt[prio[i]]), one warp per candidate: the row is staged in

@@ -7,7 +7,7 @@ the hand-written kernels of saturn_b200/csrc.
 from __future__ import annotations
 
 import ctypes as C
-from typing import Optional, Sequence, Tuple
+from typing import NamedTuple, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -18,33 +18,43 @@ from ._lib import FLAG_INTEGER_STARTS, FLAG_REDUCED, SaturnB200Error, SearchPara
 NSLOT = 8
 
 
-OBJECTIVES = ("makespan", "completion", "weighted_completion", "tardiness", "weighted_tardiness", "max_lateness",
-              "late_tasks", "weighted_late_tasks", "max_tardiness", "weighted_max_tardiness")
+class Objective(NamedTuple):
+    flags: int      # the SB_FLAG_* bits that select it
+    weighted: bool  # scores with the weights of set_weights
+    due: bool       # scores against the due dates of set_due
+
+
+# Every objective of the engine.  "tardiness" is the total tardiness against set_due, "max_lateness" the maximum
+# lateness scored as L_max + Engine.due_shift, "late_tasks" the number of tasks that complete after their due date,
+# "max_tardiness" the largest tardiness; each "weighted_" form weighs the jobs by set_weights ("weighted_max_tardiness"
+# with weights 1 / p* and due dates at the release dates is the maximum stretch).
+_SUM, _W, _DUE = _lib.FLAG_SUM_COMPLETION, _lib.FLAG_WEIGHTED, _lib.FLAG_DUE
+_OBJECTIVES = {
+    "makespan": Objective(0, False, False),
+    "completion": Objective(_SUM, False, False),
+    "weighted_completion": Objective(_SUM | _W, True, False),
+    "tardiness": Objective(_SUM | _DUE, False, True),
+    "weighted_tardiness": Objective(_SUM | _DUE | _W, True, True),
+    "max_lateness": Objective(_lib.FLAG_MAX_LATENESS, False, True),
+    "late_tasks": Objective(_SUM | _DUE | _lib.FLAG_LATE_COUNT, False, True),
+    "weighted_late_tasks": Objective(_SUM | _DUE | _lib.FLAG_LATE_COUNT | _W, True, True),
+    "max_tardiness": Objective(_SUM | _DUE | _lib.FLAG_MAX_TARDINESS, False, True),
+    "weighted_max_tardiness": Objective(_SUM | _DUE | _lib.FLAG_MAX_TARDINESS | _W, True, True),
+}
+OBJECTIVES = tuple(_OBJECTIVES)
+
+
+def objective_spec(objective: str) -> Objective:
+    """The table entry of an objective name; raises SolverError for a name that is not one."""
+    if objective not in _OBJECTIVES:
+        from .solver import SolverError
+        raise SolverError("objective must be one of %s, not %r" % (", ".join(map(repr, OBJECTIVES)), objective))
+    return _OBJECTIVES[objective]
 
 
 def objective_flag(objective: str) -> int:
-    """SB_FLAG_SUM_COMPLETION for objective="completion" (score = sum of completion times), SB_FLAG_SUM_COMPLETION |
-    SB_FLAG_WEIGHTED for "weighted_completion" (the sum weighted by the engine's set_weights), SB_FLAG_SUM_COMPLETION |
-    SB_FLAG_DUE for "tardiness" (total tardiness against the engine's set_due) and SB_FLAG_SUM_COMPLETION |
-    SB_FLAG_DUE | SB_FLAG_WEIGHTED for "weighted_tardiness", SB_FLAG_MAX_LATENESS for "max_lateness" (the maximum
-    lateness against the engine's set_due, scored as L_max + Engine.due_shift), SB_FLAG_SUM_COMPLETION | SB_FLAG_DUE |
-    SB_FLAG_LATE_COUNT for "late_tasks" (the number of tasks that complete after their set_due date), the same |
-    SB_FLAG_WEIGHTED for "weighted_late_tasks" (the sum of their set_weights weights), SB_FLAG_SUM_COMPLETION |
-    SB_FLAG_DUE | SB_FLAG_MAX_TARDINESS for "max_tardiness" (the largest tardiness against set_due), the same |
-    SB_FLAG_WEIGHTED for "weighted_max_tardiness" (the largest set_weights-weighted tardiness; with weights 1 / p* and
-    due dates at the release dates, the maximum stretch) and 0 for "makespan"."""
-    if objective not in OBJECTIVES:
-        from .solver import SolverError
-        raise SolverError("objective must be one of %s, not %r" % (", ".join(map(repr, OBJECTIVES)), objective))
-    if objective == "makespan":
-        return 0
-    if objective == "max_lateness":
-        return _lib.FLAG_MAX_LATENESS
-    late = objective.endswith("late_tasks")
-    max_t = objective.endswith("max_tardiness")
-    return _lib.FLAG_SUM_COMPLETION | (_lib.FLAG_WEIGHTED if objective.startswith("weighted_") else 0) | (
-        _lib.FLAG_DUE if objective.endswith("tardiness") or late else 0) | (_lib.FLAG_LATE_COUNT if late else 0) | (
-        _lib.FLAG_MAX_TARDINESS if max_t else 0)
+    """The SB_FLAG_* bits of an objective name (see _OBJECTIVES)."""
+    return objective_spec(objective).flags
 
 
 def weights_f32(w, J: int) -> np.ndarray:
@@ -110,8 +120,8 @@ def _require_due(due, objective: str):
     """The tardiness objectives (the maximum tardiness among them), the late counts and the maximum lateness score
     against the due dates of set_due: refuse them, before any device call, on an engine that has none (set_table
     clears them)."""
-    if (objective.endswith("tardiness") or objective.endswith("late_tasks") or objective == "max_lateness") and \
-            due is None:
+    spec = _OBJECTIVES.get(objective)
+    if spec is not None and spec.due and due is None:
         from .solver import SolverError
         raise SolverError("objective=%r needs due dates: call set_due after set_table" % (objective,))
 

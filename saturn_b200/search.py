@@ -18,7 +18,8 @@ from typing import List, Optional, Tuple
 import numpy as np
 import torch
 
-from .engine import Engine, objective_flag
+from . import _lib
+from .engine import Engine, objective_flag, objective_spec
 
 
 @dataclass
@@ -64,13 +65,13 @@ def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objecti
     "weighted_tardiness", each repaired by Moore-Hodgson's rule after the node fill (moore_hodgson).
     objective="max_tardiness" / "weighted_max_tardiness": the EDD orders of "tardiness" / "weighted_tardiness"
     unchanged."""
-    objective_flag(objective)
-    if objective.startswith("weighted_"):
+    spec = objective_spec(objective)
+    if spec.weighted:
         if weights is None:
             raise ValueError("objective=%r needs the job weights" % objective)
         w64 = np.asarray(weights, dtype=np.float32).astype(np.float64)
-    late = objective.endswith("late_tasks")
-    edd = objective.endswith("tardiness") or objective == "max_lateness" or late
+    late = bool(spec.flags & _lib.FLAG_LATE_COUNT)
+    edd = spec.due
     if edd:
         if due is None:
             raise ValueError("objective=%r needs the job due dates" % objective)
@@ -93,8 +94,7 @@ def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objecti
         col = np.argmin(cost, axis=1)
         rt = usable[np.arange(J), col]
         if edd:
-            weighted = objective in ("weighted_tardiness", "weighted_late_tasks", "weighted_max_tardiness")
-            tie = rt.astype(np.float64) / w64 if weighted else rt.astype(np.float64)
+            tie = rt.astype(np.float64) / w64 if spec.weighted else rt.astype(np.float64)
             order = np.lexsort((np.arange(J), tie, d32))
         elif objective == "weighted_completion":
             order = np.argsort(rt.astype(np.float64) / w64, kind="stable")
@@ -114,7 +114,7 @@ def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objecti
                 ob[j] |= n << 3
         if late:
             order = moore_hodgson(order, col, rt, ob >> 3 if nodes > 1 else np.zeros(J, dtype=np.int64), nodes,
-                                  w64 if objective == "weighted_late_tasks" else None, d32,
+                                  w64 if spec.weighted else None, d32,
                                   rel if release is not None else None, integer_starts)
         seeds.append((ob, order))
     return seeds
@@ -269,8 +269,8 @@ def run_search(engine: Engine, chains: int = 1 << 16, rounds: int = 200, seed: i
     if record_history:
         history.append((time.perf_counter() - t0, chains * world, key_makespan(key)))
     exchange_every = max(1, int(exchange_every))
-    # a tardiness or late count of +0 (key bits 0) cannot be beaten
-    at_zero = objective.endswith("tardiness") or objective.endswith("late_tasks")
+    # a tardiness, late count or maximum tardiness (the SB_FLAG_DUE forms) of +0 (key bits 0) cannot be beaten
+    at_zero = bool(objective_flag(objective) & _lib.FLAG_DUE)
     reason = 3 if at_zero and (best_seen >> 32) == 0 else 0
     while reason == 0 and done_rounds < rounds:
         # one group of rounds, no host synchronisation; the library resamples on its own cadence
