@@ -69,6 +69,13 @@
  * twice w = 1 (barring overflow).  The score is >= +0.  A job with no runtime (rt = +inf) gives a +inf term, so the
  * candidate scores +inf without a special case.  w_j = 1 / p*_j and d_j = max(r_j, 0), with p*_j a lower bound on
  * job j's runtime, make it the maximum stretch (slowdown) of the jobs, max_j (C_j - max(r_j, 0)) / p*_j.
+ * With SB_FLAG_SQUARED instead it is the (weighted) squared tardiness:
+ *   total = sum_j w_j max(0, start_j + rt_j - d_j)^2, from +0 in schedule order per job: e = start + rt, l = e - d,
+ *   t = max(l, +0) (the tardiness fold's t bit for bit), u = t * t, x = w * u, acc = acc + x, every step rounded on
+ *   its own (no fused multiply-add).
+ * Due dates at or past every completion give +0, w = 2 exactly twice w = 1 (barring overflow).  The score is >= +0.  A
+ * job with no runtime (rt = +inf) gives a +inf term.  d_j = max(r_j, 0) makes it the squared flow time
+ * sum_j w_j (C_j - max(r_j, 0))^2 (sum_j w_j C_j^2 without release dates).
  * The schedule, every start and every slot mask are the same under every objective.
  * With SB_FLAG_MAX_LATENESS (per-job due dates d_j, sb_set_due) the score is the maximum lateness
  * L_max = max_j (start_j + rt_j - d_j), emitted as the tail makespan L_max + D >= +0 with D = max_t d_t:
@@ -209,6 +216,22 @@ typedef enum sb_status {
                                      sum_j w_j), it stops as soon as the incumbent is +0 (stop_reason 3), and
                                      sb_search_seed_lpt plants the EDD orders of SB_FLAG_DUE.  Not available with
                                      SB_FLAG_ALT_WARPSCAN (SB_ERR_UNSUPPORTED). */
+#define SB_FLAG_SQUARED 8192u      /* with SB_FLAG_SUM_COMPLETION | SB_FLAG_DUE only (SB_FLAG_WEIGHTED optional; else
+                                     SB_ERR_ARG), and not with SB_FLAG_LATE_COUNT, SB_FLAG_MAX_TARDINESS or
+                                     SB_FLAG_MAX_LATENESS (SB_ERR_ARG): each tardiness is squared before it is
+                                     weighted, and the objective is the (weighted) squared tardiness
+                                     sum_j w_j max(0, C_j - d_j)^2 (see the evaluation rule above).  It reads the
+                                     weights and due dates of SB_FLAG_DUE and needs nothing else.  With
+                                     SB_FLAG_WEIGHTED it is SB_ERR_ARG unless J * max_j w_j * 2^50 < FLT_MAX
+                                     (recorded by sb_set_weights): a tardiness below 2^25 squares below 2^50, so
+                                     below that bound the sum cannot overflow to +inf.  Accepted by sb_eval,
+                                     sb_eval_host, sb_eval_full, sb_decode and the search, sb_search_run_multi
+                                     included; every score the library emits then holds the sum of squares, and
+                                     target_makespan targets it.  The search's temperature unit becomes
+                                     max(incumbent / sum_j w_j, sum_j w_j (min_k rt_jk)^2 / sum_j w_j) (SB_FLAG_DUE's
+                                     floor with each runtime squared), it stops as soon as the incumbent is +0
+                                     (stop_reason 3), and sb_search_seed_lpt plants the EDD orders of SB_FLAG_DUE.
+                                     Not available with SB_FLAG_ALT_WARPSCAN (SB_ERR_UNSUPPORTED). */
 #define SB_IPC_HANDLE_BYTES 64
 
 typedef struct sb_handle sb_handle;

@@ -19,6 +19,7 @@ FLAG_RELEASE = 512
 FLAG_MAX_LATENESS = 1024
 FLAG_LATE_COUNT = 2048
 FLAG_MAX_TARDINESS = 4096
+FLAG_SQUARED = 8192
 IPC_HANDLE_BYTES = 64
 # test hooks in the top bits of the same flags word: the enum in csrc/sb_internal.h says what each one forces
 HOOK_FORCE_GENERIC = 0x80000000

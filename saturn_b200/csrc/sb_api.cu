@@ -2,6 +2,7 @@
 //
 // No exceptions cross this boundary and no CPU fallback exists: every entry point either runs
 // the CUDA path on the handle's device or returns a negative sb_status with sb_last_error() set.
+#include <float.h>
 #include <math.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -111,6 +112,10 @@ struct sb_handle {
   std::vector<float> h_w;
   double w_sum = 0.0;
   bool has_w = false;
+  // SB_FLAG_SQUARED | SB_FLAG_WEIGHTED: whether J * max_j w_j * 2^50 < FLT_MAX (in double), made by sb_set_weights.  A
+  // plan inside the 2^24 horizon with |d| < 2^24 has every tardiness below 2^25, so every square below 2^50, and the
+  // weighted sum of squares stays finite below that bound; past it the flag is refused
+  bool sq_finite = false;
   // due dates (sb_set_due): device copy padded like d_w, J unit weights for SB_FLAG_DUE without SB_FLAG_WEIGHTED,
   // and the host copy (EDD seeds); has_d is cleared by sb_set_table
   float* d_d = nullptr;
@@ -362,11 +367,13 @@ int sb_set_weights(sb_handle* h, const float* w, int J) {
     return SB_OK;
   }
   if (J != h->J) return fail(SB_ERR_ARG, "J=%d differs from the table's J=%d", J, h->J);
-  double sum = 0.0;
+  double sum = 0.0, wmax = 0.0;
   for (int j = 0; j < J; ++j) {
     if (!isfinite(w[j]) || !(w[j] > 0.f)) return fail(SB_ERR_ARG, "weight %d (%g) is not finite and > 0", j, w[j]);
     sum += static_cast<double>(w[j]);
+    wmax = std::max(wmax, static_cast<double>(w[j]));
   }
+  h->sq_finite = static_cast<double>(J) * wmax * 0x1p50 < static_cast<double>(FLT_MAX);
   h->has_w = false;
   const size_t cap = static_cast<size_t>((J + 3) & ~3);
   if (h->d_w_cap < cap) {
@@ -469,13 +476,19 @@ int sb_set_release(sb_handle* h, const float* r, int J) {
 }
 
 // The one reader of the objective flags.  SB_FLAG_WEIGHTED and SB_FLAG_DUE are valid with SB_FLAG_SUM_COMPLETION only;
-// SB_FLAG_MAX_LATENESS alone among the objective flags; SB_FLAG_LATE_COUNT and SB_FLAG_MAX_TARDINESS with
-// SB_FLAG_SUM_COMPLETION | SB_FLAG_DUE only (they change what the tardiness form adds per job, and how it folds its
-// terms), and not together or with SB_FLAG_MAX_LATENESS.  Every other combination is SB_ERR_ARG.
+// SB_FLAG_MAX_LATENESS alone among the objective flags; SB_FLAG_LATE_COUNT, SB_FLAG_MAX_TARDINESS and SB_FLAG_SQUARED
+// with SB_FLAG_SUM_COMPLETION | SB_FLAG_DUE only (they change what the tardiness form adds per job, and how it folds
+// its terms), and not together or with SB_FLAG_MAX_LATENESS.  Every other combination is SB_ERR_ARG.
 static int decode_objective(unsigned flags, Objective* o) {
   const bool sum = flags & SB_FLAG_SUM_COMPLETION, weighted = flags & SB_FLAG_WEIGHTED, due = flags & SB_FLAG_DUE;
   const bool lateness = flags & SB_FLAG_MAX_LATENESS, late = flags & SB_FLAG_LATE_COUNT;
-  const bool max_tardiness = flags & SB_FLAG_MAX_TARDINESS;
+  const bool max_tardiness = flags & SB_FLAG_MAX_TARDINESS, squared = flags & SB_FLAG_SQUARED;
+  if (squared && !(sum && due))
+    return fail(SB_ERR_ARG, "SB_FLAG_SQUARED squares the tardiness form's terms: it needs SB_FLAG_SUM_COMPLETION and "
+                "SB_FLAG_DUE");
+  if (squared && (late || max_tardiness || lateness))
+    return fail(SB_ERR_ARG, "SB_FLAG_SQUARED cannot be combined with SB_FLAG_LATE_COUNT, SB_FLAG_MAX_TARDINESS or "
+                "SB_FLAG_MAX_LATENESS");
   if (late && !(sum && due))
     return fail(SB_ERR_ARG, "SB_FLAG_LATE_COUNT counts late jobs on the tardiness form: it needs SB_FLAG_SUM_COMPLETION "
                 "and SB_FLAG_DUE");
@@ -496,13 +509,16 @@ static int decode_objective(unsigned flags, Objective* o) {
   else if (!sum) o->obj = Obj::Makespan;
   else if (late) o->obj = Obj::LateCount;
   else if (max_tardiness) o->obj = Obj::MaxTardiness;
+  else if (squared) o->obj = Obj::SquaredTardiness;
   else if (due) o->obj = Obj::Tardiness;
   else o->obj = weighted ? Obj::WeightedSum : Obj::Sum;
   return SB_OK;
 }
 
 // the objectives folded from the tardiness form (SB_FLAG_DUE): their scores reach +0, which no plan can beat
-static bool tardiness_form(Obj o) { return o == Obj::Tardiness || o == Obj::LateCount || o == Obj::MaxTardiness; }
+static bool tardiness_form(Obj o) {
+  return o == Obj::Tardiness || o == Obj::LateCount || o == Obj::MaxTardiness || o == Obj::SquaredTardiness;
+}
 
 // decode_objective, then the per-job arrays the objective reads (and SB_FLAG_RELEASE's) must be set on the handle
 static int check_per_job(const sb_handle* h, unsigned flags, Objective* o) {
@@ -517,6 +533,9 @@ static int check_per_job(const sb_handle* h, unsigned flags, Objective* o) {
     return fail(SB_ERR_STATE, "SB_FLAG_WEIGHTED needs sb_set_weights (sb_set_table clears the weights)");
   if (obj_due(o->obj) && !h->has_d)
     return fail(SB_ERR_STATE, "SB_FLAG_DUE needs sb_set_due (sb_set_table clears the due dates)");
+  if (o->obj == Obj::SquaredTardiness && o->weighted && !h->sq_finite)
+    return fail(SB_ERR_ARG, "SB_FLAG_SQUARED | SB_FLAG_WEIGHTED needs J * max w * 2^50 < FLT_MAX (beyond it the sum of "
+                "squared tardiness can overflow fp32)");
   if ((flags & SB_FLAG_RELEASE) && !h->has_r)
     return fail(SB_ERR_STATE, "SB_FLAG_RELEASE needs sb_set_release (sb_set_table clears the release dates)");
   return SB_OK;
@@ -636,7 +655,7 @@ int sb_eval(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, int64
     if (c.obj != Obj::Makespan || (flags & SB_FLAG_RELEASE))
       return fail(SB_ERR_UNSUPPORTED, "SB_FLAG_ALT_WARPSCAN scores the makespan without release dates only: it "
                   "cannot be combined with SB_FLAG_SUM_COMPLETION, SB_FLAG_WEIGHTED, SB_FLAG_DUE, SB_FLAG_RELEASE, "
-                  "SB_FLAG_MAX_LATENESS, SB_FLAG_LATE_COUNT or SB_FLAG_MAX_TARDINESS");
+                  "SB_FLAG_MAX_LATENESS, SB_FLAG_LATE_COUNT, SB_FLAG_MAX_TARDINESS or SB_FLAG_SQUARED");
     if (flags & (SB_FLAG_POST_KEY | SB_FLAG_FOLD_PREV))
       return fail(SB_ERR_UNSUPPORTED, "SB_FLAG_ALT_WARPSCAN cannot be combined with the fused key exchange");
     cudaError_t e = eval_alt_launch(h->dev, c, h->stream);
@@ -1089,7 +1108,7 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
     // tardiness can be 0 or tiny at the incumbent: the unit is at least the weighted mean of each job's smallest
     // proposable runtime, the size of the score change one move makes
     const float* tmin = h->h_tmin.data();
-    double move = 0.0, move_max = 0.0;
+    double move = 0.0, move_max = 0.0, move_sq = 0.0;
     for (int j = 0; j < J; ++j) {
       double lo = HUGE_VAL, lo_any = HUGE_VAL;
       for (int k = 0; k < kSlots; ++k) {
@@ -1102,12 +1121,17 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
         const double x = (weighted ? static_cast<double>(h->h_w[j]) : 1.0) * lo;
         move += x;
         move_max = std::max(move_max, x);
+        move_sq += x * lo;
       }
     }
     // the maximum tardiness is a max, not a sum: its unit is the incumbent itself (the mean-completion division of
     // SB_FLAG_SUM_COMPLETION does not apply), and at least the largest weighted smallest runtime, the same floor taken
     // as a max.  A starting point, not a measured choice (DESIGN §3)
     if (o.obj == Obj::MaxTardiness) s.scale = std::max(mk, static_cast<float>(move_max));
+    // the squared tardiness: the same mean-per-weight unit, with the floor's runtimes squared, sum_j w_j lo_j^2 /
+    // sum_j w_j (a starting point, not a measured choice, DESIGN §3)
+    else if (o.obj == Obj::SquaredTardiness)
+      s.scale = std::max(s.scale, static_cast<float>(move_sq / (weighted ? h->w_sum : static_cast<double>(J))));
     else s.scale = std::max(s.scale, static_cast<float>(move / (weighted ? h->w_sum : static_cast<double>(J))));
   }
   // the late count moves in steps of one job's weight and is 0 at many incumbents: its unit is the count of every job,

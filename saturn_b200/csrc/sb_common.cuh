@@ -19,29 +19,34 @@ constexpr float kSentinel = 1.0e6f;  // reference's "unprofiled" runtime, Perfor
 __device__ __forceinline__ float inf_f() { return __int_as_float(0x7f800000); }
 
 // ---------------------------------------------------------------- the objective
-// The seven scores the kernels compute, and the SB_FLAG_* bits that select each (sb_api.cu: decode_objective; every
+// The eight scores the kernels compute, and the SB_FLAG_* bits that select each (sb_api.cu: decode_objective; every
 // form also runs with SB_FLAG_RELEASE).  C is a job's completion, w its weight, d its due date.
-//   Obj           flags                                              score
-//   Makespan      none                                               max C
-//   TailMakespan  MAX_LATENESS                                       max (C + q), tails q = max d - d (L_max + max d)
-//   Sum           SUM_COMPLETION                                     sum C
-//   WeightedSum   SUM_COMPLETION | WEIGHTED                          sum w C
-//   Tardiness     SUM_COMPLETION | DUE [| WEIGHTED]                  sum w max(C - d, 0), unit weights without WEIGHTED
-//   LateCount     SUM_COMPLETION | DUE | LATE_COUNT [| WEIGHTED]     sum (C > d ? w : 0)
-//   MaxTardiness  SUM_COMPLETION | DUE | MAX_TARDINESS [| WEIGHTED]  max w max(C - d, 0)
-// Every other combination of those flags is refused.  The history of each form is in DESIGN.md.
-enum class Obj { Makespan, TailMakespan, Sum, WeightedSum, Tardiness, LateCount, MaxTardiness };
+//   Obj               flags                                              score
+//   Makespan          none                                               max C
+//   TailMakespan      MAX_LATENESS                                       max (C + q), tails q = max d - d (L_max + max d)
+//   Sum               SUM_COMPLETION                                     sum C
+//   WeightedSum       SUM_COMPLETION | WEIGHTED                          sum w C
+//   Tardiness         SUM_COMPLETION | DUE [| WEIGHTED]                  sum w max(C - d, 0), unit weights without WEIGHTED
+//   LateCount         SUM_COMPLETION | DUE | LATE_COUNT [| WEIGHTED]     sum (C > d ? w : 0)
+//   MaxTardiness      SUM_COMPLETION | DUE | MAX_TARDINESS [| WEIGHTED]  max w max(C - d, 0)
+//   SquaredTardiness  SUM_COMPLETION | DUE | SQUARED [| WEIGHTED]        sum w max(C - d, 0)^2
+// Every other combination of those flags is refused.  The history of each form is in DESIGN.md.  New forms go at the
+// end: a kernel's symbol holds its form's value.
+enum class Obj { Makespan, TailMakespan, Sum, WeightedSum, Tardiness, LateCount, MaxTardiness, SquaredTardiness };
 // the score is a sum over the jobs, folded in schedule order
 __host__ __device__ constexpr bool obj_sum(Obj o) {
-  return o == Obj::Sum || o == Obj::WeightedSum || o == Obj::Tardiness || o == Obj::LateCount;
+  return o == Obj::Sum || o == Obj::WeightedSum || o == Obj::Tardiness || o == Obj::LateCount ||
+         o == Obj::SquaredTardiness;
 }
 // the score reads the job weights (the caller's, or unit weights without SB_FLAG_WEIGHTED)
 __host__ __device__ constexpr bool obj_weights(Obj o) {
-  return o == Obj::WeightedSum || o == Obj::Tardiness || o == Obj::LateCount || o == Obj::MaxTardiness;
+  return o == Obj::WeightedSum || o == Obj::Tardiness || o == Obj::LateCount || o == Obj::MaxTardiness ||
+         o == Obj::SquaredTardiness;
 }
 // the score reads the due-date array: the due dates, or TailMakespan's tails
 __host__ __device__ constexpr bool obj_due(Obj o) {
-  return o == Obj::TailMakespan || o == Obj::Tardiness || o == Obj::LateCount || o == Obj::MaxTardiness;
+  return o == Obj::TailMakespan || o == Obj::Tardiness || o == Obj::LateCount || o == Obj::MaxTardiness ||
+         o == Obj::SquaredTardiness;
 }
 
 // ---------------------------------------------------------------- mbarrier + TMA bulk copy (1-D)
@@ -191,7 +196,9 @@ __device__ __forceinline__ float fmax3_mk(float mk, float b, float c) {
 //                  bit).  Tardiness: mk + w * max(e - d, +0) (d = 0 gives WeightedSum).  LateCount: mk + (e > d ? w :
 //                  +0); a job that completes exactly at its due date is on time.  MaxTardiness: max(mk, w * max(e - d,
 //                  +0)), Tardiness's term bit for bit folded with max; a job with no runtime (rt = +inf, w > 0) gives
-//                  a +inf term.
+//                  a +inf term.  SquaredTardiness: t = max(e - d, +0), Tardiness's term before the weight bit for
+//                  bit, then mk + w * (t * t), three roundings; w = 1 gives the unweighted form bit for bit, and a
+//                  job with no runtime a +inf term.
 // The slot update is the same under every objective: only the score differs.
 // kRelease (SB_FLAG_RELEASE): the job starts no earlier than its release date `r`, s = max(f[km1], r) (ceil(r) under
 // integer starts, made once by sb_set_release, so s stays an integer).  The slot update below stays valid because it
@@ -237,6 +244,14 @@ __device__ __forceinline__ void ls_step(float (&f)[8], float& mk, float& pend, f
     else if constexpr (kObj == Obj::MaxTardiness)
       mk = __int_as_float(max(__float_as_int(mk), __float_as_int(__fmul_rn(w, __fsub_rn(e, d)))));
     else if constexpr (kObj == Obj::Tardiness) mk = __fadd_rn(mk, __fmul_rn(w, fmaxf(__fsub_rn(e, d), 0.f)));
+    // the squared tardiness, mk + w * (t * t) with t = max(e - d, +0), as mk + w * (x * max(x, +0)) with x = e - d: for
+    // x > 0 the same product, and for x <= 0 a +0 or -0 term, which adds to mk >= +0 exactly as the +0 term does.
+    // Same value; the t * t form gave one position-major search kernel (PB 1, INT, a CTA-pair table, release dates)
+    // 8 bytes of spills at the 128-register cap, where its tardiness sibling has none
+    else if constexpr (kObj == Obj::SquaredTardiness) {
+      const float x = __fsub_rn(e, d);
+      mk = __fadd_rn(mk, __fmul_rn(w, __fmul_rn(x, fmaxf(x, 0.f))));
+    }
     else if constexpr (kObj == Obj::WeightedSum) mk = __fadd_rn(mk, __fmul_rn(w, e));
     else mk = mk + e;
   } else if (kTrackMk) {

@@ -796,6 +796,10 @@ __global__ void __launch_bounds__(128) k_eval_full(const FullArgs a) {
         mk = fmaxf(mk, __fmul_rn(__ldg(a.w + j), fmaxf(__fsub_rn(s + rt, __ldg(a.d + j)), 0.f)));
       else if constexpr (OBJ == Obj::Tardiness)
         mk = __fadd_rn(mk, __fmul_rn(__ldg(a.w + j), fmaxf(__fsub_rn(s + rt, __ldg(a.d + j)), 0.f)));
+      else if constexpr (OBJ == Obj::SquaredTardiness) {
+        const float t = fmaxf(__fsub_rn(s + rt, __ldg(a.d + j)), 0.f);
+        mk = __fadd_rn(mk, __fmul_rn(__ldg(a.w + j), __fmul_rn(t, t)));
+      }
       else if constexpr (OBJ == Obj::WeightedSum) mk = __fadd_rn(mk, __fmul_rn(__ldg(a.w + j), s + rt));
       else if constexpr (OBJ == Obj::Sum) mk = mk + (s + rt);  // the left fold in schedule order
       else mk = fmaxf(mk, s + rt);

@@ -54,14 +54,18 @@ def orchestrate(task_list, log=False, interval=1000, gurobi=True, *,
     batches_to_run, interval, node_per_task, task_dependency_dict)` stands in for
     saturn.executor.execute; returns the list of per-interval records (plan makespan, tasks run).
 
-    A `due` mapping Task -> due date in `solver_kwargs` (objective="tardiness", "max_lateness" or "late_tasks") is
+    A `due` mapping Task -> due date in `solver_kwargs` (objective="tardiness", "max_lateness", "late_tasks" or "squared_tardiness") is
     measured from the first plan's t = 0: the solve for interval n plans from n * interval on, so it receives
     {t: d - n * interval}, and the lateness each solve reports is against the original due dates (both sides shift
     alike).  A sequence `due` raises SolverError, since the task list shrinks from interval to interval.  A `release`
     mapping Task -> release date is shifted the same way, {t: r - n * interval}; a sequence `release` raises
     SolverError.  Under objective="max_stretch" the shifted release dates are what each solve measures stretch
     from, and each interval's fastest runtime p*_t comes from the runtimes `forecast` has shrunk: each solve
-    minimises the stretch of the work that remains, not of the whole task.
+    minimises the stretch of the work that remains, not of the whole task.  Under objective="squared_tardiness" the
+    shifted due dates leave every tardiness unchanged (C and d move alike).  Under objective="squared_flow" each solve
+    measures flow from the shifted release dates, clamped at the interval's t = 0: a task released before the
+    interval counts its flow from the interval's start, so each solve minimises the squares of the waits that
+    remain, not of the whole flow time.
     """
     logging.basicConfig(level=logging.INFO if log else logging.WARNING,
                         format="%(asctime)s %(levelname)-8s %(message)s", datefmt="%Y-%m-%d %H:%M:%S")

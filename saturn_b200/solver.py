@@ -168,6 +168,9 @@ _ENGINE = None
 _MULTI: dict = {}
 last_stats: dict = {}
 FP32_EXACT_HORIZON = float(1 << 24)   # integer seconds are exact in the kernels' fp32 state below this
+FP32_MAX = float(np.finfo(np.float32).max)
+SQUARE_BOUND = float(1 << 50)   # a squared tardiness inside the horizon, (2^25)^2, with |d| < 2^24
+_SQUARED = ("squared_tardiness", "squared_flow")   # the solve() objectives that run as the squared tardiness
 
 
 def _engine(devices=None):
@@ -224,9 +227,10 @@ def _check_horizon(T, found_makespan=None, release=None, tails=None):
                           "options" % lower)
 
 def _check_objective(objective, hysteresis=False, release=None):
-    if objective not in ("makespan", "completion", "tardiness", "max_lateness", "late_tasks", "max_stretch"):
-        raise SolverError("objective must be 'makespan', 'completion', 'tardiness', 'max_lateness', 'late_tasks' or "
-                          "'max_stretch', not %r" % (objective,))
+    if objective not in ("makespan", "completion", "tardiness", "max_lateness", "late_tasks", "max_stretch",
+                         "squared_tardiness", "squared_flow"):
+        raise SolverError("objective must be 'makespan', 'completion', 'tardiness', 'max_lateness', 'late_tasks', "
+                          "'max_stretch', 'squared_tardiness' or 'squared_flow', not %r" % (objective,))
     if objective != "makespan" and hysteresis:
         raise SolverError("hysteresis=True compares plans by makespan (milp.py:363-442); it is not defined for "
                           "objective=%r" % (objective,))
@@ -259,26 +263,32 @@ def _resolve_weights(weights, objective, J, task_list=None):
     if objective == "max_stretch":
         raise SolverError("objective='max_stretch' weighs every task by 1 / its fastest runtime: it takes no weights "
                           "(for a weighted mean stretch use objective='completion' with weights)")
-    if objective not in ("completion", "tardiness", "late_tasks"):
-        raise SolverError("weights apply to objective='completion', 'tardiness' or 'late_tasks' only, not to %r"
-                          % (objective,))
+    if objective not in ("completion", "tardiness", "late_tasks", "squared_tardiness", "squared_flow"):
+        raise SolverError("weights apply to objective='completion', 'tardiness', 'late_tasks', 'squared_tardiness' or "
+                          "'squared_flow' only, not to %r" % (objective,))
     weights = _per_task(weights, "weights", task_list)
     from .engine import weights_f32
     w32 = weights_f32(weights, J)
+    if objective in _SQUARED and not J * float(w32.max()) * SQUARE_BOUND < FP32_MAX:
+        # a plan inside the 2^24 horizon with |d| < 2^24 has every tardiness below 2^25, so every square below 2^50:
+        # below this bound the device's fp32 sum of squares stays finite (sb_set_weights makes the same test)
+        raise SolverError("objective=%r needs J * max(weights) * 2^50 < FLT_MAX (%d tasks, largest weight %g): beyond "
+                          "it the fp32 sum of squares can overflow; scale the weights down" % (objective, J,
+                                                                                                float(w32.max())))
     return [float(x) for x in weights], w32
 
 
 def _resolve_due(due, objective, J, task_list=None):
     """The caller's per-task due dates as (float64 values in task order, fp32 array for the device), or (None, None)
-    without objective="tardiness", "max_lateness" or "late_tasks", which require them.  Raises SolverError before
-    any device call."""
-    if objective == "max_stretch" and due is not None:
-        raise SolverError("objective='max_stretch' measures every task from its release date: it takes no due dates "
-                          "(pass release=...)")
-    if objective not in ("tardiness", "max_lateness", "late_tasks"):
+    without objective="tardiness", "max_lateness", "late_tasks" or "squared_tardiness", which require them.  Raises
+    SolverError before any device call."""
+    if objective in ("max_stretch", "squared_flow") and due is not None:
+        raise SolverError("objective=%r measures every task from its release date: it takes no due dates "
+                          "(pass release=...)" % (objective,))
+    if objective not in ("tardiness", "max_lateness", "late_tasks", "squared_tardiness"):
         if due is not None:
-            raise SolverError("due dates apply to objective='tardiness', 'max_lateness' or 'late_tasks' only, not to %r"
-                              % (objective,))
+            raise SolverError("due dates apply to objective='tardiness', 'max_lateness', 'late_tasks' or "
+                              "'squared_tardiness' only, not to %r" % (objective,))
         return None, None
     if due is None:
         raise SolverError("objective=%r needs due dates (due=...)" % (objective,))
@@ -316,6 +326,8 @@ def _set_objective(eng, objective, w32, d32, r32=None):
             return "weighted_late_tasks" if w32 is not None else "late_tasks"
         if objective == "max_stretch":
             return "weighted_max_tardiness"
+        if objective in _SQUARED:
+            return "weighted_squared_tardiness" if w32 is not None else "squared_tardiness"
         return "weighted_tardiness" if w32 is not None else "tardiness"
     return "weighted_completion" if w32 is not None else objective
 
@@ -361,8 +373,13 @@ def _stretch_form(Tdev, r32):
     if not np.isfinite(scaled).all():
         raise SolverError("objective='max_stretch': 1 / the fastest runtime of task %d overflows fp32 over a 2^24 "
                           "horizon; express runtimes in finer units" % int(np.argmax(~np.isfinite(scaled))))
-    d32 = np.zeros(J, dtype=np.float32) if r32 is None else np.where(r32 > 0, r32, np.float32(0)).astype(np.float32)
-    return pstar, w32, d32
+    return pstar, w32, _release_due(r32, J)
+
+
+def _release_due(r32, J):
+    """The fp32 due dates max(r32_t, +0) (+0 without release dates) that measure every task from its release:
+    objective="max_stretch" and "squared_flow" run against them."""
+    return np.zeros(J, dtype=np.float32) if r32 is None else np.where(r32 > 0, r32, np.float32(0)).astype(np.float32)
 
 
 def _stretch_stats(start, rts, pstar, r64):
@@ -370,6 +387,25 @@ def _stretch_stats(start, rts, pstar, r64):
     r = r64 if r64 is not None else [0.0] * len(rts)
     st = [(float(s) + float(rt) - max(x, 0.0)) / float(p) for s, rt, x, p in zip(start, rts, r, pstar)]
     return {"max_stretch": max(st), "mean_stretch": sum(st) / len(st)}
+
+
+def _squared_stats(start, rts, w64, d64):
+    """squared_tardiness, sum_t w_t max(0, C_t - d_t)^2 (unit weights without w64), with weighted_tardiness and
+    late_tasks (_tardiness_stats), of a plan in float64."""
+    w = w64 if w64 is not None else [1.0] * len(rts)
+    stats = _tardiness_stats(start, rts, w64, d64)
+    stats["squared_tardiness"] = sum(wi * max(0.0, float(s) + float(r) - d) ** 2
+                                     for s, r, d, wi in zip(start, rts, d64, w))
+    return stats
+
+
+def _squared_flow_stats(start, rts, w64, r64):
+    """squared_flow, sum_t w_t (C_t - max(r_t, 0))^2 (unit weights without w64, r_t = 0 without r64), and
+    total_flow_time, sum_t (C_t - max(r_t, 0)), of a plan in float64."""
+    r = r64 if r64 is not None else [0.0] * len(rts)
+    w = w64 if w64 is not None else [1.0] * len(rts)
+    flow = [float(s) + float(rt) - max(x, 0.0) for s, rt, x in zip(start, rts, r)]
+    return {"squared_flow": sum(wi * f * f for wi, f in zip(w, flow)), "total_flow_time": sum(flow)}
 
 
 def _tails(d32):
@@ -470,6 +506,21 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     device's fp32 max stretch.  The 6th element stays the plan's makespan.  The mean stretch needs no objective of
     its own: objective="completion" with weights={t: 1 / p*_t} minimises sum_t (C_t - r_t) / p*_t up to a constant.
 
+    Squared tardiness.  objective="squared_tardiness" with `due` (as above) minimises sum_t w_t max(0, C_t - d_t)^2
+    (unit weights without `weights`): the l2 norm of the delays, between the total tardiness, which is indifferent
+    between one task late by 10 h and ten late by 1 h each, and a maximum, which ignores every task but the worst.
+    The `due` and `weights` rules and errors are those of "tardiness", as is the refusal of hysteresis=True;
+    `release` is valid.  The search stops as soon as it finds a plan with no late task.  objective="squared_flow"
+    minimises sum_t w_t (C_t - max(r_t, 0))^2, the l2 norm of each task's time from release to result (sum_t w_t C_t^2
+    without `release`): it runs as the squared tardiness against the due dates max(r_t, 0) in fp32, as
+    "max_stretch" does; `release` and `weights` are valid, `due` and hysteresis=True raise SolverError.  Under both,
+    weights with J * max(weights) * 2^50 >= FLT_MAX raise SolverError before any device call (past it the device's
+    fp32 sum of squares can overflow; unit weights never do).  last_stats["squared_tardiness"],
+    ["weighted_tardiness"] and ["late_tasks"] (squared_tardiness), or last_stats["squared_flow"] and
+    ["total_flow_time"] (squared_flow), are recomputed in float64 from the emitted plan, the tasks' own runtimes and
+    the caller's d, r and w; last_stats["device_makespan"] holds the device's fp32 score.  The 6th element stays the
+    plan's makespan.
+
     Release dates.  `release` (a sequence aligned with task_list, or a mapping keyed by Task, in the runtimes' units
     from the plan's t = 0) keeps every task from starting before its release date, under every objective: a
     dataset or a parent checkpoint that is only ready later, a job that arrives tomorrow.  r <= 0 means already
@@ -527,6 +578,8 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
         # p*_t in the tasks' own runtimes: the fastest option among the cells the device table keeps
         pstar = [min(float(list(t.strategies.values())[int(optindex[j, g])].runtime)
                      for g in range(NSLOT) if np.isfinite(Tdev[j, 0, g])) for j, t in enumerate(task_list)]
+    elif objective == "squared_flow":
+        d32 = _release_due(r32, J)
     if nodes is None:
         nodes = _default_nodes()
     nodes = int(nodes)
@@ -583,6 +636,10 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
         last_stats.update(_late_count_stats(dec["start"], rts, w64, d64))
     elif objective == "max_stretch":
         last_stats.update(_stretch_stats(dec["start"], rts, pstar, r64))
+    elif objective == "squared_tardiness":
+        last_stats.update(_squared_stats(dec["start"], rts, w64, d64))
+    elif objective == "squared_flow":
+        last_stats.update(_squared_flow_stats(dec["start"], rts, w64, r64))
     elif d64 is not None:
         last_stats.update(_tardiness_stats(dec["start"], rts, w64, d64))
     if r64 is not None:
@@ -690,6 +747,7 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     aligned with T's rows; `release` as for solve(), under every objective, a sequence aligned with T's rows
     (last_stats["total_flow_time"]).  objective="max_stretch" as for solve(), with p*_t the smallest cell of row t
     the search may propose, over every strategy (last_stats["max_stretch"] and ["mean_stretch"] from T's values).
+    objective="squared_tardiness" (with `due`) and "squared_flow" as for solve(), with their last_stats from T's values.
     Every cell of T must be
     >= 0 (-0.0 counts as zero), +inf or a sentinel: a negative or NaN cell raises SolverError, with or without `mask`.
 
@@ -728,6 +786,8 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     _check_horizon(Tdev, release=r64, tails=_tails(d32) if objective == "max_lateness" else None)
     if objective == "max_stretch":
         pstar, w32, d32 = _stretch_form(Tdev, r32)
+    elif objective == "squared_flow":
+        d32 = _release_due(r32, J)
     eng = engine if engine is not None else _engine(devices)
     nodes = int(_default_nodes() if nodes is None else nodes)
     eng.set_table(Tdev, gcount, sentinel=float("inf"), nodes=nodes)
@@ -776,6 +836,10 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
         last_stats.update(_late_count_stats(dec["start"], rts, w64, d64))
     elif objective == "max_stretch":
         last_stats.update(_stretch_stats(dec["start"], rts, pstar, r64))
+    elif objective == "squared_tardiness":
+        last_stats.update(_squared_stats(dec["start"], rts, w64, d64))
+    elif objective == "squared_flow":
+        last_stats.update(_squared_flow_stats(dec["start"], rts, w64, r64))
     elif d64 is not None:
         last_stats.update(_tardiness_stats(dec["start"], rts, w64, d64))
     if r64 is not None:

@@ -3,7 +3,7 @@ maximum lateness, of the (weighted) number of late tasks, of the maximum stretch
 prints one JSON line.
 
     python scripts/bench_objective.py [--steps 200] [--warmup 20] [--solve-chains 0] [--solve-rounds 400]
-                                      [--only max_stretch]
+                                      [--only max_stretch | squared]
 
 kernel: sb_eval on bench.py's C4 batch (J = 256, S = 8, 946,176 candidates, the same seeded inputs, integer
         starts), scored for the makespan, the sum of completion times, the weighted sum (seeded weights) and the
@@ -31,6 +31,10 @@ stretch: the same 256-task set and release dates: solve(objective="max_stretch")
         stretch and makespan (stretch (C_t - max(r_t, 0)) / p*_t, p*_t the task's fastest proposable runtime).
 --only max_stretch times only the weighted tardiness and the weighted maximum tardiness and runs only the stretch
 comparison.
+--only squared times only the weighted tardiness and the weighted squared tardiness (the same weights and due dates),
+alternated as above, and runs only the squared-flow comparison: on the same 256-task set and release dates,
+solve(objective="squared_flow") against the completion, max_stretch and makespan plans (all release-aware), each
+rescored in float64 on sum_t F_t^2, mean F_t and max F_t, the flow time F_t = C_t - max(r_t, 0).
 The card's name and power limit are read in the same run (nvidia-smi, read-only queries).
 """
 import argparse
@@ -62,7 +66,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--solve-chains", type=int, default=0, help="0 = solve()'s default population")
     ap.add_argument("--solve-rounds", type=int, default=400)
-    ap.add_argument("--only", choices=("all", "max_stretch"), default="all")
+    ap.add_argument("--only", choices=("all", "max_stretch", "squared"), default="all")
     args = ap.parse_args()
     import numpy as np
     import torch
@@ -90,6 +94,8 @@ def main():
             "release_weighted_tardiness", "max_lateness", "weighted_late_tasks", "weighted_max_tardiness")
     if args.only == "max_stretch":
         objs = ("weighted_tardiness", "weighted_max_tardiness")
+    if args.only == "squared":
+        objs = ("weighted_tardiness", "weighted_squared_tardiness")
     times = {o: [] for o in objs}
     for i in range(args.warmup + args.steps):
         for obj in objs[i % len(objs):] + objs[:i % len(objs)]:
@@ -106,6 +112,20 @@ def main():
     kernel = {o: {"median_ms": float(np.median(t)), "p10_ms": float(np.percentile(t, 10)),
                   "p90_ms": float(np.percentile(t, 90)), "candidates_per_s": B / (float(np.median(t)) * 1e-3)}
               for o, t in times.items()}
+    if args.only == "squared":
+        kernel["squared_over_weighted_tardiness"] = (kernel["weighted_squared_tardiness"]["median_ms"] /
+                                                     kernel["weighted_tardiness"]["median_ms"])
+        kernel.update(B=B, J=J, S=Sx, path=path, steps=args.steps)
+        del opt, prio, out
+        eng_r.close()
+        torch.cuda.empty_cache()
+        tasks = _tasks256()
+        kw = dict(rounds=args.solve_rounds, seed=1, engine=eng, **({"chains": args.solve_chains}
+                                                                   if args.solve_chains else {}))
+        makespan = S.solve(tasks, None, **kw)[5]
+        print(json.dumps({"card": card(0), "kernel": kernel, "squared_flow": squared_effect(S, R, tasks, makespan, kw)}))
+        eng.close()
+        return
     kernel["max_tardiness_over_weighted_tardiness"] = (kernel["weighted_max_tardiness"]["median_ms"] /
                                                        kernel["weighted_tardiness"]["median_ms"])
     if args.only == "max_stretch":
@@ -217,6 +237,26 @@ def stretch_effect(S, R, tasks, makespan, kw):
         st = [(c - max(x, 0.0)) / p for c, x, p in zip(comp, r, pstar)]
         out[name] = {"max_stretch": max(st), "mean_stretch": sum(st) / J, "makespan": max(comp), "wall_s": wall,
                      "rounds": S.last_stats["rounds"]}
+    return out
+
+
+def squared_effect(S, R, tasks, makespan, kw):
+    """The squared-flow plan against the completion, max_stretch and makespan plans on the 256-task set with the
+    release dates of release_effect, every plan rescored in float64 on the flow times F_t = C_t - max(r_t, 0) (see the
+    module doc)."""
+    import numpy as np
+    J = len(tasks)
+    tuples = [[(g, s.runtime) for g, s in t.strategies.items()] for t in tasks]
+    r = [float(x) for x in np.random.default_rng(6).integers(0, int(0.5 * makespan), size=J)]
+    out = {}
+    for obj in ("squared_flow", "completion", "max_stretch", "makespan"):
+        t0 = time.perf_counter()
+        res = S.solve(tasks, None, objective=obj, release=r, **kw)
+        wall = time.perf_counter() - t0
+        comp = [p[0] + p[2] for p in R.plan_from_arrays(tuples, res[0], res[1], res[2], res[3])]
+        flow = [c - max(x, 0.0) for c, x in zip(comp, r)]
+        out[obj] = {"sum_flow_squared": sum(f * f for f in flow), "mean_flow": sum(flow) / J, "max_flow": max(flow),
+                    "makespan": max(comp), "wall_s": wall, "rounds": S.last_stats["rounds"]}
     return out
 
 
