@@ -76,6 +76,13 @@
  * Due dates at or past every completion give +0, w = 2 exactly twice w = 1 (barring overflow).  The score is >= +0.  A
  * job with no runtime (rt = +inf) gives a +inf term.  d_j = max(r_j, 0) makes it the squared flow time
  * sum_j w_j (C_j - max(r_j, 0))^2 (sum_j w_j C_j^2 without release dates).
+ * With SB_FLAG_LATE_PENALTY as well (per-job late penalties p_j >= 0, sb_set_penalty) it is the late penalty:
+ *   total = sum_j [C_j > d_j] (p_j + w_j (C_j - d_j)), from +0 in schedule order per job: e = start + rt, x = e - d,
+ *   then acc = acc + (x > 0 ? p + (w * x) : +0), the product and the sum each rounded on their own (no fused
+ *   multiply-add).
+ * A job that completes exactly at its due date is on time.  p = 0 gives exactly the tardiness fold of SB_FLAG_DUE,
+ * due dates at or past every completion give +0, and the score is >= +0.  A job with no runtime (rt = +inf) gives a
+ * +inf term.  The comparison C > d is made in fp32, as the late count makes it.
  * The schedule, every start and every slot mask are the same under every objective.
  * With SB_FLAG_MAX_LATENESS (per-job due dates d_j, sb_set_due) the score is the maximum lateness
  * L_max = max_j (start_j + rt_j - d_j), emitted as the tail makespan L_max + D >= +0 with D = max_t d_t:
@@ -232,6 +239,20 @@ typedef enum sb_status {
                                      floor with each runtime squared), it stops as soon as the incumbent is +0
                                      (stop_reason 3), and sb_search_seed_lpt plants the EDD orders of SB_FLAG_DUE.
                                      Not available with SB_FLAG_ALT_WARPSCAN (SB_ERR_UNSUPPORTED). */
+#define SB_FLAG_LATE_PENALTY 16384u /* with SB_FLAG_SUM_COMPLETION | SB_FLAG_DUE only (SB_FLAG_WEIGHTED, the rate per
+                                     unit of time late, optional; else SB_ERR_ARG), and not with SB_FLAG_LATE_COUNT,
+                                     SB_FLAG_MAX_TARDINESS, SB_FLAG_SQUARED or SB_FLAG_MAX_LATENESS (SB_ERR_ARG),
+                                     after sb_set_penalty (else SB_ERR_STATE, checked after the due dates and before
+                                     the release dates): each late job adds its fixed penalty to its weighted
+                                     tardiness, and the objective is sum_j [C_j > d_j] (p_j + w_j (C_j - d_j)) (see
+                                     the evaluation rule above).  Accepted by sb_eval, sb_eval_host, sb_eval_full,
+                                     sb_decode and the search, sb_search_run_multi included (every handle must hold
+                                     penalties); every score the library emits then holds the total penalty, and
+                                     target_makespan targets it.  The search's temperature unit becomes
+                                     max(incumbent / sum_j w_j, (sum_j w_j min_k rt_jk + sum_j p_j) / sum_j w_j)
+                                     (SB_FLAG_DUE's floor with the penalties added), it stops as soon as the
+                                     incumbent is +0 (stop_reason 3), and sb_search_seed_lpt plants the EDD orders of
+                                     SB_FLAG_DUE.  Not available with SB_FLAG_ALT_WARPSCAN (SB_ERR_UNSUPPORTED). */
 #define SB_IPC_HANDLE_BYTES 64
 
 typedef struct sb_handle sb_handle;
@@ -282,6 +303,12 @@ int sb_set_due(sb_handle* h, const float* d, int J);
  * uses is made here, once.  sb_set_table clears the release dates; setting or clearing them ends the current
  * search (sb_search_init again). */
 int sb_set_release(sb_handle* h, const float* r, int J);
+/* Per-job late penalties for SB_FLAG_LATE_PENALTY: p host fp32 [J], the fixed cost of each job that completes after
+ * its due date, every value finite and >= 0 with J * max_j p_j < 2^126 (else SB_ERR_ARG, as is a J that differs
+ * from the table's); -0 is stored as +0.  p = NULL clears them.  SB_ERR_STATE before sb_set_table.  sb_set_table
+ * clears the penalties; setting or clearing them ends the current search (sb_search_init again).  Their sum is
+ * recorded for the search's temperature unit. */
+int sb_set_penalty(sb_handle* h, const float* p, int J);
 /* copy the reduced table back (host pointers, either may be NULL): tmin fp32 [J][8], args u8 [J][8].
  * This is the table the reference solver is actually given: Task.strategies[g] after the profiler's
  * min over executors (PerformanceEvaluator.py:101-115), read at milp.py:77-81. */

@@ -20,6 +20,7 @@ FLAG_MAX_LATENESS = 1024
 FLAG_LATE_COUNT = 2048
 FLAG_MAX_TARDINESS = 4096
 FLAG_SQUARED = 8192
+FLAG_LATE_PENALTY = 16384
 IPC_HANDLE_BYTES = 64
 # test hooks in the top bits of the same flags word: the enum in csrc/sb_internal.h says what each one forces
 HOOK_FORCE_GENERIC = 0x80000000
@@ -42,7 +43,7 @@ TILE_DEBUG_NO_STAGGER = 4
 # every symbol include/saturn_b200.h declares (tests check that the library exports them all)
 SYMBOLS = [
     "sb_abi_version", "sb_last_error", "sb_create", "sb_destroy", "sb_sync", "sb_set_table",
-    "sb_set_sentinel", "sb_set_weights", "sb_set_due", "sb_set_release", "sb_get_reduced", "sb_eval", "sb_last_eval_path", "sb_validate", "sb_eval_host", "sb_eval_full",
+    "sb_set_sentinel", "sb_set_weights", "sb_set_due", "sb_set_release", "sb_set_penalty", "sb_get_reduced", "sb_eval", "sb_last_eval_path", "sb_validate", "sb_eval_host", "sb_eval_full",
     "sb_decode", "sb_xchg_create", "sb_xchg_connect", "sb_xchg_connect_local", "sb_xchg_post", "sb_xchg_reduce", "sb_xchg_check",
     "sb_search_init", "sb_search_round", "sb_search_best_key_ptr", "sb_search_best",
     "sb_search_inject", "sb_search_resample", "sb_search_seed_lpt", "sb_search_run", "sb_search_run_multi", "sb_search_wave", "sb_search_is_fused", "sb_search_stats", "sb_search_validate", "sb_search_verify_count",
@@ -98,6 +99,7 @@ def load():
         "sb_set_weights": [vp, vp, ci],
         "sb_set_due": [vp, vp, ci],
         "sb_set_release": [vp, vp, ci],
+        "sb_set_penalty": [vp, vp, ci],
         "sb_get_reduced": [vp, vp, vp],
         "sb_eval": [vp, vp, vp, i64, i64, u32, vp, vp, C.c_uint32],
         "sb_last_eval_path": [vp],

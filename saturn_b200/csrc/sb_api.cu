@@ -71,6 +71,7 @@ struct SearchState {
   const float* due = nullptr;  // obj_due: the handle's due dates (TailMakespan: its delivery tails)
                                // (position-major kernels)
   const float* rel = nullptr;  // SB_FLAG_RELEASE: the handle's release dates as the flags read them (likewise)
+  const float* pen = nullptr;  // obj_penalty: the handle's late penalties (likewise)
 };
 
 struct sb_handle {
@@ -135,6 +136,12 @@ struct sb_handle {
   size_t d_r_cap = 0;
   std::vector<float> h_r, h_rc;
   bool has_r = false;
+  // late penalties (sb_set_penalty): device copy padded like d_w, and their sum in double (the temperature unit);
+  // has_p is cleared by sb_set_table
+  float* d_p = nullptr;
+  size_t d_p_cap = 0;
+  double p_sum = 0.0;
+  bool has_p = false;
   SearchState search;
   int last_path = -1;
   // peer-memory exchange
@@ -252,6 +259,7 @@ int sb_destroy(sb_handle* h) {
   cudaFree(h->d_q);
   cudaFree(h->d_r);
   cudaFree(h->d_rc);
+  cudaFree(h->d_p);
   for (int i = 0; i < 2; ++i)
     if (h->hs[i]) cudaStreamDestroy(h->hs[i]);
   if (h->own_stream && h->stream) cudaStreamDestroy(h->stream);
@@ -284,6 +292,7 @@ int sb_set_table(sb_handle* h, const float* T, const uint8_t* gcount, int J, int
   h->has_w = false;         // weights belong to a task set: a new table needs new ones
   h->has_d = false;         // so do due dates
   h->has_r = false;         // and release dates
+  h->has_p = false;         // and late penalties
   const size_t nT = static_cast<size_t>(J) * S * G;
   const size_t ntab = static_cast<size_t>(J) * S * kSlots;
   // a re-planning loop sets a table of the same shape every interval: keep the allocations (cudaFree /
@@ -475,14 +484,62 @@ int sb_set_release(sb_handle* h, const float* r, int J) {
   return SB_OK;
 }
 
+int sb_set_penalty(sb_handle* h, const float* p, int J) {
+  int rc = use_device(h);
+  if (rc) return rc;
+  if (h->J == 0) return fail(SB_ERR_STATE, "sb_set_table has not been called");
+  CK(cudaStreamSynchronize(h->stream));  // no queued kernel may still read the old penalties
+  h->search.ready = false;               // the running search was set up for the old penalties (scale)
+  if (!p) {
+    h->has_p = false;
+    return SB_OK;
+  }
+  if (J != h->J) return fail(SB_ERR_ARG, "J=%d differs from the table's J=%d", J, h->J);
+  double sum = 0.0, pmax = 0.0;
+  for (int j = 0; j < J; ++j) {
+    if (!isfinite(p[j]) || !(p[j] >= 0.f)) return fail(SB_ERR_ARG, "late penalty %d (%g) is not finite and >= 0", j, p[j]);
+    sum += static_cast<double>(p[j]);
+    pmax = std::max(pmax, static_cast<double>(p[j]));
+  }
+  // below J * max p < 2^126 the penalties alone sum below FLT_MAX
+  if (!(static_cast<double>(J) * pmax < 0x1p126))
+    return fail(SB_ERR_ARG, "J * max p (%g) is not below 2^126: the fp32 sum of the penalties could overflow",
+                static_cast<double>(J) * pmax);
+  h->has_p = false;
+  const size_t cap = static_cast<size_t>((J + 3) & ~3);
+  if (h->d_p_cap < cap) {
+    cudaFree(h->d_p);
+    h->d_p = nullptr;
+    h->d_p_cap = 0;
+    CK(cudaMalloc(&h->d_p, cap * sizeof(float)));
+    h->d_p_cap = cap;
+  }
+  // -0 is stored as +0 (x + 0 = x otherwise), as sb_set_release stores its release dates
+  std::vector<float> hp(cap, 0.f);
+  for (int j = 0; j < J; ++j) hp[j] = p[j] + 0.f;
+  CK(cudaMemcpyAsync(h->d_p, hp.data(), cap * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  h->p_sum = sum;
+  h->has_p = true;
+  return SB_OK;
+}
+
 // The one reader of the objective flags.  SB_FLAG_WEIGHTED and SB_FLAG_DUE are valid with SB_FLAG_SUM_COMPLETION only;
-// SB_FLAG_MAX_LATENESS alone among the objective flags; SB_FLAG_LATE_COUNT, SB_FLAG_MAX_TARDINESS and SB_FLAG_SQUARED
-// with SB_FLAG_SUM_COMPLETION | SB_FLAG_DUE only (they change what the tardiness form adds per job, and how it folds
-// its terms), and not together or with SB_FLAG_MAX_LATENESS.  Every other combination is SB_ERR_ARG.
+// SB_FLAG_MAX_LATENESS alone among the objective flags; SB_FLAG_LATE_COUNT, SB_FLAG_MAX_TARDINESS, SB_FLAG_SQUARED and
+// SB_FLAG_LATE_PENALTY with SB_FLAG_SUM_COMPLETION | SB_FLAG_DUE only (they change what the tardiness form adds per
+// job, and how it folds its terms), and not together or with SB_FLAG_MAX_LATENESS.  Every other combination is
+// SB_ERR_ARG.
 static int decode_objective(unsigned flags, Objective* o) {
   const bool sum = flags & SB_FLAG_SUM_COMPLETION, weighted = flags & SB_FLAG_WEIGHTED, due = flags & SB_FLAG_DUE;
   const bool lateness = flags & SB_FLAG_MAX_LATENESS, late = flags & SB_FLAG_LATE_COUNT;
   const bool max_tardiness = flags & SB_FLAG_MAX_TARDINESS, squared = flags & SB_FLAG_SQUARED;
+  const bool penalty = flags & SB_FLAG_LATE_PENALTY;
+  if (penalty && !(sum && due))
+    return fail(SB_ERR_ARG, "SB_FLAG_LATE_PENALTY adds a fixed penalty to the tardiness form's late terms: it needs "
+                "SB_FLAG_SUM_COMPLETION and SB_FLAG_DUE");
+  if (penalty && (late || max_tardiness || squared || lateness))
+    return fail(SB_ERR_ARG, "SB_FLAG_LATE_PENALTY cannot be combined with SB_FLAG_LATE_COUNT, SB_FLAG_MAX_TARDINESS, "
+                "SB_FLAG_SQUARED or SB_FLAG_MAX_LATENESS");
   if (squared && !(sum && due))
     return fail(SB_ERR_ARG, "SB_FLAG_SQUARED squares the tardiness form's terms: it needs SB_FLAG_SUM_COMPLETION and "
                 "SB_FLAG_DUE");
@@ -510,6 +567,7 @@ static int decode_objective(unsigned flags, Objective* o) {
   else if (late) o->obj = Obj::LateCount;
   else if (max_tardiness) o->obj = Obj::MaxTardiness;
   else if (squared) o->obj = Obj::SquaredTardiness;
+  else if (penalty) o->obj = Obj::LatePenalty;
   else if (due) o->obj = Obj::Tardiness;
   else o->obj = weighted ? Obj::WeightedSum : Obj::Sum;
   return SB_OK;
@@ -517,7 +575,8 @@ static int decode_objective(unsigned flags, Objective* o) {
 
 // the objectives folded from the tardiness form (SB_FLAG_DUE): their scores reach +0, which no plan can beat
 static bool tardiness_form(Obj o) {
-  return o == Obj::Tardiness || o == Obj::LateCount || o == Obj::MaxTardiness || o == Obj::SquaredTardiness;
+  return o == Obj::Tardiness || o == Obj::LateCount || o == Obj::MaxTardiness || o == Obj::SquaredTardiness ||
+         o == Obj::LatePenalty;
 }
 
 // decode_objective, then the per-job arrays the objective reads (and SB_FLAG_RELEASE's) must be set on the handle
@@ -536,6 +595,8 @@ static int check_per_job(const sb_handle* h, unsigned flags, Objective* o) {
   if (o->obj == Obj::SquaredTardiness && o->weighted && !h->sq_finite)
     return fail(SB_ERR_ARG, "SB_FLAG_SQUARED | SB_FLAG_WEIGHTED needs J * max w * 2^50 < FLT_MAX (beyond it the sum of "
                 "squared tardiness can overflow fp32)");
+  if (obj_penalty(o->obj) && !h->has_p)
+    return fail(SB_ERR_STATE, "SB_FLAG_LATE_PENALTY needs sb_set_penalty (sb_set_table clears the penalties)");
   if ((flags & SB_FLAG_RELEASE) && !h->has_r)
     return fail(SB_ERR_STATE, "SB_FLAG_RELEASE needs sb_set_release (sb_set_table clears the release dates)");
   return SB_OK;
@@ -550,6 +611,8 @@ static const float* job_due(const sb_handle* h, Obj obj) {
   if (!obj_due(obj)) return nullptr;
   return obj == Obj::TailMakespan ? h->d_q : h->d_d;
 }
+// the late penalties the kernels read, or none
+static const float* job_penalty(const sb_handle* h, Obj obj) { return obj_penalty(obj) ? h->d_p : nullptr; }
 // the weights the kernels read: the caller's, unit weights, or none
 static const float* job_weights(const sb_handle* h, const Objective& o) {
   if (!obj_weights(o.obj)) return nullptr;
@@ -594,6 +657,7 @@ static int make_call(sb_handle* h, const uint8_t* opt, const void* prio, int64_t
   c->w = job_weights(h, o);
   c->d = job_due(h, o.obj);
   c->r = job_release(h, flags);
+  c->p = job_penalty(h, o.obj);
   return SB_OK;
 }
 
@@ -655,7 +719,8 @@ int sb_eval(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, int64
     if (c.obj != Obj::Makespan || (flags & SB_FLAG_RELEASE))
       return fail(SB_ERR_UNSUPPORTED, "SB_FLAG_ALT_WARPSCAN scores the makespan without release dates only: it "
                   "cannot be combined with SB_FLAG_SUM_COMPLETION, SB_FLAG_WEIGHTED, SB_FLAG_DUE, SB_FLAG_RELEASE, "
-                  "SB_FLAG_MAX_LATENESS, SB_FLAG_LATE_COUNT, SB_FLAG_MAX_TARDINESS or SB_FLAG_SQUARED");
+                  "SB_FLAG_MAX_LATENESS, SB_FLAG_LATE_COUNT, SB_FLAG_MAX_TARDINESS, SB_FLAG_SQUARED or "
+                  "SB_FLAG_LATE_PENALTY");
     if (flags & (SB_FLAG_POST_KEY | SB_FLAG_FOLD_PREV))
       return fail(SB_ERR_UNSUPPORTED, "SB_FLAG_ALT_WARPSCAN cannot be combined with the fused key exchange");
     cudaError_t e = eval_alt_launch(h->dev, c, h->stream);
@@ -991,7 +1056,8 @@ static int search_eval(sb_handle* h, bool cur_rows, long long first, long long c
     SearchFuse sf = {};
     sf.cur_mk = s.d.cur_mk;
     const bool reduced = (s.p.flags & SB_FLAG_REDUCED) != 0;
-    CK(search_pos_launch(h->dev, s.d, reduced ? h->tmin : h->tab, s.w, s.due, s.rel, (reduced ? 1 : h->S) * kSlots, s.p.flags,
+    CK(search_pos_launch(h->dev, s.d, reduced ? h->tmin : h->tab, s.w, s.due, s.rel, s.pen,
+                         (reduced ? 1 : h->S) * kSlots, s.p.flags,
                          s.obj.obj, first, count, true, sf, h->stream));
     return SB_OK;
   }
@@ -1034,6 +1100,7 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
   s.w = job_weights(h, o);
   s.due = job_due(h, o.obj);
   s.rel = job_release(h, p->flags);
+  s.pen = job_penalty(h, o.obj);
   d.stride_o = (J + 31) & ~31;  // 32-byte rows: TMA bulk copies for opt, 256-bit streaming loads for prio
   // make stride_p == stride_o * pb so that one element stride describes both (sb_eval contract)
   d.stride_p = d.stride_o * pb;
@@ -1132,6 +1199,10 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
     // sum_j w_j (a starting point, not a measured choice, DESIGN §3)
     else if (o.obj == Obj::SquaredTardiness)
       s.scale = std::max(s.scale, static_cast<float>(move_sq / (weighted ? h->w_sum : static_cast<double>(J))));
+    // the late penalty: the tardiness floor with every penalty added, (sum_j w_j lo_j + sum_j p_j) / sum_j w_j,
+    // which is the tardiness unit bit for bit when every p = 0 (a starting point, not a measured choice, DESIGN §3)
+    else if (o.obj == Obj::LatePenalty)
+      s.scale = std::max(s.scale, static_cast<float>((move + h->p_sum) / (weighted ? h->w_sum : static_cast<double>(J))));
     else s.scale = std::max(s.scale, static_cast<float>(move / (weighted ? h->w_sum : static_cast<double>(J))));
   }
   // the late count moves in steps of one job's weight and is 0 at many incumbents: its unit is the count of every job,
@@ -1238,7 +1309,8 @@ int sb_search_round(sb_handle* h, int rounds) {
       SearchFuse sf = make_fuse(s, round, n);
       sf.resample_every = 0;
       const bool reduced = (s.p.flags & SB_FLAG_REDUCED) != 0;
-      CK(search_pos_launch(h->dev, s.d, reduced ? h->tmin : h->tab, s.w, s.due, s.rel, (reduced ? 1 : h->S) * kSlots, s.p.flags,
+      CK(search_pos_launch(h->dev, s.d, reduced ? h->tmin : h->tab, s.w, s.due, s.rel, s.pen,
+                         (reduced ? 1 : h->S) * kSlots, s.p.flags,
                            s.obj.obj, 0, s.d.chains, false, sf, h->stream));  // keeps the incumbent in its tail
       fused = true;
     } else if (s.fused_ok) {

@@ -19,8 +19,8 @@ constexpr float kSentinel = 1.0e6f;  // reference's "unprofiled" runtime, Perfor
 __device__ __forceinline__ float inf_f() { return __int_as_float(0x7f800000); }
 
 // ---------------------------------------------------------------- the objective
-// The eight scores the kernels compute, and the SB_FLAG_* bits that select each (sb_api.cu: decode_objective; every
-// form also runs with SB_FLAG_RELEASE).  C is a job's completion, w its weight, d its due date.
+// The nine scores the kernels compute, and the SB_FLAG_* bits that select each (sb_api.cu: decode_objective; every
+// form also runs with SB_FLAG_RELEASE).  C is a job's completion, w its weight, d its due date, p its late penalty.
 //   Obj               flags                                              score
 //   Makespan          none                                               max C
 //   TailMakespan      MAX_LATENESS                                       max (C + q), tails q = max d - d (L_max + max d)
@@ -30,24 +30,29 @@ __device__ __forceinline__ float inf_f() { return __int_as_float(0x7f800000); }
 //   LateCount         SUM_COMPLETION | DUE | LATE_COUNT [| WEIGHTED]     sum (C > d ? w : 0)
 //   MaxTardiness      SUM_COMPLETION | DUE | MAX_TARDINESS [| WEIGHTED]  max w max(C - d, 0)
 //   SquaredTardiness  SUM_COMPLETION | DUE | SQUARED [| WEIGHTED]        sum w max(C - d, 0)^2
+//   LatePenalty       SUM_COMPLETION | DUE | LATE_PENALTY [| WEIGHTED]   sum (C > d ? p + w (C - d) : 0)
 // Every other combination of those flags is refused.  The history of each form is in DESIGN.md.  New forms go at the
 // end: a kernel's symbol holds its form's value.
-enum class Obj { Makespan, TailMakespan, Sum, WeightedSum, Tardiness, LateCount, MaxTardiness, SquaredTardiness };
+enum class Obj {
+  Makespan, TailMakespan, Sum, WeightedSum, Tardiness, LateCount, MaxTardiness, SquaredTardiness, LatePenalty
+};
 // the score is a sum over the jobs, folded in schedule order
 __host__ __device__ constexpr bool obj_sum(Obj o) {
   return o == Obj::Sum || o == Obj::WeightedSum || o == Obj::Tardiness || o == Obj::LateCount ||
-         o == Obj::SquaredTardiness;
+         o == Obj::SquaredTardiness || o == Obj::LatePenalty;
 }
 // the score reads the job weights (the caller's, or unit weights without SB_FLAG_WEIGHTED)
 __host__ __device__ constexpr bool obj_weights(Obj o) {
   return o == Obj::WeightedSum || o == Obj::Tardiness || o == Obj::LateCount || o == Obj::MaxTardiness ||
-         o == Obj::SquaredTardiness;
+         o == Obj::SquaredTardiness || o == Obj::LatePenalty;
 }
 // the score reads the due-date array: the due dates, or TailMakespan's tails
 __host__ __device__ constexpr bool obj_due(Obj o) {
   return o == Obj::TailMakespan || o == Obj::Tardiness || o == Obj::LateCount || o == Obj::MaxTardiness ||
-         o == Obj::SquaredTardiness;
+         o == Obj::SquaredTardiness || o == Obj::LatePenalty;
 }
+// the score reads the late-penalty array (sb_set_penalty)
+__host__ __device__ constexpr bool obj_penalty(Obj o) { return o == Obj::LatePenalty; }
 
 // ---------------------------------------------------------------- mbarrier + TMA bulk copy (1-D)
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -181,8 +186,9 @@ __device__ __forceinline__ float fmax3_mk(float mk, float b, float c) {
 }
 
 // The job's completion e = s + rt is folded into mk by the objective kObj; `w` is the job's weight, `d` its due date
-// (TailMakespan: its tail q), each read only by the forms that use it.  Every product and sum is rounded on its own
-// (__fmul_rn, __fadd_rn: nvcc would otherwise contract them into one FFMA, which the oracle cannot reproduce).
+// (TailMakespan: its tail q), `p` its late penalty, each read only by the forms that use it.  Every product and sum is
+// rounded on its own (__fmul_rn, __fadd_rn: nvcc would otherwise contract them into one FFMA, which the oracle cannot
+// reproduce).
 //   Makespan     : only with kTrackMk (integer starts: the slot state holds s + ceil(rt), not the completion; several
 //                  nodes: no single f[7] at the end), mk = max(mk, e).  `ph` pairs the completions of two consecutive
 //                  steps into one 3-input max: 0 parks this step's completion in `pend`, 1 folds max(mk, pend, e);
@@ -198,14 +204,16 @@ __device__ __forceinline__ float fmax3_mk(float mk, float b, float c) {
 //                  +0)), Tardiness's term bit for bit folded with max; a job with no runtime (rt = +inf, w > 0) gives
 //                  a +inf term.  SquaredTardiness: t = max(e - d, +0), Tardiness's term before the weight bit for
 //                  bit, then mk + w * (t * t), three roundings; w = 1 gives the unweighted form bit for bit, and a
-//                  job with no runtime a +inf term.
+//                  job with no runtime a +inf term.  LatePenalty: x = e - d, then mk + (x > 0 ? p + w * x : +0), the
+//                  product and the sum rounded on their own; p = +0 gives Tardiness's term bit for bit (+0 added to
+//                  a positive finite value is exact), and a job with no runtime a +inf term.
 // The slot update is the same under every objective: only the score differs.
 // kRelease (SB_FLAG_RELEASE): the job starts no earlier than its release date `r`, s = max(f[km1], r) (ceil(r) under
 // integer starts, made once by sb_set_release, so s stays an integer).  The slot update below stays valid because it
 // only needs v >= f[km1]; r <= 0 gives s = f[km1] exactly.
 template <bool kIntegerStarts, bool kTrackMk = kIntegerStarts, Obj kObj = Obj::Makespan, bool kRelease = false>
 __device__ __forceinline__ void ls_step(float (&f)[8], float& mk, float& pend, float rt, int km1, int one, int ph,
-                                        float w = 0.f, float d = 0.f, float r = 0.f) {
+                                        float w = 0.f, float d = 0.f, float r = 0.f, float p = 0.f) {
   const float INF = inf_f();
   const int b2 = km1 & 4, b1 = km1 & 2, b0 = km1 & 1;
   // stage "shift by 4"
@@ -251,6 +259,10 @@ __device__ __forceinline__ void ls_step(float (&f)[8], float& mk, float& pend, f
     else if constexpr (kObj == Obj::SquaredTardiness) {
       const float x = __fsub_rn(e, d);
       mk = __fadd_rn(mk, __fmul_rn(w, __fmul_rn(x, fmaxf(x, 0.f))));
+    }
+    else if constexpr (kObj == Obj::LatePenalty) {
+      const float x = __fsub_rn(e, d);
+      mk = __fadd_rn(mk, x > 0.f ? __fadd_rn(p, __fmul_rn(w, x)) : 0.f);
     }
     else if constexpr (kObj == Obj::WeightedSum) mk = __fadd_rn(mk, __fmul_rn(w, e));
     else mk = mk + e;

@@ -28,8 +28,8 @@
 //     folded with one redux + one atomicMin per warp;
 //   * OBJ: every kernel here comes in a form per objective (sb_common.cuh: Obj), folded by ls_step; the schedule,
 //     and every start, is the same under all of them.  The per-job arrays an objective reads (weights,
-//     due dates or tails) sit beside the table wherever the table is in shared memory (same TMA phase), and are
-//     read from global memory where the table is;
+//     due dates or tails, late penalties) sit beside the table wherever the table is in shared memory (same TMA
+//     phase), and are read from global memory where the table is;
 //   * R (SB_FLAG_RELEASE, with any objective): no job starts before its release date.  Every objective form has
 //     a release twin; the release dates follow the other per-job arrays, in the same memory and TMA phase.
 #include "sb_lane.cuh"
@@ -61,6 +61,7 @@ struct TileArgs {
   int packed;    // consecutive candidates' rows lie back to back (stride_o == copy_o == row_o, stride_p == copy_p)
   int stagger;   // start the warps of a CTA at staggered phases
   unsigned long long* tile_wait;  // TILE_DEBUG_TIMING: [0] += fetch-to-wait ns, [1] += tile-loop ns, per warp
+  const float* p;  // obj_penalty(OBJ): job late penalties [J], padded like w (last: the other fields keep their offsets)
 };
 
 // TABG: the runtime table stays in global memory (read through L1/L2) — for tables larger than the
@@ -75,16 +76,18 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t tab_bytes = TABG ? 0u : static_cast<uint32_t>(a.J) * a.SG * 4u;  // a multiple of 32 (SG = S * 8)
   // the per-job arrays the objective reads follow the table in the same TMA phase, each padded to 16 bytes: the
-  // weights, the due dates (or tails), the release dates (TABG: they all stay in global memory)
-  constexpr bool kW = obj_weights(OBJ), kD = obj_due(OBJ);
+  // weights, the due dates (or tails), the release dates, the late penalties (TABG: they all stay in global memory)
+  constexpr bool kW = obj_weights(OBJ), kD = obj_due(OBJ), kP = obj_penalty(OBJ);
   const uint32_t w_bytes = (kW && !TABG) ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u;
   const uint32_t d_bytes = kD ? (kW ? w_bytes : (TABG ? 0u : ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u))) : 0u;
   const uint32_t r_bytes = (R && !TABG) ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u;
+  const uint32_t p_bytes = kP ? w_bytes : 0u;  // the penalties come with the weights (obj_weights)
   float* tab_s = reinterpret_cast<float*>(smem);
   [[maybe_unused]] float* w_s = reinterpret_cast<float*>(smem + tab_bytes);
   [[maybe_unused]] float* d_s = reinterpret_cast<float*>(smem + tab_bytes + w_bytes);
   [[maybe_unused]] float* r_s = reinterpret_cast<float*>(smem + tab_bytes + w_bytes + d_bytes);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + ((tab_bytes + w_bytes + d_bytes + r_bytes + 15u) & ~15u));
+  [[maybe_unused]] float* p_s = reinterpret_cast<float*>(smem + tab_bytes + w_bytes + d_bytes + r_bytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + ((tab_bytes + w_bytes + d_bytes + r_bytes + p_bytes + 15u) & ~15u));
   uint8_t* tiles = reinterpret_cast<uint8_t*>(bars) + (((1 + nw) * 8 + 15) & ~15);
   const uint32_t node_bytes = MULTI ? static_cast<uint32_t>(a.nodes) * 1024u : 0u;
   const uint32_t tile_bytes = 32u * (a.row_o + (STREAM ? 0 : a.row_p)) + node_bytes;
@@ -104,7 +107,7 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
   if constexpr (!TABG) {
     if (threadIdx.x == 0) {
       // stage the runtime table: TMA bulk copies of <= 32 KB each, one mbarrier phase
-      mbar_arrive_expect_tx(bar_tab, tab_bytes + w_bytes + d_bytes + r_bytes);
+      mbar_arrive_expect_tx(bar_tab, tab_bytes + w_bytes + d_bytes + r_bytes + p_bytes);
       const uint8_t* src = reinterpret_cast<const uint8_t*>(a.tab);
       for (uint32_t off = 0; off < tab_bytes; off += 32768u) {
         uint32_t n = min(32768u, tab_bytes - off);
@@ -113,6 +116,7 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
       if constexpr (kW) stage_job_array(smem + tab_bytes, a.w, w_bytes, bar_tab);
       if constexpr (kD) stage_job_array(smem + tab_bytes + w_bytes, a.d, d_bytes, bar_tab);
       if constexpr (R) stage_job_array(smem + tab_bytes + w_bytes + d_bytes, a.r, r_bytes, bar_tab);
+      if constexpr (kP) stage_job_array(smem + tab_bytes + w_bytes + d_bytes + r_bytes, a.p, p_bytes, bar_tab);
     }
   }
 
@@ -130,6 +134,10 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
   if constexpr (R) {
     st.rr = TABG ? a.r : r_s;
     st.rr_s = smem_u32(r_s);
+  }
+  if constexpr (kP) {
+    st.pp = TABG ? a.p : p_s;
+    st.pp_s = smem_u32(p_s);
   }
   st.SG = a.SG;
   st.one = a.one;
@@ -288,6 +296,7 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
         [[maybe_unused]] float wb[kBatch];  // kW: the batch's weights, gathered with its runtimes
         [[maybe_unused]] float db[kBatch];  // kD: the batch's due dates (or tails), likewise
         [[maybe_unused]] float xb[kBatch];  // R: the batch's release dates, likewise
+        [[maybe_unused]] float pb[kBatch];  // kP: the batch's late penalties, likewise
         auto resolve = [&](const uint32_t* w) {  // w: the kBatch / 4 words that hold the batch's job ids
           int js[kBatch];
 #pragma unroll
@@ -307,6 +316,10 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
           if constexpr (R) {
 #pragma unroll
             for (int i = 0; i < kBatch; ++i) xb[i] = st.gather_r(js[i]);
+          }
+          if constexpr (kP) {
+#pragma unroll
+            for (int i = 0; i < kBatch; ++i) pb[i] = st.gather_p(js[i]);
           }
         };
         if (nfull > 0) resolve(q.w);
@@ -329,6 +342,7 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
             [[maybe_unused]] float wc[kBatch];
             [[maybe_unused]] float dc[kBatch];
             [[maybe_unused]] float xc[kBatch];
+            [[maybe_unused]] float pc[kBatch];
 #pragma unroll
             for (int i = 0; i < kBatch; ++i) { oc[i] = ob[i]; rc[i] = rb[i]; }
             if constexpr (kW) {
@@ -343,11 +357,15 @@ __global__ void __launch_bounds__(STREAM ? 512 : 384, 1) k_eval_tiles(const Tile
 #pragma unroll
               for (int i = 0; i < kBatch; ++i) xc[i] = xb[i];
             }
+            if constexpr (kP) {
+#pragma unroll
+              for (int i = 0; i < kBatch; ++i) pc[i] = pb[i];
+            }
             resolve(b + 1 < STEPS / kBatch ? q.w + (b + 1) * (kBatch / 4) : head);
 #pragma unroll
             for (int i = 0; i < kBatch; ++i)
               st.step_resolved(static_cast<int>(oc[i]), rc[i], i & 1, kW ? wc[i] : 0.f, kD ? dc[i] : 0.f,
-                               R ? xc[i] : 0.f);
+                               R ? xc[i] : 0.f, kP ? pc[i] : 0.f);
           }
           q = nxt;
         }
@@ -654,6 +672,7 @@ struct GenericArgs {
   const float* w;  // obj_weights(OBJ): job weights [J], read with ld.global.nc
   const float* d;  // obj_due(OBJ): job due dates (or tails) [J], likewise
   const float* r;  // R: job release dates [J], likewise
+  const float* p;  // obj_penalty(OBJ): job late penalties [J], likewise
 };
 
 template <int PB, bool INT, bool MULTI, Obj OBJ = Obj::Makespan, bool R = false>
@@ -675,6 +694,7 @@ __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
   st.wt = a.w;
   st.dd = a.d;
   st.rr = a.r;
+  st.pp = a.p;
   st.SG = a.SG;
   st.one = a.one;
   st.ns = node_s + lane;
@@ -700,8 +720,8 @@ __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
         for (int t = 0; t < BATCH; ++t) os[t] = st.lookup_opt(js[t]);
 #pragma unroll
         for (int t = 0; t < BATCH; ++t) rts[t] = st.lookup_rt(js[t], os[t]);
-        // the batch's release dates, weights and due dates (or tails), gathered with its runtimes
-        [[maybe_unused]] float xs[BATCH], ws[BATCH], ds[BATCH];
+        // the batch's release dates, weights, due dates (or tails) and late penalties, gathered with its runtimes
+        [[maybe_unused]] float xs[BATCH], ws[BATCH], ds[BATCH], ps[BATCH];
         if constexpr (R) {
 #pragma unroll
           for (int t = 0; t < BATCH; ++t) xs[t] = st.lookup_r(js[t]);
@@ -714,10 +734,14 @@ __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
 #pragma unroll
           for (int t = 0; t < BATCH; ++t) ds[t] = st.lookup_d(js[t]);
         }
+        if constexpr (obj_penalty(OBJ)) {
+#pragma unroll
+          for (int t = 0; t < BATCH; ++t) ps[t] = st.lookup_p(js[t]);
+        }
 #pragma unroll
         for (int t = 0; t < BATCH; ++t)
           st.step_resolved(os[t], rts[t], t & 1, obj_weights(OBJ) ? ws[t] : 0.f, obj_due(OBJ) ? ds[t] : 0.f,
-                           R ? xs[t] : 0.f);
+                           R ? xs[t] : 0.f, obj_penalty(OBJ) ? ps[t] : 0.f);
       }
       for (; i < a.J; ++i) st.step(PB == 1 ? prow[i] : reinterpret_cast<const uint16_t*>(prow)[i]);
       mk = st.result(a.nodes);
@@ -747,6 +771,7 @@ struct FullArgs {
   const float* w;       // obj_weights(OBJ): job weights [J]
   const float* d;       // obj_due(OBJ): job due dates [J] (TailMakespan: the delivery tails)
   const float* r;       // R: job release dates [J] (ceiled with INT)
+  const float* p;       // obj_penalty(OBJ): job late penalties [J]
 };
 
 // The score is folded here on its own, not through ls_step: this kernel is the library's slot-exact cross-check of
@@ -799,6 +824,10 @@ __global__ void __launch_bounds__(128) k_eval_full(const FullArgs a) {
       else if constexpr (OBJ == Obj::SquaredTardiness) {
         const float t = fmaxf(__fsub_rn(s + rt, __ldg(a.d + j)), 0.f);
         mk = __fadd_rn(mk, __fmul_rn(__ldg(a.w + j), __fmul_rn(t, t)));
+      }
+      else if constexpr (OBJ == Obj::LatePenalty) {
+        const float x = __fsub_rn(s + rt, __ldg(a.d + j));
+        mk = __fadd_rn(mk, x > 0.f ? __fadd_rn(__ldg(a.p + j), __fmul_rn(__ldg(a.w + j), x)) : 0.f);
       }
       else if constexpr (OBJ == Obj::WeightedSum) mk = __fadd_rn(mk, __fmul_rn(__ldg(a.w + j), s + rt));
       else if constexpr (OBJ == Obj::Sum) mk = mk + (s + rt);  // the left fold in schedule order
@@ -893,6 +922,7 @@ static TileArgs tile_args(const EvalCall& c, const TilePlan& tp) {
   a.w = c.w;
   a.d = c.d;
   a.r = c.r;
+  a.p = c.p;
   a.ntiles = (c.B + 31) / 32;
   a.one = 1;
   a.packed = a.stagger = 0;
@@ -961,6 +991,7 @@ cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, i
   g.tab = c.tab; g.J = c.J; g.SG = c.SG; g.opt = c.opt; g.prio = c.prio; g.B = c.B;
   g.stride_o = c.stride_o; g.stride_p = c.stride_p; g.out = c.out; g.best_key = c.best_key;
   g.id_base = c.id_base; g.tab_in_smem = 0; g.nodes = c.nodes; g.one = 1; g.w = c.w; g.d = c.d; g.r = c.r;
+  g.p = c.p;
   if (path_used) *path_used = 0;
   const size_t tab_bytes = static_cast<size_t>(c.J) * c.SG * 4;
   size_t smem = multi ? static_cast<size_t>(4) * c.nodes * 1024u : 0u;  // 4 warps per CTA
@@ -1016,6 +1047,7 @@ cudaError_t eval_full_launch(const Device& dev, const EvalCall& c, float* start,
   a.tab = c.tab; a.J = c.J; a.SG = c.SG; a.opt = c.opt; a.prio = c.prio; a.B = c.B;
   a.stride_o = c.stride_o; a.stride_p = c.stride_p; a.nodes = c.nodes < 1 ? 1 : c.nodes;
   a.out = c.out; a.start = start; a.slotmask = slotmask; a.w = c.w; a.d = c.d; a.r = c.r;
+  a.p = c.p;
   long long blocks = (c.B + 127) / 128;
   long long cap = static_cast<long long>(dev.sm_count) * 16;
   int grid = static_cast<int>(blocks < cap ? blocks : cap);

@@ -33,7 +33,7 @@ static_assert(((HOOK_FORCE_GENERIC | HOOK_NO_STREAM | HOOK_NO_FUSED | HOOK_NO_IN
                (SB_FLAG_INTEGER_STARTS | SB_FLAG_REDUCED | SB_FLAG_OPT_BY_POSITION | SB_FLAG_POST_KEY |
                 SB_FLAG_FOLD_PREV | SB_FLAG_ALT_WARPSCAN | SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED |
                 SB_FLAG_DUE | SB_FLAG_RELEASE | SB_FLAG_MAX_LATENESS | SB_FLAG_LATE_COUNT |
-                SB_FLAG_MAX_TARDINESS | SB_FLAG_SQUARED)) == 0,
+                SB_FLAG_MAX_TARDINESS | SB_FLAG_SQUARED | SB_FLAG_LATE_PENALTY)) == 0,
               "the test hooks share no bit with the SB_FLAG_* flags");
 
 // Debug options of the streamed tile kernel (sb_debug_tile_options): kept on the handle, not in the flags word, and
@@ -66,6 +66,7 @@ decltype(auto) with_obj(Obj obj, F&& f) {
     case Obj::LateCount: return f(obj_c<Obj::LateCount>{});
     case Obj::MaxTardiness: return f(obj_c<Obj::MaxTardiness>{});
     case Obj::SquaredTardiness: return f(obj_c<Obj::SquaredTardiness>{});
+    case Obj::LatePenalty: return f(obj_c<Obj::LatePenalty>{});
     default: return f(obj_c<Obj::Makespan>{});
   }
 }
@@ -82,10 +83,11 @@ decltype(auto) with_eval_types(int pb, unsigned flags, Obj obj, F&& f) {
   });
 }
 // the per-job fp32 arrays a kernel stages beside the table: the weights, then the due dates (or tails), then the
-// release dates (SB_FLAG_RELEASE), each where the objective reads it (stage_job_array, sb_lane.cuh); each is padded to 16
-// bytes
+// release dates (SB_FLAG_RELEASE), then the late penalties, each where the objective reads it (stage_job_array,
+// sb_lane.cuh); each is padded to 16 bytes
 inline int job_arrays(Obj obj, unsigned flags) {
-  return (obj_weights(obj) ? 1 : 0) + (obj_due(obj) ? 1 : 0) + ((flags & SB_FLAG_RELEASE) ? 1 : 0);
+  return (obj_weights(obj) ? 1 : 0) + (obj_due(obj) ? 1 : 0) + ((flags & SB_FLAG_RELEASE) ? 1 : 0) +
+         (obj_penalty(obj) ? 1 : 0);
 }
 inline size_t job_array_bytes(int J) { return (static_cast<size_t>(J) * 4 + 15) & ~size_t(15); }
 
@@ -141,6 +143,7 @@ struct EvalCall {
                                // padded the same way
   const float* r = nullptr;    // SB_FLAG_RELEASE: the job release dates [J] (ceiled under SB_FLAG_INTEGER_STARTS),
                                // padded the same way
+  const float* p = nullptr;    // obj_penalty(obj): the job late penalties [J], padded the same way
   int J = 0, SG = 0;
   const uint8_t* opt = nullptr;
   const uint8_t* prio = nullptr;

@@ -32,9 +32,9 @@ __device__ __forceinline__ PrioChunk ld_prio32(const uint8_t* p) {
 }
 
 // The per-job fp32 arrays a kernel stages beside its table, in this order: the weights (obj_weights), the due dates or
-// tails (obj_due), the release dates (SB_FLAG_RELEASE).  Each is padded to 16 bytes (each kernel spells the padding
-// out per array: computing it once changes the generated code) and is fetched by stage_job_array with TMA bulk
-// copies in the table's mbarrier phase.
+// tails (obj_due), the release dates (SB_FLAG_RELEASE), the late penalties (obj_penalty).  Each is padded to 16 bytes
+// (each kernel spells the padding out per array: computing it once changes the generated code) and is fetched by
+// stage_job_array with TMA bulk copies in the table's mbarrier phase.
 __device__ __forceinline__ void stage_job_array(uint8_t* dst, const float* src, uint32_t bytes, uint64_t* bar) {
   const uint8_t* s = reinterpret_cast<const uint8_t*>(src);
   for (uint32_t off = 0; off < bytes; off += 32768u) tma_bulk_g2s(dst + off, s + off, min(32768u, bytes - off), bar);
@@ -50,7 +50,7 @@ __device__ __forceinline__ void stage_job_array(uint8_t* dst, const float* src, 
 // beside the table, 2: in global memory, read with ld.global.nc.
 template <bool INT, bool MULTI, int ADDR = 0, Obj OBJ = Obj::Makespan, int HOME = 0, bool REL = false>
 struct LaneState {
-  static constexpr bool kW = obj_weights(OBJ), kD = obj_due(OBJ);
+  static constexpr bool kW = obj_weights(OBJ), kD = obj_due(OBJ), kP = obj_penalty(OBJ);
   float f[8];
   float mk;
   float pend;  // a completion time parked by an even step (see ls_step; the makespan forms only)
@@ -59,10 +59,11 @@ struct LaneState {
   const float* wt;      // kW: the job weights [J]
   const float* dd;      // kD: the job due dates [J] (or delivery tails)
   const float* rr;      // REL: the job release dates [J]
+  const float* pp;      // kP: the job late penalties [J]
   int SG;
   int one;
   uint32_t orow_s, tab_s, four;  // ADDR = 1: shared-window addresses of orow / tab, and a run-time 4
-  uint32_t wt_s, dd_s, rr_s;     // ADDR = 1: shared-window addresses of wt / dd / rr
+  uint32_t wt_s, dd_s, rr_s, pp_s;  // ADDR = 1: shared-window addresses of wt / dd / rr / pp
   float4* ns;  // MULTI: lane-private node-state column; node n lives at ns[(2n)*32], ns[(2n+1)*32]
   int cur;     // MULTI: the node whose state is currently in f[] (its shared-memory copy is stale)
 
@@ -99,19 +100,20 @@ struct LaneState {
   }
   // the job's entry of a per-job array: shared memory (HOME = 1) or global memory (HOME = 2)
   __device__ __forceinline__ float job_at(const float* a, int j) const { return HOME == 1 ? a[j] : __ldg(a + j); }
-  // the job's weight, due date (or tail) and release date; 0 where the kernel reads none
+  // the job's weight, due date (or tail), release date and late penalty; 0 where the kernel reads none
   __device__ __forceinline__ float lookup_w(int j) const { if constexpr (kW) return job_at(wt, j); else return 0.f; }
   __device__ __forceinline__ float lookup_d(int j) const { if constexpr (kD) return job_at(dd, j); else return 0.f; }
   __device__ __forceinline__ float lookup_r(int j) const { if constexpr (REL) return job_at(rr, j); else return 0.f; }
-  // ph: t & 1 inside fully unrolled loops, -1 elsewhere (see ls_step); w, d, r: the job's weight, due date (or tail)
-  // and release date, each read only where the objective (or REL) uses it
+  __device__ __forceinline__ float lookup_p(int j) const { if constexpr (kP) return job_at(pp, j); else return 0.f; }
+  // ph: t & 1 inside fully unrolled loops, -1 elsewhere (see ls_step); w, d, r, p: the job's weight, due date (or
+  // tail), release date and late penalty, each read only where the objective (or REL) uses it
   __device__ __forceinline__ void step_resolved(int o, float rt, int ph = -1, float w = 0.f, float d = 0.f,
-                                                float r = 0.f) {
+                                                float r = 0.f, float p = 0.f) {
     if (!MULTI) {
-      ls_step<INT, INT, OBJ, REL>(f, mk, pend, rt, o & 7, one, ph, w, d, r);
+      ls_step<INT, INT, OBJ, REL>(f, mk, pend, rt, o & 7, one, ph, w, d, r, p);
     } else {
       switch_node(o >> 3);
-      ls_step<INT, true, OBJ, REL>(f, mk, pend, rt, o & 7, one, ph, w, d, r);
+      ls_step<INT, true, OBJ, REL>(f, mk, pend, rt, o & 7, one, ph, w, d, r, p);
     }
   }
   // ADDR = 1: the two look-ups as separate gathers, so that the streamed loop of k_eval_tiles can issue a whole
@@ -142,22 +144,25 @@ struct LaneState {
   __device__ __forceinline__ float gather_w(int j) const { if constexpr (kW) return gather_at(wt_s, j); else return 0.f; }
   __device__ __forceinline__ float gather_d(int j) const { if constexpr (kD) return gather_at(dd_s, j); else return 0.f; }
   __device__ __forceinline__ float gather_r(int j) const { if constexpr (REL) return gather_at(rr_s, j); else return 0.f; }
+  __device__ __forceinline__ float gather_p(int j) const { if constexpr (kP) return gather_at(pp_s, j); else return 0.f; }
   __device__ __forceinline__ void step(int j, int ph = -1) {
     if (!MULTI && ADDR == 1) {
       const uint32_t o = gather_opt(j);
       ls_step<INT, INT, OBJ, REL>(f, mk, pend, gather_rt(j, o), static_cast<int>(o & 7u), one, ph, gather_w(j),
-                                  gather_d(j), gather_r(j));
+                                  gather_d(j), gather_r(j), gather_p(j));
       return;
     }
     const int o = orow[j];
     if (!MULTI) {
       const float rt = tab[j * SG + o];
-      ls_step<INT, INT, OBJ, REL>(f, mk, pend, rt, o & 7, one, ph, lookup_w(j), lookup_d(j), lookup_r(j));
+      ls_step<INT, INT, OBJ, REL>(f, mk, pend, rt, o & 7, one, ph, lookup_w(j), lookup_d(j), lookup_r(j),
+                                  lookup_p(j));
     } else {
       const int col = o & 7;  // reduced table only: opt = (node << 3) | (k - 1)
       const float rt = tab[j * 8 + col];
       switch_node(o >> 3);
-      ls_step<INT, true, OBJ, REL>(f, mk, pend, rt, col, one, ph, lookup_w(j), lookup_d(j), lookup_r(j));
+      ls_step<INT, true, OBJ, REL>(f, mk, pend, rt, col, one, ph, lookup_w(j), lookup_d(j), lookup_r(j),
+                                   lookup_p(j));
     }
   }
   // the tail makespan is tracked in mk at every shape: f[7] is a completion, not a tail sum.

@@ -331,6 +331,7 @@ struct PosArgs {
   const float* w;  // obj_weights(OBJ): job weights [J], zero-padded to a multiple of 4 (16 bytes)
   const float* d;  // obj_due(OBJ): job due dates (or tails) [J], padded the same way
   const float* r;  // R: job release dates [J], padded the same way
+  const float* p;  // obj_penalty(OBJ): job late penalties [J], padded the same way
 };
 
 struct PosMove {
@@ -438,15 +439,18 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
   const uint32_t tab_off = TAB == 2 ? rank * half * 4u : 0u;
   const uint32_t tab_bytes = TAB == 1 ? 0u : (TAB == 2 ? (rank == 0 ? half * 4u : tab_all - half * 4u) : tab_all);
   const uint32_t tab_room = TAB == 1 ? 0u : (TAB == 2 ? half * 4u : tab_all);
-  constexpr bool kW = obj_weights(OBJ), kD = obj_due(OBJ);
+  constexpr bool kW = obj_weights(OBJ), kD = obj_due(OBJ), kP = obj_penalty(OBJ);
   const uint32_t w_bytes = (kW && TAB == 0) ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u;
   const uint32_t d_bytes = kD ? (kW ? w_bytes : (TAB == 0 ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u)) : 0u;
   const uint32_t r_bytes = (R && TAB == 0) ? ((static_cast<uint32_t>(a.J) * 4u + 15u) & ~15u) : 0u;
+  const uint32_t p_bytes = kP ? w_bytes : 0u;  // the penalties come with the weights (obj_weights)
   float* tab_s = reinterpret_cast<float*>(smem);
   [[maybe_unused]] float* w_s = reinterpret_cast<float*>(smem + ((tab_room + 15u) & ~15u));
   [[maybe_unused]] float* d_s = reinterpret_cast<float*>(smem + ((tab_room + 15u) & ~15u) + w_bytes);
   [[maybe_unused]] float* r_s = reinterpret_cast<float*>(smem + ((tab_room + 15u) & ~15u) + w_bytes + d_bytes);
-  uint64_t* bar_tab = reinterpret_cast<uint64_t*>(smem + ((tab_room + 15u) & ~15u) + w_bytes + d_bytes + r_bytes);
+  [[maybe_unused]] float* p_s = reinterpret_cast<float*>(smem + ((tab_room + 15u) & ~15u) + w_bytes + d_bytes + r_bytes);
+  uint64_t* bar_tab =
+      reinterpret_cast<uint64_t*>(smem + ((tab_room + 15u) & ~15u) + w_bytes + d_bytes + r_bytes + p_bytes);
   const uint32_t node_bytes = MULTI ? static_cast<uint32_t>(a.nodes) * 1024u : 0u;
   float4* node_s = reinterpret_cast<float4*>(reinterpret_cast<uint8_t*>(bar_tab) + 16 + static_cast<size_t>(warp) * node_bytes);
   if (threadIdx.x == 0) {
@@ -456,12 +460,13 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
   __syncthreads();
   if constexpr (TAB != 1) {
     if (threadIdx.x == 0) {
-      mbar_arrive_expect_tx(bar_tab, tab_bytes + w_bytes + d_bytes + r_bytes);
+      mbar_arrive_expect_tx(bar_tab, tab_bytes + w_bytes + d_bytes + r_bytes + p_bytes);
       const uint8_t* src = reinterpret_cast<const uint8_t*>(a.tab) + tab_off;
       for (uint32_t off = 0; off < tab_bytes; off += 32768u) tma_bulk_g2s(smem + off, src + off, min(32768u, tab_bytes - off), bar_tab);
       if constexpr (kW && TAB == 0) stage_job_array(reinterpret_cast<uint8_t*>(w_s), a.w, w_bytes, bar_tab);
       if constexpr (kD && TAB == 0) stage_job_array(reinterpret_cast<uint8_t*>(d_s), a.d, d_bytes, bar_tab);
       if constexpr (R && TAB == 0) stage_job_array(reinterpret_cast<uint8_t*>(r_s), a.r, r_bytes, bar_tab);
+      if constexpr (kP && TAB == 0) stage_job_array(reinterpret_cast<uint8_t*>(p_s), a.p, p_bytes, bar_tab);
     }
   }
   LaneState<INT, MULTI, 0, OBJ, TAB == 0 ? 1 : 2, R> st;
@@ -469,6 +474,7 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
   if constexpr (kW) st.wt = TAB == 0 ? w_s : a.w;
   if constexpr (kD) st.dd = TAB == 0 ? d_s : a.d;
   if constexpr (R) st.rr = TAB == 0 ? r_s : a.r;
+  if constexpr (kP) st.pp = TAB == 0 ? p_s : a.p;
   st.SG = a.SG;
   st.one = a.one;
   st.orow = nullptr;
@@ -562,7 +568,7 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
           for (int t = 0; t < 32; ++t) {
             const int j = prio_at<PB>(qp[(t * PB) / 32].w, t % (32 / PB));
             const int o = prio_at<1>(qo.w, t);
-            st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j), st.lookup_d(j), st.lookup_r(j));
+            st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j), st.lookup_d(j), st.lookup_r(j), st.lookup_p(j));
           }
         } else {
 #pragma unroll
@@ -570,7 +576,8 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
             if (base + t < J) {
               const int j = prio_at<PB>(qp[(t * PB) / 32].w, t % (32 / PB));
               const int o = prio_at<1>(qo.w, t);
-              st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j), st.lookup_d(j), st.lookup_r(j));
+              st.step_resolved(o, lookup(j, o), t & 1, st.lookup_w(j), st.lookup_d(j), st.lookup_r(j),
+                               st.lookup_p(j));
             }
           }
         }
@@ -752,7 +759,7 @@ cudaError_t search_init_population_pos(const SearchDev& s, cudaStream_t st) {
   return launch(with_pb(s.pb, [](auto PB) { return k_init_population_pos<PB>; }), grid, threads, 0, st, s);
 }
 
-// smem: table (+ weights, + due dates, + release dates) + mbarrier + per-warp node states (MULTI)
+// smem: table (+ weights, + due dates, + release dates, + late penalties) + mbarrier + per-warp node states (MULTI)
 size_t search_pos_smem(int J, int SG, int nodes, int warps, int arrays) {
   const size_t tab_bytes = (static_cast<size_t>(J) * SG * 4 + 15) & ~size_t(15);
   return tab_bytes + arrays * job_array_bytes(J) + 16 + static_cast<size_t>(warps) * (nodes > 1 ? nodes * 1024u : 0u);
@@ -803,8 +810,8 @@ static cudaError_t eval_pos_far_launch(const Device& dev, const PosArgs& a, int 
 // tab_home: 0 = the table in every CTA's shared memory (cudaErrorNotSupported when it does not fit);
 // scoring only, one node: 2 = split over CTA pairs, 1 = global memory
 cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float* tab, const float* w, const float* d,
-                              const float* r, int SG, unsigned flags, Obj obj, long long first, long long count, bool eval_only,
-                              const SearchFuse& sf, cudaStream_t st, int tab_home) {
+                              const float* r, const float* p, int SG, unsigned flags, Obj obj, long long first,
+                              long long count, bool eval_only, const SearchFuse& sf, cudaStream_t st, int tab_home) {
   if (count <= 0) return cudaSuccess;
   PosArgs a;
   a.tab = tab; a.J = s.J; a.SG = SG; a.nodes = s.nodes;
@@ -819,6 +826,7 @@ cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float
   a.w = w;
   a.d = d;
   a.r = r;
+  a.p = p;
   const bool multi = s.nodes > 1;
   if (tab_home != 0) {
     if (!eval_only || multi) return cudaErrorNotSupported;
@@ -870,7 +878,7 @@ cudaError_t eval_pos_launch(const Device& dev, const EvalCall& c, cudaStream_t s
   s.keys = c.best_key;
   SearchFuse sf = {};
   sf.cur_mk = c.out;
-  return search_pos_launch(dev, s, c.tab, c.w, c.d, c.r, c.SG, c.flags, c.obj, 0, c.B, true, sf, st, home);
+  return search_pos_launch(dev, s, c.tab, c.w, c.d, c.r, c.p, c.SG, c.flags, c.obj, 0, c.B, true, sf, st, home);
 }
 
 // Job-indexed opt rows -> schedule order (out[i] = opt[prio[i]]), one warp per candidate: the row is staged in

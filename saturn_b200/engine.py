@@ -28,7 +28,8 @@ class Objective(NamedTuple):
 # lateness scored as L_max + Engine.due_shift, "late_tasks" the number of tasks that complete after their due date,
 # "max_tardiness" the largest tardiness, "squared_tardiness" the sum of squared tardiness; each "weighted_" form weighs
 # the jobs by set_weights ("weighted_max_tardiness" with weights 1 / p* and due dates at the release dates is the
-# maximum stretch; "squared_tardiness" with due dates at the release dates the squared flow time).
+# maximum stretch; "squared_tardiness" with due dates at the release dates the squared flow time), "late_penalty" the
+# fixed penalty of set_penalty plus the (weighted) tardiness of every late task.
 _SUM, _W, _DUE = _lib.FLAG_SUM_COMPLETION, _lib.FLAG_WEIGHTED, _lib.FLAG_DUE
 _OBJECTIVES = {
     "makespan": Objective(0, False, False),
@@ -43,12 +44,17 @@ _OBJECTIVES = {
     "weighted_max_tardiness": Objective(_SUM | _DUE | _lib.FLAG_MAX_TARDINESS | _W, True, True),
     "squared_tardiness": Objective(_SUM | _DUE | _lib.FLAG_SQUARED, False, True),
     "weighted_squared_tardiness": Objective(_SUM | _DUE | _lib.FLAG_SQUARED | _W, True, True),
+    "late_penalty": Objective(_SUM | _DUE | _lib.FLAG_LATE_PENALTY, False, True),
+    "weighted_late_penalty": Objective(_SUM | _DUE | _lib.FLAG_LATE_PENALTY | _W, True, True),
 }
 # The squared forms, which the exact reference (oracle/ref_exact.py) and the cross-cutting sweeps of the test suite
 # do not fold yet; they are held to their own oracle, oracle/ref_squared_tardiness.py.
 SQUARED_OBJECTIVES = ("squared_tardiness", "weighted_squared_tardiness")
-# The objectives every cross-cutting check of the test suite covers: all of them but the squared forms.
-OBJECTIVES = tuple(o for o in _OBJECTIVES if o not in SQUARED_OBJECTIVES)
+# The late-penalty forms, which also read the penalties of set_penalty (objective_reads_penalty); like the squared
+# forms they are held to their own oracle, oracle/ref_late_penalty.py, until the cross-cutting sweeps fold them.
+PENALTY_OBJECTIVES = ("late_penalty", "weighted_late_penalty")
+# The objectives every cross-cutting check of the test suite covers: all of them but the squared and late-penalty forms.
+OBJECTIVES = tuple(o for o in _OBJECTIVES if o not in SQUARED_OBJECTIVES + PENALTY_OBJECTIVES)
 
 
 def objective_spec(objective: str) -> Objective:
@@ -62,6 +68,11 @@ def objective_spec(objective: str) -> Objective:
 def objective_flag(objective: str) -> int:
     """The SB_FLAG_* bits of an objective name (see _OBJECTIVES)."""
     return objective_spec(objective).flags
+
+
+def objective_reads_penalty(objective: str) -> bool:
+    """Whether an objective scores with the late penalties of set_penalty (SB_FLAG_LATE_PENALTY)."""
+    return bool(objective_spec(objective).flags & _lib.FLAG_LATE_PENALTY)
 
 
 def weights_f32(w, J: int) -> np.ndarray:
@@ -96,6 +107,27 @@ def due_f32(d, J: int) -> np.ndarray:
     if not (np.isfinite(d64).all() and (np.abs(d64) < 2.0 ** 24).all()):
         raise SolverError("every due date must be finite with |d| < 2^24")
     return d64.astype(np.float32)
+
+
+def penalty_f32(p, J: int) -> np.ndarray:
+    """J late penalties as fp32 (round to nearest: integers below 2^24 are exact), -0 as +0.  Every penalty must be
+    finite and >= 0, and J * max p < 2^126 once in fp32 (the fp32 sum of the penalties stays finite); raises
+    SolverError otherwise."""
+    from .solver import SolverError
+    try:
+        p64 = np.asarray(p, dtype=np.float64)
+    except (TypeError, ValueError) as e:
+        raise SolverError("penalties must be numbers: %s" % e)
+    if p64.shape != (J,):
+        raise SolverError("penalties must have one value per task (%d), got shape %s" % (J, p64.shape))
+    if not (np.isfinite(p64).all() and (p64 >= 0).all()):
+        raise SolverError("every penalty must be finite and >= 0")
+    with np.errstate(over="ignore"):
+        p32 = p64.astype(np.float32) + np.float32(0)
+    if not (np.isfinite(p32).all() and J * float(p32.max(initial=0.0)) < 2.0 ** 126):
+        raise SolverError("penalties must keep J * max(penalty) below 2^126 in fp32 (%d tasks, largest penalty %g): "
+                          "beyond it the fp32 sum can overflow" % (J, float(p64.max(initial=0.0))))
+    return p32
 
 
 def release_f32(r, J: int) -> np.ndarray:
@@ -133,6 +165,14 @@ def _require_due(due, objective: str):
         raise SolverError("objective=%r needs due dates: call set_due after set_table" % (objective,))
 
 
+def _require_penalty(penalty, objective: str):
+    """The late-penalty objectives score with the penalties of set_penalty: refuse them, before any device call, on
+    an engine that has none (set_table clears them)."""
+    if objective in _OBJECTIVES and objective_reads_penalty(objective) and penalty is None:
+        from .solver import SolverError
+        raise SolverError("objective=%r needs late penalties: call set_penalty after set_table" % (objective,))
+
+
 class Engine:
     """One solver handle bound to one CUDA device."""
 
@@ -157,6 +197,7 @@ class Engine:
         self.gcount = None
         self.nodes = 1
         self.weights = None  # fp32 job weights of objective="weighted_completion" (set_weights)
+        self.penalty = None  # fp32 job late penalties of the late-penalty objectives (set_penalty)
         self.due = None  # fp32 job due dates of the tardiness, late-count and max-lateness objectives (set_due)
         self.due_shift = None  # max of self.due: objective="max_lateness" scores L_max + due_shift (>= 0)
         self.release = None  # fp32 job release dates, under every objective (set_release)
@@ -207,6 +248,7 @@ class Engine:
         self.due = None
         self.due_shift = None
         self.release = None
+        self.penalty = None
         return self
 
     def set_weights(self, w) -> "Engine":
@@ -255,11 +297,26 @@ class Engine:
         self.release = r32
         return self
 
+    def set_penalty(self, p) -> "Engine":
+        """Per-job late penalties (J values, finite and >= 0, converted to fp32) for objective="late_penalty", which
+        scores sum_j [C_j > d_j] (p_j + (C_j - d_j)) with C_j = start_j + rt_j against the due dates of set_due, and
+        "weighted_late_penalty", which multiplies each tardiness by the set_weights weight.  None clears them;
+        set_table clears them too."""
+        if p is None:
+            check(self._lib.sb_set_penalty(self._h, None, 0))
+            self.penalty = None
+            return self
+        p32 = np.ascontiguousarray(penalty_f32(p, self.J))
+        check(self._lib.sb_set_penalty(self._h, C.c_void_p(p32.ctypes.data), int(self.J)))
+        self.penalty = p32
+        return self
+
     def _release_flag(self) -> int:
         return _lib.FLAG_RELEASE if self.release is not None else 0
 
     def _flags(self, integer_starts: bool, reduced: bool, objective: str) -> int:
         _require_due(self.due, objective)
+        _require_penalty(self.penalty, objective)
         return _flags(integer_starts, reduced, objective) | self._release_flag()
 
     def reduced_table(self) -> Tuple[np.ndarray, np.ndarray]:
@@ -468,6 +525,7 @@ class Engine:
         evaluated, rounds, stop_reason, wall_s, history [(wall s, evaluated, makespan)].  With
         objective="completion" every "makespan" there is the sum of completion times, and target_makespan targets it."""
         _require_due(self.due, objective)
+        _require_penalty(self.penalty, objective)
         return _search_run(self._lib, [self._h], self.J, chains, rounds, seed, chain_base, integer_starts, reduced,
                            t_start, t_end, warm, resample_every, sync_every, patience, time_budget_s, target_makespan,
                            heuristic_seeds, record_history, _no_fused, int(_extra_flags) | self._release_flag(),
@@ -658,6 +716,14 @@ class MultiEngine:
 
     release = property(lambda self: self.engines[0].release)
 
+    def set_penalty(self, p):
+        """Engine.set_penalty on every device."""
+        for e in self.engines:
+            e.set_penalty(p)
+        return self
+
+    penalty = property(lambda self: self.engines[0].penalty)
+
     def decode(self, *a, **kw):
         return self.engines[0].decode(*a, **kw)
 
@@ -672,6 +738,7 @@ class MultiEngine:
                    _no_fused: bool = False, _extra_flags: int = 0, objective: str = "makespan"):
         """`chains` is per device; the result's `evaluated` counts every device."""
         _require_due(self.due, objective)
+        _require_penalty(self.penalty, objective)
         return _search_run(self._lib, [e._h for e in self.engines], self.J, chains, rounds, seed, chain_base,
                            integer_starts, reduced, t_start, t_end, warm, resample_every, sync_every, patience,
                            time_budget_s, target_makespan, heuristic_seeds, record_history, _no_fused,

@@ -54,7 +54,8 @@ def orchestrate(task_list, log=False, interval=1000, gurobi=True, *,
     batches_to_run, interval, node_per_task, task_dependency_dict)` stands in for
     saturn.executor.execute; returns the list of per-interval records (plan makespan, tasks run).
 
-    A `due` mapping Task -> due date in `solver_kwargs` (objective="tardiness", "max_lateness", "late_tasks" or "squared_tardiness") is
+    A `due` mapping Task -> due date in `solver_kwargs` (objective="tardiness", "max_lateness", "late_tasks",
+    "squared_tardiness" or "late_penalty") is
     measured from the first plan's t = 0: the solve for interval n plans from n * interval on, so it receives
     {t: d - n * interval}, and the lateness each solve reports is against the original due dates (both sides shift
     alike).  A sequence `due` raises SolverError, since the task list shrinks from interval to interval.  A `release`
@@ -65,7 +66,9 @@ def orchestrate(task_list, log=False, interval=1000, gurobi=True, *,
     shifted due dates leave every tardiness unchanged (C and d move alike).  Under objective="squared_flow" each solve
     measures flow from the shifted release dates, clamped at the interval's t = 0: a task released before the
     interval counts its flow from the interval's start, so each solve minimises the squares of the waits that
-    remain, not of the whole flow time.
+    remain, not of the whole flow time.  Under objective="late_penalty" a `penalty` mapping Task -> penalty is passed
+    to every solve unchanged: a penalty is what missing the due date costs, whenever the plan is made; a sequence
+    `penalty` raises SolverError, as a sequence `due` does.
     """
     logging.basicConfig(level=logging.INFO if log else logging.WARNING,
                         format="%(asctime)s %(levelname)-8s %(message)s", datefmt="%Y-%m-%d %H:%M:%S")
@@ -73,6 +76,9 @@ def orchestrate(task_list, log=False, interval=1000, gurobi=True, *,
     due = kw.pop("due", None)
     if due is not None and not isinstance(due, Mapping):
         raise SolverError("orchestrate() needs due as a mapping Task -> due date: its task list shrinks every interval")
+    if kw.get("penalty") is not None and not isinstance(kw["penalty"], Mapping):
+        raise SolverError("orchestrate() needs penalty as a mapping Task -> penalty: its task list shrinks every "
+                          "interval")
     release = kw.pop("release", None)
     if release is not None and not isinstance(release, Mapping):
         raise SolverError("orchestrate() needs release as a mapping Task -> release date: its task list shrinks "

@@ -63,8 +63,8 @@ def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objecti
     release date (ceiled when `integer_starts`, as the device schedules them), so jobs released together keep the
     objective's order.  objective="late_tasks" / "weighted_late_tasks": the EDD orders of "tardiness" /
     "weighted_tardiness", each repaired by Moore-Hodgson's rule after the node fill (moore_hodgson).
-    objective="max_tardiness" / "weighted_max_tardiness" and "squared_tardiness" / "weighted_squared_tardiness": the
-    EDD orders of "tardiness" / "weighted_tardiness" unchanged."""
+    objective="max_tardiness" / "weighted_max_tardiness", "squared_tardiness" / "weighted_squared_tardiness" and
+    "late_penalty" / "weighted_late_penalty": the EDD orders of "tardiness" / "weighted_tardiness" unchanged."""
     spec = objective_spec(objective)
     if spec.weighted:
         if weights is None:
@@ -187,7 +187,9 @@ def run_search(engine: Engine, chains: int = 1 << 16, rounds: int = 200, seed: i
     "weighted_late_tasks" minimises the (weighted) number of tasks that complete after their due date, and stops at
     0 like the tardiness.  objective="max_tardiness" / "weighted_max_tardiness" minimises the largest (weighted)
     tardiness, and stops at 0 like the tardiness.  objective="squared_tardiness" / "weighted_squared_tardiness"
-    minimises the (weighted) sum of squared tardiness, and stops at 0 like the tardiness.
+    minimises the (weighted) sum of squared tardiness, and stops at 0 like the tardiness.  objective="late_penalty" /
+    "weighted_late_penalty" minimises the engine's set_penalty penalty plus the (weighted) tardiness of every late
+    task, and stops at 0 like the tardiness.
 
     `rounds` device rounds are issued in groups of `exchange_every` (tournament resampling every
     `resample_every` rounds inside a group is only another launch); after each group the ranks exchange

@@ -228,9 +228,10 @@ def _check_horizon(T, found_makespan=None, release=None, tails=None):
 
 def _check_objective(objective, hysteresis=False, release=None):
     if objective not in ("makespan", "completion", "tardiness", "max_lateness", "late_tasks", "max_stretch",
-                         "squared_tardiness", "squared_flow"):
+                         "squared_tardiness", "squared_flow", "late_penalty"):
         raise SolverError("objective must be 'makespan', 'completion', 'tardiness', 'max_lateness', 'late_tasks', "
-                          "'max_stretch', 'squared_tardiness' or 'squared_flow', not %r" % (objective,))
+                          "'max_stretch', 'squared_tardiness', 'squared_flow' or 'late_penalty', not %r"
+                          % (objective,))
     if objective != "makespan" and hysteresis:
         raise SolverError("hysteresis=True compares plans by makespan (milp.py:363-442); it is not defined for "
                           "objective=%r" % (objective,))
@@ -263,9 +264,9 @@ def _resolve_weights(weights, objective, J, task_list=None):
     if objective == "max_stretch":
         raise SolverError("objective='max_stretch' weighs every task by 1 / its fastest runtime: it takes no weights "
                           "(for a weighted mean stretch use objective='completion' with weights)")
-    if objective not in ("completion", "tardiness", "late_tasks", "squared_tardiness", "squared_flow"):
-        raise SolverError("weights apply to objective='completion', 'tardiness', 'late_tasks', 'squared_tardiness' or "
-                          "'squared_flow' only, not to %r" % (objective,))
+    if objective not in ("completion", "tardiness", "late_tasks", "squared_tardiness", "squared_flow", "late_penalty"):
+        raise SolverError("weights apply to objective='completion', 'tardiness', 'late_tasks', 'squared_tardiness', "
+                          "'squared_flow' or 'late_penalty' only, not to %r" % (objective,))
     weights = _per_task(weights, "weights", task_list)
     from .engine import weights_f32
     w32 = weights_f32(weights, J)
@@ -280,15 +281,15 @@ def _resolve_weights(weights, objective, J, task_list=None):
 
 def _resolve_due(due, objective, J, task_list=None):
     """The caller's per-task due dates as (float64 values in task order, fp32 array for the device), or (None, None)
-    without objective="tardiness", "max_lateness", "late_tasks" or "squared_tardiness", which require them.  Raises
-    SolverError before any device call."""
+    without objective="tardiness", "max_lateness", "late_tasks", "squared_tardiness" or "late_penalty", which require
+    them.  Raises SolverError before any device call."""
     if objective in ("max_stretch", "squared_flow") and due is not None:
         raise SolverError("objective=%r measures every task from its release date: it takes no due dates "
                           "(pass release=...)" % (objective,))
-    if objective not in ("tardiness", "max_lateness", "late_tasks", "squared_tardiness"):
+    if objective not in ("tardiness", "max_lateness", "late_tasks", "squared_tardiness", "late_penalty"):
         if due is not None:
-            raise SolverError("due dates apply to objective='tardiness', 'max_lateness', 'late_tasks' or "
-                              "'squared_tardiness' only, not to %r" % (objective,))
+            raise SolverError("due dates apply to objective='tardiness', 'max_lateness', 'late_tasks', "
+                              "'squared_tardiness' or 'late_penalty' only, not to %r" % (objective,))
         return None, None
     if due is None:
         raise SolverError("objective=%r needs due dates (due=...)" % (objective,))
@@ -299,6 +300,21 @@ def _resolve_due(due, objective, J, task_list=None):
         # the device scores the tails max d - d_t in fp32: beyond 2^24 they round even for integer due dates
         raise SolverError("objective='max_lateness' needs max(due) - min(due) < 2^24")
     return [float(x) for x in due], d32
+
+
+def _resolve_penalty(penalty, objective, J, task_list=None):
+    """The caller's per-task late penalties as (float64 values in task order, fp32 array for the device), or
+    (None, None) without objective="late_penalty", which requires them.  Raises SolverError before any device call."""
+    if objective != "late_penalty":
+        if penalty is not None:
+            raise SolverError("penalties apply to objective='late_penalty' only, not to %r" % (objective,))
+        return None, None
+    if penalty is None:
+        raise SolverError("objective='late_penalty' needs the penalty of each missed due date (penalty=...)")
+    penalty = _per_task(penalty, "penalty", task_list)
+    from .engine import penalty_f32
+    p32 = penalty_f32(penalty, J)
+    return [float(x) for x in penalty], p32
 
 
 def _resolve_release(release, J, task_list=None):
@@ -312,10 +328,13 @@ def _resolve_release(release, J, task_list=None):
     return [float(x) for x in release], r32
 
 
-def _set_objective(eng, objective, w32, d32, r32=None):
-    """Hand the weights, due dates and release dates to the engine; returns the engine objective the search runs."""
+def _set_objective(eng, objective, w32, d32, r32=None, p32=None):
+    """Hand the weights, due dates, release dates and late penalties to the engine; returns the engine objective the
+    search runs."""
     if r32 is not None:
         eng.set_release(r32)
+    if p32 is not None:
+        eng.set_penalty(p32)
     if w32 is not None:
         eng.set_weights(w32)
     if d32 is not None:
@@ -328,6 +347,8 @@ def _set_objective(eng, objective, w32, d32, r32=None):
             return "weighted_max_tardiness"
         if objective in _SQUARED:
             return "weighted_squared_tardiness" if w32 is not None else "squared_tardiness"
+        if objective == "late_penalty":
+            return "weighted_late_penalty" if w32 is not None else "late_penalty"
         return "weighted_tardiness" if w32 is not None else "tardiness"
     return "weighted_completion" if w32 is not None else objective
 
@@ -399,6 +420,16 @@ def _squared_stats(start, rts, w64, d64):
     return stats
 
 
+def _late_penalty_stats(start, rts, w64, d64, p64):
+    """late_penalty, sum_t [C_t > d_t] (p_t + w_t (C_t - d_t)) (unit rate without w64), with weighted_tardiness and
+    late_tasks (_tardiness_stats), of a plan in float64."""
+    w = w64 if w64 is not None else [1.0] * len(rts)
+    stats = _tardiness_stats(start, rts, w64, d64)
+    late = [float(s) + float(r) - d for s, r, d in zip(start, rts, d64)]
+    stats["late_penalty"] = sum(p + wi * x for x, p, wi in zip(late, p64, w) if x > 0)
+    return stats
+
+
 def _squared_flow_stats(start, rts, w64, r64):
     """squared_flow, sum_t w_t (C_t - max(r_t, 0))^2 (unit weights without w64, r_t = 0 without r64), and
     total_flow_time, sum_t (C_t - max(r_t, 0)), of a plan in float64."""
@@ -442,7 +473,7 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
           timeout=500, *, chains: Optional[int] = None, rounds: Optional[int] = None, seed: int = 0,
           integer_starts: bool = True, engine=None, hysteresis: Optional[bool] = None,
           nodes: Optional[int] = None, devices=None, objective: str = "makespan", weights=None, due=None,
-          release=None):
+          release=None, penalty=None):
     """Drop-in for saturn.solver.solve (milp.py:23).
 
     Objective.  "makespan" (the default, the reference's) or "completion": minimise the sum of the tasks'
@@ -521,6 +552,20 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     the caller's d, r and w; last_stats["device_makespan"] holds the device's fp32 score.  The 6th element stays the
     plan's makespan.
 
+    Late penalty.  objective="late_penalty" with `due` (as above) and `penalty` (a sequence aligned with task_list,
+    or a mapping keyed by Task, every value finite and >= 0) minimises sum_t [C_t > d_t] (p_t + w_t (C_t - d_t)):
+    each missed due date costs its fixed penalty p_t (a missed submission, an SLA credit) plus w_t per unit of time
+    late (unit rate without `weights`).  With every p = 0 it is "tardiness"; with penalties above any total
+    tardiness a plan can have it minimises the late count first and breaks ties by the tardiness.  The `due` and
+    `weights` rules and errors are those of "tardiness", as is the refusal of hysteresis=True; `release` is valid.
+    A missing `penalty`, `penalty` under any other objective, a wrong length, a task missing from the mapping, a
+    negative, NaN or inf value, or penalties that overflow fp32 (J * max(penalty) >= 2^126) raise SolverError before
+    any device call.  The search stops as soon as it finds a plan with no late task.  The device decides C_t > d_t
+    in fp32, so with fractional runtimes or due dates a task that completes within rounding of its due date may be
+    counted either way (integer data is exact).  last_stats["late_penalty"], ["weighted_tardiness"] and
+    ["late_tasks"] are recomputed in float64 from the emitted plan, the tasks' own runtimes and the caller's d, w and
+    p; last_stats["device_makespan"] holds the device's fp32 score.  The 6th element stays the plan's makespan.
+
     Release dates.  `release` (a sequence aligned with task_list, or a mapping keyed by Task, in the runtimes' units
     from the plan's t = 0) keeps every task from starting before its release date, under every objective: a
     dataset or a parent checkpoint that is only ready later, a job that arrives tomorrow.  r <= 0 means already
@@ -561,6 +606,7 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     J = len(task_list)
     w64, w32 = _resolve_weights(weights, objective, J, task_list)
     d64, d32 = _resolve_due(due, objective, J, task_list)
+    p64, p32 = _resolve_penalty(penalty, objective, J, task_list)
     r64, r32 = _resolve_release(release, J, task_list)
     if J == 0:
         return [[[] for _ in range(NSLOT)]], [], [], [], [], 0.0
@@ -584,7 +630,7 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
         nodes = _default_nodes()
     nodes = int(nodes)
     eng.set_table(Tdev, list(range(1, NSLOT + 1)), sentinel=float("inf"), nodes=nodes)
-    search_objective = _set_objective(eng, objective, w32, d32, r32)
+    search_objective = _set_objective(eng, objective, w32, d32, r32, p32)
     if chains is None:
         chains = int(os.environ.get("SATURN_B200_CHAINS", 0))
         if chains <= 0:
@@ -640,6 +686,8 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
         last_stats.update(_squared_stats(dec["start"], rts, w64, d64))
     elif objective == "squared_flow":
         last_stats.update(_squared_flow_stats(dec["start"], rts, w64, r64))
+    elif objective == "late_penalty":
+        last_stats.update(_late_penalty_stats(dec["start"], rts, w64, d64, p64))
     elif d64 is not None:
         last_stats.update(_tardiness_stats(dec["start"], rts, w64, d64))
     if r64 is not None:
@@ -739,7 +787,7 @@ def strategies_from_table(T, mask, executors=None, params=None, gcount=None):
 def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeout=500, *,
                 chains: Optional[int] = None, rounds: Optional[int] = None, seed: int = 0,
                 integer_starts: bool = True, engine=None, nodes: Optional[int] = None, devices=None,
-                objective: str = "makespan", weights=None, due=None, release=None):
+                objective: str = "makespan", weights=None, due=None, release=None, penalty=None):
     """solve() on the dense profiler tensor T[J][S][G] (+ mask of usable cells, + gcount[G] GPU counts).
     `objective` as for solve(): "makespan" or "completion" (sum of completion times); `weights` as for solve(),
     a sequence aligned with T's rows (the weighted sum of completion times, last_stats["weighted_completion"]);
@@ -748,6 +796,8 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     (last_stats["total_flow_time"]).  objective="max_stretch" as for solve(), with p*_t the smallest cell of row t
     the search may propose, over every strategy (last_stats["max_stretch"] and ["mean_stretch"] from T's values).
     objective="squared_tardiness" (with `due`) and "squared_flow" as for solve(), with their last_stats from T's values.
+    objective="late_penalty" (with `due` and `penalty`, sequences aligned with T's rows) as for solve(), with its
+    last_stats from T's values.
     Every cell of T must be
     >= 0 (-0.0 counts as zero), +inf or a sentinel: a negative or NaN cell raises SolverError, with or without `mask`.
 
@@ -769,6 +819,7 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     J, S, G = T.shape
     w64, w32 = _resolve_weights(weights, objective, J)
     d64, d32 = _resolve_due(due, objective, J)
+    p64, p32 = _resolve_penalty(penalty, objective, J)
     r64, r32 = _resolve_release(release, J)
     if J == 0:
         return [[[] for _ in range(NSLOT)]], [], [], [], [], 0.0, np.zeros(0, dtype=np.int64)
@@ -791,7 +842,7 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     eng = engine if engine is not None else _engine(devices)
     nodes = int(_default_nodes() if nodes is None else nodes)
     eng.set_table(Tdev, gcount, sentinel=float("inf"), nodes=nodes)
-    search_objective = _set_objective(eng, objective, w32, d32, r32)
+    search_objective = _set_objective(eng, objective, w32, d32, r32, p32)
     if chains is None:
         chains = int(os.environ.get("SATURN_B200_CHAINS", 0))
         if chains <= 0:
@@ -840,6 +891,8 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
         last_stats.update(_squared_stats(dec["start"], rts, w64, d64))
     elif objective == "squared_flow":
         last_stats.update(_squared_flow_stats(dec["start"], rts, w64, r64))
+    elif objective == "late_penalty":
+        last_stats.update(_late_penalty_stats(dec["start"], rts, w64, d64, p64))
     elif d64 is not None:
         last_stats.update(_tardiness_stats(dec["start"], rts, w64, d64))
     if r64 is not None:

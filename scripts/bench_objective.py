@@ -3,7 +3,7 @@ maximum lateness, of the (weighted) number of late tasks, of the maximum stretch
 prints one JSON line.
 
     python scripts/bench_objective.py [--steps 200] [--warmup 20] [--solve-chains 0] [--solve-rounds 400]
-                                      [--only max_stretch | squared]
+                                      [--only max_stretch | squared | late_penalty]
 
 kernel: sb_eval on bench.py's C4 batch (J = 256, S = 8, 946,176 candidates, the same seeded inputs, integer
         starts), scored for the makespan, the sum of completion times, the weighted sum (seeded weights) and the
@@ -35,6 +35,11 @@ comparison.
 alternated as above, and runs only the squared-flow comparison: on the same 256-task set and release dates,
 solve(objective="squared_flow") against the completion, max_stretch and makespan plans (all release-aware), each
 rescored in float64 on sum_t F_t^2, mean F_t and max F_t, the flow time F_t = C_t - max(r_t, 0).
+--only late_penalty times only the weighted tardiness and the weighted late penalty (the same weights and due dates,
+seeded integer penalties in [0, 100000) s), alternated as above, and runs only the late-penalty comparison: on the
+256-task set with the seeded integer due dates of the late-count row and seeded integer penalties in [0, 100000),
+solve(objective="late_penalty") against the tardiness, late_tasks and completion plans, each rescored in float64 on
+the cost sum_t [C_t > d_t] (p_t + C_t - d_t), the late tasks and the tardiness.
 The card's name and power limit are read in the same run (nvidia-smi, read-only queries).
 """
 import argparse
@@ -66,7 +71,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--solve-chains", type=int, default=0, help="0 = solve()'s default population")
     ap.add_argument("--solve-rounds", type=int, default=400)
-    ap.add_argument("--only", choices=("all", "max_stretch", "squared"), default="all")
+    ap.add_argument("--only", choices=("all", "max_stretch", "squared", "late_penalty"), default="all")
     args = ap.parse_args()
     import numpy as np
     import torch
@@ -96,6 +101,9 @@ def main():
         objs = ("weighted_tardiness", "weighted_max_tardiness")
     if args.only == "squared":
         objs = ("weighted_tardiness", "weighted_squared_tardiness")
+    if args.only == "late_penalty":
+        objs = ("weighted_tardiness", "weighted_late_penalty")
+        eng.set_penalty(np.random.default_rng(7).integers(0, 100000, size=J))
     times = {o: [] for o in objs}
     for i in range(args.warmup + args.steps):
         for obj in objs[i % len(objs):] + objs[:i % len(objs)]:
@@ -112,6 +120,19 @@ def main():
     kernel = {o: {"median_ms": float(np.median(t)), "p10_ms": float(np.percentile(t, 10)),
                   "p90_ms": float(np.percentile(t, 90)), "candidates_per_s": B / (float(np.median(t)) * 1e-3)}
               for o, t in times.items()}
+    if args.only == "late_penalty":
+        kernel["late_penalty_over_weighted_tardiness"] = (kernel["weighted_late_penalty"]["median_ms"] /
+                                                          kernel["weighted_tardiness"]["median_ms"])
+        kernel.update(B=B, J=J, S=Sx, path=path, steps=args.steps)
+        del opt, prio, out
+        eng_r.close()
+        torch.cuda.empty_cache()
+        kw = dict(rounds=args.solve_rounds, seed=1, engine=eng, **({"chains": args.solve_chains}
+                                                                   if args.solve_chains else {}))
+        print(json.dumps({"card": card(0), "kernel": kernel, "late_penalty": late_penalty_effect(S, R, _tasks256(),
+                                                                                                   kw)}))
+        eng.close()
+        return
     if args.only == "squared":
         kernel["squared_over_weighted_tardiness"] = (kernel["weighted_squared_tardiness"]["median_ms"] /
                                                      kernel["weighted_tardiness"]["median_ms"])
@@ -256,6 +277,33 @@ def squared_effect(S, R, tasks, makespan, kw):
         comp = [p[0] + p[2] for p in R.plan_from_arrays(tuples, res[0], res[1], res[2], res[3])]
         flow = [c - max(x, 0.0) for c, x in zip(comp, r)]
         out[obj] = {"sum_flow_squared": sum(f * f for f in flow), "mean_flow": sum(flow) / J, "max_flow": max(flow),
+                    "makespan": max(comp), "wall_s": wall, "rounds": S.last_stats["rounds"]}
+    return out
+
+
+def late_penalty_effect(S, R, tasks, kw):
+    """The late-penalty plan against the tardiness, late_tasks and completion plans on the 256-task set with the due
+    dates of the late-count row and seeded penalties, every plan rescored in float64 (see the module doc)."""
+    import numpy as np
+    J = len(tasks)
+    tuples = [[(g, s.runtime) for g, s in t.strategies.items()] for t in tasks]
+    due = [float(x) for x in np.random.default_rng(4).integers(0, 200000, size=J)]
+    pen = [float(x) for x in np.random.default_rng(8).integers(0, 100000, size=J)]
+    for obj in ("late_penalty", "tardiness", "late_tasks"):   # first launches load the kernels
+        S.solve(tasks, None, rounds=4, engine=kw["engine"], objective=obj, due=due,
+                **({"penalty": pen} if obj == "late_penalty" else {}))
+    out = {}
+    for obj in ("late_penalty", "tardiness", "late_tasks", "completion"):
+        extra = {"due": due} if obj != "completion" else {}
+        if obj == "late_penalty":
+            extra["penalty"] = pen
+        t0 = time.perf_counter()
+        res = S.solve(tasks, None, objective=obj, **extra, **kw)
+        wall = time.perf_counter() - t0
+        comp = [p[0] + p[2] for p in R.plan_from_arrays(tuples, res[0], res[1], res[2], res[3])]
+        late = [(c - d, p) for c, d, p in zip(comp, due, pen) if c > d]
+        out[obj] = {"cost": sum(p + x for x, p in late), "late_tasks": len(late),
+                    "tardiness": sum(x for x, _p in late), "penalties_paid": sum(p for _x, p in late),
                     "makespan": max(comp), "wall_s": wall, "rounds": S.last_stats["rounds"]}
     return out
 
