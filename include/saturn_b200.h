@@ -83,6 +83,12 @@
  * A job that completes exactly at its due date is on time.  p = 0 gives exactly the tardiness fold of SB_FLAG_DUE,
  * due dates at or past every completion give +0, and the score is >= +0.  A job with no runtime (rt = +inf) gives a
  * +inf term.  The comparison C > d is made in fp32, as the late count makes it.
+ * With SB_FLAG_COMPLETION_PENALTY instead (penalties from sb_set_penalty as well) it is the completion penalty:
+ *   total = sum_j (w_j C_j + [C_j > d_j] p_j), from +0 in schedule order per job: e = start + rt, t = w * e, then
+ *   t = t + p when e > d, then acc = acc + t, every step rounded on its own (no fused multiply-add).
+ * p = 0 gives exactly the weighted completion fold (the unweighted sum without SB_FLAG_WEIGHTED).  A job that
+ * completes exactly at its due date is on time; a job with no runtime (rt = +inf) gives a +inf term.  One due date H
+ * for every job with every p above any sum_j w_j C_j makes it min sum_j w_j C_j subject to makespan <= H.
  * The schedule, every start and every slot mask are the same under every objective.
  * With SB_FLAG_MAX_LATENESS (per-job due dates d_j, sb_set_due) the score is the maximum lateness
  * L_max = max_j (start_j + rt_j - d_j), emitted as the tail makespan L_max + D >= +0 with D = max_t d_t:
@@ -253,6 +259,18 @@ typedef enum sb_status {
                                      (SB_FLAG_DUE's floor with the penalties added), it stops as soon as the
                                      incumbent is +0 (stop_reason 3), and sb_search_seed_lpt plants the EDD orders of
                                      SB_FLAG_DUE.  Not available with SB_FLAG_ALT_WARPSCAN (SB_ERR_UNSUPPORTED). */
+#define SB_FLAG_COMPLETION_PENALTY 32768u /* with SB_FLAG_SUM_COMPLETION | SB_FLAG_DUE only (SB_FLAG_WEIGHTED optional;
+                                     else SB_ERR_ARG), and not with SB_FLAG_LATE_PENALTY, SB_FLAG_LATE_COUNT,
+                                     SB_FLAG_MAX_TARDINESS, SB_FLAG_SQUARED or SB_FLAG_MAX_LATENESS (SB_ERR_ARG), after
+                                     sb_set_penalty (else SB_ERR_STATE, checked after the due dates and before the
+                                     release dates): the (weighted) completion time plus a fixed penalty for each
+                                     missed due date, sum_j (w_j C_j + [C_j > d_j] p_j) (see the evaluation rule
+                                     above).  Accepted wherever SB_FLAG_LATE_PENALTY is; every score the library emits
+                                     then holds that total, and target_makespan targets it.  The search's temperature
+                                     unit is the completion unit (incumbent / sum_j w_j, no sum of penalties added),
+                                     it does not stop at 0, and sb_search_seed_lpt plants the completion orders (SPT,
+                                     WSPT with SB_FLAG_WEIGHTED), not the EDD orders of SB_FLAG_DUE.  Not available
+                                     with SB_FLAG_ALT_WARPSCAN (SB_ERR_UNSUPPORTED). */
 #define SB_IPC_HANDLE_BYTES 64
 
 typedef struct sb_handle sb_handle;
@@ -303,11 +321,11 @@ int sb_set_due(sb_handle* h, const float* d, int J);
  * uses is made here, once.  sb_set_table clears the release dates; setting or clearing them ends the current
  * search (sb_search_init again). */
 int sb_set_release(sb_handle* h, const float* r, int J);
-/* Per-job late penalties for SB_FLAG_LATE_PENALTY: p host fp32 [J], the fixed cost of each job that completes after
- * its due date, every value finite and >= 0 with J * max_j p_j < 2^126 (else SB_ERR_ARG, as is a J that differs
- * from the table's); -0 is stored as +0.  p = NULL clears them.  SB_ERR_STATE before sb_set_table.  sb_set_table
- * clears the penalties; setting or clearing them ends the current search (sb_search_init again).  Their sum is
- * recorded for the search's temperature unit. */
+/* Per-job late penalties for SB_FLAG_LATE_PENALTY and SB_FLAG_COMPLETION_PENALTY: p host fp32 [J], the fixed cost
+ * of each job that completes after its due date, every value finite and >= 0 with J * max_j p_j < 2^126 (else
+ * SB_ERR_ARG, as is a J that differs from the table's); -0 is stored as +0.  p = NULL clears them.  SB_ERR_STATE
+ * before sb_set_table.  sb_set_table clears the penalties; setting or clearing them ends the current search
+ * (sb_search_init again).  Their sum is recorded for the search's temperature unit. */
 int sb_set_penalty(sb_handle* h, const float* p, int J);
 /* copy the reduced table back (host pointers, either may be NULL): tmin fp32 [J][8], args u8 [J][8].
  * This is the table the reference solver is actually given: Task.strategies[g] after the profiler's

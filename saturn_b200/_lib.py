@@ -21,6 +21,7 @@ FLAG_LATE_COUNT = 2048
 FLAG_MAX_TARDINESS = 4096
 FLAG_SQUARED = 8192
 FLAG_LATE_PENALTY = 16384
+FLAG_COMPLETION_PENALTY = 32768
 IPC_HANDLE_BYTES = 64
 # test hooks in the top bits of the same flags word: the enum in csrc/sb_internal.h says what each one forces
 HOOK_FORCE_GENERIC = 0x80000000

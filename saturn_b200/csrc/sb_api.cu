@@ -525,15 +525,21 @@ int sb_set_penalty(sb_handle* h, const float* p, int J) {
 }
 
 // The one reader of the objective flags.  SB_FLAG_WEIGHTED and SB_FLAG_DUE are valid with SB_FLAG_SUM_COMPLETION only;
-// SB_FLAG_MAX_LATENESS alone among the objective flags; SB_FLAG_LATE_COUNT, SB_FLAG_MAX_TARDINESS, SB_FLAG_SQUARED and
-// SB_FLAG_LATE_PENALTY with SB_FLAG_SUM_COMPLETION | SB_FLAG_DUE only (they change what the tardiness form adds per
-// job, and how it folds its terms), and not together or with SB_FLAG_MAX_LATENESS.  Every other combination is
-// SB_ERR_ARG.
+// SB_FLAG_MAX_LATENESS alone among the objective flags; SB_FLAG_LATE_COUNT, SB_FLAG_MAX_TARDINESS, SB_FLAG_SQUARED,
+// SB_FLAG_LATE_PENALTY and SB_FLAG_COMPLETION_PENALTY with SB_FLAG_SUM_COMPLETION | SB_FLAG_DUE only (they change what
+// the tardiness form adds per job, and how it folds its terms), and not together or with SB_FLAG_MAX_LATENESS.  Every
+// other combination is SB_ERR_ARG.
 static int decode_objective(unsigned flags, Objective* o) {
   const bool sum = flags & SB_FLAG_SUM_COMPLETION, weighted = flags & SB_FLAG_WEIGHTED, due = flags & SB_FLAG_DUE;
   const bool lateness = flags & SB_FLAG_MAX_LATENESS, late = flags & SB_FLAG_LATE_COUNT;
   const bool max_tardiness = flags & SB_FLAG_MAX_TARDINESS, squared = flags & SB_FLAG_SQUARED;
-  const bool penalty = flags & SB_FLAG_LATE_PENALTY;
+  const bool penalty = flags & SB_FLAG_LATE_PENALTY, completion_penalty = flags & SB_FLAG_COMPLETION_PENALTY;
+  if (completion_penalty && !(sum && due))
+    return fail(SB_ERR_ARG, "SB_FLAG_COMPLETION_PENALTY adds a fixed penalty per missed due date to the completion "
+                "time: it needs SB_FLAG_SUM_COMPLETION and SB_FLAG_DUE");
+  if (completion_penalty && (penalty || late || max_tardiness || squared || lateness))
+    return fail(SB_ERR_ARG, "SB_FLAG_COMPLETION_PENALTY cannot be combined with SB_FLAG_LATE_PENALTY, "
+                "SB_FLAG_LATE_COUNT, SB_FLAG_MAX_TARDINESS, SB_FLAG_SQUARED or SB_FLAG_MAX_LATENESS");
   if (penalty && !(sum && due))
     return fail(SB_ERR_ARG, "SB_FLAG_LATE_PENALTY adds a fixed penalty to the tardiness form's late terms: it needs "
                 "SB_FLAG_SUM_COMPLETION and SB_FLAG_DUE");
@@ -568,6 +574,7 @@ static int decode_objective(unsigned flags, Objective* o) {
   else if (max_tardiness) o->obj = Obj::MaxTardiness;
   else if (squared) o->obj = Obj::SquaredTardiness;
   else if (penalty) o->obj = Obj::LatePenalty;
+  else if (completion_penalty) o->obj = Obj::CompletionPenalty;
   else if (due) o->obj = Obj::Tardiness;
   else o->obj = weighted ? Obj::WeightedSum : Obj::Sum;
   return SB_OK;
@@ -596,7 +603,8 @@ static int check_per_job(const sb_handle* h, unsigned flags, Objective* o) {
     return fail(SB_ERR_ARG, "SB_FLAG_SQUARED | SB_FLAG_WEIGHTED needs J * max w * 2^50 < FLT_MAX (beyond it the sum of "
                 "squared tardiness can overflow fp32)");
   if (obj_penalty(o->obj) && !h->has_p)
-    return fail(SB_ERR_STATE, "SB_FLAG_LATE_PENALTY needs sb_set_penalty (sb_set_table clears the penalties)");
+    return fail(SB_ERR_STATE, "%s needs sb_set_penalty (sb_set_table clears the penalties)",
+                o->obj == Obj::CompletionPenalty ? "SB_FLAG_COMPLETION_PENALTY" : "SB_FLAG_LATE_PENALTY");
   if ((flags & SB_FLAG_RELEASE) && !h->has_r)
     return fail(SB_ERR_STATE, "SB_FLAG_RELEASE needs sb_set_release (sb_set_table clears the release dates)");
   return SB_OK;
@@ -719,8 +727,8 @@ int sb_eval(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, int64
     if (c.obj != Obj::Makespan || (flags & SB_FLAG_RELEASE))
       return fail(SB_ERR_UNSUPPORTED, "SB_FLAG_ALT_WARPSCAN scores the makespan without release dates only: it "
                   "cannot be combined with SB_FLAG_SUM_COMPLETION, SB_FLAG_WEIGHTED, SB_FLAG_DUE, SB_FLAG_RELEASE, "
-                  "SB_FLAG_MAX_LATENESS, SB_FLAG_LATE_COUNT, SB_FLAG_MAX_TARDINESS, SB_FLAG_SQUARED or "
-                  "SB_FLAG_LATE_PENALTY");
+                  "SB_FLAG_MAX_LATENESS, SB_FLAG_LATE_COUNT, SB_FLAG_MAX_TARDINESS, SB_FLAG_SQUARED, "
+                  "SB_FLAG_LATE_PENALTY or SB_FLAG_COMPLETION_PENALTY");
     if (flags & (SB_FLAG_POST_KEY | SB_FLAG_FOLD_PREV))
       return fail(SB_ERR_UNSUPPORTED, "SB_FLAG_ALT_WARPSCAN cannot be combined with the fused key exchange");
     cudaError_t e = eval_alt_launch(h->dev, c, h->stream);
@@ -1170,6 +1178,9 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
   // fraction of a typical score difference under every objective
   const bool weighted = o.weighted;
   const float per = weighted ? static_cast<float>(h->w_sum) : static_cast<float>(J);
+  // The completion penalty keeps this completion unit, with no sum of penalties added: in a front the penalties are
+  // a barrier that the warm-started incumbent already clears, and must not heat the search past it.  With every p = 0
+  // it is the completion unit bit for bit (a starting point, not a measured choice, DESIGN §3)
   s.scale = isfinite(mk) ? (obj_sum(o.obj) ? mk / per : mk) : 1.0f;
   if (tardiness_form(o.obj) && isfinite(mk)) {
     // tardiness can be 0 or tiny at the incumbent: the unit is at least the weighted mean of each job's smallest
@@ -1481,8 +1492,10 @@ int sb_search_seed_lpt(sb_handle* h) {
   // weighted sum: Smith's rule (WSPT), ascending rt / w; with unit weights exactly the SPT order
   const bool wspt = spt && s.obj.weighted;
   // the due-date objectives: earliest due date first (EDD), ties by rt / w (rt with unit weights), then by job index;
-  // the maximum lateness the same unit-weight EDD orders (Jackson's rule, optimal for L_max on one machine)
-  const bool edd = obj_due(obj);
+  // the maximum lateness the same unit-weight EDD orders (Jackson's rule, optimal for L_max on one machine).  The
+  // completion penalty keeps the completion orders: its due dates are a barrier on the completion time (one cap for
+  // every job in a front), and WSPT is what lowers the sum below it
+  const bool edd = obj_due(obj) && obj != Obj::CompletionPenalty;
   const bool rel = (s.p.flags & SB_FLAG_RELEASE) != 0;
   // the late count: each EDD order repaired by Moore-Hodgson's rule (see moore_hodgson)
   const bool late = obj == Obj::LateCount;

@@ -19,7 +19,7 @@ constexpr float kSentinel = 1.0e6f;  // reference's "unprofiled" runtime, Perfor
 __device__ __forceinline__ float inf_f() { return __int_as_float(0x7f800000); }
 
 // ---------------------------------------------------------------- the objective
-// The nine scores the kernels compute, and the SB_FLAG_* bits that select each (sb_api.cu: decode_objective; every
+// The ten scores the kernels compute, and the SB_FLAG_* bits that select each (sb_api.cu: decode_objective; every
 // form also runs with SB_FLAG_RELEASE).  C is a job's completion, w its weight, d its due date, p its late penalty.
 //   Obj               flags                                              score
 //   Makespan          none                                               max C
@@ -31,28 +31,33 @@ __device__ __forceinline__ float inf_f() { return __int_as_float(0x7f800000); }
 //   MaxTardiness      SUM_COMPLETION | DUE | MAX_TARDINESS [| WEIGHTED]  max w max(C - d, 0)
 //   SquaredTardiness  SUM_COMPLETION | DUE | SQUARED [| WEIGHTED]        sum w max(C - d, 0)^2
 //   LatePenalty       SUM_COMPLETION | DUE | LATE_PENALTY [| WEIGHTED]   sum (C > d ? p + w (C - d) : 0)
+//   CompletionPenalty SUM_COMPLETION | DUE | COMPLETION_PENALTY [| WEIGHTED]
+//                                                                        sum (w C + (C > d ? p : 0))
 // Every other combination of those flags is refused.  The history of each form is in DESIGN.md.  New forms go at the
 // end: a kernel's symbol holds its form's value.
 enum class Obj {
-  Makespan, TailMakespan, Sum, WeightedSum, Tardiness, LateCount, MaxTardiness, SquaredTardiness, LatePenalty
+  Makespan, TailMakespan, Sum, WeightedSum, Tardiness, LateCount, MaxTardiness, SquaredTardiness, LatePenalty,
+  CompletionPenalty
 };
 // the score is a sum over the jobs, folded in schedule order
 __host__ __device__ constexpr bool obj_sum(Obj o) {
   return o == Obj::Sum || o == Obj::WeightedSum || o == Obj::Tardiness || o == Obj::LateCount ||
-         o == Obj::SquaredTardiness || o == Obj::LatePenalty;
+         o == Obj::SquaredTardiness || o == Obj::LatePenalty || o == Obj::CompletionPenalty;
 }
 // the score reads the job weights (the caller's, or unit weights without SB_FLAG_WEIGHTED)
 __host__ __device__ constexpr bool obj_weights(Obj o) {
   return o == Obj::WeightedSum || o == Obj::Tardiness || o == Obj::LateCount || o == Obj::MaxTardiness ||
-         o == Obj::SquaredTardiness || o == Obj::LatePenalty;
+         o == Obj::SquaredTardiness || o == Obj::LatePenalty || o == Obj::CompletionPenalty;
 }
 // the score reads the due-date array: the due dates, or TailMakespan's tails
 __host__ __device__ constexpr bool obj_due(Obj o) {
   return o == Obj::TailMakespan || o == Obj::Tardiness || o == Obj::LateCount || o == Obj::MaxTardiness ||
-         o == Obj::SquaredTardiness || o == Obj::LatePenalty;
+         o == Obj::SquaredTardiness || o == Obj::LatePenalty || o == Obj::CompletionPenalty;
 }
 // the score reads the late-penalty array (sb_set_penalty)
-__host__ __device__ constexpr bool obj_penalty(Obj o) { return o == Obj::LatePenalty; }
+__host__ __device__ constexpr bool obj_penalty(Obj o) {
+  return o == Obj::LatePenalty || o == Obj::CompletionPenalty;
+}
 
 // ---------------------------------------------------------------- mbarrier + TMA bulk copy (1-D)
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -206,7 +211,10 @@ __device__ __forceinline__ float fmax3_mk(float mk, float b, float c) {
 //                  bit, then mk + w * (t * t), three roundings; w = 1 gives the unweighted form bit for bit, and a
 //                  job with no runtime a +inf term.  LatePenalty: x = e - d, then mk + (x > 0 ? p + w * x : +0), the
 //                  product and the sum rounded on their own; p = +0 gives Tardiness's term bit for bit (+0 added to
-//                  a positive finite value is exact), and a job with no runtime a +inf term.
+//                  a positive finite value is exact), and a job with no runtime a +inf term.  CompletionPenalty:
+//                  t = w * e, then t + p when e > d, then mk + t, each rounded on its own; p = +0 gives WeightedSum's
+//                  term bit for bit (+0 added to a value >= +0 is exact), a job that completes exactly at its due date
+//                  is on time, and a job with no runtime gives a +inf term.  k_eval_full folds this literal form.
 // The slot update is the same under every objective: only the score differs.
 // kRelease (SB_FLAG_RELEASE): the job starts no earlier than its release date `r`, s = max(f[km1], r) (ceil(r) under
 // integer starts, made once by sb_set_release, so s stays an integer).  The slot update below stays valid because it
@@ -264,6 +272,11 @@ __device__ __forceinline__ void ls_step(float (&f)[8], float& mk, float& pend, f
       const float x = __fsub_rn(e, d);
       mk = __fadd_rn(mk, x > 0.f ? __fadd_rn(p, __fmul_rn(w, x)) : 0.f);
     }
+    // the completion penalty, t = w * e, then t + p when e > d, as t + (e > d ? p : +0): t >= +0, so adding +0 leaves
+    // it exact.  Same value; the literal branch spilled 20 bytes in one multi-node search kernel, this form 4 to 8
+    // bytes in ten single-node position-major search kernels (DESIGN §3.1, *Completion penalty*), all at 128 registers
+    else if constexpr (kObj == Obj::CompletionPenalty)
+      mk = __fadd_rn(mk, __fadd_rn(__fmul_rn(w, e), e > d ? p : 0.f));
     else if constexpr (kObj == Obj::WeightedSum) mk = __fadd_rn(mk, __fmul_rn(w, e));
     else mk = mk + e;
   } else if (kTrackMk) {

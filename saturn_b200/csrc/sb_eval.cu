@@ -829,6 +829,11 @@ __global__ void __launch_bounds__(128) k_eval_full(const FullArgs a) {
         const float x = __fsub_rn(s + rt, __ldg(a.d + j));
         mk = __fadd_rn(mk, x > 0.f ? __fadd_rn(__ldg(a.p + j), __fmul_rn(__ldg(a.w + j), x)) : 0.f);
       }
+      else if constexpr (OBJ == Obj::CompletionPenalty) {
+        float t = __fmul_rn(__ldg(a.w + j), s + rt);
+        if (s + rt > __ldg(a.d + j)) t = __fadd_rn(t, __ldg(a.p + j));
+        mk = __fadd_rn(mk, t);
+      }
       else if constexpr (OBJ == Obj::WeightedSum) mk = __fadd_rn(mk, __fmul_rn(__ldg(a.w + j), s + rt));
       else if constexpr (OBJ == Obj::Sum) mk = mk + (s + rt);  // the left fold in schedule order
       else mk = fmaxf(mk, s + rt);

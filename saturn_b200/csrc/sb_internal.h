@@ -33,7 +33,7 @@ static_assert(((HOOK_FORCE_GENERIC | HOOK_NO_STREAM | HOOK_NO_FUSED | HOOK_NO_IN
                (SB_FLAG_INTEGER_STARTS | SB_FLAG_REDUCED | SB_FLAG_OPT_BY_POSITION | SB_FLAG_POST_KEY |
                 SB_FLAG_FOLD_PREV | SB_FLAG_ALT_WARPSCAN | SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED |
                 SB_FLAG_DUE | SB_FLAG_RELEASE | SB_FLAG_MAX_LATENESS | SB_FLAG_LATE_COUNT |
-                SB_FLAG_MAX_TARDINESS | SB_FLAG_SQUARED | SB_FLAG_LATE_PENALTY)) == 0,
+                SB_FLAG_MAX_TARDINESS | SB_FLAG_SQUARED | SB_FLAG_LATE_PENALTY | SB_FLAG_COMPLETION_PENALTY)) == 0,
               "the test hooks share no bit with the SB_FLAG_* flags");
 
 // Debug options of the streamed tile kernel (sb_debug_tile_options): kept on the handle, not in the flags word, and
@@ -67,6 +67,7 @@ decltype(auto) with_obj(Obj obj, F&& f) {
     case Obj::MaxTardiness: return f(obj_c<Obj::MaxTardiness>{});
     case Obj::SquaredTardiness: return f(obj_c<Obj::SquaredTardiness>{});
     case Obj::LatePenalty: return f(obj_c<Obj::LatePenalty>{});
+    case Obj::CompletionPenalty: return f(obj_c<Obj::CompletionPenalty>{});
     default: return f(obj_c<Obj::Makespan>{});
   }
 }

@@ -55,14 +55,23 @@ SQUARED_OBJECTIVES = ("squared_tardiness", "weighted_squared_tardiness")
 PENALTY_OBJECTIVES = ("late_penalty", "weighted_late_penalty")
 # The objectives every cross-cutting check of the test suite covers: all of them but the squared and late-penalty forms.
 OBJECTIVES = tuple(o for o in _OBJECTIVES if o not in SQUARED_OBJECTIVES + PENALTY_OBJECTIVES)
+# The completion-penalty forms: the (weighted) completion time plus the set_penalty penalty of every task that completes
+# after its due date (solver.solve_front runs them with one due date, a makespan cap, for every task).  A table of their
+# own, held to oracle/ref_completion_penalty.py; objective_spec and objective_flag look names up in both tables.
+COMPLETION_PENALTY_OBJECTIVES = {
+    "completion_penalty": Objective(_SUM | _DUE | _lib.FLAG_COMPLETION_PENALTY, False, True),
+    "weighted_completion_penalty": Objective(_SUM | _DUE | _lib.FLAG_COMPLETION_PENALTY | _W, True, True),
+}
 
 
 def objective_spec(objective: str) -> Objective:
     """The table entry of an objective name; raises SolverError for a name that is not one."""
-    if objective not in _OBJECTIVES:
+    spec = _OBJECTIVES.get(objective) or COMPLETION_PENALTY_OBJECTIVES.get(objective)
+    if spec is None:
         from .solver import SolverError
-        raise SolverError("objective must be one of %s, not %r" % (", ".join(map(repr, _OBJECTIVES)), objective))
-    return _OBJECTIVES[objective]
+        names = list(_OBJECTIVES) + list(COMPLETION_PENALTY_OBJECTIVES)
+        raise SolverError("objective must be one of %s, not %r" % (", ".join(map(repr, names)), objective))
+    return spec
 
 
 def objective_flag(objective: str) -> int:
@@ -71,8 +80,9 @@ def objective_flag(objective: str) -> int:
 
 
 def objective_reads_penalty(objective: str) -> bool:
-    """Whether an objective scores with the late penalties of set_penalty (SB_FLAG_LATE_PENALTY)."""
-    return bool(objective_spec(objective).flags & _lib.FLAG_LATE_PENALTY)
+    """Whether an objective scores with the late penalties of set_penalty (SB_FLAG_LATE_PENALTY or
+    SB_FLAG_COMPLETION_PENALTY)."""
+    return bool(objective_spec(objective).flags & (_lib.FLAG_LATE_PENALTY | _lib.FLAG_COMPLETION_PENALTY))
 
 
 def weights_f32(w, J: int) -> np.ndarray:
@@ -159,7 +169,7 @@ def _require_due(due, objective: str):
     """The tardiness objectives (the maximum tardiness among them), the late counts and the maximum lateness score
     against the due dates of set_due: refuse them, before any device call, on an engine that has none (set_table
     clears them)."""
-    spec = _OBJECTIVES.get(objective)
+    spec = _OBJECTIVES.get(objective) or COMPLETION_PENALTY_OBJECTIVES.get(objective)
     if spec is not None and spec.due and due is None:
         from .solver import SolverError
         raise SolverError("objective=%r needs due dates: call set_due after set_table" % (objective,))
@@ -168,7 +178,8 @@ def _require_due(due, objective: str):
 def _require_penalty(penalty, objective: str):
     """The late-penalty objectives score with the penalties of set_penalty: refuse them, before any device call, on
     an engine that has none (set_table clears them)."""
-    if objective in _OBJECTIVES and objective_reads_penalty(objective) and penalty is None:
+    if (objective in _OBJECTIVES or objective in COMPLETION_PENALTY_OBJECTIVES) and objective_reads_penalty(objective) \
+            and penalty is None:
         from .solver import SolverError
         raise SolverError("objective=%r needs late penalties: call set_penalty after set_table" % (objective,))
 
@@ -300,8 +311,9 @@ class Engine:
     def set_penalty(self, p) -> "Engine":
         """Per-job late penalties (J values, finite and >= 0, converted to fp32) for objective="late_penalty", which
         scores sum_j [C_j > d_j] (p_j + (C_j - d_j)) with C_j = start_j + rt_j against the due dates of set_due, and
-        "weighted_late_penalty", which multiplies each tardiness by the set_weights weight.  None clears them;
-        set_table clears them too."""
+        "weighted_late_penalty", which multiplies each tardiness by the set_weights weight, and for
+        objective="completion_penalty" / "weighted_completion_penalty", which score sum_j (w_j C_j + [C_j > d_j] p_j).
+        None clears them; set_table clears them too."""
         if p is None:
             check(self._lib.sb_set_penalty(self._h, None, 0))
             self.penalty = None

@@ -55,7 +55,7 @@ def orchestrate(task_list, log=False, interval=1000, gurobi=True, *,
     saturn.executor.execute; returns the list of per-interval records (plan makespan, tasks run).
 
     A `due` mapping Task -> due date in `solver_kwargs` (objective="tardiness", "max_lateness", "late_tasks",
-    "squared_tardiness" or "late_penalty") is
+    "squared_tardiness", "late_penalty" or "completion_penalty") is
     measured from the first plan's t = 0: the solve for interval n plans from n * interval on, so it receives
     {t: d - n * interval}, and the lateness each solve reports is against the original due dates (both sides shift
     alike).  A sequence `due` raises SolverError, since the task list shrinks from interval to interval.  A `release`
@@ -66,9 +66,9 @@ def orchestrate(task_list, log=False, interval=1000, gurobi=True, *,
     shifted due dates leave every tardiness unchanged (C and d move alike).  Under objective="squared_flow" each solve
     measures flow from the shifted release dates, clamped at the interval's t = 0: a task released before the
     interval counts its flow from the interval's start, so each solve minimises the squares of the waits that
-    remain, not of the whole flow time.  Under objective="late_penalty" a `penalty` mapping Task -> penalty is passed
-    to every solve unchanged: a penalty is what missing the due date costs, whenever the plan is made; a sequence
-    `penalty` raises SolverError, as a sequence `due` does.
+    remain, not of the whole flow time.  Under objective="late_penalty" and "completion_penalty" a `penalty` mapping
+    Task -> penalty is passed to every solve unchanged: a penalty is what missing the due date costs, whenever the
+    plan is made; a sequence `penalty` raises SolverError, as a sequence `due` does.
     """
     logging.basicConfig(level=logging.INFO if log else logging.WARNING,
                         format="%(asctime)s %(levelname)-8s %(message)s", datefmt="%Y-%m-%d %H:%M:%S")

@@ -64,14 +64,17 @@ def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objecti
     objective's order.  objective="late_tasks" / "weighted_late_tasks": the EDD orders of "tardiness" /
     "weighted_tardiness", each repaired by Moore-Hodgson's rule after the node fill (moore_hodgson).
     objective="max_tardiness" / "weighted_max_tardiness", "squared_tardiness" / "weighted_squared_tardiness" and
-    "late_penalty" / "weighted_late_penalty": the EDD orders of "tardiness" / "weighted_tardiness" unchanged."""
+    "late_penalty" / "weighted_late_penalty": the EDD orders of "tardiness" / "weighted_tardiness" unchanged.
+    objective="completion_penalty" / "weighted_completion_penalty": the orders of "completion" /
+    "weighted_completion" (SPT / WSPT), not EDD: the due dates there are a barrier on the completion time."""
     spec = objective_spec(objective)
     if spec.weighted:
         if weights is None:
             raise ValueError("objective=%r needs the job weights" % objective)
         w64 = np.asarray(weights, dtype=np.float32).astype(np.float64)
     late = bool(spec.flags & _lib.FLAG_LATE_COUNT)
-    edd = spec.due
+    completion_penalty = bool(spec.flags & _lib.FLAG_COMPLETION_PENALTY)
+    edd = spec.due and not completion_penalty
     if edd:
         if due is None:
             raise ValueError("objective=%r needs the job due dates" % objective)
@@ -96,9 +99,9 @@ def lpt_seeds(tmin: np.ndarray, sentinel: float = 1.0e6, nodes: int = 1, objecti
         if edd:
             tie = rt.astype(np.float64) / w64 if spec.weighted else rt.astype(np.float64)
             order = np.lexsort((np.arange(J), tie, d32))
-        elif objective == "weighted_completion":
+        elif objective in ("weighted_completion", "weighted_completion_penalty"):
             order = np.argsort(rt.astype(np.float64) / w64, kind="stable")
-        elif objective == "completion":
+        elif objective in ("completion", "completion_penalty"):
             order = np.argsort(rt, kind="stable")
         else:
             order = np.argsort(-rt * (col + 1) ** 0.5, kind="stable")
@@ -189,7 +192,9 @@ def run_search(engine: Engine, chains: int = 1 << 16, rounds: int = 200, seed: i
     tardiness, and stops at 0 like the tardiness.  objective="squared_tardiness" / "weighted_squared_tardiness"
     minimises the (weighted) sum of squared tardiness, and stops at 0 like the tardiness.  objective="late_penalty" /
     "weighted_late_penalty" minimises the engine's set_penalty penalty plus the (weighted) tardiness of every late
-    task, and stops at 0 like the tardiness.
+    task, and stops at 0 like the tardiness.  objective="completion_penalty" / "weighted_completion_penalty" minimises
+    the (weighted) sum of completion times plus the set_penalty penalty of every late task, with no stop at 0 (the
+    score of a non-empty plan is > 0).
 
     `rounds` device rounds are issued in groups of `exchange_every` (tournament resampling every
     `resample_every` rounds inside a group is only another launch); after each group the ranks exchange
@@ -272,8 +277,10 @@ def run_search(engine: Engine, chains: int = 1 << 16, rounds: int = 200, seed: i
     if record_history:
         history.append((time.perf_counter() - t0, chains * world, key_makespan(key)))
     exchange_every = max(1, int(exchange_every))
-    # a tardiness, late count or maximum tardiness (the SB_FLAG_DUE forms) of +0 (key bits 0) cannot be beaten
-    at_zero = bool(objective_flag(objective) & _lib.FLAG_DUE)
+    # a tardiness, late count or maximum tardiness (the SB_FLAG_DUE forms) of +0 (key bits 0) cannot be beaten; the
+    # completion penalty, also an SB_FLAG_DUE form, counts every completion time and never reaches +0
+    flags = objective_flag(objective)
+    at_zero = bool(flags & _lib.FLAG_DUE) and not (flags & _lib.FLAG_COMPLETION_PENALTY)
     reason = 3 if at_zero and (best_seen >> 32) == 0 else 0
     while reason == 0 and done_rounds < rounds:
         # one group of rounds, no host synchronisation; the library resamples on its own cadence

@@ -24,7 +24,7 @@ import os
 import time
 from collections import defaultdict
 from collections.abc import Mapping
-from typing import List, Optional, Sequence
+from typing import List, NamedTuple, Optional, Sequence
 
 import numpy as np
 
@@ -228,10 +228,10 @@ def _check_horizon(T, found_makespan=None, release=None, tails=None):
 
 def _check_objective(objective, hysteresis=False, release=None):
     if objective not in ("makespan", "completion", "tardiness", "max_lateness", "late_tasks", "max_stretch",
-                         "squared_tardiness", "squared_flow", "late_penalty"):
+                         "squared_tardiness", "squared_flow", "late_penalty", "completion_penalty"):
         raise SolverError("objective must be 'makespan', 'completion', 'tardiness', 'max_lateness', 'late_tasks', "
-                          "'max_stretch', 'squared_tardiness', 'squared_flow' or 'late_penalty', not %r"
-                          % (objective,))
+                          "'max_stretch', 'squared_tardiness', 'squared_flow', 'late_penalty' or "
+                          "'completion_penalty', not %r" % (objective,))
     if objective != "makespan" and hysteresis:
         raise SolverError("hysteresis=True compares plans by makespan (milp.py:363-442); it is not defined for "
                           "objective=%r" % (objective,))
@@ -264,9 +264,10 @@ def _resolve_weights(weights, objective, J, task_list=None):
     if objective == "max_stretch":
         raise SolverError("objective='max_stretch' weighs every task by 1 / its fastest runtime: it takes no weights "
                           "(for a weighted mean stretch use objective='completion' with weights)")
-    if objective not in ("completion", "tardiness", "late_tasks", "squared_tardiness", "squared_flow", "late_penalty"):
+    if objective not in ("completion", "tardiness", "late_tasks", "squared_tardiness", "squared_flow", "late_penalty",
+                         "completion_penalty"):
         raise SolverError("weights apply to objective='completion', 'tardiness', 'late_tasks', 'squared_tardiness', "
-                          "'squared_flow' or 'late_penalty' only, not to %r" % (objective,))
+                          "'squared_flow', 'late_penalty' or 'completion_penalty' only, not to %r" % (objective,))
     weights = _per_task(weights, "weights", task_list)
     from .engine import weights_f32
     w32 = weights_f32(weights, J)
@@ -281,15 +282,17 @@ def _resolve_weights(weights, objective, J, task_list=None):
 
 def _resolve_due(due, objective, J, task_list=None):
     """The caller's per-task due dates as (float64 values in task order, fp32 array for the device), or (None, None)
-    without objective="tardiness", "max_lateness", "late_tasks", "squared_tardiness" or "late_penalty", which require
-    them.  Raises SolverError before any device call."""
+    without objective="tardiness", "max_lateness", "late_tasks", "squared_tardiness", "late_penalty" or
+    "completion_penalty", which require them.  Raises SolverError before any device call."""
     if objective in ("max_stretch", "squared_flow") and due is not None:
         raise SolverError("objective=%r measures every task from its release date: it takes no due dates "
                           "(pass release=...)" % (objective,))
-    if objective not in ("tardiness", "max_lateness", "late_tasks", "squared_tardiness", "late_penalty"):
+    if objective not in ("tardiness", "max_lateness", "late_tasks", "squared_tardiness", "late_penalty",
+                         "completion_penalty"):
         if due is not None:
             raise SolverError("due dates apply to objective='tardiness', 'max_lateness', 'late_tasks', "
-                              "'squared_tardiness' or 'late_penalty' only, not to %r" % (objective,))
+                              "'squared_tardiness', 'late_penalty' or 'completion_penalty' only, not to %r"
+                              % (objective,))
         return None, None
     if due is None:
         raise SolverError("objective=%r needs due dates (due=...)" % (objective,))
@@ -304,13 +307,15 @@ def _resolve_due(due, objective, J, task_list=None):
 
 def _resolve_penalty(penalty, objective, J, task_list=None):
     """The caller's per-task late penalties as (float64 values in task order, fp32 array for the device), or
-    (None, None) without objective="late_penalty", which requires them.  Raises SolverError before any device call."""
-    if objective != "late_penalty":
+    (None, None) without objective="late_penalty" or "completion_penalty", which require them.  Raises SolverError
+    before any device call."""
+    if objective not in ("late_penalty", "completion_penalty"):
         if penalty is not None:
-            raise SolverError("penalties apply to objective='late_penalty' only, not to %r" % (objective,))
+            raise SolverError("penalties apply to objective='completion_penalty' or 'late_penalty' only, not to %r"
+                              % (objective,))
         return None, None
     if penalty is None:
-        raise SolverError("objective='late_penalty' needs the penalty of each missed due date (penalty=...)")
+        raise SolverError("objective=%r needs the penalty of each missed due date (penalty=...)" % (objective,))
     penalty = _per_task(penalty, "penalty", task_list)
     from .engine import penalty_f32
     p32 = penalty_f32(penalty, J)
@@ -347,8 +352,8 @@ def _set_objective(eng, objective, w32, d32, r32=None, p32=None):
             return "weighted_max_tardiness"
         if objective in _SQUARED:
             return "weighted_squared_tardiness" if w32 is not None else "squared_tardiness"
-        if objective == "late_penalty":
-            return "weighted_late_penalty" if w32 is not None else "late_penalty"
+        if objective in ("late_penalty", "completion_penalty"):
+            return "weighted_" + objective if w32 is not None else objective
         return "weighted_tardiness" if w32 is not None else "tardiness"
     return "weighted_completion" if w32 is not None else objective
 
@@ -430,6 +435,17 @@ def _late_penalty_stats(start, rts, w64, d64, p64):
     return stats
 
 
+def _completion_penalty_stats(start, rts, w64, d64, p64):
+    """completion_penalty, sum_t (w_t C_t + [C_t > d_t] p_t) (unit weights without w64), with weighted_completion,
+    late_tasks and penalty_paid, sum_t [C_t > d_t] p_t, of a plan in float64."""
+    w = w64 if w64 is not None else [1.0] * len(rts)
+    comp = [float(s) + float(r) for s, r in zip(start, rts)]
+    late = [c > d for c, d in zip(comp, d64)]
+    wc = sum(wi * c for wi, c in zip(w, comp))
+    paid = sum(p for p, x in zip(p64, late) if x)
+    return {"completion_penalty": wc + paid, "weighted_completion": wc, "late_tasks": sum(late), "penalty_paid": paid}
+
+
 def _squared_flow_stats(start, rts, w64, r64):
     """squared_flow, sum_t w_t (C_t - max(r_t, 0))^2 (unit weights without w64, r_t = 0 without r64), and
     total_flow_time, sum_t (C_t - max(r_t, 0)), of a plan in float64."""
@@ -473,7 +489,7 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
           timeout=500, *, chains: Optional[int] = None, rounds: Optional[int] = None, seed: int = 0,
           integer_starts: bool = True, engine=None, hysteresis: Optional[bool] = None,
           nodes: Optional[int] = None, devices=None, objective: str = "makespan", weights=None, due=None,
-          release=None, penalty=None):
+          release=None, penalty=None, _warm=None):
     """Drop-in for saturn.solver.solve (milp.py:23).
 
     Objective.  "makespan" (the default, the reference's) or "completion": minimise the sum of the tasks'
@@ -566,6 +582,18 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     ["late_tasks"] are recomputed in float64 from the emitted plan, the tasks' own runtimes and the caller's d, w and
     p; last_stats["device_makespan"] holds the device's fp32 score.  The 6th element stays the plan's makespan.
 
+    Completion penalty.  objective="completion_penalty" with `due` and `penalty` (as for "late_penalty") minimises
+    sum_t (w_t C_t + [C_t > d_t] p_t): the (weighted) completion time, as "completion" minimises it, plus a fixed
+    penalty for each missed due date (an SLA credit) that the late penalty's rate does not stand in for, since every
+    task's completion time already counts.  With every p = 0 it is "completion", plan for plan.  A task that
+    finishes exactly at its due date is on time, decided in fp32 as "late_penalty" decides it.  One due date H for
+    every task with every penalty above any sum_t w_t C_t makes it "minimise the mean completion time subject to a
+    makespan <= H" (solve_front runs it so).  The `due`, `weights`, `penalty` and `release` rules and errors are
+    those of "late_penalty", as is the refusal of hysteresis=True; there is no stop at zero.
+    last_stats["completion_penalty"], ["weighted_completion"] (unit weights without `weights`), ["late_tasks"] and
+    ["penalty_paid"] are recomputed in float64 from the emitted plan, the tasks' own runtimes and the caller's d, w
+    and p; last_stats["device_makespan"] holds the device's fp32 score.  The 6th element stays the plan's makespan.
+
     Release dates.  `release` (a sequence aligned with task_list, or a mapping keyed by Task, in the runtimes' units
     from the plan's t = 0) keeps every task from starting before its release date, under every objective: a
     dataset or a parent checkpoint that is only ready later, a job that arrives tomorrow.  r <= 0 means already
@@ -644,7 +672,7 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
         budget = min(budget, float(timeout))
     except (TypeError, ValueError):
         pass
-    warm = candidate_from_arrays(task_list, presolved, nodes)
+    warm = _warm if _warm is not None else candidate_from_arrays(task_list, presolved, nodes)
     res = run_search(eng, chains=chains, rounds=rounds, seed=seed, integer_starts=integer_starts, reduced=True,
                      time_budget_s=budget, patience=max(40, rounds // 4), warm=warm,
                      **({"objective": search_objective} if search_objective != "makespan" else {}))
@@ -688,6 +716,8 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
         last_stats.update(_squared_flow_stats(dec["start"], rts, w64, r64))
     elif objective == "late_penalty":
         last_stats.update(_late_penalty_stats(dec["start"], rts, w64, d64, p64))
+    elif objective == "completion_penalty":
+        last_stats.update(_completion_penalty_stats(dec["start"], rts, w64, d64, p64))
     elif d64 is not None:
         last_stats.update(_tardiness_stats(dec["start"], rts, w64, d64))
     if r64 is not None:
@@ -796,8 +826,8 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     (last_stats["total_flow_time"]).  objective="max_stretch" as for solve(), with p*_t the smallest cell of row t
     the search may propose, over every strategy (last_stats["max_stretch"] and ["mean_stretch"] from T's values).
     objective="squared_tardiness" (with `due`) and "squared_flow" as for solve(), with their last_stats from T's values.
-    objective="late_penalty" (with `due` and `penalty`, sequences aligned with T's rows) as for solve(), with its
-    last_stats from T's values.
+    objective="late_penalty" and "completion_penalty" (with `due` and `penalty`, sequences aligned with T's rows) as
+    for solve(), with their last_stats from T's values.
     Every cell of T must be
     >= 0 (-0.0 counts as zero), +inf or a sentinel: a negative or NaN cell raises SolverError, with or without `mask`.
 
@@ -893,11 +923,144 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
         last_stats.update(_squared_flow_stats(dec["start"], rts, w64, r64))
     elif objective == "late_penalty":
         last_stats.update(_late_penalty_stats(dec["start"], rts, w64, d64, p64))
+    elif objective == "completion_penalty":
+        last_stats.update(_completion_penalty_stats(dec["start"], rts, w64, d64, p64))
     elif d64 is not None:
         last_stats.update(_tardiness_stats(dec["start"], rts, w64, d64))
     if r64 is not None:
         last_stats.update(_flow_stats(dec["start"], rts, r64))
     return arrays + (makespan, strategy)
+
+
+# ------------------------------------------------------------------------------------------ front
+class FrontPoint(NamedTuple):
+    """One plan of solve_front: the makespan cap it was solved under (an fp32 value), its makespan and its (weighted)
+    sum of completion times (float64, the tasks' own runtimes), solve()'s 6-tuple and that solve's last_stats."""
+    cap: float
+    makespan: float
+    completion: float
+    plan: tuple
+    stats: dict
+
+
+def _plan_schedule(task_list, plan, T):
+    """The chosen option index, start (float64) and slot runtime (fp32, the device table T's cell) of every task of
+    a solve() plan."""
+    sta, tga, bss, bna, _boa, _mk = plan
+    opt = np.array([int(np.argmax(b)) for b in bss], dtype=np.int64)
+    node = np.array([int(np.argmax(b)) for b in bna], dtype=np.int64)
+    start = np.empty(len(task_list))
+    rt32 = np.empty(len(task_list), dtype=np.float32)
+    for t, task in enumerate(task_list):
+        k = int(list(task.strategies.keys())[opt[t]])
+        g = [i for i, v in enumerate(tga[t][node[t]]) if v == 1.0][0]
+        start[t] = sta[node[t]][g][t]
+        rt32[t] = T[t, 0, k - 1]
+    return opt, start, rt32
+
+
+def _device_makespan(task_list, plan, T):
+    """A plan's makespan in the device's arithmetic: max_t fp32(start_t + rt_t) over the fp32 starts and table cells,
+    the value the kernels' makespan and due-date comparisons see."""
+    _opt, start, rt32 = _plan_schedule(task_list, plan, T)
+    return float(np.max(start.astype(np.float32) + rt32))
+
+
+def _plan_candidate(task_list, plan, nodes):
+    """A solve() plan as the exact search candidate it was decoded from: reduced opt bytes and the list order that
+    boa records (candidate_from_arrays orders by start time instead, which need not list-schedule to the same
+    plan)."""
+    _sta, _tga, bss, bna, boa, _mk = plan
+    J = len(task_list)
+    opt = np.zeros(J, dtype=np.uint8)
+    for t, task in enumerate(task_list):
+        k = int(list(task.strategies.keys())[int(np.argmax(bss[t]))])
+        opt[t] = (k - 1) | ((int(np.argmax(bna[t])) << 3) if nodes > 1 else 0)
+    before = np.array([[v == 1.0 for v in row] for row in boa], dtype=bool)   # before[a][b]: a precedes b
+    return opt, np.argsort(before.sum(axis=0), kind="stable")
+
+
+def solve_front(task_list, points=8, weights=None, release=None, nodes=None, devices=None, seed=0,
+                integer_starts=True, timeout=500, engine=None, *, chains: Optional[int] = None,
+                rounds: Optional[int] = None, **refused):
+    """The trade-off between the makespan and the (weighted) sum of completion times: up to `points` plans, each the
+    best sum_t w_t C_t found under a makespan cap, sorted by makespan ascending with the sum strictly descending.
+
+    1. solve(objective="makespan"); its makespan in the device's fp32 arithmetic, M0, is the first cap.
+    2. solve(objective="completion") (with `weights`, the weighted sum); its fp32 makespan is M1.
+    3. For `points` - 2 caps evenly spaced strictly between M0 and M1 (fp32, ascending), solve(objective=
+       "completion_penalty") with every due date at the cap and every penalty P, the smallest power of two
+       >= sum_t w_t * 2^24 (the horizon every plan's times stay below): a plan over the cap then scores above every
+       plan that meets it, so this minimises the sum subject to makespan <= cap (the epsilon-constraint method).
+       Each search starts from the previous point's plan, which meets the larger cap.
+    4. Every plan is rescored in float64 and the dominated ones are dropped.
+    If M1 <= M0 the front is the completion plan alone.  Each point is a FrontPoint(cap, makespan, completion, plan,
+    stats): `plan` is solve()'s 6-tuple (convert_into_comprehensible takes it unchanged), `stats` that solve's
+    last_stats, `completion` the float64 sum_t w_t C_t (unit weights without `weights`).  A plan's float64 makespan
+    can exceed its fp32 cap by the rounding of the device's fp32 start + runtime (half an fp32 ulp of the cap).
+
+    `weights` and `release` as for solve(); `seed`, `integer_starts`, `timeout`, `engine`, `nodes`, `devices`,
+    `chains` and `rounds` go to every solve.  points < 2, `due`, `penalty`, `hysteresis` or `presolved`, weights
+    whose P breaks the penalty bound (J * P >= 2^126), and a plan whose fp32 makespan exceeds its cap raise
+    SolverError."""
+    if not isinstance(points, (int, np.integer)) or isinstance(points, bool) or points < 2:
+        raise SolverError("solve_front needs points >= 2, not %r" % (points,))
+    for name in ("due", "penalty", "hysteresis", "presolved"):
+        if name in refused:
+            raise SolverError("solve_front sets every due date and penalty itself and starts from its own plans: it "
+                              "takes no %s" % name)
+    if refused:
+        raise TypeError("solve_front() got unexpected keyword argument(s) %s" % ", ".join(sorted(refused)))
+    task_list = list(task_list)
+    J = len(task_list)
+    w64, w32 = _resolve_weights(weights, "completion", J, task_list)
+    _resolve_release(release, J, task_list)
+    if J == 0:
+        return []
+    wsum = float(np.sum(w32, dtype=np.float64)) if w32 is not None else float(J)
+    m, e = math.frexp(wsum * FP32_EXACT_HORIZON)
+    P = math.ldexp(1.0, e - 1 if m == 0.5 else e)
+    if not J * P < 2.0 ** 126:
+        raise SolverError("solve_front's penalty P = %g (the smallest power of two >= sum(weights) * 2^24) gives "
+                          "J * P >= 2^126; scale the weights down" % P)
+    nodes = int(_default_nodes() if nodes is None else nodes)
+    T, _usable, _optindex = build_table(task_list)
+    common = dict(seed=seed, integer_starts=integer_starts, timeout=timeout, engine=engine, nodes=nodes,
+                  devices=devices, chains=chains, rounds=rounds, release=release)
+
+    def run(objective, cap=None, **extra):
+        plan = solve(task_list, None, objective=objective, **common, **extra)
+        return (cap if cap is not None else _device_makespan(task_list, plan, T)), plan, dict(last_stats)
+
+    mk = run("makespan")
+    cp = run("completion", weights=weights)
+    if not cp[0] > mk[0]:
+        runs = [cp]
+    else:
+        caps = []
+        for i in range(1, points - 1):
+            c = float(np.float32(mk[0] + (cp[0] - mk[0]) * i / (points - 1)))
+            if mk[0] < c < cp[0] and (not caps or c > caps[-1]):
+                caps.append(c)
+        runs = [mk]
+        for c in caps:
+            runs.append(run("completion_penalty", cap=c, weights=weights, due=[c] * J, penalty=[P] * J,
+                            _warm=_plan_candidate(task_list, runs[-1][1], nodes)))
+            if _device_makespan(task_list, runs[-1][1], T) > c:
+                raise SolverError("solve_front: the plan for the makespan cap %r has fp32 makespan %r over its cap"
+                                  % (c, _device_makespan(task_list, runs[-1][1], T)))
+        runs.append(cp)
+    w = w64 if w64 is not None else [1.0] * J
+    found = []
+    for cap, plan, stats in runs:
+        opt, start, _rt32 = _plan_schedule(task_list, plan, T)
+        comp = [start[t] + float(list(task.strategies.values())[opt[t]].runtime) for t, task in enumerate(task_list)]
+        found.append(FrontPoint(cap, max(comp), sum(wi * c for wi, c in zip(w, comp)), plan, stats))
+    front = []
+    for p in sorted(found, key=lambda p: (p.makespan, p.completion)):
+        if not front or p.completion < front[-1].completion:
+            front.append(p)
+    return front
 
 
 # ------------------------------------------------------------------------------------------ decode

@@ -3,7 +3,7 @@ maximum lateness, of the (weighted) number of late tasks, of the maximum stretch
 prints one JSON line.
 
     python scripts/bench_objective.py [--steps 200] [--warmup 20] [--solve-chains 0] [--solve-rounds 400]
-                                      [--only max_stretch | squared | late_penalty]
+                                      [--only max_stretch | squared | late_penalty | completion_penalty]
 
 kernel: sb_eval on bench.py's C4 batch (J = 256, S = 8, 946,176 candidates, the same seeded inputs, integer
         starts), scored for the makespan, the sum of completion times, the weighted sum (seeded weights) and the
@@ -40,6 +40,10 @@ seeded integer penalties in [0, 100000) s), alternated as above, and runs only t
 256-task set with the seeded integer due dates of the late-count row and seeded integer penalties in [0, 100000),
 solve(objective="late_penalty") against the tardiness, late_tasks and completion plans, each rescored in float64 on
 the cost sum_t [C_t > d_t] (p_t + C_t - d_t), the late tasks and the tardiness.
+--only completion_penalty times only the weighted completion and the weighted completion penalty (the same weights,
+the due dates of the kernel rows, seeded integer penalties in [0, 100000) s), alternated as above, and runs only
+solve_front(points=8) on the 256-task set with the release dates of the stretch comparison: per point its cap, its
+makespan and its mean flow time (C_t - max(r_t, 0)) in float64, and the front's total wall time.
 The card's name and power limit are read in the same run (nvidia-smi, read-only queries).
 """
 import argparse
@@ -71,7 +75,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--solve-chains", type=int, default=0, help="0 = solve()'s default population")
     ap.add_argument("--solve-rounds", type=int, default=400)
-    ap.add_argument("--only", choices=("all", "max_stretch", "squared", "late_penalty"), default="all")
+    ap.add_argument("--only", choices=("all", "max_stretch", "squared", "late_penalty", "completion_penalty"),
+                    default="all")
     args = ap.parse_args()
     import numpy as np
     import torch
@@ -104,6 +109,9 @@ def main():
     if args.only == "late_penalty":
         objs = ("weighted_tardiness", "weighted_late_penalty")
         eng.set_penalty(np.random.default_rng(7).integers(0, 100000, size=J))
+    if args.only == "completion_penalty":
+        objs = ("weighted_completion", "weighted_completion_penalty")
+        eng.set_penalty(np.random.default_rng(7).integers(0, 100000, size=J))
     times = {o: [] for o in objs}
     for i in range(args.warmup + args.steps):
         for obj in objs[i % len(objs):] + objs[:i % len(objs)]:
@@ -120,6 +128,20 @@ def main():
     kernel = {o: {"median_ms": float(np.median(t)), "p10_ms": float(np.percentile(t, 10)),
                   "p90_ms": float(np.percentile(t, 90)), "candidates_per_s": B / (float(np.median(t)) * 1e-3)}
               for o, t in times.items()}
+    if args.only == "completion_penalty":
+        kernel["completion_penalty_over_weighted_completion"] = (kernel["weighted_completion_penalty"]["median_ms"] /
+                                                                 kernel["weighted_completion"]["median_ms"])
+        kernel.update(B=B, J=J, S=Sx, path=path, steps=args.steps)
+        del opt, prio, out
+        eng_r.close()
+        torch.cuda.empty_cache()
+        tasks = _tasks256()
+        kw = dict(rounds=args.solve_rounds, seed=1, engine=eng, **({"chains": args.solve_chains}
+                                                                   if args.solve_chains else {}))
+        makespan = S.solve(tasks, None, **kw)[5]
+        print(json.dumps({"card": card(0), "kernel": kernel, "front": front_effect(S, tasks, makespan, kw)}))
+        eng.close()
+        return
     if args.only == "late_penalty":
         kernel["late_penalty_over_weighted_tardiness"] = (kernel["weighted_late_penalty"]["median_ms"] /
                                                           kernel["weighted_tardiness"]["median_ms"])
@@ -306,6 +328,22 @@ def late_penalty_effect(S, R, tasks, kw):
                     "tardiness": sum(x for x, _p in late), "penalties_paid": sum(p for _x, p in late),
                     "makespan": max(comp), "wall_s": wall, "rounds": S.last_stats["rounds"]}
     return out
+
+
+def front_effect(S, tasks, makespan, kw):
+    """solve_front(points=8) on the 256-task set with the release dates of release_effect: per point the cap, the
+    makespan and the mean flow time in float64, and the front's wall time (see the module doc)."""
+    import numpy as np
+    J = len(tasks)
+    r = [float(x) for x in np.random.default_rng(6).integers(0, int(0.5 * makespan), size=J)]
+    S.solve_front(tasks, points=3, release=r, **dict(kw, rounds=4))   # first launches load the kernels
+    t0 = time.perf_counter()
+    front = S.solve_front(tasks, points=8, release=r, **kw)
+    wall = time.perf_counter() - t0
+    shift = sum(max(x, 0.0) for x in r)
+    return {"wall_s": wall, "points": [{"cap": p.cap, "makespan": p.makespan, "mean_flow": (p.completion - shift) / J,
+                                        "objective": p.stats["objective"], "rounds": p.stats["rounds"],
+                                        "solve_wall_s": p.stats["total_wall_s"]} for p in front]}
 
 
 def late_unit_effect(S, R, tasks, due, w, kw):
