@@ -271,6 +271,23 @@ typedef enum sb_status {
                                      it does not stop at 0, and sb_search_seed_lpt plants the completion orders (SPT,
                                      WSPT with SB_FLAG_WEIGHTED), not the EDD orders of SB_FLAG_DUE.  Not available
                                      with SB_FLAG_ALT_WARPSCAN (SB_ERR_UNSUPPORTED). */
+#define SB_FLAG_WORST_MAKESPAN 65536u /* after sb_set_scenarios (else SB_ERR_STATE): the objective is the worst makespan
+                                     over the K runtime scenarios, max_k M_k, where M_k is the makespan of the same
+                                     candidate (options and order, the list rule re-run) on scenario table k,
+                                     T_k[j][c] = fp32(f[k][j] * T[j][c]).  Not combinable with SB_FLAG_MEAN_MAKESPAN,
+                                     SB_FLAG_SUM_COMPLETION, SB_FLAG_WEIGHTED, SB_FLAG_DUE, SB_FLAG_MAX_LATENESS,
+                                     SB_FLAG_LATE_COUNT, SB_FLAG_MAX_TARDINESS, SB_FLAG_SQUARED, SB_FLAG_LATE_PENALTY or
+                                     SB_FLAG_COMPLETION_PENALTY (SB_ERR_ARG); valid with SB_FLAG_RELEASE and several
+                                     nodes.  The K tables must fit in one CTA's shared memory beside the release dates
+                                     and the node states (else SB_ERR_UNSUPPORTED).  Accepted by sb_eval, sb_eval_host,
+                                     sb_eval_full, sb_eval_scenarios, sb_decode and the search, sb_search_run_multi
+                                     included; sb_eval_full and sb_decode report the start times and GPU slots of the
+                                     nominal schedule (on T).  The search runs without incremental rounds, with the
+                                     makespan's temperature unit (the incumbent's score) and seeds.  Not available with
+                                     SB_FLAG_ALT_WARPSCAN (SB_ERR_UNSUPPORTED). */
+#define SB_FLAG_MEAN_MAKESPAN 131072u /* as SB_FLAG_WORST_MAKESPAN, but the score is the sum of the K makespans, the
+                                     left fold acc = acc + M_k (fp32, each add rounded) in scenario order from +0: K
+                                     times the mean makespan, with the same arg-min. */
 #define SB_IPC_HANDLE_BYTES 64
 
 typedef struct sb_handle sb_handle;
@@ -327,6 +344,12 @@ int sb_set_release(sb_handle* h, const float* r, int J);
  * before sb_set_table.  sb_set_table clears the penalties; setting or clearing them ends the current search
  * (sb_search_init again).  Their sum is recorded for the search's temperature unit. */
 int sb_set_penalty(sb_handle* h, const float* p, int J);
+/* Runtime scenarios for SB_FLAG_WORST_MAKESPAN and SB_FLAG_MEAN_MAKESPAN: f fp32 [K][J], host or device, one positive
+ * factor per scenario and job; scenario k's table is T_k[j][c] = fp32(f[k][j] * T[j][c]) for every cell of row j, of
+ * the full and of the reduced table alike (+inf stays +inf).  K outside 1..8, a J that differs from the table's, or a
+ * factor that is <= 0, NaN or inf is SB_ERR_ARG.  f = NULL clears them.  SB_ERR_STATE before sb_set_table.
+ * sb_set_table clears the scenarios; setting or clearing them ends the current search (sb_search_init again). */
+int sb_set_scenarios(sb_handle* h, const float* f, int K, int J);
 /* copy the reduced table back (host pointers, either may be NULL): tmin fp32 [J][8], args u8 [J][8].
  * This is the table the reference solver is actually given: Task.strategies[g] after the profiler's
  * min over executors (PerformanceEvaluator.py:101-115), read at milp.py:77-81. */
@@ -376,6 +399,10 @@ int sb_eval_host(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, 
  * may be NULL. */
 int sb_eval_full(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, int64_t row_stride,
                  unsigned flags, float* makespan_out, float* start_out, uint32_t* slotmask_out);
+/* Under SB_FLAG_WORST_MAKESPAN or SB_FLAG_MEAN_MAKESPAN (else SB_ERR_ARG): the slot-exact score of B candidates and
+ * every scenario's makespan M_k, makespans_out fp32 [B][K] (device pointers; score_out may be NULL). */
+int sb_eval_scenarios(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, int64_t row_stride,
+                      unsigned flags, float* score_out, float* makespans_out);
 
 /* decode ONE candidate given in host memory into host arrays (all [J]; any may be NULL) — everything
  * milp.py:330-352 extracts per task (start, occupied GPUs, selected option, node):

@@ -22,6 +22,8 @@ FLAG_MAX_TARDINESS = 4096
 FLAG_SQUARED = 8192
 FLAG_LATE_PENALTY = 16384
 FLAG_COMPLETION_PENALTY = 32768
+FLAG_WORST_MAKESPAN = 65536
+FLAG_MEAN_MAKESPAN = 131072
 IPC_HANDLE_BYTES = 64
 # test hooks in the top bits of the same flags word: the enum in csrc/sb_internal.h says what each one forces
 HOOK_FORCE_GENERIC = 0x80000000
@@ -44,7 +46,7 @@ TILE_DEBUG_NO_STAGGER = 4
 # every symbol include/saturn_b200.h declares (tests check that the library exports them all)
 SYMBOLS = [
     "sb_abi_version", "sb_last_error", "sb_create", "sb_destroy", "sb_sync", "sb_set_table",
-    "sb_set_sentinel", "sb_set_weights", "sb_set_due", "sb_set_release", "sb_set_penalty", "sb_get_reduced", "sb_eval", "sb_last_eval_path", "sb_validate", "sb_eval_host", "sb_eval_full",
+    "sb_set_sentinel", "sb_set_weights", "sb_set_due", "sb_set_release", "sb_set_penalty", "sb_set_scenarios", "sb_get_reduced", "sb_eval", "sb_last_eval_path", "sb_validate", "sb_eval_host", "sb_eval_full", "sb_eval_scenarios",
     "sb_decode", "sb_xchg_create", "sb_xchg_connect", "sb_xchg_connect_local", "sb_xchg_post", "sb_xchg_reduce", "sb_xchg_check",
     "sb_search_init", "sb_search_round", "sb_search_best_key_ptr", "sb_search_best",
     "sb_search_inject", "sb_search_resample", "sb_search_seed_lpt", "sb_search_run", "sb_search_run_multi", "sb_search_wave", "sb_search_is_fused", "sb_search_stats", "sb_search_validate", "sb_search_verify_count",
@@ -101,12 +103,14 @@ def load():
         "sb_set_due": [vp, vp, ci],
         "sb_set_release": [vp, vp, ci],
         "sb_set_penalty": [vp, vp, ci],
+        "sb_set_scenarios": [vp, vp, ci, ci],
         "sb_get_reduced": [vp, vp, vp],
         "sb_eval": [vp, vp, vp, i64, i64, u32, vp, vp, C.c_uint32],
         "sb_last_eval_path": [vp],
         "sb_validate": [vp, vp, vp, i64, i64, u32, C.POINTER(i64)],
         "sb_eval_host": [vp, vp, vp, i64, i64, u32, vp],
         "sb_eval_full": [vp, vp, vp, i64, i64, u32, vp, vp, vp],
+        "sb_eval_scenarios": [vp, vp, vp, i64, i64, u32, vp, vp],
         "sb_decode": [vp, vp, vp, u32, vp, vp, vp, vp, vp, vp],
         "sb_xchg_create": [vp, ci, ci, vp],
         "sb_xchg_connect": [vp, vp],

@@ -142,6 +142,14 @@ struct sb_handle {
   size_t d_p_cap = 0;
   double p_sum = 0.0;
   bool has_p = false;
+  // runtime scenarios (sb_set_scenarios): the K scaled copies of the full table ([K][J][S][8]) and of the reduced
+  // table ([K][J][8]), built on the device from the factors; has_f is cleared by sb_set_table
+  float* d_scen = nullptr;
+  float* d_scen_min = nullptr;
+  float* d_f = nullptr;  // the factors [K][J]
+  size_t d_scen_cap = 0, d_scen_min_cap = 0, d_f_cap = 0;
+  int scen_K = 0;
+  bool has_f = false;
   SearchState search;
   int last_path = -1;
   // peer-memory exchange
@@ -254,6 +262,9 @@ int sb_destroy(sb_handle* h) {
   cudaFree(h->dec_buf);
   cudaFree(h->stage_T);
   cudaFree(h->d_w);
+  cudaFree(h->d_f);
+  cudaFree(h->d_scen);
+  cudaFree(h->d_scen_min);
   cudaFree(h->d_d);
   cudaFree(h->d_one);
   cudaFree(h->d_q);
@@ -293,6 +304,7 @@ int sb_set_table(sb_handle* h, const float* T, const uint8_t* gcount, int J, int
   h->has_d = false;         // so do due dates
   h->has_r = false;         // and release dates
   h->has_p = false;         // and late penalties
+  h->has_f = false;         // and runtime scenarios
   const size_t nT = static_cast<size_t>(J) * S * G;
   const size_t ntab = static_cast<size_t>(J) * S * kSlots;
   // a re-planning loop sets a table of the same shape every interval: keep the allocations (cudaFree /
@@ -524,6 +536,51 @@ int sb_set_penalty(sb_handle* h, const float* p, int J) {
   return SB_OK;
 }
 
+// a device buffer of at least `bytes`, grown (contents dropped) when smaller
+static int grow(float** p, size_t* cap, size_t bytes) {
+  if (*cap >= bytes) return SB_OK;
+  cudaFree(*p);
+  *p = nullptr;
+  *cap = 0;
+  CK(cudaMalloc(p, bytes));
+  *cap = bytes;
+  return SB_OK;
+}
+
+int sb_set_scenarios(sb_handle* h, const float* f, int K, int J) {
+  int rc = use_device(h);
+  if (rc) return rc;
+  if (h->J == 0) return fail(SB_ERR_STATE, "sb_set_table has not been called");
+  CK(cudaStreamSynchronize(h->stream));  // no queued kernel may still read the old scenario tables
+  h->search.ready = false;               // the running search was set up for the old scenarios
+  if (!f) {
+    h->has_f = false;
+    return SB_OK;
+  }
+  if (K < 1 || K > 8) return fail(SB_ERR_ARG, "K=%d scenarios outside 1..8", K);
+  if (J != h->J) return fail(SB_ERR_ARG, "J=%d differs from the table's J=%d", J, h->J);
+  // host or device memory: the factors are checked on the host either way
+  const size_t n = static_cast<size_t>(K) * J;
+  std::vector<float> hf(n);
+  CK(cudaMemcpy(hf.data(), f, n * sizeof(float), cudaMemcpyDefault));
+  for (size_t i = 0; i < n; ++i)
+    if (!isfinite(hf[i]) || !(hf[i] > 0.f))
+      return fail(SB_ERR_ARG, "scenario %d, job %d: factor %g is not finite and > 0", static_cast<int>(i / J),
+                  static_cast<int>(i % J), hf[i]);
+  h->has_f = false;
+  const int SG = h->S * kSlots;
+  if ((rc = grow(&h->d_f, &h->d_f_cap, n * sizeof(float)))) return rc;
+  if ((rc = grow(&h->d_scen, &h->d_scen_cap, n * SG * sizeof(float)))) return rc;
+  if ((rc = grow(&h->d_scen_min, &h->d_scen_min_cap, n * kSlots * sizeof(float)))) return rc;
+  CK(cudaMemcpyAsync(h->d_f, hf.data(), n * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+  CK(scale_tables_launch(h->tab, J, SG, h->d_f, K, h->d_scen, h->stream));
+  CK(scale_tables_launch(h->tmin, J, kSlots, h->d_f, K, h->d_scen_min, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  h->scen_K = K;
+  h->has_f = true;
+  return SB_OK;
+}
+
 // The one reader of the objective flags.  SB_FLAG_WEIGHTED and SB_FLAG_DUE are valid with SB_FLAG_SUM_COMPLETION only;
 // SB_FLAG_MAX_LATENESS alone among the objective flags; SB_FLAG_LATE_COUNT, SB_FLAG_MAX_TARDINESS, SB_FLAG_SQUARED,
 // SB_FLAG_LATE_PENALTY and SB_FLAG_COMPLETION_PENALTY with SB_FLAG_SUM_COMPLETION | SB_FLAG_DUE only (they change what
@@ -534,6 +591,15 @@ static int decode_objective(unsigned flags, Objective* o) {
   const bool lateness = flags & SB_FLAG_MAX_LATENESS, late = flags & SB_FLAG_LATE_COUNT;
   const bool max_tardiness = flags & SB_FLAG_MAX_TARDINESS, squared = flags & SB_FLAG_SQUARED;
   const bool penalty = flags & SB_FLAG_LATE_PENALTY, completion_penalty = flags & SB_FLAG_COMPLETION_PENALTY;
+  const bool worst = flags & SB_FLAG_WORST_MAKESPAN, mean = flags & SB_FLAG_MEAN_MAKESPAN;
+  if (worst && mean)
+    return fail(SB_ERR_ARG, "SB_FLAG_WORST_MAKESPAN and SB_FLAG_MEAN_MAKESPAN are two objectives: pass one");
+  if ((worst || mean) && (sum || weighted || due || lateness || late || max_tardiness || squared || penalty ||
+                          completion_penalty))
+    return fail(SB_ERR_ARG, "%s scores makespans over runtime scenarios: it cannot be combined with "
+                "SB_FLAG_SUM_COMPLETION, SB_FLAG_WEIGHTED, SB_FLAG_DUE, SB_FLAG_MAX_LATENESS, SB_FLAG_LATE_COUNT, "
+                "SB_FLAG_MAX_TARDINESS, SB_FLAG_SQUARED, SB_FLAG_LATE_PENALTY or SB_FLAG_COMPLETION_PENALTY",
+                worst ? "SB_FLAG_WORST_MAKESPAN" : "SB_FLAG_MEAN_MAKESPAN");
   if (completion_penalty && !(sum && due))
     return fail(SB_ERR_ARG, "SB_FLAG_COMPLETION_PENALTY adds a fixed penalty per missed due date to the completion "
                 "time: it needs SB_FLAG_SUM_COMPLETION and SB_FLAG_DUE");
@@ -568,7 +634,9 @@ static int decode_objective(unsigned flags, Objective* o) {
   if (due && !sum)
     return fail(SB_ERR_ARG, "SB_FLAG_DUE scores the tardiness of the completion times: it needs SB_FLAG_SUM_COMPLETION");
   o->weighted = weighted;
-  if (lateness) o->obj = Obj::TailMakespan;
+  if (worst) o->obj = Obj::WorstMakespan;
+  else if (mean) o->obj = Obj::MeanMakespan;
+  else if (lateness) o->obj = Obj::TailMakespan;
   else if (!sum) o->obj = Obj::Makespan;
   else if (late) o->obj = Obj::LateCount;
   else if (max_tardiness) o->obj = Obj::MaxTardiness;
@@ -607,6 +675,18 @@ static int check_per_job(const sb_handle* h, unsigned flags, Objective* o) {
                 o->obj == Obj::CompletionPenalty ? "SB_FLAG_COMPLETION_PENALTY" : "SB_FLAG_LATE_PENALTY");
   if ((flags & SB_FLAG_RELEASE) && !h->has_r)
     return fail(SB_ERR_STATE, "SB_FLAG_RELEASE needs sb_set_release (sb_set_table clears the release dates)");
+  if (obj_scenario(o->obj)) {
+    const char* name = o->obj == Obj::WorstMakespan ? "SB_FLAG_WORST_MAKESPAN" : "SB_FLAG_MEAN_MAKESPAN";
+    if (!h->has_f) return fail(SB_ERR_STATE, "%s needs sb_set_scenarios (sb_set_table clears the scenarios)", name);
+    if (flags & SB_FLAG_ALT_WARPSCAN)
+      return fail(SB_ERR_UNSUPPORTED, "%s is not available with SB_FLAG_ALT_WARPSCAN", name);
+    const int SG = ((flags & SB_FLAG_REDUCED) ? 1 : h->S) * kSlots;
+    const size_t need = scenario_smem(h->J, SG, h->scen_K, h->nodes, flags);
+    if (need > h->dev.smem_optin)
+      return fail(SB_ERR_UNSUPPORTED, "%s: the %d scenario tables of %d x %d cells (%zu bytes with the release dates "
+                  "and node states) must fit in one CTA's shared memory (%zu bytes); pass SB_FLAG_REDUCED or fewer "
+                  "scenarios", name, h->scen_K, h->J, SG, need, h->dev.smem_optin);
+  }
   return SB_OK;
 }
 // the release dates the kernels read: ceiled under SB_FLAG_INTEGER_STARTS, as given otherwise, or none
@@ -653,6 +733,10 @@ static int make_call(sb_handle* h, const uint8_t* opt, const void* prio, int64_t
                 "(opt byte = (node << 3) | (k - 1))", h->nodes);
   c->nodes = h->nodes;
   c->tab = reduced ? h->tmin : h->tab;
+  if (obj_scenario(o.obj)) {
+    c->tab = reduced ? h->d_scen_min : h->d_scen;
+    c->K = h->scen_K;
+  }
   c->J = h->J;
   c->SG = (reduced ? 1 : h->S) * kSlots;
   c->opt = opt;
@@ -700,11 +784,13 @@ int sb_eval(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, int64
   // and score them with the position-major kernel, which keeps no tile and streams both rows.
   // HOOK_REORDER takes this route at any size.
   {
+    // the scenario forms take this route under HOOK_REORDER only: their tables fit the generic kernel's shared memory
     const bool hooks = (flags & (HOOK_FORCE_GENERIC | HOOK_NO_STREAM | HOOK_NO_REORDER | SB_FLAG_POST_KEY |
-                                 SB_FLAG_FOLD_PREV | SB_FLAG_ALT_WARPSCAN)) != 0;
+                                 SB_FLAG_FOLD_PREV | SB_FLAG_ALT_WARPSCAN)) != 0 ||
+                       (obj_scenario(c.obj) && !(flags & HOOK_REORDER));
     const bool aligned = row_stride % 32 == 0 && reinterpret_cast<uintptr_t>(opt) % 32 == 0 &&
                          reinterpret_cast<uintptr_t>(prio) % 32 == 0;
-    const int home = eval_pos_home(h->dev, c.J, c.SG, c.nodes, flags, c.obj);
+    const int home = eval_pos_home(h->dev, c.J, c.SG, c.nodes, flags, c.obj, c.K);
     if (!hooks && aligned && B > 0 && c.J <= 6144 && home >= 0 && (home != 0 || c.J >= 1024 || (flags & HOOK_REORDER))) {
       const size_t need = static_cast<size_t>(B) * static_cast<size_t>(row_stride);
       if (need > h->by_pos_bytes) {
@@ -780,6 +866,7 @@ int sb_validate(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, i
   rc = make_call(h, opt, prio, B, row_stride, flags, &c);
   if (rc) return rc;
   if (!bad_rows) return fail(SB_ERR_ARG, "bad_rows is null");
+  c.tab = (flags & SB_FLAG_REDUCED) ? h->tmin : h->tab;  // the cells a candidate selects exist in the nominal table
   CK(cudaMemsetAsync(h->d_scratch, 0, sizeof(unsigned long long), h->stream));
   CK(validate_launch(h->dev, c, h->d_scratch, h->stream));
   unsigned long long bad = 0;
@@ -787,6 +874,22 @@ int sb_validate(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, i
   CK(cudaStreamSynchronize(h->stream));
   *bad_rows = static_cast<int64_t>(bad);
   return SB_OK;
+}
+
+// The slot-exact kernel under any objective.  The scenario forms score on their tables, and their start times and slot
+// masks are those of the nominal schedule: the makespan form on the nominal table writes them.
+static cudaError_t eval_full_any(sb_handle* h, const EvalCall& c, float* start, uint32_t* slotmask, float* mks) {
+  if (!obj_scenario(c.obj)) return eval_full_launch(h->dev, c, start, slotmask, h->stream);
+  if (start || slotmask) {
+    EvalCall nominal = c;
+    nominal.obj = Obj::Makespan;
+    nominal.K = 0;
+    nominal.tab = (c.flags & SB_FLAG_REDUCED) ? h->tmin : h->tab;
+    nominal.out = nullptr;
+    cudaError_t e = eval_full_launch(h->dev, nominal, start, slotmask, h->stream);
+    if (e != cudaSuccess) return e;
+  }
+  return eval_full_scenarios_launch(h->dev, c, mks, h->stream);
 }
 
 int sb_eval_full(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, int64_t row_stride, unsigned flags,
@@ -797,7 +900,21 @@ int sb_eval_full(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, 
   rc = make_call(h, opt, prio, B, row_stride, flags, &c);
   if (rc) return rc;
   c.out = makespan_out;
-  CK(eval_full_launch(h->dev, c, start_out, slotmask_out, h->stream));
+  CK(eval_full_any(h, c, start_out, slotmask_out, nullptr));
+  return SB_OK;
+}
+
+int sb_eval_scenarios(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, int64_t row_stride, unsigned flags,
+                      float* score_out, float* makespans_out) {
+  int rc = use_device(h);
+  if (rc) return rc;
+  EvalCall c;
+  rc = make_call(h, opt, prio, B, row_stride, flags, &c);
+  if (rc) return rc;
+  if (!obj_scenario(c.obj)) return fail(SB_ERR_ARG, "sb_eval_scenarios needs SB_FLAG_WORST_MAKESPAN or SB_FLAG_MEAN_MAKESPAN");
+  if (B > 0 && !makespans_out) return fail(SB_ERR_ARG, "makespans_out is null");
+  c.out = score_out;
+  CK(eval_full_scenarios_launch(h->dev, c, makespans_out, h->stream));
   return SB_OK;
 }
 
@@ -880,7 +997,7 @@ int sb_decode(sb_handle* h, const uint8_t* opt, const void* prio, unsigned flags
   rc = make_call(h, d_opt, d_prio, 1, J, flags, &c);
   if (rc) return rc;
   c.out = d_mk;
-  CK(eval_full_launch(h->dev, c, d_start, d_mask, h->stream));
+  CK(eval_full_any(h, c, d_start, d_mask, nullptr));
   std::vector<float> hs(J);
   std::vector<uint32_t> hm(J);
   float mk = 0.f;
@@ -1057,6 +1174,16 @@ static int search_alloc(SearchState& s, void** p, size_t bytes) {
   return SB_OK;
 }
 
+// the tables the search's position-major kernel reads: the nominal table, or under the scenario forms the K scenario
+// tables (*K = their number)
+static const float* search_tables(const sb_handle* h, int* K) {
+  const SearchState& s = h->search;
+  const bool reduced = (s.p.flags & SB_FLAG_REDUCED) != 0;
+  *K = obj_scenario(s.obj.obj) ? h->scen_K : 0;
+  if (*K) return reduced ? h->d_scen_min : h->d_scen;
+  return reduced ? h->tmin : h->tab;
+}
+
 static int search_eval(sb_handle* h, bool cur_rows, long long first, long long count) {
   SearchState& s = h->search;
   if (s.d.pos) {  // position-major rows are only ever scored in place, by their own kernel
@@ -1064,9 +1191,11 @@ static int search_eval(sb_handle* h, bool cur_rows, long long first, long long c
     SearchFuse sf = {};
     sf.cur_mk = s.d.cur_mk;
     const bool reduced = (s.p.flags & SB_FLAG_REDUCED) != 0;
-    CK(search_pos_launch(h->dev, s.d, reduced ? h->tmin : h->tab, s.w, s.due, s.rel, s.pen,
+    int K = 0;
+    const float* tab = search_tables(h, &K);
+    CK(search_pos_launch(h->dev, s.d, tab, s.w, s.due, s.rel, s.pen,
                          (reduced ? 1 : h->S) * kSlots, s.p.flags,
-                         s.obj.obj, first, count, true, sf, h->stream));
+                         s.obj.obj, first, count, true, sf, h->stream, 0, K));
     return SB_OK;
   }
   EvalCall c;
@@ -1148,8 +1277,13 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
   // Rows that do not fit in shared memory: keep the population in schedule order and stream both rows.
   const int SGs = (reduced ? 1 : h->S) * kSlots;
   const bool no_fused = (p->flags & HOOK_NO_FUSED) != 0;
-  const int mode = search_round_mode(h->dev, J, SGs, h->nodes, arrays);
-  d.pos = (!no_fused && mode != 2 && search_pos_smem(J, SGs, h->nodes, 16, arrays) <= h->dev.smem_optin) ? 1 : 0;
+  // the scenario forms have no tile kernel: their population is always position-major (check_per_job has held their
+  // tables to the position-major kernel's shared memory), or unfused under HOOK_NO_FUSED
+  const bool scen = obj_scenario(o.obj);
+  const int mode = scen ? 0 : search_round_mode(h->dev, J, SGs, h->nodes, arrays);
+  const size_t pos_smem = scen ? scenario_smem(J, SGs, h->scen_K, h->nodes, p->flags)
+                               : search_pos_smem(J, SGs, h->nodes, 16, arrays);
+  d.pos = (!no_fused && mode != 2 && pos_smem <= h->dev.smem_optin) ? 1 : 0;
   if (d.pos) CK(search_init_population_pos(d, h->stream));
   else CK(search_init_population(d, h->stream));
   s.ready = true;
@@ -1231,7 +1365,9 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
     nwin = (nout + wblk - 1) / wblk;
   }
   s.win = s.fused_ok && h->nodes == 1 && nwin >= 2 && nwin <= 32 && !(p->flags & HOOK_ROUND1_MOVES);
-  s.inc = s.win && !(p->flags & HOOK_NO_INCREMENTAL);
+  // the scenario forms score every proposal from position 0, as HOOK_NO_INCREMENTAL does (K snapshot sets per window
+  // boundary are not kept)
+  s.inc = s.win && !(p->flags & HOOK_NO_INCREMENTAL) && !scen;
   s.verify = s.inc && (p->flags & HOOK_VERIFY_INCREMENTAL);
   // automatic cadence: resampling is nearly free inside the tile kernel; elsewhere it is a full copy of the
   // population and ends a launch (an incremental launch starts with one unmodified pass, so longer is better)
@@ -1320,9 +1456,11 @@ int sb_search_round(sb_handle* h, int rounds) {
       SearchFuse sf = make_fuse(s, round, n);
       sf.resample_every = 0;
       const bool reduced = (s.p.flags & SB_FLAG_REDUCED) != 0;
-      CK(search_pos_launch(h->dev, s.d, reduced ? h->tmin : h->tab, s.w, s.due, s.rel, s.pen,
+      int K = 0;
+      const float* tab = search_tables(h, &K);
+      CK(search_pos_launch(h->dev, s.d, tab, s.w, s.due, s.rel, s.pen,
                          (reduced ? 1 : h->S) * kSlots, s.p.flags,
-                           s.obj.obj, 0, s.d.chains, false, sf, h->stream));  // keeps the incumbent in its tail
+                           s.obj.obj, 0, s.d.chains, false, sf, h->stream, 0, K));  // keeps the incumbent in its tail
       fused = true;
     } else if (s.fused_ok) {
       EvalCall c;
@@ -1488,7 +1626,8 @@ int sb_search_seed_lpt(sb_handle* h) {
   const float* tmin = h->h_tmin.data();
   const Obj obj = s.obj.obj;
   // shortest first: the order that favours the sum (and, below, the tie-break of the due-date orders)
-  const bool spt = obj != Obj::Makespan && obj != Obj::TailMakespan;
+  // the scenario forms seed as the makespan does, on the nominal table
+  const bool spt = obj != Obj::Makespan && obj != Obj::TailMakespan && !obj_scenario(obj);
   // weighted sum: Smith's rule (WSPT), ascending rt / w; with unit weights exactly the SPT order
   const bool wspt = spt && s.obj.weighted;
   // the due-date objectives: earliest due date first (EDD), ties by rt / w (rt with unit weights), then by job index;
@@ -1776,7 +1915,9 @@ int sb_search_wave(sb_handle* h, unsigned flags, int64_t* chains) {
   const int arrays = job_arrays(o.obj, flags);
   int warps = 0;
   TilePlan tp;
-  if (search_round_mode(h->dev, h->J, SG, h->nodes, arrays) == 2) {
+  if (obj_scenario(o.obj)) {  // the position-major kernel, 16 warps per CTA (sb_search_init)
+    warps = 16;
+  } else if (search_round_mode(h->dev, h->J, SG, h->nodes, arrays) == 2) {
     plan_tiles(h->dev, h->J, SG, pb, false, h->nodes, &tp, false, arrays);
     warps = tp.warps;
   } else if (search_pos_smem(h->J, SG, h->nodes, 16, arrays) <= h->dev.smem_optin) {

@@ -33,12 +33,23 @@ __device__ __forceinline__ float inf_f() { return __int_as_float(0x7f800000); }
 //   LatePenalty       SUM_COMPLETION | DUE | LATE_PENALTY [| WEIGHTED]   sum (C > d ? p + w (C - d) : 0)
 //   CompletionPenalty SUM_COMPLETION | DUE | COMPLETION_PENALTY [| WEIGHTED]
 //                                                                        sum (w C + (C > d ? p : 0))
+//   WorstMakespan     WORST_MAKESPAN                                     max_k M_k, M_k the makespan on scenario table k
+//   MeanMakespan      MEAN_MAKESPAN                                      sum_k M_k, left fold in scenario order
 // Every other combination of those flags is refused.  The history of each form is in DESIGN.md.  New forms go at the
 // end: a kernel's symbol holds its form's value.
 enum class Obj {
   Makespan, TailMakespan, Sum, WeightedSum, Tardiness, LateCount, MaxTardiness, SquaredTardiness, LatePenalty,
-  CompletionPenalty
+  CompletionPenalty, WorstMakespan, MeanMakespan
 };
+// the score folds the makespans of K scenario tables (sb_set_scenarios); each pass is the makespan form's
+__host__ __device__ constexpr bool obj_scenario(Obj o) { return o == Obj::WorstMakespan || o == Obj::MeanMakespan; }
+// the form ls_step folds inside one pass: the makespan for the scenario forms, the objective itself otherwise
+__host__ __device__ constexpr Obj step_obj(Obj o) { return obj_scenario(o) ? Obj::Makespan : o; }
+// one scenario's makespan m folded into the score: an exact max, or a sum rounded at every add (both start at +0)
+template <Obj kObj>
+__device__ __forceinline__ float scenario_fold(float score, float m) {
+  return kObj == Obj::WorstMakespan ? fmaxf(score, m) : __fadd_rn(score, m);
+}
 // the score is a sum over the jobs, folded in schedule order
 __host__ __device__ constexpr bool obj_sum(Obj o) {
   return o == Obj::Sum || o == Obj::WeightedSum || o == Obj::Tardiness || o == Obj::LateCount ||

@@ -673,23 +673,58 @@ struct GenericArgs {
   const float* d;  // obj_due(OBJ): job due dates (or tails) [J], likewise
   const float* r;  // R: job release dates [J], likewise
   const float* p;  // obj_penalty(OBJ): job late penalties [J], likewise
+  int K;           // obj_scenario(OBJ): the scenario tables at tab, [K][J][SG] (last: the other fields keep their offsets)
+  int pad;         // keeps the struct free of implicit padding: a padding hole changes the code of every kernel taking it
 };
 
+// One pass of the scenario forms over a candidate's J steps on the table st.tab points to: the batched loop of
+// k_eval_generic below, with the makespan form's step (whose kernels keep their own copy of the loop, so that their
+// code stays what it was).
+template <int PB, Obj OBJ, bool R, class Lane>
+__device__ __forceinline__ float generic_pass(Lane& st, const GenericArgs& a, const uint8_t* prow) {
+  static_assert(obj_scenario(OBJ), "the scenario forms only");
+  st.reset(a.nodes);
+  constexpr int BATCH = 16;
+  int i = 0;
+  for (; i + BATCH <= a.J; i += BATCH) {
+    int js[BATCH], os[BATCH];
+    float rts[BATCH];
+    [[maybe_unused]] float xs[BATCH];
+#pragma unroll
+    for (int t = 0; t < BATCH; ++t) js[t] = PB == 1 ? prow[i + t] : reinterpret_cast<const uint16_t*>(prow)[i + t];
+#pragma unroll
+    for (int t = 0; t < BATCH; ++t) os[t] = st.lookup_opt(js[t]);
+#pragma unroll
+    for (int t = 0; t < BATCH; ++t) rts[t] = st.lookup_rt(js[t], os[t]);
+    if constexpr (R) {
+#pragma unroll
+      for (int t = 0; t < BATCH; ++t) xs[t] = st.lookup_r(js[t]);
+    }
+#pragma unroll
+    for (int t = 0; t < BATCH; ++t) st.step_resolved(os[t], rts[t], t & 1, 0.f, 0.f, R ? xs[t] : 0.f, 0.f);
+  }
+  for (; i < a.J; ++i) st.step(PB == 1 ? prow[i] : reinterpret_cast<const uint16_t*>(prow)[i]);
+  return st.result(a.nodes);
+}
+
+// obj_scenario(OBJ): each lane runs its candidate's J steps once per scenario table, with the makespan form's step,
+// and folds the K makespans into the score (scenario_fold); one slot state, whatever K.
 template <int PB, bool INT, bool MULTI, Obj OBJ = Obj::Makespan, bool R = false>
 __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
   extern __shared__ __align__(128) uint8_t smem[];
+  constexpr bool kScen = obj_scenario(OBJ);
   const float* tab = a.tab;
   const uint32_t node_bytes = MULTI ? static_cast<uint32_t>(a.nodes) * 1024u : 0u;  // per warp
   float4* node_s = reinterpret_cast<float4*>(smem) + (threadIdx.x >> 5) * (node_bytes / 16);
   if (a.tab_in_smem) {
     float* tab_s = reinterpret_cast<float*>(smem + (blockDim.x >> 5) * node_bytes);
-    const int n = a.J * a.SG;
+    const int n = kScen ? a.J * a.SG * a.K : a.J * a.SG;
     for (int i = threadIdx.x; i < n; i += blockDim.x) tab_s[i] = a.tab[i];
     __syncthreads();
     tab = tab_s;
   }
   const int lane = threadIdx.x & 31;
-  LaneState<INT, MULTI, 0, OBJ, 2, R> st;
+  LaneState<INT, MULTI, 0, step_obj(OBJ), 2, R> st;
   st.tab = tab;
   st.wt = a.w;
   st.dd = a.d;
@@ -706,6 +741,12 @@ __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
     if (active) {
       st.orow = a.opt + b * a.stride_o;
       const uint8_t* prow = a.prio + b * a.stride_p;
+      if constexpr (kScen) {
+        for (int k = 0; k < a.K; ++k) {
+          st.tab = tab + static_cast<size_t>(k) * a.J * a.SG;
+          mk = scenario_fold<OBJ>(mk, generic_pass<PB, OBJ, R>(st, a, prow));
+        }
+      } else {
       st.reset(a.nodes);
       // batches of 16 positions: 16 independent opt loads, then 16 independent table loads, then the
       // 16 dependent scheduling steps — the global-memory latency is paid once per batch
@@ -745,6 +786,7 @@ __global__ void __launch_bounds__(128) k_eval_generic(const GenericArgs a) {
       }
       for (; i < a.J; ++i) st.step(PB == 1 ? prow[i] : reinterpret_cast<const uint16_t*>(prow)[i]);
       mk = st.result(a.nodes);
+      }
       a.out[b] = mk;
     }
     if (a.best_key != nullptr) fold_best(a.best_key, active, mk, a.id_base + static_cast<uint32_t>(b), lane);
@@ -772,12 +814,75 @@ struct FullArgs {
   const float* d;       // obj_due(OBJ): job due dates [J] (TailMakespan: the delivery tails)
   const float* r;       // R: job release dates [J] (ceiled with INT)
   const float* p;       // obj_penalty(OBJ): job late penalties [J]
+  int K;                // obj_scenario(OBJ): the scenario tables at tab, [K][J][SG] (last: the other fields keep their
+                        // offsets); `start` (nullable) then receives every scenario's makespan, [B][K]
+  int pad;              // keeps the struct free of implicit padding: a padding hole changes the code of every kernel
+                        // taking it
 };
 
 // The score is folded here on its own, not through ls_step: this kernel is the library's slot-exact cross-check of
 // the fast kernels, so it restates every objective's fold (in the same fp32 operations).
 template <int PB, bool INT, Obj OBJ = Obj::Makespan, bool R = false>
+__global__ void __launch_bounds__(128) k_eval_full(const FullArgs a);
+
+// obj_scenario(OBJ): the slot-exact makespan of each scenario table (start times and slot masks are not written: the
+// host takes them from the makespan form on the nominal table), M_k into a.start ([B][K]), folded into the score in
+// scenario order
+template <int PB, bool INT, Obj OBJ, bool R>
+__device__ __forceinline__ void eval_full_scenarios(const FullArgs& a) {
+  const long long nthreads = static_cast<long long>(gridDim.x) * blockDim.x;
+  const bool multi = a.nodes > 1;
+  for (long long b = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; b < a.B; b += nthreads) {
+    const uint8_t* orow = a.opt + b * a.stride_o;
+    const uint8_t* prow = a.prio + b * a.stride_p;
+    float score = 0.f;
+    for (int sc = 0; sc < a.K; ++sc) {
+      const float* tab = a.tab + static_cast<size_t>(sc) * a.J * a.SG;
+      float ready[kMaxNodes * kSlots];
+      for (int g = 0; g < a.nodes * kSlots; ++g) ready[g] = 0.f;
+      float mk = 0.f;
+      for (int i = 0; i < a.J; ++i) {
+        const int j = PB == 1 ? prow[i] : reinterpret_cast<const uint16_t*>(prow)[i];
+        const int o = orow[j];
+        const int k = (o & 7) + 1;
+        const int node = multi ? (o >> 3) : 0;
+        const float rt = __ldg(tab + static_cast<size_t>(j) * a.SG + (multi ? (o & 7) : o));
+        float* rd = ready + node * kSlots;
+        uint32_t taken = 0;
+        float s = 0.f;
+        for (int q = 0; q < k; ++q) {
+          int best = -1;
+          float bv = 0.f;
+          for (int g = 0; g < kSlots; ++g) {
+            const bool free_slot = ((taken >> g) & 1u) == 0u;
+            if (free_slot && (best < 0 || rd[g] < bv)) {
+              best = g;
+              bv = rd[g];
+            }
+          }
+          taken |= 1u << best;
+          s = bv;
+        }
+        if constexpr (R) s = fmaxf(s, __ldg(a.r + j));
+        const float hold = (INT && isfinite(rt)) ? ceilf(rt) : rt;
+        const float nxt = s + hold;
+        for (int g = 0; g < kSlots; ++g)
+          if ((taken >> g) & 1u) rd[g] = nxt;
+        mk = fmaxf(mk, s + rt);
+      }
+      if (a.start) a.start[b * a.K + sc] = mk;
+      score = scenario_fold<OBJ>(score, mk);
+    }
+    if (a.out) a.out[b] = score;
+  }
+}
+
+template <int PB, bool INT, Obj OBJ, bool R>
 __global__ void __launch_bounds__(128) k_eval_full(const FullArgs a) {
+  if constexpr (obj_scenario(OBJ)) {
+    eval_full_scenarios<PB, INT, OBJ, R>(a);
+    return;
+  } else {
   const long long nthreads = static_cast<long long>(gridDim.x) * blockDim.x;
   const bool multi = a.nodes > 1;
   for (long long b = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; b < a.B; b += nthreads) {
@@ -841,6 +946,7 @@ __global__ void __launch_bounds__(128) k_eval_full(const FullArgs a) {
       if (a.slotmask) a.slotmask[b * a.J + j] = (static_cast<uint32_t>(node) << 16) | taken;
     }
     if (a.out) a.out[b] = mk;
+  }
   }
 }
 
@@ -953,7 +1059,8 @@ cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, i
   TilePlan tp;
   int nw = 0;
   bool stream = false, tabg = false;
-  if (!c.force_generic) {
+  const bool scen = obj_scenario(c.obj);  // the tile kernels have no scenario forms: the generic kernel scores them
+  if (!c.force_generic && !scen) {
     if (stream_ok) {
       nw = plan_tiles(dev, c.J, c.SG, pb, true, c.nodes, &tp, false, arrays);
       stream = nw >= 2 && c.stride_o >= tp.copy_o && c.stride_p >= ((c.J * pb + 31) & ~31);
@@ -997,10 +1104,13 @@ cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, i
   g.stride_o = c.stride_o; g.stride_p = c.stride_p; g.out = c.out; g.best_key = c.best_key;
   g.id_base = c.id_base; g.tab_in_smem = 0; g.nodes = c.nodes; g.one = 1; g.w = c.w; g.d = c.d; g.r = c.r;
   g.p = c.p;
+  g.K = c.K;
+  g.pad = 0;
   if (path_used) *path_used = 0;
-  const size_t tab_bytes = static_cast<size_t>(c.J) * c.SG * 4;
+  // the scenario tables always fit (check_per_job holds them to scenario_smem, which asks for more than this)
+  const size_t tab_bytes = static_cast<size_t>(c.J) * c.SG * 4 * (scen ? c.K : 1);
   size_t smem = multi ? static_cast<size_t>(4) * c.nodes * 1024u : 0u;  // 4 warps per CTA
-  if (tab_bytes <= dev.smem_optin / 2) {
+  if (tab_bytes <= dev.smem_optin / 2 || scen) {
     g.tab_in_smem = 1;
     smem += tab_bytes;
   }
@@ -1008,9 +1118,11 @@ cudaError_t eval_launch(const Device& dev, const EvalCall& c, cudaStream_t st, i
   long long cap = static_cast<long long>(dev.sm_count) * 8;
   int grid = static_cast<int>(blocks < cap ? blocks : cap);
   if (grid < 1) grid = 1;
-  const auto kern = with_eval_types(pb, c.flags, c.obj, [&](auto PB, auto INT, auto OBJ, auto R) {
-    return with_bool(multi, [&](auto MULTI) { return k_eval_generic<PB, INT, MULTI, OBJ, R>; });
-  });
+  using GenericKernel = void (*)(GenericArgs);
+  const auto pick = [&](auto PB, auto INT, auto OBJ, auto R) -> GenericKernel {
+    return with_bool(multi, [&](auto MULTI) -> GenericKernel { return k_eval_generic<PB, INT, MULTI, OBJ, R>; });
+  };
+  const GenericKernel kern = scen ? with_scenario_types(pb, c.flags, c.obj, pick) : with_eval_types(pb, c.flags, c.obj, pick);
   return launch(kern, grid, 128, smem, st, g);
 }
 
@@ -1053,13 +1165,33 @@ cudaError_t eval_full_launch(const Device& dev, const EvalCall& c, float* start,
   a.stride_o = c.stride_o; a.stride_p = c.stride_p; a.nodes = c.nodes < 1 ? 1 : c.nodes;
   a.out = c.out; a.start = start; a.slotmask = slotmask; a.w = c.w; a.d = c.d; a.r = c.r;
   a.p = c.p;
+  a.K = c.K;
+  a.pad = 0;
   long long blocks = (c.B + 127) / 128;
   long long cap = static_cast<long long>(dev.sm_count) * 16;
   int grid = static_cast<int>(blocks < cap ? blocks : cap);
-  const auto kern = with_eval_types(pb, c.flags, c.obj, [](auto PB, auto INT, auto OBJ, auto R) {
-    return k_eval_full<PB, INT, OBJ, R>;
-  });
-  return launch(kern, grid, 128, 0, st, a);
+  using FullKernel = void (*)(FullArgs);
+  const auto pick = [](auto PB, auto INT, auto OBJ, auto R) -> FullKernel { return k_eval_full<PB, INT, OBJ, R>; };
+  if (obj_scenario(c.obj)) return cudaErrorInvalidValue;  // eval_full_scenarios_launch
+  return launch(with_eval_types(pb, c.flags, c.obj, pick), grid, 128, 0, st, a);
+}
+
+cudaError_t eval_full_scenarios_launch(const Device& dev, const EvalCall& c, float* mks, cudaStream_t st) {
+  if (c.B <= 0) return cudaSuccess;
+  if (!obj_scenario(c.obj)) return cudaErrorInvalidValue;
+  const int pb = c.J <= 256 ? 1 : 2;
+  FullArgs a = {};
+  a.tab = c.tab; a.J = c.J; a.SG = c.SG; a.opt = c.opt; a.prio = c.prio; a.B = c.B;
+  a.stride_o = c.stride_o; a.stride_p = c.stride_p; a.nodes = c.nodes < 1 ? 1 : c.nodes;
+  a.out = c.out; a.r = c.r;
+  a.K = c.K;
+  a.start = mks;
+  long long blocks = (c.B + 127) / 128;
+  long long cap = static_cast<long long>(dev.sm_count) * 16;
+  int grid = static_cast<int>(blocks < cap ? blocks : cap);
+  using FullKernel = void (*)(FullArgs);
+  const auto pick = [](auto PB, auto INT, auto OBJ, auto R) -> FullKernel { return k_eval_full<PB, INT, OBJ, R>; };
+  return launch(with_scenario_types(pb, c.flags, c.obj, pick), grid, 128, 0, st, a);
 }
 
 cudaError_t validate_launch(const Device& dev, const EvalCall& c, unsigned long long* bad, cudaStream_t st, bool by_pos) {

@@ -33,7 +33,8 @@ static_assert(((HOOK_FORCE_GENERIC | HOOK_NO_STREAM | HOOK_NO_FUSED | HOOK_NO_IN
                (SB_FLAG_INTEGER_STARTS | SB_FLAG_REDUCED | SB_FLAG_OPT_BY_POSITION | SB_FLAG_POST_KEY |
                 SB_FLAG_FOLD_PREV | SB_FLAG_ALT_WARPSCAN | SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED |
                 SB_FLAG_DUE | SB_FLAG_RELEASE | SB_FLAG_MAX_LATENESS | SB_FLAG_LATE_COUNT |
-                SB_FLAG_MAX_TARDINESS | SB_FLAG_SQUARED | SB_FLAG_LATE_PENALTY | SB_FLAG_COMPLETION_PENALTY)) == 0,
+                SB_FLAG_MAX_TARDINESS | SB_FLAG_SQUARED | SB_FLAG_LATE_PENALTY | SB_FLAG_COMPLETION_PENALTY |
+                SB_FLAG_WORST_MAKESPAN | SB_FLAG_MEAN_MAKESPAN)) == 0,
               "the test hooks share no bit with the SB_FLAG_* flags");
 
 // Debug options of the streamed tile kernel (sb_debug_tile_options): kept on the handle, not in the flags word, and
@@ -79,6 +80,19 @@ decltype(auto) with_eval_types(int pb, unsigned flags, Obj obj, F&& f) {
     return with_bool(flags & SB_FLAG_INTEGER_STARTS, [&](auto INT) {
       return with_bool(flags & SB_FLAG_RELEASE, [&](auto R) {
         return with_obj(obj, [&](auto OBJ) { return f(PB, INT, OBJ, R); });
+      });
+    });
+  });
+}
+// The scenario forms run on k_eval_generic, k_eval_full and k_search_pos only, never on the tile kernels: with_obj
+// above does not name them, and their launch sites dispatch with this instead.
+template <class F>
+decltype(auto) with_scenario_types(int pb, unsigned flags, Obj obj, F&& f) {
+  return with_pb(pb, [&](auto PB) {
+    return with_bool(flags & SB_FLAG_INTEGER_STARTS, [&](auto INT) {
+      return with_bool(flags & SB_FLAG_RELEASE, [&](auto R) {
+        return obj == Obj::WorstMakespan ? f(PB, INT, obj_c<Obj::WorstMakespan>{}, R)
+                                         : f(PB, INT, obj_c<Obj::MeanMakespan>{}, R);
       });
     });
   });
@@ -137,7 +151,9 @@ struct TilePlan {
 };
 
 struct EvalCall {
-  const float* tab = nullptr;  // canonical table actually used (full or reduced)
+  const float* tab = nullptr;  // canonical table actually used (full or reduced); obj_scenario(obj): the K scaled
+                               // copies of it, scenario-major [K][J][SG]
+  int K = 0;                   // obj_scenario(obj): the number of scenario tables
   const float* w = nullptr;    // obj_weights(obj): the job weights [J], padded with zeros to a multiple of 4 (unit
                                // weights without SB_FLAG_WEIGHTED)
   const float* d = nullptr;    // obj_due(obj): the job due dates [J] (TailMakespan: the delivery tails max_t d_t - d_j),
@@ -212,6 +228,8 @@ cudaError_t eval_alt_launch(const Device& dev, const EvalCall& c, cudaStream_t s
 int search_round_mode(const Device& dev, int J, int SG, int nodes, int arrays = 0);
 cudaError_t search_round_launch(const Device& dev, const EvalCall& c, const SearchFuse& sf, cudaStream_t st);
 cudaError_t eval_full_launch(const Device& dev, const EvalCall& c, float* start, uint32_t* slotmask, cudaStream_t st);
+// the scenario forms of k_eval_full: the score into c.out and (mks != nullptr) every scenario's makespan, [B][K]
+cudaError_t eval_full_scenarios_launch(const Device& dev, const EvalCall& c, float* mks, cudaStream_t st);
 cudaError_t validate_launch(const Device& dev, const EvalCall& c, unsigned long long* bad, cudaStream_t st,
                             bool by_pos = false);
 
@@ -221,5 +239,11 @@ cudaError_t build_table_launch(const float* T, int J, int S, int G, uint64_t gco
 // valid (non-dominated, non-sentinel) option lists for the search: vopt[J][8] opt bytes, nvalid[J]
 cudaError_t build_valid_launch(const float* tmin, const uint8_t* args, int J, int reduced, float sentinel, uint8_t* vopt,
                                int* nvalid, cudaStream_t st);
+// scenario tables: out[k][j][c] = fp32(f[k][j] * tab[j][c]) for the K factor rows f[K][J] (device) and a table of J
+// rows of SG cells
+cudaError_t scale_tables_launch(const float* tab, int J, int SG, const float* f, int K, float* out, cudaStream_t st);
+// shared memory the position-major kernel needs for K scenario tables of J x SG cells beside what it already stages;
+// every scenario route is held to it (sb_api.cu: check_per_job)
+size_t scenario_smem(int J, int SG, int K, int nodes, unsigned flags);
 
 }  // namespace sb

@@ -332,6 +332,8 @@ struct PosArgs {
   const float* d;  // obj_due(OBJ): job due dates (or tails) [J], padded the same way
   const float* r;  // R: job release dates [J], padded the same way
   const float* p;  // obj_penalty(OBJ): job late penalties [J], padded the same way
+  int K;           // obj_scenario(OBJ): the scenario tables at tab, [K][J][SG] (last: the other fields keep their offsets)
+  int pad;         // keeps the struct free of implicit padding: a padding hole changes the code of every kernel taking it
 };
 
 struct PosMove {
@@ -425,14 +427,19 @@ __device__ __forceinline__ PosMove make_pos_move_win(const SearchFuse& sf, int r
 // alternative to 1, kept behind a test hook.
 // OBJ: the objective (sb_common.cuh), folded by ls_step.  R: no job starts before its release date (SB_FLAG_RELEASE,
 // any objective).  The per-job arrays they read (stage_job_array, sb_lane.cuh) follow the table in shared memory with TAB = 0 and are
-// read from global memory (ld.global.nc) with TAB = 1 / 2.
+// read from global memory (ld.global.nc) with TAB = 1 / 2.  obj_scenario(OBJ): the K scenario tables are staged back to
+// back (TAB = 0 only), and every evaluation runs one pass of the makespan form per table (no snapshots: the host runs
+// these forms without incremental rounds) and folds the K makespans into the score.
 template <int PB, bool INT, bool MULTI, bool EVAL = false, int TAB = 0, Obj OBJ = Obj::Makespan, bool R = false>
 __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
   static_assert(TAB == 0 || (EVAL && !MULTI), "tables outside the CTA's shared memory: scoring only, one node");
+  constexpr bool kScen = obj_scenario(OBJ);
+  static_assert(TAB == 0 || !kScen, "the scenario tables live in the CTA's shared memory");
   extern __shared__ __align__(128) uint8_t smem[];
   const int nw = blockDim.x >> 5;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t tab_all = static_cast<uint32_t>(a.J) * a.SG * 4u;
+  const uint32_t tab_all = kScen ? static_cast<uint32_t>(a.J) * a.SG * 4u * static_cast<uint32_t>(a.K)
+                                 : static_cast<uint32_t>(a.J) * a.SG * 4u;
   // TAB = 2: rank r of the pair keeps entries [r * half, (r + 1) * half)
   [[maybe_unused]] const uint32_t half = pos_tab_half(a.J, a.SG);
   [[maybe_unused]] const uint32_t rank = TAB == 2 ? cluster_ctarank() : 0u;
@@ -469,7 +476,7 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
       if constexpr (kP && TAB == 0) stage_job_array(reinterpret_cast<uint8_t*>(p_s), a.p, p_bytes, bar_tab);
     }
   }
-  LaneState<INT, MULTI, 0, OBJ, TAB == 0 ? 1 : 2, R> st;
+  LaneState<INT, MULTI, 0, step_obj(OBJ), TAB == 0 ? 1 : 2, R> st;
   st.tab = tab_s;
   if constexpr (kW) st.wt = TAB == 0 ? w_s : a.w;
   if constexpr (kD) st.dd = TAB == 0 ? d_s : a.d;
@@ -518,7 +525,7 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
     // rounds: `oc0` > 0 resumes at that 32-position block from the snapshot in front of it (buffer bit of
     // `par`), `save` stores the state in front of every later window boundary into the other buffer
     // (see SearchFuse::snap; a window is `wblk` blocks, chosen so that there are at most 32 windows).
-    auto evaluate = [&](const PosMove& mv, int oc0, uint32_t par, bool save, float* snap_t, int wblk) -> float {
+    auto pass = [&](const PosMove& mv, int oc0, uint32_t par, bool save, float* snap_t, int wblk) -> float {
       const int nout = (J + 31) / 32;  // outer iterations of 32 positions
       if (oc0 == 0) {
         st.reset(a.nodes);
@@ -586,6 +593,18 @@ __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
         for (int h = 0; h < PCH; ++h) qp[h] = np[h];
       }
       return st.result(a.nodes);
+    };
+    auto evaluate = [&](const PosMove& mv, int oc0, uint32_t par, bool save, float* snap_t, int wblk) -> float {
+      if constexpr (kScen) {
+        float score = 0.f;
+        for (int k = 0; k < a.K; ++k) {
+          st.tab = tab_s + static_cast<size_t>(k) * J * a.SG;
+          score = scenario_fold<OBJ>(score, pass(mv, 0, par, false, snap_t, wblk));
+        }
+        return score;
+      } else {
+        return pass(mv, oc0, par, save, snap_t, wblk);
+      }
     };
     PosMove none;
     none.kind = 0; none.a = none.b = none.va = none.vb = none.oa = none.ob = 0;
@@ -765,6 +784,10 @@ size_t search_pos_smem(int J, int SG, int nodes, int warps, int arrays) {
   return tab_bytes + arrays * job_array_bytes(J) + 16 + static_cast<size_t>(warps) * (nodes > 1 ? nodes * 1024u : 0u);
 }
 
+size_t scenario_smem(int J, int SG, int K, int nodes, unsigned flags) {
+  return search_pos_smem(J, SG * K, nodes, 16, (flags & SB_FLAG_RELEASE) ? 1 : 0);
+}
+
 using PosKernel = void (*)(PosArgs);
 
 // Scoring-only launches with the table outside the CTA's own shared memory (TAB = tab_home = 1 / 2 of k_search_pos).
@@ -811,7 +834,8 @@ static cudaError_t eval_pos_far_launch(const Device& dev, const PosArgs& a, int 
 // scoring only, one node: 2 = split over CTA pairs, 1 = global memory
 cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float* tab, const float* w, const float* d,
                               const float* r, const float* p, int SG, unsigned flags, Obj obj, long long first,
-                              long long count, bool eval_only, const SearchFuse& sf, cudaStream_t st, int tab_home) {
+                              long long count, bool eval_only, const SearchFuse& sf, cudaStream_t st, int tab_home,
+                              int K) {
   if (count <= 0) return cudaSuccess;
   PosArgs a;
   a.tab = tab; a.J = s.J; a.SG = SG; a.nodes = s.nodes;
@@ -827,24 +851,29 @@ cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float
   a.d = d;
   a.r = r;
   a.p = p;
+  a.K = K;
+  a.pad = 0;
   const bool multi = s.nodes > 1;
+  const bool scen = obj_scenario(obj);
   if (tab_home != 0) {
-    if (!eval_only || multi) return cudaErrorNotSupported;
+    if (!eval_only || multi || scen) return cudaErrorNotSupported;
     return eval_pos_far_launch(dev, a, tab_home, s.pb, flags, obj, st);
   }
   const int warps = 16;
-  const size_t smem = search_pos_smem(s.J, SG, s.nodes, warps, job_arrays(obj, flags));
+  const size_t smem = scen ? scenario_smem(s.J, SG, K, s.nodes, flags)
+                           : search_pos_smem(s.J, SG, s.nodes, warps, job_arrays(obj, flags));
   if (smem > dev.smem_optin) return cudaErrorNotSupported;
   const long long ntiles = (count + 31) / 32;
   const long long ctas = (ntiles + warps - 1) / warps;
   const int grid = static_cast<int>(ctas < dev.sm_count ? ctas : dev.sm_count);
-  const PosKernel kern = with_eval_types(s.pb, flags, obj, [&](auto PB, auto INT, auto OBJ, auto R) {
+  const auto pick = [&](auto PB, auto INT, auto OBJ, auto R) -> PosKernel {
     return with_bool(multi, [&](auto MULTI) {
       return with_bool(eval_only, [&](auto EVAL) -> PosKernel {
         return k_search_pos<PB, INT, MULTI, EVAL, 0, OBJ, R>;
       });
     });
-  });
+  };
+  const PosKernel kern = scen ? with_scenario_types(s.pb, flags, obj, pick) : with_eval_types(s.pb, flags, obj, pick);
   return launch(kern, grid, warps * 32, smem, st, a);
 }
 
@@ -852,7 +881,10 @@ cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float
 // a one-node table that does not fit there: 1 = global memory, read through L1 / L2 (with no tile in shared
 // memory the SM's whole array is L1); -1 = nowhere (multi-node table beyond shared memory).
 // HOOK_TABLE_PAIR forces 2 (split over CTA pairs: scattered 4-byte ld.shared::cluster), HOOK_TABLE_GLOBAL forces 1.
-int eval_pos_home(const Device& dev, int J, int SG, int nodes, unsigned flags, Obj obj) {
+int eval_pos_home(const Device& dev, int J, int SG, int nodes, unsigned flags, Obj obj, int K) {
+  // the scenario tables: shared memory or nowhere (check_per_job has already held them to scenario_smem)
+  if (obj_scenario(obj))
+    return !(flags & (HOOK_TABLE_PAIR | HOOK_TABLE_GLOBAL)) && scenario_smem(J, SG, K, nodes, flags) <= dev.smem_optin ? 0 : -1;
   const bool pair_ok = nodes == 1 && static_cast<size_t>(pos_tab_half(J, SG)) * 4 + 16 <= dev.smem_optin;
   if (flags & HOOK_TABLE_PAIR) return pair_ok ? 2 : -1;
   if (flags & HOOK_TABLE_GLOBAL) return nodes == 1 ? 1 : -1;
@@ -865,7 +897,7 @@ int eval_pos_home(const Device& dev, int J, int SG, int nodes, unsigned flags, O
 cudaError_t eval_pos_launch(const Device& dev, const EvalCall& c, cudaStream_t st, int* path) {
   if (c.stride_o % 32 != 0 || reinterpret_cast<uintptr_t>(c.opt) % 32 != 0 || reinterpret_cast<uintptr_t>(c.prio) % 32 != 0)
     return cudaErrorNotSupported;
-  const int home = eval_pos_home(dev, c.J, c.SG, c.nodes, c.flags, c.obj);
+  const int home = eval_pos_home(dev, c.J, c.SG, c.nodes, c.flags, c.obj, c.K);
   if (home < 0) return cudaErrorNotSupported;
   if (path) *path = home == 0 ? 5 : (home == 2 ? 7 : 8);
   if (c.B <= 0) return cudaSuccess;
@@ -878,7 +910,7 @@ cudaError_t eval_pos_launch(const Device& dev, const EvalCall& c, cudaStream_t s
   s.keys = c.best_key;
   SearchFuse sf = {};
   sf.cur_mk = c.out;
-  return search_pos_launch(dev, s, c.tab, c.w, c.d, c.r, c.p, c.SG, c.flags, c.obj, 0, c.B, true, sf, st, home);
+  return search_pos_launch(dev, s, c.tab, c.w, c.d, c.r, c.p, c.SG, c.flags, c.obj, 0, c.B, true, sf, st, home, c.K);
 }
 
 // Job-indexed opt rows -> schedule order (out[i] = opt[prio[i]]), one warp per candidate: the row is staged in

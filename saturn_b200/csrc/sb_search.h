@@ -29,11 +29,13 @@ cudaError_t search_accept(const SearchDev& s, int round, float temperature, cuda
 cudaError_t search_init_population_pos(const SearchDev& s, cudaStream_t st);
 size_t search_pos_smem(int J, int SG, int nodes, int warps, int arrays = 0);  // arrays: job_arrays(obj, flags)
 // w: the job weights [J] (obj_weights(obj)), else nullptr; d: the due dates or tails [J] (obj_due(obj)); r: the
-// release dates [J] (SB_FLAG_RELEASE; ceiled with SB_FLAG_INTEGER_STARTS)
+// release dates [J] (SB_FLAG_RELEASE; ceiled with SB_FLAG_INTEGER_STARTS); K: obj_scenario(obj), the number of scenario
+// tables at tab ([K][J][SG])
 cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float* tab, const float* w, const float* d,
                               const float* r, const float* p, int SG, unsigned flags, Obj obj, long long first,
-                              long long count, bool eval_only, const SearchFuse& sf, cudaStream_t st, int tab_home = 0);
-int eval_pos_home(const Device& dev, int J, int SG, int nodes, unsigned flags, Obj obj);
+                              long long count, bool eval_only, const SearchFuse& sf, cudaStream_t st, int tab_home = 0,
+                              int K = 0);
+int eval_pos_home(const Device& dev, int J, int SG, int nodes, unsigned flags, Obj obj, int K = 0);
 cudaError_t eval_pos_launch(const Device& dev, const EvalCall& c, cudaStream_t st, int* path = nullptr);
 cudaError_t opt_by_position_launch(const Device& dev, const EvalCall& c, uint8_t* out, cudaStream_t st);
 cudaError_t search_resample(const SearchDev& s, int round, cudaStream_t st);

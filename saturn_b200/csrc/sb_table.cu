@@ -64,6 +64,27 @@ cudaError_t build_table_launch(const float* T, int J, int S, int G, uint64_t gco
   return cudaGetLastError();
 }
 
+// one thread per (k, j, c): scenario k's cell, one fp32 product rounded to nearest (f > 0 finite: +inf stays +inf, a
+// sentinel scales like any runtime).  One factor per job scales every option of the job alike, so the reduced
+// table's arg-min is the same in every scenario and the factor may scale the reduced table directly.
+__global__ void k_scale_tables(const float* __restrict__ tab, int J, int SG, const float* __restrict__ f, int K,
+                               float* __restrict__ out) {
+  const long long n = static_cast<long long>(K) * J * SG;
+  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (idx >= n) return;
+  const long long cells = static_cast<long long>(J) * SG;
+  const int k = static_cast<int>(idx / cells);
+  const long long jc = idx % cells;
+  const int j = static_cast<int>(jc / SG);
+  out[idx] = __fmul_rn(f[static_cast<size_t>(k) * J + j], tab[jc]);
+}
+
+cudaError_t scale_tables_launch(const float* tab, int J, int SG, const float* f, int K, float* out, cudaStream_t st) {
+  const long long n = static_cast<long long>(K) * J * SG;
+  k_scale_tables<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(tab, J, SG, f, K, out);
+  return cudaGetLastError();
+}
+
 // Valid option list per job for the search's proposals.  Only non-dominated cells are proposed:
 // for each gpu count the fastest strategy (a slower strategy with the same footprint can never
 // improve the optimum), and only cells below the reference's sentinel runtimes (1e6 "not

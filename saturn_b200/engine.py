@@ -62,14 +62,22 @@ COMPLETION_PENALTY_OBJECTIVES = {
     "completion_penalty": Objective(_SUM | _DUE | _lib.FLAG_COMPLETION_PENALTY, False, True),
     "weighted_completion_penalty": Objective(_SUM | _DUE | _lib.FLAG_COMPLETION_PENALTY | _W, True, True),
 }
+# The scenario forms: the worst makespan, max_k M_k, and the mean makespan, scored as sum_k M_k, over the K runtime
+# scenarios of set_scenarios (M_k: the same options and order, the list schedule re-run on scenario table k).  A table
+# of their own, held to oracle/ref_scenarios.py; objective_spec and objective_flag look names up here as well.
+SCENARIO_OBJECTIVES = {
+    "worst_makespan": Objective(_lib.FLAG_WORST_MAKESPAN, False, False),
+    "mean_makespan": Objective(_lib.FLAG_MEAN_MAKESPAN, False, False),
+}
 
 
 def objective_spec(objective: str) -> Objective:
     """The table entry of an objective name; raises SolverError for a name that is not one."""
-    spec = _OBJECTIVES.get(objective) or COMPLETION_PENALTY_OBJECTIVES.get(objective)
+    spec = _OBJECTIVES.get(objective) or COMPLETION_PENALTY_OBJECTIVES.get(objective) or \
+        SCENARIO_OBJECTIVES.get(objective)
     if spec is None:
         from .solver import SolverError
-        names = list(_OBJECTIVES) + list(COMPLETION_PENALTY_OBJECTIVES)
+        names = list(_OBJECTIVES) + list(COMPLETION_PENALTY_OBJECTIVES) + list(SCENARIO_OBJECTIVES)
         raise SolverError("objective must be one of %s, not %r" % (", ".join(map(repr, names)), objective))
     return spec
 
@@ -161,6 +169,25 @@ def release_f32(r, J: int) -> np.ndarray:
     return r32
 
 
+def scenarios_f32(f, J: int) -> np.ndarray:
+    """K runtime scenarios [K][J] as fp32 (round to nearest), 1 <= K <= 8.  Every factor must be finite and > 0, and
+    stay so in fp32; raises SolverError otherwise."""
+    from .solver import SolverError
+    try:
+        f64 = np.asarray(f, dtype=np.float64)
+    except (TypeError, ValueError) as e:
+        raise SolverError("scenario factors must be numbers: %s" % e)
+    if f64.ndim != 2 or f64.shape[1] != J or not 1 <= f64.shape[0] <= 8:
+        raise SolverError("scenarios must be K x %d factors with 1 <= K <= 8, got shape %s" % (J, f64.shape))
+    if not (np.isfinite(f64).all() and (f64 > 0).all()):
+        raise SolverError("every scenario factor must be finite and > 0")
+    with np.errstate(over="ignore", under="ignore"):
+        f32 = f64.astype(np.float32)
+    if not (np.isfinite(f32).all() and (f32 > 0).all()):
+        raise SolverError("every scenario factor must stay finite and > 0 in fp32 (a factor rounds to 0 or to inf)")
+    return f32
+
+
 def _flags(integer_starts: bool, reduced: bool, objective: str = "makespan") -> int:
     return (FLAG_INTEGER_STARTS if integer_starts else 0) | (FLAG_REDUCED if reduced else 0) | objective_flag(objective)
 
@@ -212,6 +239,7 @@ class Engine:
         self.due = None  # fp32 job due dates of the tardiness, late-count and max-lateness objectives (set_due)
         self.due_shift = None  # max of self.due: objective="max_lateness" scores L_max + due_shift (>= 0)
         self.release = None  # fp32 job release dates, under every objective (set_release)
+        self.scenarios = None  # fp32 runtime factors [K][J] of the scenario objectives (set_scenarios)
 
     # ------------------------------------------------------------------ lifecycle
     def close(self):
@@ -260,6 +288,7 @@ class Engine:
         self.due_shift = None
         self.release = None
         self.penalty = None
+        self.scenarios = None
         return self
 
     def set_weights(self, w) -> "Engine":
@@ -323,12 +352,29 @@ class Engine:
         self.penalty = p32
         return self
 
+    def set_scenarios(self, f) -> "Engine":
+        """K runtime scenarios, f[K][J] factors (1 <= K <= 8, each finite and > 0, converted to fp32), for
+        objective="worst_makespan", which scores max_k M_k, and "mean_makespan", which scores sum_k M_k: M_k is the
+        makespan of the same options and order on the table whose row j is fp32(f[k][j] * T[j]).  None clears them;
+        set_table clears them too."""
+        if f is None:
+            check(self._lib.sb_set_scenarios(self._h, None, 0, 0))
+            self.scenarios = None
+            return self
+        f32 = np.ascontiguousarray(scenarios_f32(f, self.J))
+        check(self._lib.sb_set_scenarios(self._h, C.c_void_p(f32.ctypes.data), int(f32.shape[0]), int(self.J)))
+        self.scenarios = f32
+        return self
+
     def _release_flag(self) -> int:
         return _lib.FLAG_RELEASE if self.release is not None else 0
 
     def _flags(self, integer_starts: bool, reduced: bool, objective: str) -> int:
         _require_due(self.due, objective)
         _require_penalty(self.penalty, objective)
+        if objective in SCENARIO_OBJECTIVES and self.scenarios is None:
+            from .solver import SolverError
+            raise SolverError("objective=%r needs runtime scenarios: call set_scenarios after set_table" % (objective,))
         return _flags(integer_starts, reduced, objective) | self._release_flag()
 
     def reduced_table(self) -> Tuple[np.ndarray, np.ndarray]:
@@ -435,6 +481,18 @@ class Engine:
                                      self._flags(integer_starts, reduced, objective), C.c_void_p(mk.data_ptr()),
                                      C.c_void_p(start.data_ptr()), C.c_void_p(mask.data_ptr())))
         return mk, start, mask
+
+    def eval_scenarios(self, opt: torch.Tensor, prio: torch.Tensor, integer_starts: bool = True, reduced: bool = False,
+                       objective: str = "worst_makespan"):
+        """(score[B], makespans[B][K]) of every candidate under a scenario objective, slot-exact (sb_eval_scenarios)."""
+        B, stride = self._check_cands(opt, prio, True)
+        K = 0 if self.scenarios is None else self.scenarios.shape[0]
+        score = torch.empty(B, dtype=torch.float32, device=self.device)
+        mks = torch.empty((B, max(K, 1)), dtype=torch.float32, device=self.device)
+        check(self._lib.sb_eval_scenarios(self._h, C.c_void_p(opt.data_ptr()), C.c_void_p(prio.data_ptr()), B, stride,
+                                          self._flags(integer_starts, reduced, objective),
+                                          C.c_void_p(score.data_ptr()), C.c_void_p(mks.data_ptr())))
+        return score, mks
 
     def decode(self, opt: np.ndarray, prio: np.ndarray, integer_starts: bool = True, reduced: bool = False,
                objective: str = "makespan"):
@@ -727,6 +785,14 @@ class MultiEngine:
         return self
 
     release = property(lambda self: self.engines[0].release)
+
+    def set_scenarios(self, f):
+        """Engine.set_scenarios on every device."""
+        for e in self.engines:
+            e.set_scenarios(f)
+        return self
+
+    scenarios = property(lambda self: self.engines[0].scenarios)
 
     def set_penalty(self, p):
         """Engine.set_penalty on every device."""

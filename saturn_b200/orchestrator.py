@@ -68,7 +68,10 @@ def orchestrate(task_list, log=False, interval=1000, gurobi=True, *,
     interval counts its flow from the interval's start, so each solve minimises the squares of the waits that
     remain, not of the whole flow time.  Under objective="late_penalty" and "completion_penalty" a `penalty` mapping
     Task -> penalty is passed to every solve unchanged: a penalty is what missing the due date costs, whenever the
-    plan is made; a sequence `penalty` raises SolverError, as a sequence `due` does.
+    plan is made; a sequence `penalty` raises SolverError, as a sequence `due` does.  Under
+    objective="worst_makespan" and "mean_makespan" a `scenarios` mapping Task -> K runtime factors is passed to every
+    solve unchanged: a factor scales a task's remaining work as it scales the whole task; a sequence `scenarios`
+    raises SolverError, as a sequence `due` does.
     """
     logging.basicConfig(level=logging.INFO if log else logging.WARNING,
                         format="%(asctime)s %(levelname)-8s %(message)s", datefmt="%Y-%m-%d %H:%M:%S")
@@ -79,6 +82,9 @@ def orchestrate(task_list, log=False, interval=1000, gurobi=True, *,
     if kw.get("penalty") is not None and not isinstance(kw["penalty"], Mapping):
         raise SolverError("orchestrate() needs penalty as a mapping Task -> penalty: its task list shrinks every "
                           "interval")
+    if kw.get("scenarios") is not None and not isinstance(kw["scenarios"], Mapping):
+        raise SolverError("orchestrate() needs scenarios as a mapping Task -> runtime factors: its task list shrinks "
+                          "every interval")
     release = kw.pop("release", None)
     if release is not None and not isinstance(release, Mapping):
         raise SolverError("orchestrate() needs release as a mapping Task -> release date: its task list shrinks "

@@ -171,6 +171,7 @@ FP32_EXACT_HORIZON = float(1 << 24)   # integer seconds are exact in the kernels
 FP32_MAX = float(np.finfo(np.float32).max)
 SQUARE_BOUND = float(1 << 50)   # a squared tardiness inside the horizon, (2^25)^2, with |d| < 2^24
 _SQUARED = ("squared_tardiness", "squared_flow")   # the solve() objectives that run as the squared tardiness
+_SCENARIO = ("worst_makespan", "mean_makespan")    # the solve() objectives over runtime scenarios (scenarios=...)
 
 
 def _engine(devices=None):
@@ -228,10 +229,10 @@ def _check_horizon(T, found_makespan=None, release=None, tails=None):
 
 def _check_objective(objective, hysteresis=False, release=None):
     if objective not in ("makespan", "completion", "tardiness", "max_lateness", "late_tasks", "max_stretch",
-                         "squared_tardiness", "squared_flow", "late_penalty", "completion_penalty"):
+                         "squared_tardiness", "squared_flow", "late_penalty", "completion_penalty") + _SCENARIO:
         raise SolverError("objective must be 'makespan', 'completion', 'tardiness', 'max_lateness', 'late_tasks', "
-                          "'max_stretch', 'squared_tardiness', 'squared_flow', 'late_penalty' or "
-                          "'completion_penalty', not %r" % (objective,))
+                          "'max_stretch', 'squared_tardiness', 'squared_flow', 'late_penalty', "
+                          "'completion_penalty', 'worst_makespan' or 'mean_makespan', not %r" % (objective,))
     if objective != "makespan" and hysteresis:
         raise SolverError("hysteresis=True compares plans by makespan (milp.py:363-442); it is not defined for "
                           "objective=%r" % (objective,))
@@ -320,6 +321,66 @@ def _resolve_penalty(penalty, objective, J, task_list=None):
     from .engine import penalty_f32
     p32 = penalty_f32(penalty, J)
     return [float(x) for x in penalty], p32
+
+
+def _resolve_scenarios(scenarios, objective, J, task_list=None):
+    """The caller's runtime scenarios, J rows of K factors each (a sequence aligned with the tasks or T's rows, or with
+    `task_list` a mapping Task -> K factors), as (float64 [K][J], fp32 [K][J] for the device), or (None, None) without
+    objective="worst_makespan" or "mean_makespan", which require them.  Raises SolverError before any device call."""
+    if objective not in _SCENARIO:
+        if scenarios is not None:
+            raise SolverError("scenarios apply to objective='worst_makespan' or 'mean_makespan' only, not to %r"
+                              % (objective,))
+        return None, None
+    if scenarios is None:
+        raise SolverError("objective=%r needs runtime scenarios (scenarios=...)" % (objective,))
+    rows = _per_task(scenarios, "scenarios", task_list)
+    if len(rows) != J:
+        raise SolverError("scenarios must have one row per task (%d), got %d" % (J, len(rows)))
+    try:
+        lens = {len(r) for r in rows}
+    except TypeError:
+        raise SolverError("each task's scenarios must be a sequence of K factors")
+    if len(lens) > 1:
+        raise SolverError("every task must have the same number of scenario factors, got %s" % sorted(lens))
+    try:
+        f64 = np.asarray([list(r) for r in rows], dtype=np.float64).reshape(J, -1).T.copy()
+    except (TypeError, ValueError) as e:
+        raise SolverError("scenario factors must be numbers: %s" % e)
+    from .engine import scenarios_f32
+    return f64, scenarios_f32(f64, J)
+
+
+def _check_scenario_horizon(Tdev, f32, release=None):
+    """_check_horizon on every scenario table T_k, formed in fp32 as the device forms it (one rounded product)."""
+    with np.errstate(over="ignore"):
+        for k in range(f32.shape[0]):
+            _check_horizon((f32[k][:, None, None] * Tdev).astype(np.float32), release=release)
+
+
+def _scenario_stats(rts, gpus, node, prio, f64, integer_starts, r64=None):
+    """scenario_makespans (each scenario's makespan, K values), worst_makespan and mean_makespan of a plan's options and
+    order, in float64: the list rule re-run on every scenario's runtimes f[k][t] * rt_t (the tasks' own runtimes), with
+    integer starts rounding each hold up as the device does."""
+    J = len(rts)
+    mks = []
+    for k in range(f64.shape[0]):
+        ready = {}
+        mk = 0.0
+        for j in (int(x) for x in prio):
+            rt = float(f64[k, j]) * float(rts[j])
+            rd = ready.setdefault(int(node[j]), [0.0] * NSLOT)
+            sel = sorted(range(NSLOT), key=lambda g: (rd[g], g))[:int(gpus[j])]
+            st = rd[sel[-1]]
+            if r64 is not None:
+                rel = float(r64[j])
+                st = max(st, math.ceil(rel) if integer_starts else rel)
+            nxt = st + (math.ceil(rt) if integer_starts and math.isfinite(rt) else rt)
+            for g in sel:
+                rd[g] = nxt
+            mk = max(mk, st + rt)
+        mks.append(mk)
+    return {"scenario_makespans": mks, "worst_makespan": max(mks), "mean_makespan": sum(mks) / len(mks)}
 
 
 def _resolve_release(release, J, task_list=None):
@@ -489,7 +550,7 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
           timeout=500, *, chains: Optional[int] = None, rounds: Optional[int] = None, seed: int = 0,
           integer_starts: bool = True, engine=None, hysteresis: Optional[bool] = None,
           nodes: Optional[int] = None, devices=None, objective: str = "makespan", weights=None, due=None,
-          release=None, penalty=None, _warm=None):
+          release=None, penalty=None, scenarios=None, _warm=None):
     """Drop-in for saturn.solver.solve (milp.py:23).
 
     Objective.  "makespan" (the default, the reference's) or "completion": minimise the sum of the tasks'
@@ -594,6 +655,18 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     ["penalty_paid"] are recomputed in float64 from the emitted plan, the tasks' own runtimes and the caller's d, w
     and p; last_stats["device_makespan"] holds the device's fp32 score.  The 6th element stays the plan's makespan.
 
+    Runtime scenarios.  objective="worst_makespan" or "mean_makespan" with `scenarios` (a sequence aligned with
+    task_list of K factors each, or a mapping Task -> K factors, 1 <= K <= 8, every factor finite and > 0) plans for
+    runtimes that are estimates: scenario k runs every option of task t f[t][k] times as long (fp32(f * rt), one
+    rounding), and the plan — its options and list order — minimises the largest makespan over the K scenarios, or
+    their mean, the list rule re-run on each scenario's runtimes (not the same gangs replayed).  `release` is valid.
+    A missing `scenarios`, `scenarios` under any other objective, ragged or out-of-range K, a bad factor,
+    hysteresis=True, or a scenario whose table breaks the 2^24 s integer-start horizon raises SolverError before any
+    device call.  The 6-tuple is the plan on the nominal runtimes (what the executor runs) and its 6th element the
+    nominal makespan; last_stats["scenario_makespans"] (K values), ["worst_makespan"] and ["mean_makespan"] are
+    re-run in float64 from the plan's options and order on f * the tasks' own runtimes; last_stats["device_makespan"]
+    holds the device's fp32 score (the worst makespan, or the sum of the K makespans).
+
     Release dates.  `release` (a sequence aligned with task_list, or a mapping keyed by Task, in the runtimes' units
     from the plan's t = 0) keeps every task from starting before its release date, under every objective: a
     dataset or a parent checkpoint that is only ready later, a job that arrives tomorrow.  r <= 0 means already
@@ -635,6 +708,7 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     w64, w32 = _resolve_weights(weights, objective, J, task_list)
     d64, d32 = _resolve_due(due, objective, J, task_list)
     p64, p32 = _resolve_penalty(penalty, objective, J, task_list)
+    f64, f32 = _resolve_scenarios(scenarios, objective, J, task_list)
     r64, r32 = _resolve_release(release, J, task_list)
     if J == 0:
         return [[[] for _ in range(NSLOT)]], [], [], [], [], 0.0
@@ -647,6 +721,8 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
         if usable[j].any():
             Tdev[j, 0, ~usable[j]] = np.inf
     _check_horizon(Tdev, release=r64, tails=_tails(d32) if objective == "max_lateness" else None)
+    if f32 is not None:
+        _check_scenario_horizon(Tdev, f32, r64)
     if objective == "max_stretch":
         _, w32, d32 = _stretch_form(Tdev, r32)
         # p*_t in the tasks' own runtimes: the fastest option among the cells the device table keeps
@@ -659,11 +735,14 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     nodes = int(nodes)
     eng.set_table(Tdev, list(range(1, NSLOT + 1)), sentinel=float("inf"), nodes=nodes)
     search_objective = _set_objective(eng, objective, w32, d32, r32, p32)
+    if f32 is not None:
+        eng.set_scenarios(f32)
     if chains is None:
         chains = int(os.environ.get("SATURN_B200_CHAINS", 0))
         if chains <= 0:
             # about 131072 chains, rounded to whole waves of the round kernel (no partially filled last wave)
-            wave = eng.search_wave(reduced=True) if hasattr(eng, "search_wave") else 0
+            wave = (eng.search_wave(reduced=True, **({"objective": objective} if objective in _SCENARIO else {}))
+                    if hasattr(eng, "search_wave") else 0)
             chains = max(1, round((1 << 17) / wave)) * wave if wave > 0 else 1 << 17
     if rounds is None:
         rounds = int(os.environ.get("SATURN_B200_ROUNDS", 400))
@@ -718,6 +797,9 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
         last_stats.update(_late_penalty_stats(dec["start"], rts, w64, d64, p64))
     elif objective == "completion_penalty":
         last_stats.update(_completion_penalty_stats(dec["start"], rts, w64, d64, p64))
+    elif objective in _SCENARIO:
+        last_stats.update(_scenario_stats(rts, gpus, dec["node"], res.prio, f64, integer_starts, r64))
+        _check_horizon(Tdev, max(last_stats["scenario_makespans"]))
     elif d64 is not None:
         last_stats.update(_tardiness_stats(dec["start"], rts, w64, d64))
     if r64 is not None:
@@ -817,7 +899,7 @@ def strategies_from_table(T, mask, executors=None, params=None, gcount=None):
 def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeout=500, *,
                 chains: Optional[int] = None, rounds: Optional[int] = None, seed: int = 0,
                 integer_starts: bool = True, engine=None, nodes: Optional[int] = None, devices=None,
-                objective: str = "makespan", weights=None, due=None, release=None, penalty=None):
+                objective: str = "makespan", weights=None, due=None, release=None, penalty=None, scenarios=None):
     """solve() on the dense profiler tensor T[J][S][G] (+ mask of usable cells, + gcount[G] GPU counts).
     `objective` as for solve(): "makespan" or "completion" (sum of completion times); `weights` as for solve(),
     a sequence aligned with T's rows (the weighted sum of completion times, last_stats["weighted_completion"]);
@@ -827,7 +909,9 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     the search may propose, over every strategy (last_stats["max_stretch"] and ["mean_stretch"] from T's values).
     objective="squared_tardiness" (with `due`) and "squared_flow" as for solve(), with their last_stats from T's values.
     objective="late_penalty" and "completion_penalty" (with `due` and `penalty`, sequences aligned with T's rows) as
-    for solve(), with their last_stats from T's values.
+    for solve(), with their last_stats from T's values.  objective="worst_makespan" and "mean_makespan" with
+    `scenarios`, an array [J][K] of factors aligned with T's rows, as for solve(), with their last_stats from T's
+    values.
     Every cell of T must be
     >= 0 (-0.0 counts as zero), +inf or a sentinel: a negative or NaN cell raises SolverError, with or without `mask`.
 
@@ -850,6 +934,7 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     w64, w32 = _resolve_weights(weights, objective, J)
     d64, d32 = _resolve_due(due, objective, J)
     p64, p32 = _resolve_penalty(penalty, objective, J)
+    f64, f32 = _resolve_scenarios(scenarios, objective, J)
     r64, r32 = _resolve_release(release, J)
     if J == 0:
         return [[[] for _ in range(NSLOT)]], [], [], [], [], 0.0, np.zeros(0, dtype=np.int64)
@@ -865,6 +950,8 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     if not np.isfinite(Tdev.reshape(J, -1)).any(axis=1).all():
         raise SolverError("a task has no finite cell in T")
     _check_horizon(Tdev, release=r64, tails=_tails(d32) if objective == "max_lateness" else None)
+    if f32 is not None:
+        _check_scenario_horizon(Tdev, f32, r64)
     if objective == "max_stretch":
         pstar, w32, d32 = _stretch_form(Tdev, r32)
     elif objective == "squared_flow":
@@ -873,10 +960,12 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     nodes = int(_default_nodes() if nodes is None else nodes)
     eng.set_table(Tdev, gcount, sentinel=float("inf"), nodes=nodes)
     search_objective = _set_objective(eng, objective, w32, d32, r32, p32)
+    if f32 is not None:
+        eng.set_scenarios(f32)
     if chains is None:
         chains = int(os.environ.get("SATURN_B200_CHAINS", 0))
         if chains <= 0:
-            wave = eng.search_wave(reduced=True)
+            wave = eng.search_wave(reduced=True, **({"objective": objective} if objective in _SCENARIO else {}))
             chains = max(1, round((1 << 17) / wave)) * wave if wave > 0 else 1 << 17
     if rounds is None:
         rounds = int(os.environ.get("SATURN_B200_ROUNDS", 400))
@@ -925,6 +1014,9 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
         last_stats.update(_late_penalty_stats(dec["start"], rts, w64, d64, p64))
     elif objective == "completion_penalty":
         last_stats.update(_completion_penalty_stats(dec["start"], rts, w64, d64, p64))
+    elif objective in _SCENARIO:
+        last_stats.update(_scenario_stats(rts, gpus, dec["node"], res.prio, f64, integer_starts, r64))
+        _check_horizon(Tdev, max(last_stats["scenario_makespans"]))
     elif d64 is not None:
         last_stats.update(_tardiness_stats(dec["start"], rts, w64, d64))
     if r64 is not None:

@@ -3,7 +3,7 @@ maximum lateness, of the (weighted) number of late tasks, of the maximum stretch
 prints one JSON line.
 
     python scripts/bench_objective.py [--steps 200] [--warmup 20] [--solve-chains 0] [--solve-rounds 400]
-                                      [--only max_stretch | squared | late_penalty | completion_penalty]
+                                      [--only max_stretch | squared | late_penalty | completion_penalty | scenarios]
 
 kernel: sb_eval on bench.py's C4 batch (J = 256, S = 8, 946,176 candidates, the same seeded inputs, integer
         starts), scored for the makespan, the sum of completion times, the weighted sum (seeded weights) and the
@@ -44,6 +44,13 @@ the cost sum_t [C_t > d_t] (p_t + C_t - d_t), the late tasks and the tardiness.
 the due dates of the kernel rows, seeded integer penalties in [0, 100000) s), alternated as above, and runs only
 solve_front(points=8) on the 256-task set with the release dates of the stretch comparison: per point its cap, its
 makespan and its mean flow time (C_t - max(r_t, 0)) in float64, and the front's total wall time.
+--only scenarios times, on the same C4 batch read through the reduced table (opt bytes k - 1), the makespan and the
+worst makespan over K = 1, 4 and 8 seeded log-normal scenarios (sigma 0.3, median 1) on the two routes that score the
+scenario forms: the generic kernel on job-indexed rows and the position-major kernel on rows by position, the eight
+launches alternated as above.  Then solve() on the 256-task set with K = 8 seeded log-normal factors per task (sigma
+0.3, median 1): the worst- and mean-makespan plans against the nominal makespan plan, each rescored in float64 under
+the same 8 scenarios and under 64 held-out scenarios drawn from the same distribution (another seed): the worst and
+mean makespan over each set, and the nominal makespan.
 The card's name and power limit are read in the same run (nvidia-smi, read-only queries).
 """
 import argparse
@@ -75,9 +82,12 @@ def main():
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--solve-chains", type=int, default=0, help="0 = solve()'s default population")
     ap.add_argument("--solve-rounds", type=int, default=400)
-    ap.add_argument("--only", choices=("all", "max_stretch", "squared", "late_penalty", "completion_penalty"),
-                    default="all")
+    ap.add_argument("--only", choices=("all", "max_stretch", "squared", "late_penalty", "completion_penalty",
+                                       "scenarios"), default="all")
     args = ap.parse_args()
+    if args.only == "scenarios":
+        scenarios_main(args)
+        return
     import numpy as np
     import torch
     from oracle import ref_eval as R
@@ -236,6 +246,89 @@ def main():
     print(json.dumps({"card": card(0), "kernel": kernel, "solve": solve, "late_unit": late_unit,
                       "release": release_effect(S, R, tasks, due, solve["makespan"]["makespan"], kw),
                       "stretch": stretch_effect(S, R, tasks, solve["makespan"]["makespan"], kw)}))
+    eng.close()
+
+
+def _median(t):
+    import numpy as np
+    return {"median_ms": float(np.median(t)), "p10_ms": float(np.percentile(t, 10)),
+            "p90_ms": float(np.percentile(t, 90))}
+
+
+def scenarios_main(args):
+    import numpy as np
+    import torch
+    from saturn_b200 import solver as S
+    from saturn_b200.engine import Engine, opt_by_position, random_candidates
+    from saturn_b200.synth import synth_table
+    torch.cuda.set_device(0)
+    J, Sx, G = 256, 8, 8
+    B = 132 * 8 * 32 * 28                                   # bench.py's B_PER_GPU
+    T, valid = synth_table(J, Sx, G, seed=0)
+    opt, prio = random_candidates(Engine(0).set_table(T), B, valid, seed=1)
+    opt &= 7                                                # the reduced table's opt bytes: k - 1
+    obp = opt_by_position(opt, prio)
+    out = torch.empty(B, dtype=torch.float32, device=opt.device)
+    engines = {}
+    for K in (1, 4, 8):                                     # one handle per scenario count, the same table
+        e = Engine(0)
+        e.set_table(T)
+        e.set_scenarios(np.random.default_rng(40 + K).lognormal(0.0, 0.3, size=(K, J)))
+        engines[K] = e
+    runs = []
+    for route, o, kw in (("generic", opt, {}), ("position_major", obp, {"by_position": True})):
+        runs.append((route + "/makespan", engines[1], o,
+                     dict(kw, objective="makespan", **({"_force_generic": True} if route == "generic" else {}))))
+        for K in (1, 4, 8):
+            runs.append((route + "/worst_K%d" % K, engines[K], o, dict(kw, objective="worst_makespan")))
+    times = {name: [] for name, _, _, _ in runs}
+    paths = {}
+    for i in range(args.warmup + args.steps):
+        for name, e, o, kw in runs[i % len(runs):] + runs[:i % len(runs)]:
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record()
+            e.eval(o, prio, out=out, reduced=True, **kw)
+            b.record()
+            b.synchronize()
+            paths[name] = e.last_eval_path()
+            if i >= args.warmup:
+                times[name].append(a.elapsed_time(b))
+    kernel = {name: dict(_median(t), path=paths[name]) for name, t in times.items()}
+    for route in ("generic", "position_major"):
+        base = kernel[route + "/makespan"]["median_ms"]
+        for K in (1, 4, 8):
+            kernel[route + "/worst_K%d" % K]["over_makespan"] = kernel[route + "/worst_K%d" % K]["median_ms"] / base
+    kernel.update(B=B, J=J, S=Sx, steps=args.steps)
+    del opt, prio, obp, out
+    for e in engines.values():
+        e.close()
+    torch.cuda.empty_cache()
+
+    eng = Engine(0)
+    tasks = _tasks256()
+    J = len(tasks)
+    f8 = np.random.default_rng(50).lognormal(0.0, 0.3, size=(J, 8))
+    held = np.random.default_rng(51).lognormal(0.0, 0.3, size=(64, J))
+    kw = dict(rounds=args.solve_rounds, seed=1, engine=eng, **({"chains": args.solve_chains}
+                                                               if args.solve_chains else {}))
+
+    def rescore(plan):
+        opt, order = S._plan_candidate(tasks, plan, 1)
+        gpus = (opt & 7).astype(np.int64) + 1
+        rts = [float(t.strategies[int(g)].runtime) for t, g in zip(tasks, gpus)]
+        node = np.zeros(J, dtype=np.int64)
+        same = S._scenario_stats(rts, gpus, node, order, f8.T, True)
+        other = S._scenario_stats(rts, gpus, node, order, held, True)
+        return {"nominal_makespan": plan[5], "worst_8": same["worst_makespan"], "mean_8": same["mean_makespan"],
+                "worst_64_held_out": other["worst_makespan"], "mean_64_held_out": other["mean_makespan"]}
+    solve = {}
+    for name, obj in (("makespan", "makespan"), ("worst_makespan", "worst_makespan"), ("mean_makespan", "mean_makespan")):
+        t0 = time.perf_counter()
+        plan = S.solve(tasks, None, objective=obj, **({"scenarios": f8} if obj != "makespan" else {}), **kw)
+        wall = time.perf_counter() - t0
+        solve[name] = dict(rescore(plan), wall_s=wall, rounds=S.last_stats["rounds"],
+                           candidates=S.last_stats["candidates"])
+    print(json.dumps({"card": card(0), "kernel": kernel, "scenarios": solve}))
     eng.close()
 
 
