@@ -288,6 +288,29 @@ typedef enum sb_status {
 #define SB_FLAG_MEAN_MAKESPAN 131072u /* as SB_FLAG_WORST_MAKESPAN, but the score is the sum of the K makespans, the
                                      left fold acc = acc + M_k (fp32, each add rounded) in scenario order from +0: K
                                      times the mean makespan, with the same arg-min. */
+#define SB_FLAG_WORST_TARDINESS 262144u /* modifies SB_FLAG_SUM_COMPLETION | SB_FLAG_DUE [| SB_FLAG_WEIGHTED], after
+                                     sb_set_scenarios (else SB_ERR_STATE): the objective is the worst total (weighted)
+                                     tardiness over the K runtime scenarios, max_k S_k, where S_k is the tardiness
+                                     form's score, the left fold from +0 in schedule order of
+                                     fp32(w_j * max(C_jk - d_j, 0)) (each add rounded), of the same candidate (options
+                                     and order, the list rule re-run) on scenario table k.  Not the largest per-job
+                                     tardiness (that is SB_FLAG_MAX_TARDINESS).  With every d = +0 the score is the worst
+                                     (weighted) sum of completion times bit for bit.  Without SB_FLAG_SUM_COMPLETION |
+                                     SB_FLAG_DUE, with SB_FLAG_MEAN_TARDINESS, SB_FLAG_LATE_COUNT,
+                                     SB_FLAG_MAX_TARDINESS, SB_FLAG_SQUARED, SB_FLAG_LATE_PENALTY,
+                                     SB_FLAG_COMPLETION_PENALTY, SB_FLAG_MAX_LATENESS, SB_FLAG_WORST_MAKESPAN or
+                                     SB_FLAG_MEAN_MAKESPAN it is SB_ERR_ARG; valid with SB_FLAG_RELEASE and several
+                                     nodes.  The K tables, the weights and the due dates must fit in one CTA's shared
+                                     memory beside the release dates and the node states (else SB_ERR_UNSUPPORTED).
+                                     Accepted where SB_FLAG_WORST_MAKESPAN is, with the same routes; sb_eval_full and
+                                     sb_decode report the start times and GPU slots of the nominal schedule (on T).  The
+                                     search runs without incremental rounds, plants the EDD seeds of SB_FLAG_DUE on the
+                                     nominal table, stops at a score of 0, and takes the tardiness form's temperature
+                                     unit.  Not available with SB_FLAG_ALT_WARPSCAN (SB_ERR_UNSUPPORTED). */
+#define SB_FLAG_MEAN_TARDINESS 524288u /* as SB_FLAG_WORST_TARDINESS, but the score is the sum of the K totals, the
+                                     left fold acc = acc + S_k (fp32, each add rounded) in scenario order from +0: K
+                                     times the mean total tardiness, with the same arg-min; the search's temperature
+                                     floor is K times the tardiness form's. */
 #define SB_IPC_HANDLE_BYTES 64
 
 typedef struct sb_handle sb_handle;
@@ -344,7 +367,8 @@ int sb_set_release(sb_handle* h, const float* r, int J);
  * before sb_set_table.  sb_set_table clears the penalties; setting or clearing them ends the current search
  * (sb_search_init again).  Their sum is recorded for the search's temperature unit. */
 int sb_set_penalty(sb_handle* h, const float* p, int J);
-/* Runtime scenarios for SB_FLAG_WORST_MAKESPAN and SB_FLAG_MEAN_MAKESPAN: f fp32 [K][J], host or device, one positive
+/* Runtime scenarios for SB_FLAG_WORST_MAKESPAN, SB_FLAG_MEAN_MAKESPAN, SB_FLAG_WORST_TARDINESS and
+ * SB_FLAG_MEAN_TARDINESS: f fp32 [K][J], host or device, one positive
  * factor per scenario and job; scenario k's table is T_k[j][c] = fp32(f[k][j] * T[j][c]) for every cell of row j, of
  * the full and of the reduced table alike (+inf stays +inf).  K outside 1..8, a J that differs from the table's, or a
  * factor that is <= 0, NaN or inf is SB_ERR_ARG.  f = NULL clears them.  SB_ERR_STATE before sb_set_table.
@@ -399,8 +423,9 @@ int sb_eval_host(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, 
  * may be NULL. */
 int sb_eval_full(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, int64_t row_stride,
                  unsigned flags, float* makespan_out, float* start_out, uint32_t* slotmask_out);
-/* Under SB_FLAG_WORST_MAKESPAN or SB_FLAG_MEAN_MAKESPAN (else SB_ERR_ARG): the slot-exact score of B candidates and
- * every scenario's makespan M_k, makespans_out fp32 [B][K] (device pointers; score_out may be NULL). */
+/* Under SB_FLAG_WORST_MAKESPAN, SB_FLAG_MEAN_MAKESPAN, SB_FLAG_WORST_TARDINESS or SB_FLAG_MEAN_TARDINESS (else
+ * SB_ERR_ARG): the slot-exact score of B candidates and every scenario's score, the makespan M_k or the total
+ * tardiness S_k, makespans_out fp32 [B][K] (device pointers; score_out may be NULL). */
 int sb_eval_scenarios(sb_handle* h, const uint8_t* opt, const void* prio, int64_t B, int64_t row_stride,
                       unsigned flags, float* score_out, float* makespans_out);
 

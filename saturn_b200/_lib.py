@@ -24,6 +24,8 @@ FLAG_LATE_PENALTY = 16384
 FLAG_COMPLETION_PENALTY = 32768
 FLAG_WORST_MAKESPAN = 65536
 FLAG_MEAN_MAKESPAN = 131072
+FLAG_WORST_TARDINESS = 262144
+FLAG_MEAN_TARDINESS = 524288
 IPC_HANDLE_BYTES = 64
 # test hooks in the top bits of the same flags word: the enum in csrc/sb_internal.h says what each one forces
 HOOK_FORCE_GENERIC = 0x80000000

@@ -592,6 +592,17 @@ static int decode_objective(unsigned flags, Objective* o) {
   const bool max_tardiness = flags & SB_FLAG_MAX_TARDINESS, squared = flags & SB_FLAG_SQUARED;
   const bool penalty = flags & SB_FLAG_LATE_PENALTY, completion_penalty = flags & SB_FLAG_COMPLETION_PENALTY;
   const bool worst = flags & SB_FLAG_WORST_MAKESPAN, mean = flags & SB_FLAG_MEAN_MAKESPAN;
+  const bool worst_t = flags & SB_FLAG_WORST_TARDINESS, mean_t = flags & SB_FLAG_MEAN_TARDINESS;
+  if (worst_t && mean_t)
+    return fail(SB_ERR_ARG, "SB_FLAG_WORST_TARDINESS and SB_FLAG_MEAN_TARDINESS are two objectives: pass one");
+  if ((worst_t || mean_t) && !(sum && due))
+    return fail(SB_ERR_ARG, "%s scores the tardiness form over runtime scenarios: it needs SB_FLAG_SUM_COMPLETION and "
+                "SB_FLAG_DUE", worst_t ? "SB_FLAG_WORST_TARDINESS" : "SB_FLAG_MEAN_TARDINESS");
+  if ((worst_t || mean_t) && (late || max_tardiness || squared || penalty || completion_penalty || lateness || worst ||
+                              mean))
+    return fail(SB_ERR_ARG, "%s cannot be combined with SB_FLAG_LATE_COUNT, SB_FLAG_MAX_TARDINESS, SB_FLAG_SQUARED, "
+                "SB_FLAG_LATE_PENALTY, SB_FLAG_COMPLETION_PENALTY, SB_FLAG_MAX_LATENESS, SB_FLAG_WORST_MAKESPAN or "
+                "SB_FLAG_MEAN_MAKESPAN", worst_t ? "SB_FLAG_WORST_TARDINESS" : "SB_FLAG_MEAN_TARDINESS");
   if (worst && mean)
     return fail(SB_ERR_ARG, "SB_FLAG_WORST_MAKESPAN and SB_FLAG_MEAN_MAKESPAN are two objectives: pass one");
   if ((worst || mean) && (sum || weighted || due || lateness || late || max_tardiness || squared || penalty ||
@@ -643,15 +654,27 @@ static int decode_objective(unsigned flags, Objective* o) {
   else if (squared) o->obj = Obj::SquaredTardiness;
   else if (penalty) o->obj = Obj::LatePenalty;
   else if (completion_penalty) o->obj = Obj::CompletionPenalty;
+  else if (worst_t) o->obj = Obj::WorstTardiness;
+  else if (mean_t) o->obj = Obj::MeanTardiness;
   else if (due) o->obj = Obj::Tardiness;
   else o->obj = weighted ? Obj::WeightedSum : Obj::Sum;
   return SB_OK;
 }
 
-// the objectives folded from the tardiness form (SB_FLAG_DUE): their scores reach +0, which no plan can beat
+// the objectives folded from the tardiness form (SB_FLAG_DUE): their scores reach +0, which no plan can beat (run with
+// every due date +0, as the worst and mean completion time, the scenario forms never do with a nonzero runtime)
 static bool tardiness_form(Obj o) {
   return o == Obj::Tardiness || o == Obj::LateCount || o == Obj::MaxTardiness || o == Obj::SquaredTardiness ||
-         o == Obj::LatePenalty;
+         o == Obj::LatePenalty || o == Obj::WorstTardiness || o == Obj::MeanTardiness;
+}
+// the flag that names a scenario form, for messages
+static const char* scenario_flag_name(Obj o) {
+  switch (o) {
+    case Obj::WorstMakespan: return "SB_FLAG_WORST_MAKESPAN";
+    case Obj::MeanMakespan: return "SB_FLAG_MEAN_MAKESPAN";
+    case Obj::WorstTardiness: return "SB_FLAG_WORST_TARDINESS";
+    default: return "SB_FLAG_MEAN_TARDINESS";
+  }
 }
 
 // decode_objective, then the per-job arrays the objective reads (and SB_FLAG_RELEASE's) must be set on the handle
@@ -676,14 +699,14 @@ static int check_per_job(const sb_handle* h, unsigned flags, Objective* o) {
   if ((flags & SB_FLAG_RELEASE) && !h->has_r)
     return fail(SB_ERR_STATE, "SB_FLAG_RELEASE needs sb_set_release (sb_set_table clears the release dates)");
   if (obj_scenario(o->obj)) {
-    const char* name = o->obj == Obj::WorstMakespan ? "SB_FLAG_WORST_MAKESPAN" : "SB_FLAG_MEAN_MAKESPAN";
+    const char* name = scenario_flag_name(o->obj);
     if (!h->has_f) return fail(SB_ERR_STATE, "%s needs sb_set_scenarios (sb_set_table clears the scenarios)", name);
     if (flags & SB_FLAG_ALT_WARPSCAN)
       return fail(SB_ERR_UNSUPPORTED, "%s is not available with SB_FLAG_ALT_WARPSCAN", name);
     const int SG = ((flags & SB_FLAG_REDUCED) ? 1 : h->S) * kSlots;
-    const size_t need = scenario_smem(h->J, SG, h->scen_K, h->nodes, flags);
+    const size_t need = scenario_smem(h->J, SG, h->scen_K, h->nodes, flags, o->obj);
     if (need > h->dev.smem_optin)
-      return fail(SB_ERR_UNSUPPORTED, "%s: the %d scenario tables of %d x %d cells (%zu bytes with the release dates "
+      return fail(SB_ERR_UNSUPPORTED, "%s: the %d scenario tables of %d x %d cells (%zu bytes with the per-job arrays "
                   "and node states) must fit in one CTA's shared memory (%zu bytes); pass SB_FLAG_REDUCED or fewer "
                   "scenarios", name, h->scen_K, h->J, SG, need, h->dev.smem_optin);
   }
@@ -911,7 +934,9 @@ int sb_eval_scenarios(sb_handle* h, const uint8_t* opt, const void* prio, int64_
   EvalCall c;
   rc = make_call(h, opt, prio, B, row_stride, flags, &c);
   if (rc) return rc;
-  if (!obj_scenario(c.obj)) return fail(SB_ERR_ARG, "sb_eval_scenarios needs SB_FLAG_WORST_MAKESPAN or SB_FLAG_MEAN_MAKESPAN");
+  if (!obj_scenario(c.obj))
+    return fail(SB_ERR_ARG, "sb_eval_scenarios needs SB_FLAG_WORST_MAKESPAN, SB_FLAG_MEAN_MAKESPAN, "
+                "SB_FLAG_WORST_TARDINESS or SB_FLAG_MEAN_TARDINESS");
   if (B > 0 && !makespans_out) return fail(SB_ERR_ARG, "makespans_out is null");
   c.out = score_out;
   CK(eval_full_scenarios_launch(h->dev, c, makespans_out, h->stream));
@@ -1281,7 +1306,7 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
   // tables to the position-major kernel's shared memory), or unfused under HOOK_NO_FUSED
   const bool scen = obj_scenario(o.obj);
   const int mode = scen ? 0 : search_round_mode(h->dev, J, SGs, h->nodes, arrays);
-  const size_t pos_smem = scen ? scenario_smem(J, SGs, h->scen_K, h->nodes, p->flags)
+  const size_t pos_smem = scen ? scenario_smem(J, SGs, h->scen_K, h->nodes, p->flags, o.obj)
                                : search_pos_smem(J, SGs, h->nodes, 16, arrays);
   d.pos = (!no_fused && mode != 2 && pos_smem <= h->dev.smem_optin) ? 1 : 0;
   if (d.pos) CK(search_init_population_pos(d, h->stream));
@@ -1315,7 +1340,11 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
   // The completion penalty keeps this completion unit, with no sum of penalties added: in a front the penalties are
   // a barrier that the warm-started incumbent already clears, and must not heat the search past it.  With every p = 0
   // it is the completion unit bit for bit (a starting point, not a measured choice, DESIGN §3)
-  s.scale = isfinite(mk) ? (obj_sum(o.obj) ? mk / per : mk) : 1.0f;
+  // The tardiness scenario forms take the tardiness unit: the incumbent's score per unit weight (the worst or the sum
+  // over K scenarios of a total, so per job as the sum forms), floored below (a starting point, not a measured choice,
+  // DESIGN §3)
+  const bool scen_t = o.obj == Obj::WorstTardiness || o.obj == Obj::MeanTardiness;
+  s.scale = isfinite(mk) ? ((obj_sum(o.obj) || scen_t) ? mk / per : mk) : 1.0f;
   if (tardiness_form(o.obj) && isfinite(mk)) {
     // tardiness can be 0 or tiny at the incumbent: the unit is at least the weighted mean of each job's smallest
     // proposable runtime, the size of the score change one move makes
@@ -1348,6 +1377,9 @@ int sb_search_init(sb_handle* h, const sb_search_params* p, const uint8_t* warm_
     // which is the tardiness unit bit for bit when every p = 0 (a starting point, not a measured choice, DESIGN §3)
     else if (o.obj == Obj::LatePenalty)
       s.scale = std::max(s.scale, static_cast<float>((move + h->p_sum) / (weighted ? h->w_sum : static_cast<double>(J))));
+    // the mean tardiness scores the sum of K totals: K times the floor of one
+    else if (o.obj == Obj::MeanTardiness)
+      s.scale = std::max(s.scale, static_cast<float>(h->scen_K * move / (weighted ? h->w_sum : static_cast<double>(J))));
     else s.scale = std::max(s.scale, static_cast<float>(move / (weighted ? h->w_sum : static_cast<double>(J))));
   }
   // the late count moves in steps of one job's weight and is 0 at many incumbents: its unit is the count of every job,
@@ -1626,8 +1658,9 @@ int sb_search_seed_lpt(sb_handle* h) {
   const float* tmin = h->h_tmin.data();
   const Obj obj = s.obj.obj;
   // shortest first: the order that favours the sum (and, below, the tie-break of the due-date orders)
-  // the scenario forms seed as the makespan does, on the nominal table
-  const bool spt = obj != Obj::Makespan && obj != Obj::TailMakespan && !obj_scenario(obj);
+  // the scenario forms seed as their step's form does, on the nominal table: the makespan's orders, or the tardiness
+  // form's EDD orders (which with every due date +0 are the SPT / WSPT orders of the completion forms)
+  const bool spt = step_obj(obj) != Obj::Makespan && obj != Obj::TailMakespan;
   // weighted sum: Smith's rule (WSPT), ascending rt / w; with unit weights exactly the SPT order
   const bool wspt = spt && s.obj.weighted;
   // the due-date objectives: earliest due date first (EDD), ties by rt / w (rt with unit weights), then by job index;

@@ -19,7 +19,7 @@ constexpr float kSentinel = 1.0e6f;  // reference's "unprofiled" runtime, Perfor
 __device__ __forceinline__ float inf_f() { return __int_as_float(0x7f800000); }
 
 // ---------------------------------------------------------------- the objective
-// The ten scores the kernels compute, and the SB_FLAG_* bits that select each (sb_api.cu: decode_objective; every
+// The fourteen scores the kernels compute, and the SB_FLAG_* bits that select each (sb_api.cu: decode_objective; every
 // form also runs with SB_FLAG_RELEASE).  C is a job's completion, w its weight, d its due date, p its late penalty.
 //   Obj               flags                                              score
 //   Makespan          none                                               max C
@@ -35,20 +35,32 @@ __device__ __forceinline__ float inf_f() { return __int_as_float(0x7f800000); }
 //                                                                        sum (w C + (C > d ? p : 0))
 //   WorstMakespan     WORST_MAKESPAN                                     max_k M_k, M_k the makespan on scenario table k
 //   MeanMakespan      MEAN_MAKESPAN                                      sum_k M_k, left fold in scenario order
+//   WorstTardiness    SUM_COMPLETION | DUE | WORST_TARDINESS [| WEIGHTED] max_k S_k, S_k Tardiness's score on table k
+//   MeanTardiness     SUM_COMPLETION | DUE | MEAN_TARDINESS [| WEIGHTED]  sum_k S_k, left fold in scenario order
+// (the host runs the worst and mean completion time as these two with every due date +0: C >= +0, so the term
+// w max(C - 0, 0) is w C bit for bit)
 // Every other combination of those flags is refused.  The history of each form is in DESIGN.md.  New forms go at the
 // end: a kernel's symbol holds its form's value.
 enum class Obj {
   Makespan, TailMakespan, Sum, WeightedSum, Tardiness, LateCount, MaxTardiness, SquaredTardiness, LatePenalty,
-  CompletionPenalty, WorstMakespan, MeanMakespan
+  CompletionPenalty, WorstMakespan, MeanMakespan, WorstTardiness, MeanTardiness
 };
-// the score folds the makespans of K scenario tables (sb_set_scenarios); each pass is the makespan form's
-__host__ __device__ constexpr bool obj_scenario(Obj o) { return o == Obj::WorstMakespan || o == Obj::MeanMakespan; }
-// the form ls_step folds inside one pass: the makespan for the scenario forms, the objective itself otherwise
-__host__ __device__ constexpr Obj step_obj(Obj o) { return obj_scenario(o) ? Obj::Makespan : o; }
-// one scenario's makespan m folded into the score: an exact max, or a sum rounded at every add (both start at +0)
+// the score folds one score per scenario table (sb_set_scenarios): the makespans, or the total tardiness
+__host__ __device__ constexpr bool obj_scenario(Obj o) {
+  return o == Obj::WorstMakespan || o == Obj::MeanMakespan || o == Obj::WorstTardiness || o == Obj::MeanTardiness;
+}
+// the form ls_step folds inside one pass: the makespan or the tardiness for the scenario forms, the objective itself
+// otherwise
+__host__ __device__ constexpr Obj step_obj(Obj o) {
+  return (o == Obj::WorstMakespan || o == Obj::MeanMakespan)     ? Obj::Makespan
+         : (o == Obj::WorstTardiness || o == Obj::MeanTardiness) ? Obj::Tardiness
+                                                                 : o;
+}
+// one scenario's score m folded into the score: an exact max (the worst forms), or a sum rounded at every add (the
+// mean forms); both start at +0
 template <Obj kObj>
 __device__ __forceinline__ float scenario_fold(float score, float m) {
-  return kObj == Obj::WorstMakespan ? fmaxf(score, m) : __fadd_rn(score, m);
+  return (kObj == Obj::WorstMakespan || kObj == Obj::WorstTardiness) ? fmaxf(score, m) : __fadd_rn(score, m);
 }
 // the score is a sum over the jobs, folded in schedule order
 __host__ __device__ constexpr bool obj_sum(Obj o) {
@@ -58,12 +70,14 @@ __host__ __device__ constexpr bool obj_sum(Obj o) {
 // the score reads the job weights (the caller's, or unit weights without SB_FLAG_WEIGHTED)
 __host__ __device__ constexpr bool obj_weights(Obj o) {
   return o == Obj::WeightedSum || o == Obj::Tardiness || o == Obj::LateCount || o == Obj::MaxTardiness ||
-         o == Obj::SquaredTardiness || o == Obj::LatePenalty || o == Obj::CompletionPenalty;
+         o == Obj::SquaredTardiness || o == Obj::LatePenalty || o == Obj::CompletionPenalty ||
+         o == Obj::WorstTardiness || o == Obj::MeanTardiness;
 }
 // the score reads the due-date array: the due dates, or TailMakespan's tails
 __host__ __device__ constexpr bool obj_due(Obj o) {
   return o == Obj::TailMakespan || o == Obj::Tardiness || o == Obj::LateCount || o == Obj::MaxTardiness ||
-         o == Obj::SquaredTardiness || o == Obj::LatePenalty || o == Obj::CompletionPenalty;
+         o == Obj::SquaredTardiness || o == Obj::LatePenalty || o == Obj::CompletionPenalty ||
+         o == Obj::WorstTardiness || o == Obj::MeanTardiness;
 }
 // the score reads the late-penalty array (sb_set_penalty)
 __host__ __device__ constexpr bool obj_penalty(Obj o) {

@@ -678,18 +678,21 @@ struct GenericArgs {
 };
 
 // One pass of the scenario forms over a candidate's J steps on the table st.tab points to: the batched loop of
-// k_eval_generic below, with the makespan form's step (whose kernels keep their own copy of the loop, so that their
-// code stays what it was).
+// k_eval_generic below, with step_obj(OBJ)'s step (whose kernels keep their own copy of the loop, so that their code
+// stays what it was).  The tardiness forms gather the batch's weights and due dates with its runtimes; the makespan
+// forms read neither.
 template <int PB, Obj OBJ, bool R, class Lane>
 __device__ __forceinline__ float generic_pass(Lane& st, const GenericArgs& a, const uint8_t* prow) {
   static_assert(obj_scenario(OBJ), "the scenario forms only");
+  constexpr bool kWD = obj_weights(step_obj(OBJ));  // the tardiness step: weights and due dates
+  static_assert(kWD == obj_due(step_obj(OBJ)), "a scenario step reads both arrays or neither");
   st.reset(a.nodes);
   constexpr int BATCH = 16;
   int i = 0;
   for (; i + BATCH <= a.J; i += BATCH) {
     int js[BATCH], os[BATCH];
     float rts[BATCH];
-    [[maybe_unused]] float xs[BATCH];
+    [[maybe_unused]] float xs[BATCH], ws[BATCH], ds[BATCH];
 #pragma unroll
     for (int t = 0; t < BATCH; ++t) js[t] = PB == 1 ? prow[i + t] : reinterpret_cast<const uint16_t*>(prow)[i + t];
 #pragma unroll
@@ -700,8 +703,15 @@ __device__ __forceinline__ float generic_pass(Lane& st, const GenericArgs& a, co
 #pragma unroll
       for (int t = 0; t < BATCH; ++t) xs[t] = st.lookup_r(js[t]);
     }
+    if constexpr (kWD) {
 #pragma unroll
-    for (int t = 0; t < BATCH; ++t) st.step_resolved(os[t], rts[t], t & 1, 0.f, 0.f, R ? xs[t] : 0.f, 0.f);
+      for (int t = 0; t < BATCH; ++t) ws[t] = st.lookup_w(js[t]);
+#pragma unroll
+      for (int t = 0; t < BATCH; ++t) ds[t] = st.lookup_d(js[t]);
+    }
+#pragma unroll
+    for (int t = 0; t < BATCH; ++t)
+      st.step_resolved(os[t], rts[t], t & 1, kWD ? ws[t] : 0.f, kWD ? ds[t] : 0.f, R ? xs[t] : 0.f, 0.f);
   }
   for (; i < a.J; ++i) st.step(PB == 1 ? prow[i] : reinterpret_cast<const uint16_t*>(prow)[i]);
   return st.result(a.nodes);
@@ -825,9 +835,9 @@ struct FullArgs {
 template <int PB, bool INT, Obj OBJ = Obj::Makespan, bool R = false>
 __global__ void __launch_bounds__(128) k_eval_full(const FullArgs a);
 
-// obj_scenario(OBJ): the slot-exact makespan of each scenario table (start times and slot masks are not written: the
-// host takes them from the makespan form on the nominal table), M_k into a.start ([B][K]), folded into the score in
-// scenario order
+// obj_scenario(OBJ): the slot-exact score of each scenario table, the makespan M_k or the tardiness form's total S_k
+// (start times and slot masks are not written: the host takes them from the makespan form on the nominal table), into
+// a.start ([B][K]), folded into the score in scenario order
 template <int PB, bool INT, Obj OBJ, bool R>
 __device__ __forceinline__ void eval_full_scenarios(const FullArgs& a) {
   const long long nthreads = static_cast<long long>(gridDim.x) * blockDim.x;
@@ -868,7 +878,10 @@ __device__ __forceinline__ void eval_full_scenarios(const FullArgs& a) {
         const float nxt = s + hold;
         for (int g = 0; g < kSlots; ++g)
           if ((taken >> g) & 1u) rd[g] = nxt;
-        mk = fmaxf(mk, s + rt);
+        if constexpr (step_obj(OBJ) == Obj::Tardiness)
+          mk = __fadd_rn(mk, __fmul_rn(__ldg(a.w + j), fmaxf(__fsub_rn(s + rt, __ldg(a.d + j)), 0.f)));
+        else
+          mk = fmaxf(mk, s + rt);
       }
       if (a.start) a.start[b * a.K + sc] = mk;
       score = scenario_fold<OBJ>(score, mk);
@@ -1183,7 +1196,7 @@ cudaError_t eval_full_scenarios_launch(const Device& dev, const EvalCall& c, flo
   FullArgs a = {};
   a.tab = c.tab; a.J = c.J; a.SG = c.SG; a.opt = c.opt; a.prio = c.prio; a.B = c.B;
   a.stride_o = c.stride_o; a.stride_p = c.stride_p; a.nodes = c.nodes < 1 ? 1 : c.nodes;
-  a.out = c.out; a.r = c.r;
+  a.out = c.out; a.r = c.r; a.w = c.w; a.d = c.d;
   a.K = c.K;
   a.start = mks;
   long long blocks = (c.B + 127) / 128;

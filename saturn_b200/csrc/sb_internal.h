@@ -34,8 +34,11 @@ static_assert(((HOOK_FORCE_GENERIC | HOOK_NO_STREAM | HOOK_NO_FUSED | HOOK_NO_IN
                 SB_FLAG_FOLD_PREV | SB_FLAG_ALT_WARPSCAN | SB_FLAG_SUM_COMPLETION | SB_FLAG_WEIGHTED |
                 SB_FLAG_DUE | SB_FLAG_RELEASE | SB_FLAG_MAX_LATENESS | SB_FLAG_LATE_COUNT |
                 SB_FLAG_MAX_TARDINESS | SB_FLAG_SQUARED | SB_FLAG_LATE_PENALTY | SB_FLAG_COMPLETION_PENALTY |
-                SB_FLAG_WORST_MAKESPAN | SB_FLAG_MEAN_MAKESPAN)) == 0,
+                SB_FLAG_WORST_MAKESPAN | SB_FLAG_MEAN_MAKESPAN | SB_FLAG_WORST_TARDINESS | SB_FLAG_MEAN_TARDINESS)) == 0,
               "the test hooks share no bit with the SB_FLAG_* flags");
+// The flag space is full up to the hooks: SB_FLAG_MEAN_TARDINESS (0x80000) is the last free bit below HOOK_NO_REORDER.
+// A new objective needs a bit freed, or a second word.
+static_assert((SB_FLAG_MEAN_TARDINESS << 1) == HOOK_NO_REORDER, "the flags end where the hooks begin");
 
 // Debug options of the streamed tile kernel (sb_debug_tile_options): kept on the handle, not in the flags word, and
 // read by sb_eval only.  saturn_b200/_lib.py mirrors the names.
@@ -91,8 +94,12 @@ decltype(auto) with_scenario_types(int pb, unsigned flags, Obj obj, F&& f) {
   return with_pb(pb, [&](auto PB) {
     return with_bool(flags & SB_FLAG_INTEGER_STARTS, [&](auto INT) {
       return with_bool(flags & SB_FLAG_RELEASE, [&](auto R) {
-        return obj == Obj::WorstMakespan ? f(PB, INT, obj_c<Obj::WorstMakespan>{}, R)
-                                         : f(PB, INT, obj_c<Obj::MeanMakespan>{}, R);
+        switch (obj) {
+          case Obj::WorstMakespan: return f(PB, INT, obj_c<Obj::WorstMakespan>{}, R);
+          case Obj::WorstTardiness: return f(PB, INT, obj_c<Obj::WorstTardiness>{}, R);
+          case Obj::MeanTardiness: return f(PB, INT, obj_c<Obj::MeanTardiness>{}, R);
+          default: return f(PB, INT, obj_c<Obj::MeanMakespan>{}, R);
+        }
       });
     });
   });
@@ -242,8 +249,8 @@ cudaError_t build_valid_launch(const float* tmin, const uint8_t* args, int J, in
 // scenario tables: out[k][j][c] = fp32(f[k][j] * tab[j][c]) for the K factor rows f[K][J] (device) and a table of J
 // rows of SG cells
 cudaError_t scale_tables_launch(const float* tab, int J, int SG, const float* f, int K, float* out, cudaStream_t st);
-// shared memory the position-major kernel needs for K scenario tables of J x SG cells beside what it already stages;
-// every scenario route is held to it (sb_api.cu: check_per_job)
-size_t scenario_smem(int J, int SG, int K, int nodes, unsigned flags);
+// shared memory the position-major kernel needs for K scenario tables of J x SG cells beside the per-job arrays the
+// objective reads (job_arrays) and the node states; every scenario route is held to it (sb_api.cu: check_per_job)
+size_t scenario_smem(int J, int SG, int K, int nodes, unsigned flags, Obj obj);
 
 }  // namespace sb

@@ -428,8 +428,9 @@ __device__ __forceinline__ PosMove make_pos_move_win(const SearchFuse& sf, int r
 // OBJ: the objective (sb_common.cuh), folded by ls_step.  R: no job starts before its release date (SB_FLAG_RELEASE,
 // any objective).  The per-job arrays they read (stage_job_array, sb_lane.cuh) follow the table in shared memory with TAB = 0 and are
 // read from global memory (ld.global.nc) with TAB = 1 / 2.  obj_scenario(OBJ): the K scenario tables are staged back to
-// back (TAB = 0 only), and every evaluation runs one pass of the makespan form per table (no snapshots: the host runs
-// these forms without incremental rounds) and folds the K makespans into the score.
+// back (TAB = 0 only), and every evaluation runs one pass of step_obj(OBJ) per table (no snapshots: the host runs
+// these forms without incremental rounds) and folds the K scores into the score; the tardiness forms stage and read
+// the weights and due dates as the tardiness form does.
 template <int PB, bool INT, bool MULTI, bool EVAL = false, int TAB = 0, Obj OBJ = Obj::Makespan, bool R = false>
 __global__ void __launch_bounds__(512, 1) k_search_pos(const PosArgs a) {
   static_assert(TAB == 0 || (EVAL && !MULTI), "tables outside the CTA's shared memory: scoring only, one node");
@@ -784,8 +785,8 @@ size_t search_pos_smem(int J, int SG, int nodes, int warps, int arrays) {
   return tab_bytes + arrays * job_array_bytes(J) + 16 + static_cast<size_t>(warps) * (nodes > 1 ? nodes * 1024u : 0u);
 }
 
-size_t scenario_smem(int J, int SG, int K, int nodes, unsigned flags) {
-  return search_pos_smem(J, SG * K, nodes, 16, (flags & SB_FLAG_RELEASE) ? 1 : 0);
+size_t scenario_smem(int J, int SG, int K, int nodes, unsigned flags, Obj obj) {
+  return search_pos_smem(J, SG * K, nodes, 16, job_arrays(obj, flags));
 }
 
 using PosKernel = void (*)(PosArgs);
@@ -860,7 +861,7 @@ cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float
     return eval_pos_far_launch(dev, a, tab_home, s.pb, flags, obj, st);
   }
   const int warps = 16;
-  const size_t smem = scen ? scenario_smem(s.J, SG, K, s.nodes, flags)
+  const size_t smem = scen ? scenario_smem(s.J, SG, K, s.nodes, flags, obj)
                            : search_pos_smem(s.J, SG, s.nodes, warps, job_arrays(obj, flags));
   if (smem > dev.smem_optin) return cudaErrorNotSupported;
   const long long ntiles = (count + 31) / 32;
@@ -884,7 +885,7 @@ cudaError_t search_pos_launch(const Device& dev, const SearchDev& s, const float
 int eval_pos_home(const Device& dev, int J, int SG, int nodes, unsigned flags, Obj obj, int K) {
   // the scenario tables: shared memory or nowhere (check_per_job has already held them to scenario_smem)
   if (obj_scenario(obj))
-    return !(flags & (HOOK_TABLE_PAIR | HOOK_TABLE_GLOBAL)) && scenario_smem(J, SG, K, nodes, flags) <= dev.smem_optin ? 0 : -1;
+    return !(flags & (HOOK_TABLE_PAIR | HOOK_TABLE_GLOBAL)) && scenario_smem(J, SG, K, nodes, flags, obj) <= dev.smem_optin ? 0 : -1;
   const bool pair_ok = nodes == 1 && static_cast<size_t>(pos_tab_half(J, SG)) * 4 + 16 <= dev.smem_optin;
   if (flags & HOOK_TABLE_PAIR) return pair_ok ? 2 : -1;
   if (flags & HOOK_TABLE_GLOBAL) return nodes == 1 ? 1 : -1;

@@ -69,15 +69,27 @@ SCENARIO_OBJECTIVES = {
     "worst_makespan": Objective(_lib.FLAG_WORST_MAKESPAN, False, False),
     "mean_makespan": Objective(_lib.FLAG_MEAN_MAKESPAN, False, False),
 }
+# The tardiness forms over the same scenarios: the worst total (weighted) tardiness, max_k S_k, and the mean, scored as
+# sum_k S_k, where S_k is the "tardiness" / "weighted_tardiness" score of the same options and order on scenario table
+# k.  Not the per-task maximum tardiness ("max_tardiness").  With every due date 0 they score the worst and the mean
+# (weighted) completion time (solver.solve's "worst_completion" and "mean_completion").  A table of their own, held to
+# oracle/ref_scenario_tardiness.py; objective_spec and objective_flag look names up here as well.
+SCENARIO_TARDINESS_OBJECTIVES = {
+    "worst_tardiness": Objective(_SUM | _DUE | _lib.FLAG_WORST_TARDINESS, False, True),
+    "weighted_worst_tardiness": Objective(_SUM | _DUE | _lib.FLAG_WORST_TARDINESS | _W, True, True),
+    "mean_tardiness": Objective(_SUM | _DUE | _lib.FLAG_MEAN_TARDINESS, False, True),
+    "weighted_mean_tardiness": Objective(_SUM | _DUE | _lib.FLAG_MEAN_TARDINESS | _W, True, True),
+}
 
 
 def objective_spec(objective: str) -> Objective:
     """The table entry of an objective name; raises SolverError for a name that is not one."""
     spec = _OBJECTIVES.get(objective) or COMPLETION_PENALTY_OBJECTIVES.get(objective) or \
-        SCENARIO_OBJECTIVES.get(objective)
+        SCENARIO_OBJECTIVES.get(objective) or SCENARIO_TARDINESS_OBJECTIVES.get(objective)
     if spec is None:
         from .solver import SolverError
-        names = list(_OBJECTIVES) + list(COMPLETION_PENALTY_OBJECTIVES) + list(SCENARIO_OBJECTIVES)
+        names = list(_OBJECTIVES) + list(COMPLETION_PENALTY_OBJECTIVES) + list(SCENARIO_OBJECTIVES) + \
+            list(SCENARIO_TARDINESS_OBJECTIVES)
         raise SolverError("objective must be one of %s, not %r" % (", ".join(map(repr, names)), objective))
     return spec
 
@@ -196,7 +208,8 @@ def _require_due(due, objective: str):
     """The tardiness objectives (the maximum tardiness among them), the late counts and the maximum lateness score
     against the due dates of set_due: refuse them, before any device call, on an engine that has none (set_table
     clears them)."""
-    spec = _OBJECTIVES.get(objective) or COMPLETION_PENALTY_OBJECTIVES.get(objective)
+    spec = _OBJECTIVES.get(objective) or COMPLETION_PENALTY_OBJECTIVES.get(objective) or \
+        SCENARIO_TARDINESS_OBJECTIVES.get(objective)
     if spec is not None and spec.due and due is None:
         from .solver import SolverError
         raise SolverError("objective=%r needs due dates: call set_due after set_table" % (objective,))
@@ -355,8 +368,9 @@ class Engine:
     def set_scenarios(self, f) -> "Engine":
         """K runtime scenarios, f[K][J] factors (1 <= K <= 8, each finite and > 0, converted to fp32), for
         objective="worst_makespan", which scores max_k M_k, and "mean_makespan", which scores sum_k M_k: M_k is the
-        makespan of the same options and order on the table whose row j is fp32(f[k][j] * T[j]).  None clears them;
-        set_table clears them too."""
+        makespan of the same options and order on the table whose row j is fp32(f[k][j] * T[j]).  The same scenarios
+        serve SCENARIO_TARDINESS_OBJECTIVES, which score max_k S_k or sum_k S_k with S_k the (weighted) tardiness total
+        on that table.  None clears them; set_table clears them too."""
         if f is None:
             check(self._lib.sb_set_scenarios(self._h, None, 0, 0))
             self.scenarios = None
@@ -372,7 +386,7 @@ class Engine:
     def _flags(self, integer_starts: bool, reduced: bool, objective: str) -> int:
         _require_due(self.due, objective)
         _require_penalty(self.penalty, objective)
-        if objective in SCENARIO_OBJECTIVES and self.scenarios is None:
+        if (objective in SCENARIO_OBJECTIVES or objective in SCENARIO_TARDINESS_OBJECTIVES) and self.scenarios is None:
             from .solver import SolverError
             raise SolverError("objective=%r needs runtime scenarios: call set_scenarios after set_table" % (objective,))
         return _flags(integer_starts, reduced, objective) | self._release_flag()
@@ -484,7 +498,9 @@ class Engine:
 
     def eval_scenarios(self, opt: torch.Tensor, prio: torch.Tensor, integer_starts: bool = True, reduced: bool = False,
                        objective: str = "worst_makespan"):
-        """(score[B], makespans[B][K]) of every candidate under a scenario objective, slot-exact (sb_eval_scenarios)."""
+        """(score[B], per_scenario[B][K]) of every candidate under a scenario objective, slot-exact
+        (sb_eval_scenarios): per_scenario holds each scenario's makespan M_k, or under the tardiness forms its total
+        (weighted) tardiness S_k."""
         B, stride = self._check_cands(opt, prio, True)
         K = 0 if self.scenarios is None else self.scenarios.shape[0]
         score = torch.empty(B, dtype=torch.float32, device=self.device)

@@ -55,7 +55,7 @@ def orchestrate(task_list, log=False, interval=1000, gurobi=True, *,
     saturn.executor.execute; returns the list of per-interval records (plan makespan, tasks run).
 
     A `due` mapping Task -> due date in `solver_kwargs` (objective="tardiness", "max_lateness", "late_tasks",
-    "squared_tardiness", "late_penalty" or "completion_penalty") is
+    "squared_tardiness", "late_penalty", "completion_penalty", "worst_tardiness" or "mean_tardiness") is
     measured from the first plan's t = 0: the solve for interval n plans from n * interval on, so it receives
     {t: d - n * interval}, and the lateness each solve reports is against the original due dates (both sides shift
     alike).  A sequence `due` raises SolverError, since the task list shrinks from interval to interval.  A `release`
@@ -69,9 +69,12 @@ def orchestrate(task_list, log=False, interval=1000, gurobi=True, *,
     remain, not of the whole flow time.  Under objective="late_penalty" and "completion_penalty" a `penalty` mapping
     Task -> penalty is passed to every solve unchanged: a penalty is what missing the due date costs, whenever the
     plan is made; a sequence `penalty` raises SolverError, as a sequence `due` does.  Under
-    objective="worst_makespan" and "mean_makespan" a `scenarios` mapping Task -> K runtime factors is passed to every
-    solve unchanged: a factor scales a task's remaining work as it scales the whole task; a sequence `scenarios`
-    raises SolverError, as a sequence `due` does.
+    objective="worst_makespan", "mean_makespan", "worst_tardiness", "mean_tardiness", "worst_completion" and
+    "mean_completion" a `scenarios` mapping Task -> K runtime factors is passed to every solve unchanged: a factor
+    scales a task's remaining work as it scales the whole task; a sequence `scenarios` raises SolverError, as a
+    sequence `due` does.  Under "worst_tardiness" and "mean_tardiness" the due dates shift as above, so every
+    scenario's tardiness is against the original due dates; "worst_completion" and "mean_completion" take no due
+    dates and, like "completion", count each interval's completion times from its start.
     """
     logging.basicConfig(level=logging.INFO if log else logging.WARNING,
                         format="%(asctime)s %(levelname)-8s %(message)s", datefmt="%Y-%m-%d %H:%M:%S")

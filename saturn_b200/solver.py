@@ -172,6 +172,11 @@ FP32_MAX = float(np.finfo(np.float32).max)
 SQUARE_BOUND = float(1 << 50)   # a squared tardiness inside the horizon, (2^25)^2, with |d| < 2^24
 _SQUARED = ("squared_tardiness", "squared_flow")   # the solve() objectives that run as the squared tardiness
 _SCENARIO = ("worst_makespan", "mean_makespan")    # the solve() objectives over runtime scenarios (scenarios=...)
+# the worst and mean (weighted) total tardiness and completion time over the same scenarios: the completion forms run
+# as the tardiness forms with every due date +0
+_SCENARIO_TARDINESS = ("worst_tardiness", "mean_tardiness")
+_SCENARIO_COMPLETION = ("worst_completion", "mean_completion")
+_SCENARIO_ALL = _SCENARIO + _SCENARIO_TARDINESS + _SCENARIO_COMPLETION
 
 
 def _engine(devices=None):
@@ -229,10 +234,11 @@ def _check_horizon(T, found_makespan=None, release=None, tails=None):
 
 def _check_objective(objective, hysteresis=False, release=None):
     if objective not in ("makespan", "completion", "tardiness", "max_lateness", "late_tasks", "max_stretch",
-                         "squared_tardiness", "squared_flow", "late_penalty", "completion_penalty") + _SCENARIO:
+                         "squared_tardiness", "squared_flow", "late_penalty", "completion_penalty") + _SCENARIO_ALL:
         raise SolverError("objective must be 'makespan', 'completion', 'tardiness', 'max_lateness', 'late_tasks', "
                           "'max_stretch', 'squared_tardiness', 'squared_flow', 'late_penalty', "
-                          "'completion_penalty', 'worst_makespan' or 'mean_makespan', not %r" % (objective,))
+                          "'completion_penalty', 'worst_makespan', 'mean_makespan', 'worst_tardiness', "
+                          "'mean_tardiness', 'worst_completion' or 'mean_completion', not %r" % (objective,))
     if objective != "makespan" and hysteresis:
         raise SolverError("hysteresis=True compares plans by makespan (milp.py:363-442); it is not defined for "
                           "objective=%r" % (objective,))
@@ -266,9 +272,10 @@ def _resolve_weights(weights, objective, J, task_list=None):
         raise SolverError("objective='max_stretch' weighs every task by 1 / its fastest runtime: it takes no weights "
                           "(for a weighted mean stretch use objective='completion' with weights)")
     if objective not in ("completion", "tardiness", "late_tasks", "squared_tardiness", "squared_flow", "late_penalty",
-                         "completion_penalty"):
+                         "completion_penalty") + _SCENARIO_TARDINESS + _SCENARIO_COMPLETION:
         raise SolverError("weights apply to objective='completion', 'tardiness', 'late_tasks', 'squared_tardiness', "
-                          "'squared_flow', 'late_penalty' or 'completion_penalty' only, not to %r" % (objective,))
+                          "'squared_flow', 'late_penalty', 'completion_penalty', 'worst_tardiness', "
+                          "'mean_tardiness', 'worst_completion' or 'mean_completion' only, not to %r" % (objective,))
     weights = _per_task(weights, "weights", task_list)
     from .engine import weights_f32
     w32 = weights_f32(weights, J)
@@ -288,12 +295,18 @@ def _resolve_due(due, objective, J, task_list=None):
     if objective in ("max_stretch", "squared_flow") and due is not None:
         raise SolverError("objective=%r measures every task from its release date: it takes no due dates "
                           "(pass release=...)" % (objective,))
+    if objective in _SCENARIO_COMPLETION:
+        if due is not None:
+            raise SolverError("objective=%r scores completion times: it takes no due dates (for the tardiness over "
+                              "scenarios use objective='worst_tardiness' or 'mean_tardiness')" % (objective,))
+        # the tardiness forms with every due date +0 (C >= +0, so max(C - 0, 0) is C bit for bit)
+        return [0.0] * J, np.zeros(J, dtype=np.float32)
     if objective not in ("tardiness", "max_lateness", "late_tasks", "squared_tardiness", "late_penalty",
-                         "completion_penalty"):
+                         "completion_penalty") + _SCENARIO_TARDINESS:
         if due is not None:
             raise SolverError("due dates apply to objective='tardiness', 'max_lateness', 'late_tasks', "
-                              "'squared_tardiness', 'late_penalty' or 'completion_penalty' only, not to %r"
-                              % (objective,))
+                              "'squared_tardiness', 'late_penalty', 'completion_penalty', 'worst_tardiness' or "
+                              "'mean_tardiness' only, not to %r" % (objective,))
         return None, None
     if due is None:
         raise SolverError("objective=%r needs due dates (due=...)" % (objective,))
@@ -326,10 +339,12 @@ def _resolve_penalty(penalty, objective, J, task_list=None):
 def _resolve_scenarios(scenarios, objective, J, task_list=None):
     """The caller's runtime scenarios, J rows of K factors each (a sequence aligned with the tasks or T's rows, or with
     `task_list` a mapping Task -> K factors), as (float64 [K][J], fp32 [K][J] for the device), or (None, None) without
-    objective="worst_makespan" or "mean_makespan", which require them.  Raises SolverError before any device call."""
-    if objective not in _SCENARIO:
+    a scenario objective ("worst_makespan", "mean_makespan", "worst_tardiness", "mean_tardiness", "worst_completion"
+    or "mean_completion"), which require them.  Raises SolverError before any device call."""
+    if objective not in _SCENARIO_ALL:
         if scenarios is not None:
-            raise SolverError("scenarios apply to objective='worst_makespan' or 'mean_makespan' only, not to %r"
+            raise SolverError("scenarios apply to objective='worst_makespan', 'mean_makespan', 'worst_tardiness', "
+                              "'mean_tardiness', 'worst_completion' or 'mean_completion' only, not to %r"
                               % (objective,))
         return None, None
     if scenarios is None:
@@ -358,15 +373,21 @@ def _check_scenario_horizon(Tdev, f32, release=None):
             _check_horizon((f32[k][:, None, None] * Tdev).astype(np.float32), release=release)
 
 
-def _scenario_stats(rts, gpus, node, prio, f64, integer_starts, r64=None):
+def _scenario_stats(rts, gpus, node, prio, f64, integer_starts, r64=None, w64=None, d64=None, objective=None):
     """scenario_makespans (each scenario's makespan, K values), worst_makespan and mean_makespan of a plan's options and
     order, in float64: the list rule re-run on every scenario's runtimes f[k][t] * rt_t (the tasks' own runtimes), with
-    integer starts rounding each hold up as the device does."""
+    integer starts rounding each hold up as the device does.  With objective="worst_tardiness" / "mean_tardiness" also
+    scenario_tardiness (each scenario's total tardiness sum_t w_t max(C_tk - d_t, 0), unit weights without w64),
+    worst_tardiness and mean_tardiness; with "worst_completion" / "mean_completion" scenario_completion (each scenario's
+    sum_t w_t C_tk), worst_completion and mean_completion."""
     J = len(rts)
-    mks = []
+    w = [1.0] * J if w64 is None else [float(x) for x in w64]
+    d = [0.0] * J if d64 is None else [float(x) for x in d64]
+    mks, sums = [], []
     for k in range(f64.shape[0]):
         ready = {}
         mk = 0.0
+        total = 0.0
         for j in (int(x) for x in prio):
             rt = float(f64[k, j]) * float(rts[j])
             rd = ready.setdefault(int(node[j]), [0.0] * NSLOT)
@@ -379,8 +400,14 @@ def _scenario_stats(rts, gpus, node, prio, f64, integer_starts, r64=None):
             for g in sel:
                 rd[g] = nxt
             mk = max(mk, st + rt)
+            total += w[j] * max(st + rt - d[j], 0.0)
         mks.append(mk)
-    return {"scenario_makespans": mks, "worst_makespan": max(mks), "mean_makespan": sum(mks) / len(mks)}
+        sums.append(total)
+    out = {"scenario_makespans": mks, "worst_makespan": max(mks), "mean_makespan": sum(mks) / len(mks)}
+    if objective in _SCENARIO_TARDINESS + _SCENARIO_COMPLETION:
+        what = "tardiness" if objective in _SCENARIO_TARDINESS else "completion"
+        out.update({"scenario_" + what: sums, "worst_" + what: max(sums), "mean_" + what: sum(sums) / len(sums)})
+    return out
 
 
 def _resolve_release(release, J, task_list=None):
@@ -415,6 +442,9 @@ def _set_objective(eng, objective, w32, d32, r32=None, p32=None):
             return "weighted_squared_tardiness" if w32 is not None else "squared_tardiness"
         if objective in ("late_penalty", "completion_penalty"):
             return "weighted_" + objective if w32 is not None else objective
+        if objective in _SCENARIO_TARDINESS + _SCENARIO_COMPLETION:
+            form = objective.split("_")[0] + "_tardiness"   # the completion forms: every due date 0
+            return "weighted_" + form if w32 is not None else form
         return "weighted_tardiness" if w32 is not None else "tardiness"
     return "weighted_completion" if w32 is not None else objective
 
@@ -667,6 +697,18 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
     re-run in float64 from the plan's options and order on f * the tasks' own runtimes; last_stats["device_makespan"]
     holds the device's fp32 score (the worst makespan, or the sum of the K makespans).
 
+    The same scenarios serve the completion-time and tardiness users.  objective="worst_tardiness" or
+    "mean_tardiness" (with `due`, `weights` optional) minimises the largest, or the mean, over the K scenarios of the
+    TOTAL (weighted) tardiness sum_t w_t max(C_tk - d_t, 0) — the worst or mean of objective="tardiness", not the
+    per-task maximum tardiness of the engine's "max_tardiness".  objective="worst_completion" or "mean_completion"
+    (`weights` optional, `due` refused) does the same for the (weighted) completion time sum_t w_t C_tk, the classical
+    stochastic objective sum w E[C] for "mean_completion"; the device runs them as the tardiness forms with every due
+    date 0.  All four take `scenarios` (required), `release`, `nodes` and `devices`, and refuse `penalty` and
+    hysteresis=True, with SolverError before any device call.  last_stats then also holds ["scenario_tardiness"] (K
+    values), ["worst_tardiness"] and ["mean_tardiness"], or ["scenario_completion"], ["worst_completion"] and
+    ["mean_completion"], re-run in float64 as the makespans are; last_stats["device_makespan"] holds the device's
+    fp32 score (the worst total, or the sum of the K totals).
+
     Release dates.  `release` (a sequence aligned with task_list, or a mapping keyed by Task, in the runtimes' units
     from the plan's t = 0) keeps every task from starting before its release date, under every objective: a
     dataset or a parent checkpoint that is only ready later, a job that arrives tomorrow.  r <= 0 means already
@@ -741,7 +783,8 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
         chains = int(os.environ.get("SATURN_B200_CHAINS", 0))
         if chains <= 0:
             # about 131072 chains, rounded to whole waves of the round kernel (no partially filled last wave)
-            wave = (eng.search_wave(reduced=True, **({"objective": objective} if objective in _SCENARIO else {}))
+            wave = (eng.search_wave(reduced=True, **({"objective": search_objective} if objective in _SCENARIO_ALL
+                                                     else {}))
                     if hasattr(eng, "search_wave") else 0)
             chains = max(1, round((1 << 17) / wave)) * wave if wave > 0 else 1 << 17
     if rounds is None:
@@ -797,8 +840,9 @@ def solve(task_list, presolved=None, gurobi=True, threads=max(1, (os.cpu_count()
         last_stats.update(_late_penalty_stats(dec["start"], rts, w64, d64, p64))
     elif objective == "completion_penalty":
         last_stats.update(_completion_penalty_stats(dec["start"], rts, w64, d64, p64))
-    elif objective in _SCENARIO:
-        last_stats.update(_scenario_stats(rts, gpus, dec["node"], res.prio, f64, integer_starts, r64))
+    elif objective in _SCENARIO_ALL:
+        last_stats.update(_scenario_stats(rts, gpus, dec["node"], res.prio, f64, integer_starts, r64, w64, d64,
+                                          objective))
         _check_horizon(Tdev, max(last_stats["scenario_makespans"]))
     elif d64 is not None:
         last_stats.update(_tardiness_stats(dec["start"], rts, w64, d64))
@@ -911,7 +955,8 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     objective="late_penalty" and "completion_penalty" (with `due` and `penalty`, sequences aligned with T's rows) as
     for solve(), with their last_stats from T's values.  objective="worst_makespan" and "mean_makespan" with
     `scenarios`, an array [J][K] of factors aligned with T's rows, as for solve(), with their last_stats from T's
-    values.
+    values; likewise "worst_tardiness" and "mean_tardiness" (with `due`) and "worst_completion" and
+    "mean_completion" (no `due`), each with `weights` optional.
     Every cell of T must be
     >= 0 (-0.0 counts as zero), +inf or a sentinel: a negative or NaN cell raises SolverError, with or without `mask`.
 
@@ -965,7 +1010,8 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
     if chains is None:
         chains = int(os.environ.get("SATURN_B200_CHAINS", 0))
         if chains <= 0:
-            wave = eng.search_wave(reduced=True, **({"objective": objective} if objective in _SCENARIO else {}))
+            wave = eng.search_wave(reduced=True, **({"objective": search_objective} if objective in _SCENARIO_ALL
+                                                    else {}))
             chains = max(1, round((1 << 17) / wave)) * wave if wave > 0 else 1 << 17
     if rounds is None:
         rounds = int(os.environ.get("SATURN_B200_ROUNDS", 400))
@@ -1014,8 +1060,9 @@ def solve_table(T, mask=None, gcount=None, presolved=None, interval=1000, timeou
         last_stats.update(_late_penalty_stats(dec["start"], rts, w64, d64, p64))
     elif objective == "completion_penalty":
         last_stats.update(_completion_penalty_stats(dec["start"], rts, w64, d64, p64))
-    elif objective in _SCENARIO:
-        last_stats.update(_scenario_stats(rts, gpus, dec["node"], res.prio, f64, integer_starts, r64))
+    elif objective in _SCENARIO_ALL:
+        last_stats.update(_scenario_stats(rts, gpus, dec["node"], res.prio, f64, integer_starts, r64, w64, d64,
+                                          objective))
         _check_horizon(Tdev, max(last_stats["scenario_makespans"]))
     elif d64 is not None:
         last_stats.update(_tardiness_stats(dec["start"], rts, w64, d64))

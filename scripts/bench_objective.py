@@ -51,7 +51,17 @@ launches alternated as above.  Then solve() on the 256-task set with K = 8 seede
 0.3, median 1): the worst- and mean-makespan plans against the nominal makespan plan, each rescored in float64 under
 the same 8 scenarios and under 64 held-out scenarios drawn from the same distribution (another seed): the worst and
 mean makespan over each set, and the nominal makespan.
-The card's name and power limit are read in the same run (nvidia-smi, read-only queries).
+--only scenario_tardiness times, on the same C4 batch read through the reduced table, the weighted tardiness on its
+normal route (the tile kernel on job-indexed rows, and the position-major kernel on rows by position) and the weighted
+mean tardiness over K = 1, 4 and 8 seeded log-normal scenarios on the two scenario routes (the generic kernel on
+job-indexed rows, the position-major kernel on rows by position), with the weights and due dates of the kernel rows,
+the eight launches alternated as above.  Then solve() on the 256-task set with the seeded integer due dates of the
+tardiness row and K = 8 seeded log-normal factors per task (sigma 0.3, median 1): the mean-tardiness plan against the
+nominal tardiness plan, and the mean-completion plan against the nominal completion plan, each rescored in float64
+under the same 8 scenarios and under 64 held-out scenarios drawn from the same distribution (another seed): the mean
+and worst total tardiness (or completion time) over each set, and the nominal value.
+The card's name, power limit and maximum SM clock are read in the same run (nvidia-smi, read-only queries), and with
+--only scenario_tardiness also the SM clock at the end of the kernel timing.
 """
 import argparse
 import json
@@ -83,10 +93,13 @@ def main():
     ap.add_argument("--solve-chains", type=int, default=0, help="0 = solve()'s default population")
     ap.add_argument("--solve-rounds", type=int, default=400)
     ap.add_argument("--only", choices=("all", "max_stretch", "squared", "late_penalty", "completion_penalty",
-                                       "scenarios"), default="all")
+                                       "scenarios", "scenario_tardiness"), default="all")
     args = ap.parse_args()
     if args.only == "scenarios":
         scenarios_main(args)
+        return
+    if args.only == "scenario_tardiness":
+        scenario_tardiness_main(args)
         return
     import numpy as np
     import torch
@@ -329,6 +342,110 @@ def scenarios_main(args):
         solve[name] = dict(rescore(plan), wall_s=wall, rounds=S.last_stats["rounds"],
                            candidates=S.last_stats["candidates"])
     print(json.dumps({"card": card(0), "kernel": kernel, "scenarios": solve}))
+    eng.close()
+
+
+def _sm_clock(index):
+    """The SM clock now, in MHz (a read-only nvidia-smi query), or None."""
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=clocks.sm", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=20).stdout.strip()
+        return float(out)
+    except Exception:  # noqa: BLE001
+        return None
+
+
+def scenario_tardiness_main(args):
+    import numpy as np
+    import torch
+    from saturn_b200 import solver as S
+    from saturn_b200.engine import Engine, opt_by_position, random_candidates
+    from saturn_b200.synth import synth_table
+    torch.cuda.set_device(0)
+    J, Sx, G = 256, 8, 8
+    B = 132 * 8 * 32 * 28                                   # bench.py's B_PER_GPU
+    T, valid = synth_table(J, Sx, G, seed=0)
+    opt, prio = random_candidates(Engine(0).set_table(T), B, valid, seed=1)
+    opt &= 7                                                # the reduced table's opt bytes: k - 1
+    obp = opt_by_position(opt, prio)
+    out = torch.empty(B, dtype=torch.float32, device=opt.device)
+    w = np.random.default_rng(2).choice([1.0, 2.0, 3.0, 5.0, 8.0, 0.25, 0.5, 1.5], size=J)
+    d = np.random.default_rng(3).integers(0, 20000, size=J)
+    engines = {}
+    for K in (1, 4, 8):                                     # one handle per scenario count, the same inputs
+        e = Engine(0)
+        e.set_table(T)
+        e.set_weights(w)
+        e.set_due(d)
+        e.set_scenarios(np.random.default_rng(40 + K).lognormal(0.0, 0.3, size=(K, J)))
+        engines[K] = e
+    runs = []
+    for route, o, kw in (("generic", opt, {}), ("position_major", obp, {"by_position": True})):
+        runs.append((route + "/weighted_tardiness", engines[1], o, dict(kw, objective="weighted_tardiness")))
+        for K in (1, 4, 8):
+            runs.append((route + "/weighted_mean_K%d" % K, engines[K], o, dict(kw, objective="weighted_mean_tardiness")))
+    times = {name: [] for name, _, _, _ in runs}
+    paths = {}
+    for i in range(args.warmup + args.steps):
+        for name, e, o, kw in runs[i % len(runs):] + runs[:i % len(runs)]:
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record()
+            e.eval(o, prio, out=out, reduced=True, **kw)
+            b.record()
+            b.synchronize()
+            paths[name] = e.last_eval_path()
+            if i >= args.warmup:
+                times[name].append(a.elapsed_time(b))
+    sm_clock = _sm_clock(0)
+    kernel = {name: dict(_median(t), path=paths[name]) for name, t in times.items()}
+    for route in ("generic", "position_major"):
+        base = kernel[route + "/weighted_tardiness"]["median_ms"]
+        for K in (1, 4, 8):
+            kernel[route + "/weighted_mean_K%d" % K]["over_tardiness"] = \
+                kernel[route + "/weighted_mean_K%d" % K]["median_ms"] / base
+    kernel.update(B=B, J=J, S=Sx, steps=args.steps, sm_clock_mhz_after=sm_clock)
+    del opt, prio, obp, out
+    for e in engines.values():
+        e.close()
+    torch.cuda.empty_cache()
+
+    eng = Engine(0)
+    tasks = _tasks256()
+    J = len(tasks)
+    due = [float(x) for x in np.random.default_rng(4).integers(0, 200000, size=J)]
+    f8 = np.random.default_rng(50).lognormal(0.0, 0.3, size=(J, 8))
+    held = np.random.default_rng(51).lognormal(0.0, 0.3, size=(64, J))
+    kw = dict(rounds=args.solve_rounds, seed=1, engine=eng, **({"chains": args.solve_chains}
+                                                               if args.solve_chains else {}))
+
+    def rescore(plan, what):
+        opt, order = S._plan_candidate(tasks, plan, 1)
+        gpus = (opt & 7).astype(np.int64) + 1
+        rts = [float(t.strategies[int(g)].runtime) for t, g in zip(tasks, gpus)]
+        node = np.zeros(J, dtype=np.int64)
+        dd = due if what == "tardiness" else None
+        obj = "mean_" + what
+        same = S._scenario_stats(rts, gpus, node, order, f8.T, True, None, None, dd, obj)
+        other = S._scenario_stats(rts, gpus, node, order, held, True, None, None, dd, obj)
+        nominal = S._scenario_stats(rts, gpus, node, order, np.ones((1, J)), True, None, None, dd, obj)
+        return {"nominal": nominal["mean_" + what], "mean_8": same["mean_" + what], "worst_8": same["worst_" + what],
+                "mean_64_held_out": other["mean_" + what], "worst_64_held_out": other["worst_" + what],
+                "nominal_makespan": plan[5]}
+    solve = {}
+    for name, obj, what in (("tardiness", "tardiness", "tardiness"), ("mean_tardiness", "mean_tardiness", "tardiness"),
+                            ("completion", "completion", "completion"),
+                            ("mean_completion", "mean_completion", "completion")):
+        okw = dict(kw)
+        if what == "tardiness":
+            okw["due"] = due
+        if obj.startswith("mean_"):
+            okw["scenarios"] = f8
+        t0 = time.perf_counter()
+        plan = S.solve(tasks, None, objective=obj, **okw)
+        wall = time.perf_counter() - t0
+        solve[name] = dict(rescore(plan, what), wall_s=wall, rounds=S.last_stats["rounds"],
+                           candidates=S.last_stats["candidates"])
+    print(json.dumps({"card": card(0), "kernel": kernel, "scenario_tardiness": solve}))
     eng.close()
 
 
